@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- RSPrompter inference hot path on B200 (contract: see the task brief / DESIGN.md section 6).
+"""bench.py -- RSPrompter inference hot path on H100 (DESIGN.md section 6).
 
     python bench.py --gpus N --steps K --warmup W [--config NAME]   # this repo's CUDA path
+    python bench.py ... --dump-outputs DIR                          # + what the last timed step computed, as .npy
     python bench.py --impl reference --gpus N --steps K ...         # the CPU oracle (reference arm)
 
 Configs (BASELINE.json `configs`):
@@ -36,7 +37,7 @@ if ROOT not in sys.path:
 import torch  # noqa: E402
 
 NUM_CLASSES, BATCH, SIZE, NQ = 10, 8, 1024, 100
-N_INPUT_SETS = 6   # distinct uint8 input batches rotated through the timed loop (6 x 25 MB > 126 MB L2)
+N_INPUT_SETS = 6   # distinct uint8 input batches rotated through the timed loop (6 x 25 MB > 50 MB L2)
 # DetDataPreprocessor of every rsprompter config (configs/rsprompter/_base_/rsprompter_anchor.py:39-48)
 PREPROC = dict(type="DetDataPreprocessor", mean=[123.675, 116.28, 103.53], std=[58.395, 57.12, 57.375], bgr_to_rgb=True,
                pad_size_divisor=32)
@@ -62,13 +63,8 @@ CONFIGS = {
 
 
 def _peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.isfile(path):
-        with open(path) as f:
-            p = json.load(f)
-        return dict(tflops=float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 1400.0))),
-                    hbm=float(p.get("hbm_gbs", 6650.0)), source="measured (MEASURED_PEAKS.json, sustained)")
-    return dict(tflops=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md: 1.4 PF sustained, 6.65 TB/s)")
+    return dict(tflops=989.0, hbm=3350.0,
+                source="H100 SXM data sheet, dense bf16 / HBM3 at 700 W (a lower power limit lowers what is reachable)")
 
 
 def _host_threads() -> int:
@@ -132,7 +128,7 @@ def _workload_config(args, n_gpus: int) -> dict:
                num_classes=NUM_CLASSES, global_batch=BATCH * n_gpus,
                parallelism=f"dp{n_gpus} (batch-sharded, weights replicated)",
                l2_policy=f"{N_INPUT_SETS} distinct uint8 input batches rotated ({N_INPUT_SETS * BATCH * 3 * size * size >> 20} MB "
-                         "in total; 126 MB L2); every step also streams tens of GB of activations through HBM, so "
+                         "in total; 50 MB L2); every step also streams tens of GB of activations through HBM, so "
                          "nothing of a step survives in L2 until the next",
                input="uint8 CHW images (PackDetInputs layout) through DetDataPreprocessor (BGR->RGB, mean/std)",
                weights="seeded random init of the exact architecture")
@@ -267,8 +263,8 @@ def run_reference(args) -> None:
 # ================================================================================================
 # this repo's arm
 # ================================================================================================
-KERNEL_GROUPS = (("gemm", "gemm_bf16_tcgen05"), ("attention_global", "vit_attention_kernel"),
-                 ("attention_window", "vit_window_attention_kernel"))
+KERNEL_GROUPS = (("gemm", r"gemm_bf16_wgmma"), ("attention_global", r"vit_attention_kernel<\d+, (32|64)>"),
+                 ("attention_window", r"vit_attention_kernel<\d+, 14>"))
 
 
 def _profile_kernels(step_fn, n_steps: int) -> list:
@@ -294,8 +290,9 @@ def _profile_kernels(step_fn, n_steps: int) -> list:
 
 
 def _roofline(model_step, trace_fn, inst_steps: int, step_ms: float, peaks: dict, args) -> dict:
-    """roofline of the dominant kernel family (the tcgen05 GEMM): sum(2MNK) / sum(kernel time), plus the encoder-only
+    """roofline of the dominant kernel family (the wgmma GEMM): sum(2MNK) / sum(kernel time), plus the encoder-only
     GEMM figure, the attention kernels and the whole step (SURVEY 8(d) i-iii)."""
+    import re
     from rsprompter_b200 import _lib
     _lib.trace = []
     trace_fn()
@@ -303,14 +300,14 @@ def _roofline(model_step, trace_fn, inst_steps: int, step_ms: float, peaks: dict
     trace, _lib.trace = _lib.trace, None
     kernels = _profile_kernels(model_step, inst_steps)
     total_ms = sum(t for _, t in kernels) / inst_steps
-    out = dict(bound="tensor", kernel="gemm_bf16_tcgen05_*_kernel (all tile shapes / epilogues)", peak=peaks["tflops"],
+    out = dict(bound="tensor", kernel="gemm_bf16_wgmma_*_kernel (all tile shapes / epilogues)", peak=peaks["tflops"],
                unit="TFLOP/s", peak_source=peaks["source"],
                method="per-kernel durations from CUPTI activity records of %d graph-replayed steps; FLOP = 2*M*N*K "
                       "(4*T^2*hd per head for attention) logged per launch" % inst_steps,
                kernel_ms_per_step=total_ms, kernels_per_step=len(kernels) // inst_steps)
     groups = {}
     for gname, pat in KERNEL_GROUPS:
-        ts = [t for n, t in kernels if pat in n]
+        ts = [t for n, t in kernels if re.search(pat, n)]
         want = [r for r in trace if r["kind"] == gname]
         g = dict(launches_per_step=len(ts) // inst_steps, ms_per_step=sum(ts) / inst_steps,
                  tflop_per_step=sum(r["flops"] for r in want) / 1e12)
@@ -328,10 +325,9 @@ def _roofline(model_step, trace_fn, inst_steps: int, step_ms: float, peaks: dict
                                                 frac=fl / (ms * 1e-3) / peaks["tflops"] if ms > 0 else 0.0)
         groups[gname] = g
     import collections
-    import re
     agg = collections.defaultdict(lambda: [0, 0.0])
     for n, t in kernels:
-        short = re.sub(r"^void |rsp::|v2::|win::", "", n)
+        short = re.sub(r"^void |rsp::|v2::", "", n)
         short = re.sub(r"\(.*", "", short)[:70]
         agg[short][0] += 1
         agg[short][1] += t
@@ -345,17 +341,34 @@ def _roofline(model_step, trace_fn, inst_steps: int, step_ms: float, peaks: dict
                              frac=tfl / (step_ms * 1e-3) / peaks["tflops"])
     # a dominant-kernel time above the step time would mean the measurement is broken (round-1 bug): refuse it
     assert gm["ms_per_step"] <= step_ms * 1.02, f"GEMM time {gm['ms_per_step']:.2f} ms exceeds the step {step_ms:.2f} ms"
-    # ncu dram bytes of the same step, per GEMM launch, from the committed capture (null until one exists)
-    out["traffic"], out["traffic_source"] = None, None
-    tpath = os.path.join(ROOT, "profiles", f"r02_traffic_{args.config}.json")
-    if os.path.exists(tpath):
-        with open(tpath) as f:
-            tj = json.load(f)
-        g = [k for k in tj["kernels"] if "gemm_bf16_tcgen05" in k["kernel"]]
-        if g:
-            out["traffic"] = sum(k["dram_read_bytes"] + k["dram_write_bytes"] for k in g) / sum(k["launches"] for k in g)
-            out["traffic_source"] = f"profiles/r02_traffic_{args.config}.json (ncu capture of one step, mean bytes per GEMM launch)"
     return out
+
+
+DUMP_MASK_SAMPLES = 1 << 22   # mask pixels sampled (fixed seed) for --dump-outputs; 16 MB as float32
+
+
+def dump_outputs(out_dir: str, variant: str, result) -> None:
+    """What a caller of the timed path receives from its last step, as float32 / float64 .npy (< 64 MB in all).  A
+    result record is written as its rows and counts, the foreground area of every mask slot, and a fixed, seeded
+    sample of its unpacked mask pixels; the encoder config writes its image embeddings."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    if variant == "encoder":
+        arrays = dict(image_embeddings=result.float().cpu().numpy())
+    else:
+        bits = result.mask_bits
+        lut = torch.tensor([bin(v).count("1") for v in range(256)], dtype=torch.int64, device=bits.device)
+        area = lut[bits.long()].sum(dim=(2, 3))
+        flat = bits.reshape(-1)
+        g = torch.Generator().manual_seed(0)
+        pix = torch.randint(0, flat.numel() * 8, (DUMP_MASK_SAMPLES,), generator=g).to(bits.device)
+        sample = (flat[pix // 8].long() >> (pix % 8)) & 1
+        arrays = dict(rows=result.rows.float().cpu().numpy(), counts=result.counts.double().cpu().numpy(),
+                      mask_area=area.double().cpu().numpy(), mask_pixel_sample=sample.float().cpu().numpy(),
+                      mask_pixel_sample_index=pix.double().cpu().numpy())
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def run_ours(args) -> None:
@@ -452,6 +465,7 @@ def run_ours(args) -> None:
         hbuf = [torch.empty(rec0.nbytes, dtype=torch.uint8).pin_memory() for _ in range(2)]
         d2h_bytes = rec0.nbytes
     side_done = [None, None]
+    last = {}   # the result of the most recent step (device buffers the next step overwrites)
 
     def compute(x):
         if variant == "encoder":
@@ -478,17 +492,19 @@ def run_ours(args) -> None:
     def step_resident(i):
         if side_done[i % 2] is not None:        # the buffer pair written two steps ago must have left
             torch.cuda.current_stream().wait_event(side_done[i % 2])
-        leave(i, compute(resident[i % N_INPUT_SETS]), to_host=False)
+        last["result"] = compute(resident[i % N_INPUT_SETS])
+        leave(i, last["result"], to_host=False)
 
     def step_e2e(i):
         if side_done[i % 2] is not None:
             torch.cuda.current_stream().wait_event(side_done[i % 2])
         if variant == "encoder":
             x = prep(dict(inputs=host[i % N_INPUT_SETS]), False, fuse_patch_embed=True)["inputs"]
-            leave(i, encoder_forward(x), to_host=True)
+            last["result"] = encoder_forward(x)
         else:   # the user-facing call: uint8 host batch -> data preprocessor -> predict -> record -> host
             data = model._preprocess(dict(inputs=host[i % N_INPUT_SETS]))
-            leave(i, model.predict_records(data["inputs"]), to_host=True)
+            last["result"] = model.predict_records(data["inputs"])
+        leave(i, last["result"], to_host=True)
 
     def barrier():
         if world > 1:
@@ -523,6 +539,8 @@ def run_ours(args) -> None:
         ms = timed(step_resident, args.steps)
         launches = _lib.launch_count - l0
         ms_e2e = timed(step_e2e, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, variant, last["result"])
 
     peaks = _peaks()
     roof, roof_err = None, None
@@ -590,7 +608,11 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="query_vith", choices=sorted(CONFIGS))
     ap.add_argument("--size", type=int, default=1024, help="image size of the encoder_vith config (512/768/1024/1280)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         run_reference(args)
     else:

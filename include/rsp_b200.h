@@ -1,4 +1,4 @@
-/* rsp_b200.h -- C ABI of librsp_b200.so: the B200 (sm_100a) kernels behind the RSPrompter
+/* rsp_b200.h -- C ABI of librsp_b200.so: the H100 (sm_90a) kernels behind the RSPrompter
  * inference hot path (SAM ViT encoder -> prompt-generator heads -> SAM mask decoder).
  *
  * The reference (KyanChen/RSPrompter) has no native code and no FFI: every operation below
@@ -32,7 +32,7 @@ extern "C" {
 int rsp_abi_version(void);
 const char* rsp_last_error(void);
 
-/* Dense contraction with fused epilogue (tcgen05 + TMA):
+/* Dense contraction with fused epilogue (wgmma + TMA):
  *   out[row_map[m], n] = act(sum_k A[m,k] * W[n,k] + bias[n]) + residual[row_map[m] % res_mod, n]
  * A bf16 [M,K]; W bf16 [N,K] (nn.Linear layout); out bf16 (out_fp32=0) or fp32.
  * act: 0 none, 1 GELU(erf), 2 ReLU.  row_map NULL = identity, -1 entries drop the row
@@ -299,7 +299,7 @@ int rsp_query_postprocess(const float* logits, const int32_t* sel, const float* 
                           int H, int W, uint8_t* masks, float* part_ws, float* scores, float* boxes, void* stream);
 
 /* ---- global attention on grids the flash kernel does not specialise (S = 48 / 80: 768^2 / 1280^2 inputs, VS:570-602):
- * three passes per image, all heads batched (rows stacked [H*T]), the two contractions on the tcgen05 GEMM:
+ * three passes per image, all heads batched (rows stacked [H*T]), the two contractions on the wgmma GEMM:
  *   Qh, Kh = rsp_split_heads(qkv)  (bf16 [H*T, hd] each),  Vt = rsp_transpose_cols(qkv)  (bf16 [H*hd, T])
  *   scores = rsp_gemm_bf16_grouped(Qh, Kh)            fp32 [H*T, T]    (group h: Q_h K_h^T)
  *   tab    = rsp_gemm_bf16(Qh, [Rh; Rw])              fp32 [H*T, 2*NT] (NT >= 2S-1 zero-padded table rows)

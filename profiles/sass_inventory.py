@@ -1,13 +1,13 @@
-"""Per-kernel SASS inventory of librsp_b200.so: counts of the Blackwell mnemonics that prove which hardware path a
-kernel uses (UTCHMMA/UTCQMMA = tcgen05.mma, LDTM/STTM = tcgen05.ld/st (TMEM), UTMALDG/UTMASTG = TMA load/store,
-UTCBAR = tcgen05.commit, HMMA = mma.sync, MUFU.EX2 = exp2).  Usage: python profiles/sass_inventory.py [out.txt]"""
+"""Per-kernel SASS inventory of librsp_b200.so: counts of the Hopper mnemonics that prove which hardware path a
+kernel uses (HGMMA = wgmma, HMMA = mma.sync, UTMALDG/UTMASTG = TMA load/store, LDSM = ldmatrix, LDGSTS = cp.async,
+SYNCS = mbarrier, MUFU.EX2 = exp2).  Usage: python profiles/sass_inventory.py [out.txt]"""
 import collections
 import re
 import subprocess
 import sys
 
 LIB = "rsprompter_b200/librsp_b200.so"
-PATS = ["UTCHMMA", "UTCQMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UTCBAR", "HMMA", "MUFU.EX2", "SYNCS", "LDGSTS"]
+PATS = ["HGMMA", "HMMA", "UTMALDG", "UTMASTG", "LDSM", "LDGSTS", "SYNCS", "MUFU.EX2"]
 
 
 def main(out=None):

@@ -1,4 +1,4 @@
-"""rsprompter_b200 -- B200-native (sm_100a) implementation of the RSPrompter inference hot path.
+"""rsprompter_b200 -- H100-native (sm_90a) implementation of the RSPrompter inference hot path.
 
 Importing the package registers the reference's model names (``RSSamVisionEncoder``,
 ``RSPrompterAnchor`` ...) in the mmengine-style ``MODELS`` registry, the same effect as the

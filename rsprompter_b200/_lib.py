@@ -23,7 +23,7 @@ class RspError(RuntimeError):
 
 
 def build_library(verbose: bool = False) -> Path:
-    """Compile every CUDA source for sm_100a into ``librsp_b200.so`` (in-tree, via make)."""
+    """Compile every CUDA source for sm_90a into ``librsp_b200.so`` (in-tree, via make)."""
     cmd = ["make", "-C", str(CSRC_DIR), "-j", str(os.cpu_count() or 4), "all"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
@@ -426,7 +426,7 @@ _head_scatter_maps: dict = {}
 def vit_attention_generic(qkv: torch.Tensor, rel_h: torch.Tensor, rel_w: torch.Tensor, n_seq: int, S: int, H: int,
                           hd: int, out: torch.Tensor | None = None) -> torch.Tensor:
     """Global attention on any grid with S % 4 == 0 and T % 128 == 0 (S = 48 / 80 for 768^2 / 1280^2 inputs): per
-    image, all heads batched along the rows - grouped tcgen05 GEMMs for Q K^T and P V, one GEMM for Q [Rh; Rw]^T, the
+    image, all heads batched along the rows - grouped wgmma GEMMs for Q K^T and P V, one GEMM for Q [Rh; Rw]^T, the
     softmax + decomposed rel-pos row kernel in between.  Intermediates per image: fp32 [H*T, T] scores, bf16 [H*T, T]
     probabilities (2.6 + 1.3 GB for ViT-H at 1280^2), reused across images."""
     global launch_count

@@ -1,4 +1,4 @@
-"""RSPrompter-anchor heads on the B200 kernels: RPNHead -> RSPrompterAnchorRoIPromptHead
+"""RSPrompter-anchor heads on the H100 kernels: RPNHead -> RSPrompterAnchorRoIPromptHead
 (SingleRoIExtractor + Shared2FCBBoxHead) -> RSPrompterAnchorMaskHead -> SAM mask decoder.
 
 Reference: mmdet/models/dense_heads/rpn_head.py:22-304, roi_heads/standard_roi_head.py:292-345,

@@ -1,537 +1,334 @@
-// ViT-SAM attention core for sm_100a: softmax(scale * q k^T + rel_h + rel_w) v per
-// (sequence, head), sequences being 14x14 windows (T = 196) or whole 64x64 images
-// (T = 4096).  Reference: transformers modeling_sam.py SamVisionAttention.forward
+// ViT-SAM attention core for sm_90a: softmax(scale * q k^T + rel_h + rel_w) v per
+// (sequence, head), sequences being 14x14 windows (T = 196) or whole 32x32 / 64x64 images
+// (T = 1024 / 4096).  Reference: transformers modeling_sam.py SamVisionAttention.forward
 // (:803-831), get_rel_pos / get_decomposed_rel_pos (:729-801); mmpretrain vit_sam.py
 // Attention.forward (:202-221), add_decomposed_rel_pos (:117-157).
 //
-// One CTA = 128 query rows of one (sequence, head); 320 threads:
-//   warps 0-7  softmax: thread (r, h) owns query row r and the 32-key chunks c with c % 2 == h of every
-//              128-key tile (warps w and w + 4 share TMEM lane quarter w).  The two key halves of a row are
-//              two independent online-softmax streams (own running max m_h, own sum l_h, own accumulator O_h
-//              in TMEM, the MMA warp routes each 16-key step of P V to the accumulator of the half that owns
-//              it), merged once at the end like a split-K flash decode:
-//                  O = (O_0 2^(m_0 - m) + O_1 2^(m_1 - m)) / (l_0 2^(m_0 - m) + l_1 2^(m_1 - m)).
-//              Nothing is exchanged inside the key loop, each thread keeps only 32 rel_w values in registers,
-//              and 16 softmax warps per SM (2 CTAs) hide the TMEM / MUFU latencies that 8 could not.
-//              Exponentials use the running max as reference and are redone only when a score exceeds it by
-//              more than 2^8 (O_h rescaled then); fp32 statistics; P (bf16) goes to 128B-swizzled smem.
-//   warp 8     TMA producer (Q once; K_j / V_j tiles; the two rel-pos tables) + TMEM alloc
-//   warp 9     tcgen05.mma issuer: S_j = Q K_j^T (128x128x hd), O_h += P_j V_j over the key steps of half h,
-//              V consumed straight from the qkv matrix as an MN-major operand
-// hd 80 (ViT-H) cannot afford two 80-column accumulators next to two score tiles in the 256 TMEM columns a CTA gets
-// at 2 CTAs / SM, and with a single score tile every key tile is a serial  Q K^T -> softmax -> P V  chain (ncu: 46 %
-// of all warp samples sat on the "S ready" barrier).  For HD > 64 the two key halves of a row therefore share ONE
-// accumulator and one running reference: the pair exchanges its chunk bounds through shared memory once per tile
-// (one bar.sync of the two warps of a lane quarter), both threads take the same rescale decision and each rescales
-// its share of the accumulator's columns.  That frees the columns for a second score tile: Q K_{j+1}^T runs while the
-// softmax warps work on tile j, as in the hd 64 pipeline.  K is double-buffered in shared memory (the second stage
-// lives in the half of the rel_w table region that relh_s does not use), V stays single-buffered (its load hides
-// behind the softmax of the same tile).
-// The decomposed relative-position bias is never materialised as a T x T tensor: a
-// prologue MMA computes Q (unscaled) x table^T for both tables (the reference's two
-// einsums), each thread gathers the values its row / key half needs, and the bias is added
-// inside the softmax FMA.  Scores stay fp32 until the exp (reference: softmax in fp32).
+// Flash-style, everything in registers: one CTA = 64 query rows of one (sequence, head), 4 warps of 16 rows each.
+// Scores and the output accumulator are bf16 mma.sync m16n8k16 fragments with fp32 accumulation; the score fragment
+// of a 64-key tile becomes, after the online softmax, the A operand of P V without leaving the registers.  P V runs in
+// fp16 (P in [0, 1] keeps 11 mantissa bits instead of bf16's 8; each V tile is converted in shared memory, exactly for
+// |v| in fp16's normal range).  K / V tiles stream through a two-stage cp.async ring (rows padded by 16 bytes:
+// conflict-free ldmatrix).
+// The decomposed relative-position bias is never materialised as a T x T tensor: a prologue runs Q x table^T for both
+// tables on the same tensor-core path (the reference's two einsums), scatters each row's S + S values (pre-multiplied
+// by log2 e) into shared memory, and the bias is added to the scores before the exp.  Scores stay fp32 until the exp
+// (reference: softmax in fp32).
 #include <cstdlib>
 
 #include "attention.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace rsp {
 
-constexpr int ATT_THREADS = 320;
 constexpr float LOG2E = 1.4426950408889634f;
 
-__device__ __forceinline__ float max3(float a, float b, float c) {   // one FMNMX3
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+// d (+)= a[16 x 16] * b[16 x 8], bf16 (or fp16) in, fp32 accumulators (row.col)
+__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void mma_f16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
+  __half2 v = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
 
-template <int HD>
+template <int HD, int S>
 struct AttCfg {
-  static constexpr int NA = (HD + 63) / 64;           // 64-wide swizzle atoms per head
-  static constexpr bool ONE_ACC = HD > 64;            // hd 80: one shared accumulator, pair-exchanged running max
-  static constexpr int VBUF = ONE_ACC ? 1 : 2;        // V stages in shared memory (K and S always have 2)
-  static constexpr int Q_BYTES = NA * 16384;          // 128 rows x NA x 128 B
-  static constexpr int KV_BYTES = NA * 8192;          // one 64-key stage of K or V
-  static constexpr int TAB_BYTES = NA * 16384;        // a rel-pos table in the prologue (<= 128 rows x NA x 128 B)
-  static constexpr int SCRATCH_BYTES = 32768;         // prologue gather scratch: [kw <= 64][128] fp32
-  static constexpr int RELH_BYTES = 64 * 128 * 2;     // global: [kh][row] fp16
-  // hd 64: [Q | K x2 (rel_h table) | V x2 (rel_w table) | scratch | relh_s]
-  // hd 80: [Q | A: rel_h table -> scratch -> K_0, V | B: rel_w table -> relh_s, K_1]   (K / V loads wait for the gather)
-  static constexpr int SMEM_BYTES = ONE_ACC ? Q_BYTES + 2 * TAB_BYTES + 1024
-                                            : Q_BYTES + 4 * KV_BYTES + SCRATCH_BYTES + RELH_BYTES + 1024;
-  static constexpr int O_STRIDE = 64;                 // hd 64: column distance between the two accumulators
-  static constexpr int O_COL = 128;                   // S_0 [0,64) S_1 [64,128) | hd 64: O_0 [128,192) O_1 [192,256)
-  static constexpr int TMEM_COLS = 256;               //                          | hd 80: O [128,208)
-  static_assert(!ONE_ACC || (KV_BYTES * 2 <= TAB_BYTES && RELH_BYTES + KV_BYTES <= TAB_BYTES), "hd 80 smem aliasing");
+  static constexpr int T = S * S;
+  static constexpr int HDP = HD + 8;                  // padded smem row (bf16): 16-byte rows shift banks
+  static constexpr int CH = HD / 8;                   // 16-byte chunks per row
+  static constexpr int NKT = (T + 63) / 64;           // 64-key tiles
+  static constexpr int NREL = 2 * S - 1;              // rel-pos table rows
+  static constexpr int NTG = (NREL + 63) / 64;        // 64-row groups of a table
+  static constexpr int SP = S + 4;                    // row stride of the gathered bias (floats)
+  static constexpr int Q_ELEMS = 64 * HDP;
+  static constexpr int KV_ELEMS = 128 * HDP;          // two 64-key stages (in the prologue: one whole table)
+  static constexpr int SMEM_BYTES = (Q_ELEMS + 2 * KV_ELEMS) * 2 + 2 * 64 * SP * 4;
+  static_assert(NREL <= 128, "table rows");
 };
 
 struct AttDev {
+  const __nv_bfloat16* qkv;
+  const __nv_bfloat16* rel_h;
+  const __nv_bfloat16* rel_w;
   __nv_bfloat16* out;  // [M_tok, D]
-  int T;               // tokens per sequence
-  int S;               // sqrt(T)
   int H;
   int D;
-  int n_qt;            // 128-query tiles per sequence
-  int n_kt;            // 64-key tiles per sequence
+  int n_qt;            // 64-query tiles per sequence
   float scale2;        // hd^-0.5 * log2(e)
   const int* out_row_map;   // window_unpartition + crop fused into the store (HF:925-952), or null
 };
 
-// barriers: two-slot rings indexed by tile parity; phase of slot use n is (n >> 1) & 1
-enum { B_Q = 0, B_REL, B_RELC, B_KF, B_KE = B_KF + 2, B_VF = B_KE + 2, B_VE = B_VF + 2, B_SF = B_VE + 2,
-       B_PF = B_SF + 2, B_PV = B_PF + 2, B_COUNT = B_PV + 2 };
+template <int HD, int S>
+__global__ void __launch_bounds__(128)
+vit_attention_kernel(const AttDev p) {
+  using C = AttCfg<HD, S>;
+  constexpr int T = C::T, HDP = C::HDP, CH = C::CH, SP = C::SP;
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_raw);
+  __nv_bfloat16* sK = sQ + C::Q_ELEMS;
+  __nv_bfloat16* sV = sK + C::KV_ELEMS;
+  float* relh = reinterpret_cast<float*>(sV + C::KV_ELEMS);   // [64][SP]: rel_h term of (row, key row kh)
+  float* relw = relh + 64 * SP;                               // [64][SP]: rel_w term of (row, key column kw)
 
-template <int HD, int GS>   // GS = 0: 14x14 windows; GS = 64 / 32: global attention over a GS x GS grid
-__global__ void __launch_bounds__(ATT_THREADS, 2)
-vit_attention_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_kv,
-                     const __grid_constant__ CUtensorMap tm_relh,
-                     const __grid_constant__ CUtensorMap tm_relw, const AttDev p) {
-  using Cfg = AttCfg<HD>;
-  constexpr int NA = Cfg::NA;
-  constexpr bool GLOBAL = GS > 0;
-  constexpr int NREL = GLOBAL ? 2 * GS : 32;  // padded table rows (2S-1 = 127 / 63 / 27)
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bars[B_COUNT];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ float2 xchg[2][128];            // hd 64: (m, l) of each key half, exchanged once at the end;
-                                             // hd 80: per-tile chunk bounds [tile parity][row] (.x / .y = key half 0 / 1)
-
-  constexpr bool ONE_ACC = Cfg::ONE_ACC;
-  constexpr int VBUF = Cfg::VBUF;
-  const uint32_t sQ = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sTabH = sQ + Cfg::Q_BYTES;                               // rel_h table (prologue)
-  const uint32_t sTabW = sTabH + (ONE_ACC ? Cfg::TAB_BYTES : 2 * Cfg::KV_BYTES);   // rel_w table (prologue)
-  const uint32_t sK0 = sTabH;                                            // K stage 0
-  const uint32_t sK1 = ONE_ACC ? sTabW + Cfg::RELH_BYTES : sTabH + Cfg::KV_BYTES;   // K stage 1
-  const uint32_t sV = ONE_ACC ? sTabH + Cfg::KV_BYTES : sTabW;           // V stage(s)
-  const uint32_t sScr = ONE_ACC ? sTabH : sTabW + 2 * Cfg::KV_BYTES;     // gather scratch
-  const uint32_t sRH = ONE_ACC ? sTabW : sScr + Cfg::SCRATCH_BYTES;      // relh_s
-  uint8_t* gP = smem_raw + (sScr - smem_u32(smem_raw));
-  uint8_t* gRH = smem_raw + (sRH - smem_u32(smem_raw));
-  // two-slot rings (K, S, P): slot = t & 1, phase of use n of a slot = (n >> 1) & 1; the V ring has VBUF slots
-  auto slot = [](int t) { return t & 1; };
-  auto phase = [](int t) -> uint32_t { return (t >> 1) & 1; };
-  auto vslot = [](int t) { return VBUF == 1 ? 0 : (t & 1); };
-  auto vphase = [](int t) -> uint32_t { return VBUF == 1 ? (t & 1) : ((t >> 1) & 1); };
-  auto sK = [&](int sl) { return sl ? sK1 : sK0; };
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int bid = blockIdx.x;
   const int qt = bid % p.n_qt; bid /= p.n_qt;
   const int head = bid % p.H;
   const int seq = bid / p.H;
-  const int row0 = seq * p.T;            // first token row of this sequence in qkv
-  const int q0 = qt * 128;               // first query of this tile inside the sequence
-  const int colq = head * HD;
-  const int colk = p.D + head * HD;
-  const int colv = 2 * p.D + head * HD;
+  const int q0 = qt * 64;
+  const size_t ld = static_cast<size_t>(3) * p.D;
+  const __nv_bfloat16* base = p.qkv + static_cast<size_t>(seq) * T * ld;
+  const int colq = head * HD, colk = p.D + head * HD, colv = 2 * p.D + head * HD;
 
-  auto bar = [&](int i) { return smem_u32(&bars[i]); };
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tm_qkv);
-    tma_prefetch_desc(&tm_kv);
-    tma_prefetch_desc(&tm_relh);
-    tma_prefetch_desc(&tm_relw);
-    for (int i = 0; i < B_COUNT; ++i)
-      mbar_init(bar(i), (i == B_RELC || i == B_PF || i == B_PF + 1) ? 256 : 1);
-    fence_barrier_init();
-  }
-  if (warp == 8) tmem_alloc(smem_u32(&tmem_base_s), Cfg::TMEM_COLS);
-  tc_fence_before();
+  // rows [r0, r0 + nrows) of a [*, ldr] bf16 matrix (columns col0 .. col0 + HD) -> padded smem; rows >= nvalid -> 0
+  auto load_rows = [&](__nv_bfloat16* dst, const __nv_bfloat16* src, size_t ldr, int col0, int r0, int nrows,
+                       int nvalid) {
+    for (int i = tid; i < nrows * CH; i += 128) {
+      const int r = i / CH, c = i - (i / CH) * CH;
+      const bool ok = r0 + r < nvalid;
+      const __nv_bfloat16* g = src + static_cast<size_t>(ok ? r0 + r : 0) * ldr + col0 + c * 8;
+      cp_async16(smem_u32(dst + r * HDP + c * 8), g, ok);
+    }
+  };
+  load_rows(sQ, base, ld, colq, q0, 64, T);
+  load_rows(sK, p.rel_h, HD, 0, 0, C::NTG * 64, C::NREL);
+  load_rows(sV, p.rel_w, HD, 0, 0, C::NTG * 64, C::NREL);
+  cp_async_commit();
+  cp_async_wait<0>();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
-  const uint32_t tS = tmem_base;                             // S_0 | S_1 (and the rel_h prologue product)
-  const uint32_t tOpro = tmem_base + 128;                    // rel_w prologue product
-  const uint32_t tO = tmem_base + Cfg::O_COL;                // accumulator (hd 64: of key half 0)
-  const uint32_t tO1 = ONE_ACC ? tO : tO + Cfg::O_STRIDE;    // hd 64: accumulator of key half 1
-  const int n_kt = GLOBAL ? p.n_kt : 4;
 
-  if (warp == 8 && lane == 0) {
-    // ------------------------------------------------------------ TMA producer
-    mbar_expect_tx(bar(B_Q), Cfg::Q_BYTES + 2 * NA * NREL * 128);
+  // this thread's fragment coordinates: rows rl + 8 i (i = 0, 1) of the warp's 16, columns 2 (lane % 4) + {0, 1}
+  const int rl = warp * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  uint32_t qf[HD / 16][4];
 #pragma unroll
-    for (int a = 0; a < NA; ++a) {
-      tma_load_2d(sQ + a * 16384, &tm_qkv, bar(B_Q), colq + a * 64, row0 + q0);
-      tma_load_2d(sTabH + a * 16384, &tm_relh, bar(B_Q), a * 64, 0);
-      tma_load_2d(sTabW + a * 16384, &tm_relw, bar(B_Q), a * 64, 0);
-    }
-    if (ONE_ACC) mbar_wait(bar(B_RELC), 0);   // the gather scratch / dead tables live where K / V land
-    auto load_k = [&](int t) {
-      const int s = slot(t);
-      mbar_wait(bar(B_KE + s), phase(t));     // phase 0 of the "empty" slots completes with the prologue MMAs
-      mbar_expect_tx(bar(B_KF + s), Cfg::KV_BYTES);
-#pragma unroll
-      for (int a = 0; a < NA; ++a)
-        tma_load_2d(sK(s) + a * 8192, &tm_kv, bar(B_KF + s), colk + a * 64, row0 + t * 64);
-    };
-    auto load_v = [&](int t) {
-      const int vs = vslot(t);
-      mbar_wait(bar(B_VE + vs), vphase(t));
-      mbar_expect_tx(bar(B_VF + vs), Cfg::KV_BYTES);
-#pragma unroll
-      for (int a = 0; a < NA; ++a)
-        tma_load_2d(sV + vs * Cfg::KV_BYTES + a * 8192, &tm_kv, bar(B_VF + vs), colv + a * 64, row0 + t * 64);
-    };
-    if (ONE_ACC) {
-      // single V stage: V_j can only be fetched once P V_{j-1} has drained it, so K runs one tile ahead of that wait
-      // (otherwise Q K_{j+1}^T - which only needs K - would sit behind V_j's wait and the second S tile buys nothing)
-      load_k(0);
-      for (int j = 0; j < n_kt; ++j) {
-        if (j + 1 < n_kt) load_k(j + 1);
-        load_v(j);
-      }
-    } else {
-      for (int j = 0; j < n_kt; ++j) { load_k(j); load_v(j); }
-    }
-  } else if (warp == 9 && lane == 0) {
-    // ------------------------------------------------------------ MMA issuer (own warp: sharing the producer's
-    // warp makes the two spin loops diverge inside one warp, measured 20 % slower)
-    constexpr uint32_t idesc_s = make_idesc_bf16(128, 64, 0, 0);
-    constexpr uint32_t idesc_rel = make_idesc_bf16(128, NREL, 0, 0);
-    constexpr uint32_t idesc_pv = make_idesc_bf16(128, HD, 0, 1);
-    mbar_wait(bar(B_Q), 0);
-    tc_fence_after();
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks) {
-      const uint32_t off = (ks >> 2) * 16384 + (ks & 3) * 32;
-      umma_ss(tS, make_sdesc(sQ + off, 0, 1024), make_sdesc(sTabH + off, 0, 1024), idesc_rel, ks != 0);
-    }
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks) {
-      const uint32_t off = (ks >> 2) * 16384 + (ks & 3) * 32;
-      umma_ss(tOpro, make_sdesc(sQ + off, 0, 1024), make_sdesc(sTabW + off, 0, 1024), idesc_rel, ks != 0);
-    }
-    umma_commit(bar(B_REL));
-    umma_commit(bar(B_KE));
-    umma_commit(bar(B_KE + 1));
-    umma_commit(bar(B_VE));
-    if (Cfg::VBUF == 2) umma_commit(bar(B_VE + 1));
-    mbar_wait(bar(B_RELC), 0);
-    tc_fence_after();
-    auto issue_qk = [&](int t) {   // S_slot(t) = Q K_t^T
-      const int s = slot(t);
-      mbar_wait(bar(B_KF + s), phase(t));
-      if (t >= 2) mbar_wait(bar(B_PV + s), phase(t - 2));   // P V of the previous user has consumed S_s / P_s
-      tc_fence_after();
-#pragma unroll
-      for (int ks = 0; ks < HD / 16; ++ks) {
-        const uint32_t qoff = (ks >> 2) * 16384 + (ks & 3) * 32;
-        const uint32_t koff = (ks >> 2) * 8192 + (ks & 3) * 32;
-        umma_ss(tS + s * 64, make_sdesc(sQ + qoff, 0, 1024), make_sdesc(sK(s) + koff, 0, 1024), idesc_s, ks != 0);
-      }
-      umma_commit(bar(B_SF + s));
-      if (t + 2 < n_kt) umma_commit(bar(B_KE + s));   // "empty" is only signalled when load_k(t + 2) will wait for it
-    };
-    issue_qk(0);
-    for (int j = 0; j < n_kt; ++j) {
-      if (j + 1 < n_kt) issue_qk(j + 1);      // runs while the softmax warps work on tile j
-      const int s = slot(j), vs = vslot(j);
-      mbar_wait(bar(B_PF + s), phase(j));
-      mbar_wait(bar(B_VF + vs), vphase(j));
-      tc_fence_after();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {   // 16 keys per step; 32-key chunk ks >> 1 belongs to key half ks >> 1
-        // A = P straight from TMEM: 8 packed bf16x2 columns per step, written in place over the chunk's scores
-        const uint32_t a_tmem = tS + s * 64 + (ks >> 1) * 32 + (ks & 1) * 8;
-        const uint64_t bdesc = make_sdesc(sV + vs * Cfg::KV_BYTES + ks * 2048, 8192, 1024);
-        if (ONE_ACC) umma_ts(tO, a_tmem, bdesc, idesc_pv, (j | ks) != 0);
-        else umma_ts((ks >> 1) ? tO1 : tO, a_tmem, bdesc, idesc_pv, (j | (ks & 1)) != 0);
-      }
-      umma_commit(bar(B_PV + s));
-      if (j + Cfg::VBUF < n_kt) umma_commit(bar(B_VE + vs));
-    }
-  } else if (warp < 8) {
-    // ------------------------------------------------------------ softmax / correction / output
-    const int q4 = warp & 3, hf = warp >> 2;
-    const int r = q4 * 32 + lane;            // query row inside the tile == TMEM lane
-    const uint32_t lane_off = static_cast<uint32_t>(q4 * 32) << 16;
-    const int tq = q0 + r;                    // query index inside the sequence
-    const int qh = tq / p.S;
-    const int qw = tq - qh * p.S;
-    constexpr int NW = GLOBAL ? 32 : 14;      // rel_w values kept in registers (this thread's key columns)
-    constexpr int NH = GLOBAL ? 1 : 14;       // rel_h in registers (window) or smem (global)
-    float relw[NW];
-    float relh[NH];
-    (void)relh;
-    auto pair_sync = [&]() { asm volatile("bar.sync %0, 64;" ::"r"(1 + q4) : "memory"); };
+  for (int kk = 0; kk < HD / 16; ++kk)
+    ldsm_x4(smem_u32(sQ + (warp * 16 + (lane & 15)) * HDP + kk * 16 + (lane >> 4) * 8), qf[kk][0], qf[kk][1],
+            qf[kk][2], qf[kk][3]);
+  // B operand (x4: two 8-row blocks of K-like [rows][HD] smem at k-step kk)
+  const int b_row = (lane & 7) + ((lane >> 4) << 3), b_col = ((lane >> 3) & 1) * 8;
 
-    // ---- prologue: gather this row's rel-pos terms (pre-multiplied by log2 e); half 0 takes rel_h, half 1 rel_w
-    mbar_wait(bar(B_REL), 0);
-    tc_fence_after();
-    float* scratch = reinterpret_cast<float*>(gP);  // aliases the P buffers (unused yet): [kw][128] fp32, 32 KB
-    __half* relh_s = reinterpret_cast<__half*>(gRH);
-    if (GLOBAL) {
-      // table index t <-> key coordinate k: t = q - k + (GS - 1)
-      if (hf == 0) {
+  // ---- prologue: Q x table^T for both tables, gathered into relh / relw (this warp's 16 rows only)
 #pragma unroll 1
-        for (int c = 0; c < NREL / 16; ++c) {
-          uint32_t v[16];
-          tmem_ld_32x32b_x16(tS + lane_off + c * 16, v);
-          tmem_ld_wait();
+  for (int tab = 0; tab < 2; ++tab) {
+    const __nv_bfloat16* tb = tab ? sV : sK;
+    float* dst = tab ? relw : relh;
+#pragma unroll 1
+    for (int g = 0; g < C::NTG; ++g) {
+      float acc[8][4];
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int kh = qh + (GS - 1) - (c * 16 + i);
-            if (kh >= 0 && kh < GS) relh_s[kh * 128 + r] = __float2half_rn(__uint_as_float(v[i]) * LOG2E);
+      for (int nb = 0; nb < 8; ++nb) acc[nb][0] = acc[nb][1] = acc[nb][2] = acc[nb][3] = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < HD / 16; ++kk) {
+#pragma unroll
+        for (int np = 0; np < 4; ++np) {
+          uint32_t b0, b1, b2, b3;
+          ldsm_x4(smem_u32(tb + (g * 64 + np * 16 + b_row) * HDP + kk * 16 + b_col), b0, b1, b2, b3);
+          mma_bf16(acc[2 * np], qf[kk], b0, b1);
+          mma_bf16(acc[2 * np + 1], qf[kk], b2, b3);
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int r = rl + 8 * i;
+        const int tq = q0 + r;
+        const int qc = tab ? tq % S : tq / S;   // query coordinate along the table's axis
+#pragma unroll
+        for (int nb = 0; nb < 8; ++nb) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int t = g * 64 + nb * 8 + cq + e;   // table index t = q - k + S - 1
+            const int k = qc + S - 1 - t;
+            if (t < C::NREL && k >= 0 && k < S) dst[r * SP + k] = acc[nb][2 * i + e] * LOG2E;
           }
         }
-      } else {
-#pragma unroll 1
-        for (int c = 0; c < NREL / 16; ++c) {
-          uint32_t v[16];
-          tmem_ld_32x32b_x16(tOpro + lane_off + c * 16, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int kw = qw + (GS - 1) - (c * 16 + i);
-            if (kw >= 0 && kw < GS) scratch[kw * 128 + r] = __uint_as_float(v[i]) * LOG2E;
-          }
-        }
-      }
-      pair_sync();
-      const int kw0 = (GS == 64) ? 32 * hf : 0;   // key column of this thread's 32-key chunk
-#pragma unroll
-      for (int i = 0; i < NW; ++i) relw[i] = scratch[(kw0 + i) * 128 + r];
-    } else {
-      uint32_t v[32];
-      if (hf == 0) {
-        tmem_ld_32x32b_x32(tS + lane_off, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 27; ++i) {
-          const int kh = qh + 13 - i;
-          if (kh >= 0 && kh < 14) scratch[kh * 128 + r] = __uint_as_float(v[i]) * LOG2E;
-        }
-      } else {
-        tmem_ld_32x32b_x32(tOpro + lane_off, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 27; ++i) {
-          const int kw = qw + 13 - i;
-          if (kw >= 0 && kw < 14) scratch[(14 + kw) * 128 + r] = __uint_as_float(v[i]) * LOG2E;
-        }
-      }
-      pair_sync();
-      if (qh < 14) {
-#pragma unroll
-        for (int i = 0; i < 14; ++i) { relh[i] = scratch[i * 128 + r]; relw[i] = scratch[(14 + i) * 128 + r]; }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 14; ++i) { relh[i] = 0.f; relw[i] = 0.f; }
-      }
-    }
-    tc_fence_before();
-    mbar_arrive(bar(B_RELC));
-
-    float m_run = -INFINITY, l_run = 0.f;
-    const float scale2 = p.scale2;
-    const int T = GLOBAL ? p.T : 196;          // window: compile-time so key -> (kh, kw) folds
-    const uint32_t tOme = hf ? tO1 : tO;
-    // largest bias this thread can add to a score (bounds the tile maximum from the raw accumulator maximum)
-    float bias_max = -INFINITY;
-    if (GLOBAL) {
-#pragma unroll
-      for (int i = 0; i < NW; ++i) bias_max = fmaxf(bias_max, relw[i]);
-    } else {
-      float a = -INFINITY, b = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 14; ++i) { a = fmaxf(a, relh[i]); b = fmaxf(b, relw[i]); }
-      bias_max = a + b;
-    }
-    // hd 80: the accumulator's 16-column chunks this thread rescales / stores (its share of the shared accumulator)
-    constexpr int NC0 = (HD / 16 + 1) / 2;     // chunks of half 0 (hd 80: 3 of 5; hd 64: 2 of 4)
-    const int c_lo = hf ? NC0 : 0, c_hi = hf ? HD / 16 : NC0;
-
-#pragma unroll(GLOBAL ? 1 : 4)
-    for (int j = 0; j < n_kt; ++j) {
-      const int s = slot(j);
-      const uint32_t ph = phase(j);
-      mbar_wait(bar(B_SF + s), ph);
-      tc_fence_after();
-      float rh = 0.f;
-      if (GLOBAL) rh = __half2float(relh_s[((GS == 64 ? j : 2 * j + hf)) * 128 + r]);   // image row of my chunk
-      const int key0 = j * 64 + hf * 32;                 // first key of my 32-key chunk
-      const uint32_t t_chunk = tS + lane_off + s * 64 + hf * 32;
-      // ---- upper bound of this chunk's scores from the raw accumulator maximum (scale2 > 0): the exponent
-      // reference only has to be an upper bound that is not absurdly loose, so no second look at the scores is
-      // ever needed and P can overwrite them in place
-      float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int h16 = 0; h16 < 2; ++h16) {
-        uint32_t v[16];
-        tmem_ld_32x32b_x16(t_chunk + h16 * 16, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 8; ++i) mx4[i & 3] = max3(mx4[i & 3], __uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]));
-      }
-      float bound = fmaf(fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3])), scale2, rh + bias_max);
-      if (ONE_ACC) {
-        // one reference per ROW: the two threads of a row see both chunk bounds and take the same decision
-        float* xb = reinterpret_cast<float*>(&xchg[j & 1][r]);
-        xb[hf] = bound;
-        pair_sync();
-        bound = fmaxf(bound, xb[hf ^ 1]);
-      }
-      const bool need = bound > m_run + 8.0f;
-      if (__any_sync(0xffffffffu, need)) {
-        // the reference moves up (always on the first tile, rarely later): the accumulator / l are rescaled
-        const float alpha = need ? fast_exp2(m_run - bound) : 1.0f;
-        l_run *= alpha;
-        m_run = need ? bound : m_run;
-        if (j > 0) {
-          mbar_wait(bar(B_PV + slot(j - 1)), phase(j - 1));     // P V of tile j-1 has landed in the accumulator
-          tc_fence_after();
-          if (ONE_ACC) {
-#pragma unroll 1
-            for (int c = c_lo; c < c_hi; ++c) {                 // my share of the shared accumulator's columns
-              uint32_t o[16];
-              tmem_ld_32x32b_x16(tO + lane_off + c * 16, o);
-              tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-              tmem_st_32x32b_x16(tO + lane_off + c * 16, o);
-            }
-          } else {
-#pragma unroll
-            for (int c = 0; c < HD / 16; ++c) {
-              uint32_t o[16];
-              tmem_ld_32x32b_x16(tOme + lane_off + c * 16, o);
-              tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-              tmem_st_32x32b_x16(tOme + lane_off + c * 16, o);
-            }
-          }
-          tmem_st_wait();
-        }
-      }
-      // ---- P = exp2(t - m_run) (bf16, packed, written over the chunk's own scores), row sum
-      const float rhm = rh - m_run;
-      float ls4[4] = {0.f, 0.f, 0.f, 0.f};
-      uint32_t pk[16];
-#pragma unroll
-      for (int h16 = 0; h16 < 2; ++h16) {
-        if (!GLOBAL && key0 + h16 * 16 >= T) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) pk[h16 * 8 + i] = 0u;
-        } else {
-          uint32_t v[16];
-          tmem_ld_32x32b_x16(t_chunk + h16 * 16, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float e0, e1;
-            if (GLOBAL) {
-              e0 = fast_exp2(fmaf(__uint_as_float(v[2 * i]), scale2, rhm) + relw[h16 * 16 + 2 * i]);
-              e1 = fast_exp2(fmaf(__uint_as_float(v[2 * i + 1]), scale2, rhm) + relw[h16 * 16 + 2 * i + 1]);
-            } else {
-              const int k0 = key0 + h16 * 16 + 2 * i, k1 = k0 + 1;   // resolved after unrolling j
-              const int kh0 = k0 / 14, kw0 = k0 - kh0 * 14, kh1 = k1 / 14, kw1 = k1 - kh1 * 14;
-              e0 = (k0 < T) ? fast_exp2(fmaf(__uint_as_float(v[2 * i]), scale2, relh[kh0 < 14 ? kh0 : 0] - m_run) + relw[kw0]) : 0.f;
-              e1 = (k1 < T) ? fast_exp2(fmaf(__uint_as_float(v[2 * i + 1]), scale2, relh[kh1 < 14 ? kh1 : 0] - m_run) + relw[kw1]) : 0.f;
-            }
-            ls4[i & 3] += e0 + e1;
-            pk[h16 * 8 + i] = pack_bf16x2(e0, e1);
-          }
-        }
-      }
-      tmem_st_32x32b_x16(t_chunk, pk);
-      l_run += (ls4[0] + ls4[1]) + (ls4[2] + ls4[3]);
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(bar(B_PF + s));
-    }
-
-    // ---- epilogue: O / l -> out[token, head*HD .. ]  (hd 64: merge the two key halves first)
-    mbar_wait(bar(B_PV + slot(n_kt - 1)), phase(n_kt - 1));
-    tc_fence_after();
-    pair_sync();                               // hd 80: the last tile's bound exchange has been read by both threads
-    xchg[hf][r] = make_float2(m_run, l_run);
-    pair_sync();
-    const float2 other = xchg[hf ^ 1][r];
-    float w_me, w_ot;
-    if (ONE_ACC) {                             // same reference in both halves: the sums simply add
-      w_me = 1.0f / (l_run + other.y);
-      w_ot = 0.f;
-    } else {
-      const float m_all = fmaxf(m_run, other.x);
-      const float a_me = fast_exp2(m_run - m_all), a_ot = fast_exp2(other.x - m_all);
-      const float inv = 1.0f / (l_run * a_me + other.y * a_ot);
-      w_me = a_me * inv; w_ot = a_ot * inv;
-    }
-    const uint32_t tOot = hf ? tO : tO1;
-    int dst_row = row0 + tq;
-    if (p.out_row_map && tq < T) dst_row = __ldg(p.out_row_map + dst_row);
-    const bool store = tq < T && dst_row >= 0;
-    __nv_bfloat16* orow = p.out + static_cast<size_t>(store ? dst_row : 0) * p.D + colq;
-#pragma unroll 1
-    for (int c = c_lo; c < c_hi; ++c) {
-      uint32_t o[16], o2[16];
-      tmem_ld_32x32b_x16(tOme + lane_off + c * 16, o);
-      if (!ONE_ACC) tmem_ld_32x32b_x16(tOot + lane_off + c * 16, o2);
-      tmem_ld_wait();
-      if (store) {
-        float f[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-          f[i] = ONE_ACC ? __uint_as_float(o[i]) * w_me : __uint_as_float(o[i]) * w_me + __uint_as_float(o2[i]) * w_ot;
-        uint4 w0 = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]),
-                              pack_bf16x2(f[6], f[7]));
-        uint4 w1 = make_uint4(pack_bf16x2(f[8], f[9]), pack_bf16x2(f[10], f[11]), pack_bf16x2(f[12], f[13]),
-                              pack_bf16x2(f[14], f[15]));
-        reinterpret_cast<uint4*>(orow + c * 16)[0] = w0;
-        reinterpret_cast<uint4*>(orow + c * 16)[1] = w1;
       }
     }
   }
+  __syncthreads();   // the tables' smem becomes the K / V ring
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  auto load_kv = [&](int j) {
+    const int st = j & 1;
+    load_rows(sK + st * 64 * HDP, base, ld, colk, j * 64, 64, T);
+    load_rows(sV + st * 64 * HDP, base, ld, colv, j * 64, 64, T);
+    cp_async_commit();
+  };
+  load_kv(0);
+
+  float o[HD / 8][4];
+#pragma unroll
+  for (int nb = 0; nb < HD / 8; ++nb) o[nb][0] = o[nb][1] = o[nb][2] = o[nb][3] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const float scale2 = p.scale2;
+  const float* bh[2] = {relh + rl * SP, relh + (rl + 8) * SP};
+  const float* bw[2] = {relw + rl * SP, relw + (rl + 8) * SP};
+  // V operand (x4 trans: two 8-key halves of a 16-key step, two 8-column blocks)
+  const int v_row = (lane & 7) + ((lane >> 3) & 1) * 8, v_col = (lane >> 4) * 8;
+
+#pragma unroll 1
+  for (int j = 0; j < C::NKT; ++j) {
+    if (j + 1 < C::NKT) {
+      load_kv(j + 1);
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    const __nv_bfloat16* Ks = sK + (j & 1) * 64 * HDP;
+    const __nv_bfloat16* Vs = sV + (j & 1) * 64 * HDP;
+    {   // V tile bf16 -> fp16 in place
+      uint32_t* v32 = reinterpret_cast<uint32_t*>(sV + (j & 1) * 64 * HDP);
+      for (int i = tid; i < 64 * HDP / 2; i += 128) {
+        const uint32_t w = v32[i];
+        v32[i] = pack_f16x2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
+      }
+    }
+
+    float sc[8][4];
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) sc[nb][0] = sc[nb][1] = sc[nb][2] = sc[nb][3] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk) {
+#pragma unroll
+      for (int np = 0; np < 4; ++np) {
+        uint32_t b0, b1, b2, b3;
+        ldsm_x4(smem_u32(Ks + (np * 16 + b_row) * HDP + kk * 16 + b_col), b0, b1, b2, b3);
+        mma_bf16(sc[2 * np], qf[kk], b0, b1);
+        mma_bf16(sc[2 * np + 1], qf[kk], b2, b3);
+      }
+    }
+    // scores in the log2 domain with the bias; keys past T (last window tile) drop out
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int key = j * 64 + nb * 8 + cq + (e & 1);
+        const int i = e >> 1;
+        float t = -INFINITY;
+        if (T % 64 == 0 || key < T) {
+          const int kh = key / S, kw = key - kh * S;
+          t = fmaf(sc[nb][e], scale2, bh[i][kh] + bw[i][kw]);
+        }
+        sc[nb][e] = t;
+        mx[i] = fmaxf(mx[i], t);
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+      const float m_new = fmaxf(m_run[i], mx[i]);
+      alpha[i] = fast_exp2(m_run[i] - m_new);
+      m_run[i] = m_new;
+      l_run[i] *= alpha[i];
+    }
+#pragma unroll
+    for (int nb = 0; nb < HD / 8; ++nb) {
+      o[nb][0] *= alpha[0]; o[nb][1] *= alpha[0];
+      o[nb][2] *= alpha[1]; o[nb][3] *= alpha[1];
+    }
+    // P = exp2(t - m) -> fp16 A fragments of P V
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+      const float p0 = fast_exp2(sc[nb][0] - m_run[0]), p1 = fast_exp2(sc[nb][1] - m_run[0]);
+      const float p2 = fast_exp2(sc[nb][2] - m_run[1]), p3 = fast_exp2(sc[nb][3] - m_run[1]);
+      l_run[0] += p0 + p1;
+      l_run[1] += p2 + p3;
+      pa[nb >> 1][(nb & 1) * 2 + 0] = pack_f16x2(p0, p1);
+      pa[nb >> 1][(nb & 1) * 2 + 1] = pack_f16x2(p2, p3);
+    }
+    __syncthreads();   // the whole V tile is fp16
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+      for (int np = 0; np < HD / 16; ++np) {
+        uint32_t b0, b1, b2, b3;
+        ldsm_x4_t(smem_u32(Vs + (kk * 16 + v_row) * HDP + np * 16 + v_col), b0, b1, b2, b3);
+        mma_f16(o[2 * np], pa[kk], b0, b1);
+        mma_f16(o[2 * np + 1], pa[kk], b2, b3);
+      }
+    }
+    __syncthreads();   // this stage may be refilled by the next iteration's load
+  }
+
+  // ---- epilogue: O / l -> out[token, head*HD .. ]
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float l = l_run[i];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.0f / l;
+    const int tq = q0 + rl + 8 * i;
+    if (tq >= T) continue;
+    int dst = seq * T + tq;
+    if (p.out_row_map) dst = __ldg(p.out_row_map + dst);
+    if (dst < 0) continue;
+    __nv_bfloat16* orow = p.out + static_cast<size_t>(dst) * p.D + colq + cq;
+#pragma unroll
+    for (int nb = 0; nb < HD / 8; ++nb)
+      *reinterpret_cast<uint32_t*>(orow + nb * 8) = pack_bf16x2(o[nb][2 * i] * inv, o[nb][2 * i + 1] * inv);
   }
 }
 
-template <int HD, int GS>
+template <int HD, int S>
 static int launch_att(const AttentionArgs& a, cudaStream_t stream) {
-  using Cfg = AttCfg<HD>;
-  constexpr int NREL = GS > 0 ? 2 * GS : 32;
-  const int D = a.H * HD;
-  const long long m_tok = static_cast<long long>(a.n_seq) * a.T;
-  CUtensorMap tq, tkv, th, tw;
-  RSP_TRY(make_tmap_bf16_2d(&tq, a.qkv, m_tok, 3 * D, static_cast<uint64_t>(3 * D) * 2, 128, 64));
-  RSP_TRY(make_tmap_bf16_2d(&tkv, a.qkv, m_tok, 3 * D, static_cast<uint64_t>(3 * D) * 2, 64, 64));
-  RSP_TRY(make_tmap_bf16_2d(&th, a.rel_h, 2 * a.S - 1, HD, static_cast<uint64_t>(HD) * 2, NREL, 64));
-  RSP_TRY(make_tmap_bf16_2d(&tw, a.rel_w, 2 * a.S - 1, HD, static_cast<uint64_t>(HD) * 2, NREL, 64));
+  using C = AttCfg<HD, S>;
   AttDev p;
+  p.qkv = static_cast<const __nv_bfloat16*>(a.qkv);
+  p.rel_h = static_cast<const __nv_bfloat16*>(a.rel_h);
+  p.rel_w = static_cast<const __nv_bfloat16*>(a.rel_w);
   p.out = static_cast<__nv_bfloat16*>(a.out);
-  p.T = a.T; p.S = a.S; p.H = a.H; p.D = D;
-  p.n_qt = (a.T + 127) / 128;
-  p.n_kt = (a.T + 63) / 64;
+  p.H = a.H; p.D = a.H * HD;
+  p.n_qt = (C::T + 63) / 64;
   p.scale2 = (1.0f / sqrtf(static_cast<float>(HD))) * LOG2E;
   p.out_row_map = a.out_row_map;
-  auto kern = vit_attention_kernel<HD, GS>;
+  RSP_CHECK_ARG((reinterpret_cast<uintptr_t>(a.qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.rel_h) & 15) == 0 &&
+                (reinterpret_cast<uintptr_t>(a.rel_w) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.out) & 3) == 0,
+                "attention: qkv / tables must be 16-byte aligned");
+  auto kern = vit_attention_kernel<HD, S>;
   static bool attr_set_dev[kMaxDevices] = {};   // the attribute is per device (one flag per ordinal)
   bool& attr_set = attr_set_dev[current_device()];
   if (!attr_set) {
-    RSP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg::SMEM_BYTES));
+    RSP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr_set = true;
   }
   const long long grid = static_cast<long long>(a.n_seq) * a.H * p.n_qt;
   RSP_CHECK_ARG(grid > 0 && grid < (1ll << 31), "attention: grid %lld", grid);
-  kern<<<static_cast<unsigned>(grid), ATT_THREADS, Cfg::SMEM_BYTES, stream>>>(tq, tkv, th, tw, p);
+  kern<<<static_cast<unsigned>(grid), 128, C::SMEM_BYTES, stream>>>(p);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
 }
@@ -542,19 +339,15 @@ int vit_attention(const AttentionArgs& a, cudaStream_t stream) {
   RSP_CHECK_ARG(a.n_seq > 0 && a.H > 0, "attention: bad n_seq/H");
   if (a.S != 14 && a.S != 32 && a.S != 64)   // other grids (768^2 / 1280^2 inputs): CUDA-core kernel
     return vit_attention_simt(a, stream);
-  if (a.S == 14 && (a.hd == 64 || a.hd == 80)) {
-    static const bool old_path = getenv("RSP_ATT_WINDOW_GENERIC") != nullptr;   // A/B switch for the self-test
-    if (!old_path) return vit_window_attention(a, stream);
-  }
   if (a.hd == 64) {
     if (a.S == 64) return launch_att<64, 64>(a, stream);
     if (a.S == 32) return launch_att<64, 32>(a, stream);
-    return launch_att<64, 0>(a, stream);
+    return launch_att<64, 14>(a, stream);
   }
   if (a.hd == 80) {
     if (a.S == 64) return launch_att<80, 64>(a, stream);
     if (a.S == 32) return launch_att<80, 32>(a, stream);
-    return launch_att<80, 0>(a, stream);
+    return launch_att<80, 14>(a, stream);
   }
   set_last_error("attention: head dim %d unsupported (64, 80)", a.hd);
   return RSP_ERR_UNSUPPORTED;
@@ -562,7 +355,7 @@ int vit_attention(const AttentionArgs& a, cudaStream_t stream) {
 
 // ---------------------------------------------------------------------------------------
 // SIMT restatement (one thread per query row, fp32 throughout): the device-side check of
-// the tcgen05 kernel in the native self-test, and the path for grid sizes the tensor-core
+// the tensor-core kernel in the native self-test, and the path for grid sizes the tensor-core
 // kernel does not specialise (S other than 14 / 64).
 __global__ void vit_attention_simt_kernel(const __nv_bfloat16* __restrict__ qkv,
                                           const __nv_bfloat16* __restrict__ rel_h,

@@ -21,7 +21,6 @@ struct AttentionArgs {
 
 int vit_attention(const AttentionArgs& a, cudaStream_t stream);
 int vit_attention_simt(const AttentionArgs& a, cudaStream_t stream);
-int vit_window_attention(const AttentionArgs& a, cudaStream_t stream);   // S = 14 sequences (attention_window.cu)
 // pieces of the three-pass path for other grids (attention_generic.cu)
 int attn_softmax_bias(const float* scores, int lds, const float* tab, int ldt, int NT, void* P, int ldp, int n_rows,
                       int T, int S, float scale, cudaStream_t stream);

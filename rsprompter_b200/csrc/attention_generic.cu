@@ -1,12 +1,12 @@
 // Global attention for grids the flash kernel does not specialise (S = 48 / 80: 768^2 / 1280^2 inputs of the
 // encoder-size sweep, VS:570-602 with img_size != 1024).  Three passes per (image, head), the two contractions on
-// the tcgen05 GEMM:  scores = Q K^T (fp32 [T, T]) and tab = Q [Rh; Rw]^T (fp32 [T, 2*NT]) -> this file's row kernel
+// the wgmma GEMM:  scores = Q K^T (fp32 [T, T]) and tab = Q [Rh; Rw]^T (fp32 [T, 2*NT]) -> this file's row kernel
 // P = softmax(scale * scores + rel_h + rel_w) (bf16) -> out = P V with V pre-transposed to [hd, T].
 // Reference: HF:803-831 (SamVisionAttention.forward), HF:760-801 (decomposed rel-pos); VS:202-221, 117-157.
 // HBM-bound on the T x T intermediates (12 bytes per score); the CUDA-core kernel it replaces took 108 ms (768^2) /
 // 810 ms (1280^2) per ViT-H layer at batch 8.
 #include "attention.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace rsp {
 

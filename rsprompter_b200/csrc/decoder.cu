@@ -1,6 +1,6 @@
 // Small-sequence attention pieces of SAM's two-way mask decoder (HF modeling_sam.py
 // SamAttention :231-270 as used by SamTwoWayAttentionBlock :306-348).  The heavy image-token
-// projections run on the tcgen05 GEMM; what is left has 10 prompt tokens on one side, far
+// projections run on the wgmma GEMM; what is left has 10 prompt tokens on one side, far
 // below a tensor-core tile, so these are CUDA-core kernels organised for coalesced HBM
 // access (the image-token matrices they stream are the dominant cost).
 //
@@ -9,7 +9,7 @@
 //   i2t_attention          every image token attends to the Tq prompt tokens
 //   add_cast_bf16          out = bf16(a + b)  (query + point embedding before a projection)
 #include "decoder.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace rsp {
 
@@ -133,7 +133,7 @@ int token_self_attention(const void* q, const void* k, const void* v, void* out,
 // t2i: CTA = one prompt, warp = one head.  K / V tiles of 64 image tokens x 128 channels are staged
 // in smem with cp.async (double buffered, rows padded to 272 B so the fragment loads are
 // conflict-free); S = Q K^T and O += P V run on mma.sync m16n8k16 (bf16 -> fp32): the 10 prompt
-// tokens are the M dimension padded to 16, far too few rows for a tcgen05 tile, but enough to keep
+// tokens are the M dimension padded to 16, far too few rows for a wgmma tile, but enough to keep
 // this kernel on the K / V byte stream (2 MB per prompt) instead of on CUDA-core FMAs.
 constexpr int T2I_TILE = 64;
 constexpr int T2I_ROWB = 272;  // bytes per staged row (256 + 16 pad)

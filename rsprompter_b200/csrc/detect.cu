@@ -15,7 +15,7 @@
 //   pool2_nhwc        MaxPool2d(2,2) and max_pool2d(k=1, s=2) on channels-last maps (M:1307,1362)
 //   sin_fold          x[..., ::2].sin() + x[..., 1::2]  (M:348, M:1672)
 #include "detect.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include "upsample4.cuh"
 
 namespace rsp {

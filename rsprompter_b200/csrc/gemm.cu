@@ -1,10 +1,10 @@
-// Persistent, warp-specialised bf16 GEMM for sm_100a:  out = epilogue(A[M,K] * W[N,K]^T)
+// Persistent, warp-specialised bf16 GEMM for sm_90a:  out = epilogue(A[M,K] * W[N,K]^T)
 //
-//   warp 0 (1 lane)  TMA producer: A and W tiles -> 128B-swizzled smem ring (mbarrier tx)
-//   warp 1 (1 lane)  tcgen05.mma issuer: 128 x BN x 16 UMMAs, fp32 accumulators in TMEM,
-//                    two accumulator stages so the epilogue of tile i overlaps tile i+1
-//   warp 2           TMEM allocator
-//   warps 4-7        epilogue: tcgen05.ld (thread = output row), bias / GELU / ReLU /
+//   warp 0 (1 lane)  TMA producer: A and W tiles -> 128B-swizzled smem ring (mbarrier tx);
+//                    runs ahead into the next tile while the consumers are in their epilogue
+//   warps 4-11       two consumer warpgroups: wgmma 64 x BN x 16 (rows 64 wg ..), fp32
+//                    accumulators in registers, then through a shared-memory tile to
+//   warps 4-7        the epilogue (thread = output row): bias / GELU / ReLU /
 //                    residual add / row scatter, bf16 or fp32 stores
 //
 // This one kernel is every dense contraction on the RSPrompter inference path:
@@ -14,7 +14,7 @@
 // projections.  window_unpartition (modeling_sam.py:925-952) is the `row_map` scatter in
 // the epilogue, the residual adds of SamVisionLayer.forward (:966-971) are `residual`.
 #include "gemm.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 #include <stdlib.h>
 
@@ -22,16 +22,17 @@ namespace rsp {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = one 128-byte swizzle row
-constexpr int GEMM_THREADS = 256;
+constexpr int GEMM_THREADS = 384;
 constexpr int A_STAGE_BYTES = BM * BK * 2;
 
 template <int BN>
 struct GemmCfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128) ? 6 : 8;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;  // + alignment slack
-  static constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
+  static constexpr int ACC_LD = BN + 4;                       // fp32 accumulator tile row stride
+  static constexpr int ACC_BYTES = BM * ACC_LD * 4;
+  static constexpr int STAGES = (BN == 256) ? 1 : (BN == 128) ? 4 : (BN == 64) ? 6 : 8;   // 227 KB per block
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024;  // + alignment slack
 };
 
 enum { EPI_STD = 0, EPI_LN_ROW = 1, EPI_LN64_GELU = 2, EPI_GELU_HYPER = 3 };
@@ -121,7 +122,7 @@ __device__ __forceinline__ void store32(const GemmDev& p, const float (&v)[32], 
 }
 
 // EPI_LN_ROW: out = LayerNorm_N(acc + bias + residual) (N <= BN, one n-block: the thread owns the
-// whole row in TMEM; two passes over TMEM, statistics in fp32).  SamTwoWayAttentionBlock
+// whole row in the accumulator tile; two passes over it, statistics in fp32).  SamTwoWayAttentionBlock
 // layer_norm4 fused into cross_attn_image_to_token.out_proj (HF:341-347).
 template <int BN>
 __device__ __forceinline__ void epilogue_ln_row(const GemmDev& p, uint32_t t_row, int orow, int rrow) {
@@ -130,8 +131,7 @@ __device__ __forceinline__ void epilogue_ln_row(const GemmDev& p, uint32_t t_row
   const int nch = p.N / 32;
   for (int c = 0; c < nch; ++c) {
     uint32_t r[32];
-    tmem_ld_32x32b_x32(t_row + c * 32, r);
-    tmem_ld_wait();
+    acc_ld32(t_row + (c * 32) * 4, r);
     if (orow < 0) continue;
     float v[32];
 #pragma unroll
@@ -146,8 +146,7 @@ __device__ __forceinline__ void epilogue_ln_row(const GemmDev& p, uint32_t t_row
   const float rstd = rsqrtf(fmaxf(sq / p.N - dmean * dmean, 0.f) + p.ln_eps);
   for (int c = 0; c < nch; ++c) {
     uint32_t r[32];
-    tmem_ld_32x32b_x32(t_row + c * 32, r);
-    tmem_ld_wait();
+    acc_ld32(t_row + (c * 32) * 4, r);
     if (orow < 0) continue;
     float v[32];
 #pragma unroll
@@ -174,9 +173,8 @@ __device__ __forceinline__ void epilogue_ln64_gelu(const GemmDev& p, uint32_t t_
   for (int gi = 0; gi < BN / 64; ++gi) {
     const int col0 = n_blk * BN + gi * 64;
     uint32_t r0[32], r1[32];
-    tmem_ld_32x32b_x32(t_row + gi * 64, r0);
-    tmem_ld_32x32b_x32(t_row + gi * 64 + 32, r1);
-    tmem_ld_wait();
+    acc_ld32(t_row + (gi * 64) * 4, r0);
+    acc_ld32(t_row + (gi * 64 + 32) * 4, r1);
     if (orow < 0 || col0 >= p.N) continue;
     float v[64];
 #pragma unroll
@@ -228,8 +226,7 @@ __device__ __forceinline__ void epilogue_gelu_hyper(const GemmDev& p, uint32_t t
 #pragma unroll
   for (int t2 = 0; t2 < 4; ++t2) {
     uint32_t r[32];
-    tmem_ld_32x32b_x32(t_row + t2 * 32, r);
-    tmem_ld_wait();
+    acc_ld32(t_row + (t2 * 32) * 4, r);
     float acc = 0.f;
     if (valid) {
 #pragma unroll
@@ -249,18 +246,16 @@ __device__ __forceinline__ void epilogue_gelu_hyper(const GemmDev& p, uint32_t t
 
 template <int BN, bool B_MN_MAJOR>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tma_a,
-                         const __grid_constant__ CUtensorMap tma_b, const GemmDev p) {
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a,
+                       const __grid_constant__ CUtensorMap tma_b, const GemmDev p) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[STAGES];
   __shared__ __align__(8) uint64_t bar_empty[STAGES];
-  __shared__ __align__(8) uint64_t bar_tmem_full[2];
-  __shared__ __align__(8) uint64_t bar_tmem_empty[2];
-  __shared__ uint32_t tmem_base_s;
 
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t acc_base = smem_base + STAGES * Cfg::STAGE_BYTES;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_kb = (p.K + BK - 1) / BK;
@@ -270,19 +265,11 @@ gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tma_a,
     tma_prefetch_desc(&tma_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&bar_tmem_full[s]), 1);
-      mbar_init(smem_u32(&bar_tmem_empty[s]), 4);
+      mbar_init(smem_u32(&bar_empty[s]), 8);
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(&tmem_base_s), Cfg::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
 
   if (warp == 0 && lane == 0) {
     // ------------------------------------------------------------ TMA producer
@@ -312,55 +299,31 @@ gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tma_a,
       mbar_wait(smem_u32(&bar_empty[stage]), phase ^ 1);
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp == 1 && lane == 0) {
-    // ------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = make_idesc_bf16(BM, BN, 0, B_MN_MAJOR ? 1 : 0);
+  } else if (warp >= 4) {
+    // ------------------------------------------------------------ consumers: wgmma, then epilogue (warps 4-7)
+    const int wg = (warp - 4) >> 2;
+    const int ew = warp - 4;
     int stage = 0;
     uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      mbar_wait(smem_u32(&bar_tmem_empty[as]), aphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(smem_u32(&bar_full[stage]), phase);
-        tc_fence_after();
-        const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-        const uint32_t sb = sa + A_STAGE_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          const uint64_t adesc = make_sdesc(sa + k * 32, 0, 1024);
-          const uint64_t bdesc = B_MN_MAJOR ? make_sdesc(sb + k * 2048, BK * 128, 1024)
-                                            : make_sdesc(sb + k * 32, 0, 1024);
-          umma_ss(d_tmem, adesc, bdesc, idesc, (kb | k) != 0);
-        }
-        umma_commit(smem_u32(&bar_empty[stage]));
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(smem_u32(&bar_tmem_full[as]));
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------ epilogue
-    const int ew = warp - 4;
-    int it = 0;
     const bool vec_ok = (p.ldo % 8 == 0) && (p.residual == nullptr || p.ldr % 8 == 0) &&
                         ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0) &&
                         ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0) &&
                         ((reinterpret_cast<uintptr_t>(p.bias) & 15) == 0);
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int m_blk = tile / p.num_n_blocks;
       const int n_blk = tile % p.num_n_blocks;
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      mbar_wait(smem_u32(&bar_tmem_full[as]), aphase);
-      tc_fence_after();
+      float acc[BN / 2];
+      wg_mainloop<BN, B_MN_MAJOR>(acc, smem_base, Cfg::STAGE_BYTES, A_STAGE_BYTES, STAGES, num_kb, wg, stage, phase,
+                                  bar_full, bar_empty);
+      named_bar_sync(1, 256);   // the previous tile's epilogue has read the accumulator tile
+      acc_store<BN>(acc, acc_base, Cfg::ACC_LD, wg, threadIdx.x & 127);
+      named_bar_sync(1, 256);
+      if (ew >= 4) continue;
       const int row = m_blk * BM + ew * 32 + lane;
       int orow = -1;
       if (row < p.M) orow = p.row_map ? p.row_map[row] : row;
       const int rrow = (orow >= 0 && p.residual) ? residual_row(p, orow) : orow;
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * BN;
+      const uint32_t t_row = acc_row(acc_base, Cfg::ACC_LD, ew * 32 + lane);
       if (p.epi_mode == EPI_LN_ROW) {
         epilogue_ln_row<BN>(p, t_row, orow, rrow);
       } else if (p.epi_mode == EPI_LN64_GELU) {
@@ -371,8 +334,7 @@ gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tma_a,
 #pragma unroll 1
       for (int c = 0; c < BN / 32; ++c) {
         uint32_t r[32];
-        tmem_ld_32x32b_x32(t_row + c * 32, r);
-        tmem_ld_wait();
+        acc_ld32(t_row + (c * 32) * 4, r);
         const int col0 = n_blk * BN + c * 32;
         if (orow < 0 || col0 >= p.N) continue;
         float v[32];
@@ -457,17 +419,7 @@ gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tma_a,
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&bar_tmem_empty[as]));
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
@@ -498,7 +450,7 @@ static int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   const int num_m_blocks = (a.M + BM - 1) / BM;
   p.num_n_blocks = (a.N + BN - 1) / BN;
   p.num_tiles = num_m_blocks * p.num_n_blocks;
-  auto kern = gemm_bf16_tcgen05_kernel<BN, B_MN>;
+  auto kern = gemm_bf16_wgmma_kernel<BN, B_MN>;
   static bool attr_set_dev[kMaxDevices] = {};   // the attribute is per device (one flag per ordinal)
   bool& attr_set = attr_set_dev[current_device()];
   if (!attr_set) {
@@ -534,7 +486,6 @@ int gemm_bf16(const GemmArgs& a, cudaStream_t stream) {
     static const bool v1 = getenv("RSP_GEMM_V1") != nullptr;
     if (!v1 && a.N % 128 == 0 && (reinterpret_cast<uintptr_t>(a.out) & 7) == 0 && a.ldo % 4 == 0)
       return gemm_bf16_v2_ln64_gelu(a, stream);
-    if (a.N % 256 == 0) return launch_gemm<256, false>(a, stream);
     if (a.N % 128 == 0) return launch_gemm<128, false>(a, stream);
     return launch_gemm<64, false>(a, stream);
   }
@@ -557,16 +508,10 @@ int gemm_bf16(const GemmArgs& a, cudaStream_t stream) {
   }
   int bn = a.force_bn;
   if (bn == 0) {
-    if (a.N > 128) bn = 256;
-    else if (a.N > 64) bn = 128;
+    // 128 at most: a 256-wide tile's fp32 accumulator tile leaves shared memory for a single pipeline stage
+    if (a.N > 64) bn = 128;
     else if (a.N > 32) bn = 64;
     else bn = 32;
-    // prefer 128-wide tiles when 256 would leave most of the last tile empty or the grid short
-    if (bn == 256) {
-      const int mt = (a.M + BM - 1) / BM;
-      const int t256 = mt * ((a.N + 255) / 256);
-      if ((a.N % 256 != 0 && a.N % 256 <= 128) || t256 < num_sms()) bn = 128;
-    }
   }
   {
     static const bool force_v1 = getenv("RSP_GEMM_V1") != nullptr;
@@ -606,17 +551,13 @@ int conv3x3_bf16(const GemmArgs& a, cudaStream_t stream) {
                 "conv3x3: M / K do not match the map");
   RSP_CHECK_ARG(a.epi_mode == EPI_STD && !a.w_is_kn && !a.row_map && a.act >= 0 && a.act <= 2, "conv3x3: epilogue");
   RSP_CHECK_ARG(gemm_v2_eligible(a), "conv3x3: output / residual alignment");
-  int bn = a.N > 128 ? 256 : a.N > 64 ? 128 : a.N > 32 ? 64 : 32;
-  if (bn == 256) {
-    const int t256 = ((a.M + BM - 1) / BM) * ((a.N + 255) / 256);
-    if ((a.N % 256 != 0 && a.N % 256 <= 128) || t256 < num_sms()) bn = 128;
-  }
+  const int bn = a.N > 64 ? 128 : a.N > 32 ? 64 : 32;
   return gemm_bf16_v2(a, bn, stream);
 }
 
 // ---------------------------------------------------------------------------------------
 // Plain SIMT GEMM with the same epilogue contract.  Used (a) by the device self-test as an
-// independent check of the tcgen05 path and (b) for contractions too small to fill one
+// independent check of the wgmma path and (b) for contractions too small to fill one
 // 128-row tile (hypernetwork / IoU MLPs on a handful of tokens).
 __global__ void gemm_bf16_simt_kernel(const __nv_bfloat16* __restrict__ A, int lda,
                                       const __nv_bfloat16* __restrict__ W, int ldw, int w_is_kn,

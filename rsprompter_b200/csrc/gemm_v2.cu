@@ -1,19 +1,19 @@
-// Second-generation epilogue for the persistent tcgen05 GEMM (standard epilogue only: bias,
-// GELU / ReLU, residual, row scatter, bf16 / fp32 out).  Same mainloop as gemm.cu; what changes is
-// how the accumulator leaves the SM:
-//   * 8 epilogue warps (2 per TMEM lane quarter, each owning half of the tile's columns) instead
-//     of 4, so the GELU / conversion work and the TMEM drain are spread over twice the issue slots;
+// Second-generation epilogue for the persistent wgmma GEMM (bias, GELU / ReLU, residual, row scatter,
+// bf16 / fp32 out, and the fused LayerNorm / upscaler epilogues).  Same mainloop as gemm.cu; what changes
+// is how the accumulator leaves the SM:
+//   * 8 epilogue warps (2 per 32-row quarter of the accumulator tile, each owning half of the tile's
+//     columns) instead of 4, so the GELU / conversion work is spread over twice the issue slots;
 //   * every warp transposes its 32-row x 128-byte slab through a private, bank-conflict-free smem
 //     staging buffer, so global traffic is fully coalesced: each half-warp reads (residual) and
 //     writes one whole 128-byte line per instruction instead of 32 lanes touching 32 different
 //     lines (the thread-per-row pattern of the first version, which left K = 768 GEMMs
 //     epilogue-bound at ~35-55 % of the large-K rate).
 // All shared memory is dynamic (1024-byte aligned by declaration), barriers live at its end:
-//   [ STAGES x (A 16 KB + B BN*128 B) | 8 x 32 x 136 B staging | barriers ]
+//   [ STAGES x (A 16 KB + B BN*128 B) | 8 x 32 x 136 B staging | 128 x (BN + 4) fp32 accumulators | barriers ]
 #include <cstdlib>
 
 #include "gemm.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace rsp {
 
@@ -21,7 +21,7 @@ namespace v2 {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int THREADS = 384;          // 4 control warps + 8 epilogue warps
+constexpr int THREADS = 384;          // 4 control warps + 2 consumer warpgroups (wgmma, then epilogue)
 constexpr int A_BYTES = BM * BK * 2;
 constexpr int STG_ROW = 136;          // 128-byte payload + 8 pad: conflict-free 8-byte accesses
 constexpr int STG_WARP = 32 * STG_ROW;
@@ -32,9 +32,10 @@ template <int BN>
 struct Cfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128) ? 6 : 8;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + BAR_BYTES;
-  static constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
+  static constexpr int ACC_LD = BN + 4;
+  static constexpr int ACC_BYTES = BM * ACC_LD * 4;
+  static constexpr int STAGES = (BN == 256) ? 1 : (BN == 128) ? 3 : (BN == 64) ? 6 : 8;   // 227 KB per block
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + ACC_BYTES + BAR_BYTES;
   static constexpr int NHALF = (BN >= 128) ? 2 : 1;   // epilogue warps per lane quarter that have work
   static constexpr int COLS_PER_WARP = BN / NHALF;
 };
@@ -79,7 +80,7 @@ __device__ __forceinline__ int residual_row(const Dev& p, int orow) {
 
 template <int BN, int EPI>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+gemm_bf16_wgmma_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                             const __grid_constant__ CUtensorMap tma_c, const __grid_constant__ CUtensorMap tma_r,
                             const Dev p) {
   using C = Cfg<BN>;
@@ -87,13 +88,11 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t smem_base = smem_u32(smem);
   uint8_t* stg_all = smem + STAGES * C::STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stg_all + STG_BYTES);
+  const uint32_t acc_base = smem_u32(stg_all + STG_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stg_all + STG_BYTES + C::ACC_BYTES);
   uint64_t* bar_full = bars;
   uint64_t* bar_empty = bars + STAGES;
-  uint64_t* bar_tmem_full = bars + 2 * STAGES;
-  uint64_t* bar_tmem_empty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  uint64_t* bar_res = bars + 2 * STAGES + 5;   // one per epilogue warp: residual slab landed
+  uint64_t* bar_res = bars + 2 * STAGES;   // one per epilogue warp: residual slab landed
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -104,20 +103,12 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
     tma_prefetch_desc(&tma_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&bar_tmem_full[s]), 1);
-      mbar_init(smem_u32(&bar_tmem_empty[s]), 4 * C::NHALF);
+      mbar_init(smem_u32(&bar_empty[s]), 8);
     }
     for (int s = 0; s < 8; ++s) mbar_init(smem_u32(&bar_res[s]), 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(tmem_base_s), C::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_s;
 
   if (warp == 0 && lane == 0) {
     // ------------------------------------------------------------ TMA producer
@@ -151,41 +142,16 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-    // tail: consume the ring's last "empty" completions, so that no tcgen05.commit arrive is left without a waiter when
-    // the CTA retires (compute-sanitizer synccheck "missing wait"); never-used slots pass at once
+    // tail: consume the ring's last "empty" completions, so that no consumer arrive is left without a waiter when the
+    // CTA retires; never-used slots pass at once
     for (int i = 0; i < STAGES; ++i) {
       mbar_wait(smem_u32(&bar_empty[stage]), phase ^ 1);
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp == 1 && lane == 0) {
-    // ------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = make_idesc_bf16(BM, BN, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      mbar_wait(smem_u32(&bar_tmem_empty[as]), ((it >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(smem_u32(&bar_full[stage]), phase);
-        tc_fence_after();
-        const uint32_t sa = smem_base + stage * C::STAGE_BYTES;
-        const uint32_t sb = sa + A_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          umma_ss(d_tmem, make_sdesc(sa + k * 32, 0, 1024), make_sdesc(sb + k * 32, 0, 1024), idesc,
-                  (kb | k) != 0);
-        umma_commit(smem_u32(&bar_empty[stage]));
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(smem_u32(&bar_tmem_full[as]));
-    }
-  } else if (warp >= 4 && ((warp - 4) >> 2) < C::NHALF) {
-    // ------------------------------------------------------------ epilogue (8 warps)
+  } else if (warp >= 4) {
+    // ------------------------------------------------------------ consumers: wgmma, then epilogue (8 warps)
     const int e = warp - 4;
-    const int q = e & 3, hf = e >> 2;
+    const int q = e & 3, hf = e >> 2;   // hf is also the warpgroup: rows [64 hf, 64 hf + 64) of the wgmma tile
     uint8_t* stg = stg_all + e * STG_WARP;
     const uint32_t stg_s = smem_u32(stg);
     const bool stage_f32 = p.out_fp32 || (p.residual != nullptr);
@@ -194,17 +160,24 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
     const int lpr = stage_f32 ? 16 : (W * 2) / 8;     // lanes per row at 8 bytes each
     const int rpi = 32 / lpr;                          // rows per write-out iteration
     const int epl = stage_f32 ? 2 : 4;                 // elements per lane (8 bytes)
-    int it = 0;
+    int kstage = 0;
+    uint32_t kphase = 0;
     uint32_t rphase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int m_blk = tile / p.num_n_blocks;
       const int n_blk = tile % p.num_n_blocks;
-      const int as = it & 1;
+      {
+        float acc[BN / 2];
+        wg_mainloop<BN, false>(acc, smem_base, C::STAGE_BYTES, A_BYTES, STAGES, num_kb, hf, kstage, kphase, bar_full,
+                               bar_empty);
+        named_bar_sync(5, 256);   // the previous tile's epilogue has read the accumulator tile
+        acc_store<BN>(acc, acc_base, C::ACC_LD, hf, threadIdx.x & 127);
+        named_bar_sync(5, 256);
+      }
+      if (hf >= C::NHALF) continue;
       if constexpr (EPI == EPI_GELU_HYPER) {
         // rows = (prompt, y, x, tap1); this warp owns tap2 in {2hf, 2hf+1} = output row 4y + 2ty1 + hf.
         // 16 consecutive lanes (4 x-positions... 8 with both tx1) write one contiguous 128-byte run.
-        mbar_wait(smem_u32(&bar_tmem_full[as]), (it >> 1) & 1);
-        tc_fence_after();
         const int row = m_blk * BM + q * 32 + lane;
         const bool valid = row < p.M;
         const int rows_per_prompt = p.grid_h * p.grid_w * 4;
@@ -221,13 +194,12 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
             hyp[4 * i] = h.x; hyp[4 * i + 1] = h.y; hyp[4 * i + 2] = h.z; hyp[4 * i + 3] = h.w;
           }
         }
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN + hf * 64;
+        const uint32_t t_row = acc_row(acc_base, C::ACC_LD, q * 32 + lane) + 4 * hf * 64;
         float m2[2];
 #pragma unroll
         for (int t = 0; t < 2; ++t) {
           uint32_t r[32];
-          tmem_ld_32x32b_x32(t_row + t * 32, r);
-          tmem_ld_wait();
+          acc_ld32(t_row + (t * 32) * 4, r);
           const float4* b4 = reinterpret_cast<const float4*>(p.bias + hf * 64 + t * 32);
           float acc = 0.f;
 #pragma unroll
@@ -249,10 +221,10 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
       } else if constexpr (EPI == EPI_LN_ROW) {
         // out = LayerNorm_256(acc + bias + residual), bf16 (N == BN == 256: the tile holds whole rows).  Two warps
         // share a row (128 columns each).  Pass 1: v = acc + bias + residual (residual slabs arrive by TMA in the
-        // staging buffer) is written back over the accumulator in TMEM while sum / sum of squares accumulate;
-        // the pair exchanges its partial statistics through shared memory; pass 2 re-reads v from TMEM (TMEM
-        // reads are ~900 B/clk/SM), normalises, and leaves through the same staging buffer as TMA stores.
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN + hf * 128;
+        // staging buffer) is written back over the accumulator tile while sum / sum of squares accumulate;
+        // the pair exchanges its partial statistics through shared memory; pass 2 re-reads v from the tile
+        // in shared memory, normalises, and leaves through the same staging buffer as TMA stores.
+        const uint32_t t_row = acc_row(acc_base, C::ACC_LD, q * 32 + lane) + 4 * hf * 128;
         const int col_warp = hf * 128;
         const int row0 = m_blk * BM + q * 32;
         const uint32_t sbuf = smem_u32(stg_all) + e * 4096;
@@ -274,8 +246,6 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
           }
         };
         if (valid) issue_res(col_warp);
-        mbar_wait(smem_u32(&bar_tmem_full[as]), (it >> 1) & 1);
-        tc_fence_after();
         // shifted sums: d = v - pivot with the pivot = this half row's first value, so a large common offset of the
         // row (keys with a big mean) does not cancel in E[d^2] - E[d]^2; the halves are merged with Chan's formula
         float sum = 0.f, sumsq = 0.f, piv = 0.f;
@@ -289,8 +259,7 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
 #pragma unroll
             for (int c = 0; c < 2; ++c) {
               uint32_t r[32];
-              tmem_ld_32x32b_x32(t_row + ps * 64 + c * 32, r);
-              tmem_ld_wait();
+              acc_ld32(t_row + (ps * 64 + c * 32) * 4, r);
               const float4* b4 = reinterpret_cast<const float4*>(p.bias + col0 + c * 32);
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
@@ -316,12 +285,11 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
                   r[8 * j + k] = __float_as_uint(v[k]);
                 }
               }
-              tmem_st_32x32b_x32(t_row + ps * 64 + c * 32, r);
+              acc_st32(t_row + (ps * 64 + c * 32) * 4, r);
             }
             __syncwarp();                         // every lane has read its residual row: the buffer is free
             if (ps == 0) issue_res(col0 + 64);
           }
-          tmem_st_wait();
         }
         const float mean_h = piv + sum * (1.0f / 128.0f);
         const float m2_h = fmaxf(sumsq - sum * sum * (1.0f / 128.0f), 0.f);
@@ -341,8 +309,7 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
 #pragma unroll
             for (int c = 0; c < 2; ++c) {
               uint32_t r[32];
-              tmem_ld_32x32b_x32(t_row + ps * 64 + c * 32, r);
-              tmem_ld_wait();
+              acc_ld32(t_row + (ps * 64 + c * 32) * 4, r);
               const float4* g4 = reinterpret_cast<const float4*>(p.ln_gamma + col0 + c * 32);
               const float4* e4 = reinterpret_cast<const float4*>(p.ln_beta + col0 + c * 32);
 #pragma unroll
@@ -371,11 +338,9 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
       } else if constexpr (EPI == EPI_LN64_GELU) {
         // this warp owns two 64-column groups (taps); per group: bias, LayerNorm over the 64
         // channels, GELU, bf16 -> staging -> coalesced 128-byte rows
-        mbar_wait(smem_u32(&bar_tmem_full[as]), (it >> 1) & 1);
-        tc_fence_after();
         const int my_row = m_blk * BM + q * 32 + lane;
         const int my_orow = my_row < p.M ? my_row : -1;
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN + hf * C::COLS_PER_WARP;
+        const uint32_t t_row = acc_row(acc_base, C::ACC_LD, q * 32 + lane) + 4 * hf * C::COLS_PER_WARP;
         const int col_warp = n_blk * BN + hf * C::COLS_PER_WARP;
         const int sub = lane >> 4, cl = lane & 15;
 #pragma unroll 1
@@ -385,9 +350,8 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
           float v[64];
           {
             uint32_t r0[32], r1[32];
-            tmem_ld_32x32b_x32(t_row + gi * 64, r0);
-            tmem_ld_32x32b_x32(t_row + gi * 64 + 32, r1);
-            tmem_ld_wait();
+            acc_ld32(t_row + (gi * 64) * 4, r0);
+            acc_ld32(t_row + (gi * 64 + 32) * 4, r1);
 #pragma unroll
             for (int i = 0; i < 32; ++i) { v[i] = __uint_as_float(r0[i]); v[32 + i] = __uint_as_float(r1[i]); }
           }
@@ -460,11 +424,11 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
           __syncwarp();
         }
       } else if (p.tma_store) {
-        // ---- lean path: TMEM -> registers -> bias / activation -> 128-byte-swizzled staging -> one TMA store per
+        // ---- lean path: accumulator tile -> registers -> bias / activation -> 128-byte-swizzled staging -> one TMA store per
         // 32 x 128 B slab.  No per-element address or bounds arithmetic: the tensor map clips rows >= M / cols >= N.
         // With a residual, its slab is TMA-loaded into the same staging buffer (issued as soon as the previous
         // store has drained it), added in place by the lane that owns the row, and stored from there.
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN + hf * C::COLS_PER_WARP;
+        const uint32_t t_row = acc_row(acc_base, C::ACC_LD, q * 32 + lane) + 4 * hf * C::COLS_PER_WARP;
         const int col_warp = n_blk * BN + hf * C::COLS_PER_WARP;
         const int row0 = m_blk * BM + q * 32;
         const uint32_t sbuf = smem_u32(stg_all) + e * 4096;
@@ -489,8 +453,6 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
           }
         };
         if (has_res && col_warp < p.N) issue_res(col_warp);
-        mbar_wait(smem_u32(&bar_tmem_full[as]), (it >> 1) & 1);
-        tc_fence_after();
         const int act = p.act;
         const float* bias = p.bias;
         const int N = p.N;
@@ -522,8 +484,7 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
             const int col0 = col_warp + ps * 32;
             if (col0 >= N) break;
             uint32_t r[32];
-            tmem_ld_32x32b_x32(t_row + ps * 32, r);
-            tmem_ld_wait();
+            acc_ld32(t_row + (ps * 32) * 4, r);
             float v[32];
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
@@ -558,9 +519,8 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
             const int col0 = col_warp + ps * 64;
             if (col0 >= N) break;
             uint32_t r0[32], r1[32];
-            tmem_ld_32x32b_x32(t_row + ps * 64, r0);
-            tmem_ld_32x32b_x32(t_row + ps * 64 + 32, r1);
-            tmem_ld_wait();
+            acc_ld32(t_row + (ps * 64) * 4, r0);
+            acc_ld32(t_row + (ps * 64 + 32) * 4, r1);
             float v0[32], v1[32];
 #pragma unroll
             for (int i = 0; i < 32; ++i) { v0[i] = __uint_as_float(r0[i]); v1[i] = __uint_as_float(r1[i]); }
@@ -606,7 +566,7 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
       int my_orow = -1;
       if (my_row < p.M) my_orow = p.row_map ? p.row_map[my_row] : my_row;
       const int my_rrow = (my_orow >= 0 && p.residual) ? residual_row(p, my_orow) : 0;
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN + hf * C::COLS_PER_WARP;
+      const uint32_t t_row = acc_row(acc_base, C::ACC_LD, q * 32 + lane) + 4 * hf * C::COLS_PER_WARP;
       const int col_warp = n_blk * BN + hf * C::COLS_PER_WARP;
       const int sub = lane / lpr, cl = lane - sub * lpr;
       // destination / residual row of tile-local row rr: plain arithmetic when there is no scatter map
@@ -624,7 +584,7 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
       };
       // residual prefetch (fp32-staged path: 16 lanes x 8 B per row, 2 rows per instruction): the 16
       // loads of a pass are issued back to back before the accumulator is touched, so ~4 KB per warp
-      // is in flight while the TMEM drain / activation of the same pass runs
+      // is in flight while the accumulator read / activation of the same pass runs
       float2 resv[16];
       auto load_residual = [&](int col_pass) {
         const int col = col_pass + cl * 2;
@@ -648,19 +608,16 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
         }
       };
       if (p.residual && col_warp < p.N) load_residual(col_warp);
-      mbar_wait(smem_u32(&bar_tmem_full[as]), (it >> 1) & 1);
-      tc_fence_after();
 #pragma unroll 1
       for (int ps = 0; ps < n_pass; ++ps) {
         const int col_pass = col_warp + ps * W;
         if (col_pass < p.N) {
           if (p.residual && ps > 0) load_residual(col_pass);
-          // ---- phase 1: TMEM -> registers -> bias / activation -> staging row `lane`
+          // ---- phase 1: accumulator tile -> registers -> bias / activation -> staging row `lane`
 #pragma unroll 1
           for (int c = 0; c < W / 32; ++c) {
             uint32_t r[32];
-            tmem_ld_32x32b_x32(t_row + ps * W + c * 32, r);
-            tmem_ld_wait();
+            acc_ld32(t_row + (ps * W + c * 32) * 4, r);
             const int col0 = col_pass + c * 32;
             float v[32];
 #pragma unroll
@@ -742,18 +699,8 @@ gemm_bf16_tcgen05_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __g
         }
       }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&bar_tmem_empty[as]));
     }
     if (p.tma_store && lane == 0) bulk_wait0();   // every slab is in global memory before the CTA retires
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
   }
 }
 
@@ -826,7 +773,7 @@ static int launch(const GemmArgs& a, cudaStream_t stream) {
   p.num_tiles = ((a.M + BM - 1) / BM) * p.num_n_blocks;
   p.ln_gamma = a.ln_gamma; p.ln_beta = a.ln_beta; p.ln_eps = a.ln_eps;
   p.hyper = a.hyper; p.mask_out = a.mask_out; p.grid_h = a.grid_h; p.grid_w = a.grid_w;
-  auto kern = gemm_bf16_tcgen05_v2_kernel<BN, EPI>;
+  auto kern = gemm_bf16_wgmma_v2_kernel<BN, EPI>;
   static bool attr_set_dev[kMaxDevices] = {};   // the attribute is per device (one flag per ordinal)
   bool& attr_set = attr_set_dev[current_device()];
   if (!attr_set) {
@@ -881,7 +828,6 @@ int gemm_bf16_v2_ln_row(const GemmArgs& a, cudaStream_t stream) { return v2::lau
 
 // mask-decoder upscaler epilogues on the 8-warp kernel (called from gemm_bf16 for epi_mode 2 / 3)
 int gemm_bf16_v2_ln64_gelu(const GemmArgs& a, cudaStream_t stream) {
-  if (a.N % 256 == 0) return v2::launch<256, v2::EPI_LN64_GELU>(a, stream);
   return v2::launch<128, v2::EPI_LN64_GELU>(a, stream);
 }
 

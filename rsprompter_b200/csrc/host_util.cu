@@ -87,7 +87,7 @@ int num_sms() {
   const int dev = current_device();
   if (n[dev] == 0) {
     cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (n[dev] <= 0) n[dev] = 148;
+    if (n[dev] <= 0) n[dev] = 132;
   }
   return n[dev];
 }

@@ -18,7 +18,7 @@
 #include <cstdlib>
 
 #include "query.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include "upsample4.cuh"
 
 namespace rsp {

@@ -7,7 +7,7 @@
 //   patchify16_u8                       the same arithmetic fused into the patch-embed operand loader: uint8 HWC batch
 //                                       -> bf16 [B*gh*gw, 768] patch rows (the fp32 NCHW image never exists)
 #include "records.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace rsp {
 

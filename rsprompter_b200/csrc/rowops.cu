@@ -9,7 +9,7 @@
 //   im2col_nhwc      NHWC bf16 -> [B*Ho*Wo, kh*kw*C] rows (3x3 convs of neck / FPN / RPN)
 //   nhwc_to_nchw     layout change at module boundaries that must hand back NCHW tensors
 #include "rowops.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace rsp {
 

@@ -1,6 +1,6 @@
 // Native device self-test / micro-benchmark (no Python, no torch): fast to run on a GPU box.
 //   ./rsp_selftest [gemm|attn|all] [bench]
-// Every tcgen05 kernel is compared with a plain SIMT implementation of the same contract.
+// Every tensor-core kernel is compared with a plain SIMT implementation of the same contract.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -9,7 +9,7 @@
 #include <vector>
 
 #include "gemm.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace rsp { const char* last_error(); }
 using namespace rsp;
@@ -180,52 +180,6 @@ static void bench_gemm(int M, int N, int K, int bn, int act, int out_fp32, int r
 int selftest_attention(int bench);
 
 
-// ---- microbenchmark: TMEM read bandwidth (tcgen05.ld 32x32b.x32) with NW warps reading (informs how many
-// passes over an accumulator an epilogue / softmax can afford)
-__global__ void tmem_read_bench_kernel(int iters, long long* cycles, float* sink) {
-  __shared__ uint32_t tmem_base_s;
-  const int warp = threadIdx.x >> 5;
-  if (warp == 0) rsp::tmem_alloc(rsp::smem_u32(&tmem_base_s), 512);
-  rsp::tc_fence_before();
-  __syncthreads();
-  rsp::tc_fence_after();
-  const uint32_t base = tmem_base_s + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-  float acc = 0.f;
-  __syncthreads();
-  const long long t0 = clock64();
-  for (int it = 0; it < iters; ++it) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      uint32_t v[32];
-      rsp::tmem_ld_32x32b_x32(base + ((it * 4 + c) & 15) * 32, v);
-      rsp::tmem_ld_wait();
-      acc += __uint_as_float(v[0]) + __uint_as_float(v[31]);
-    }
-  }
-  const long long t1 = clock64();
-  __syncthreads();
-  if (threadIdx.x == 0) cycles[blockIdx.x] = t1 - t0;
-  if (acc == 123.456f) sink[0] = acc;
-  __syncthreads();
-  if (warp == 0) { rsp::tc_fence_after(); rsp::tmem_dealloc(tmem_base_s, 512); }
-}
-
-static void tmem_read_bench() {
-  long long* d_cyc; float* d_sink;
-  cudaMalloc(&d_cyc, 8 * 148); cudaMalloc(&d_sink, 4);
-  const int iters = 2000;
-  for (int nw : {1, 2, 4, 8, 16}) {
-    tmem_read_bench_kernel<<<148, nw * 32>>>(iters, d_cyc, d_sink);
-    cudaDeviceSynchronize();
-    long long c = 0;
-    cudaMemcpy(&c, d_cyc, 8, cudaMemcpyDeviceToHost);
-    const double bytes = static_cast<double>(iters) * 4 * 4096 * nw;
-    printf("tmem read: %2d warps/SM  %lld cycles  %.1f B/clk/SM  (%.1f B/clk/warp), err=%s\n", nw, c, bytes / c, bytes / c / nw,
-           cudaGetErrorString(cudaGetLastError()));
-  }
-  cudaFree(d_cyc); cudaFree(d_sink);
-}
-
 int main(int argc, char** argv) {
   const char* what = argc > 1 ? argv[1] : "all";
   const int bench = argc > 2 && !strcmp(argv[2], "bench");
@@ -263,7 +217,6 @@ int main(int argc, char** argv) {
       bench_gemm(8192, 8192, 8192, 128, 0, 0, 0);
     }
   }
-  if (!strcmp(what, "tmembench")) tmem_read_bench();
   if (!strcmp(what, "gemmprof")) {
     // mask-decoder shapes (N prompts * 4096 image tokens rows)
     bench_gemm(1 << 20, 256, 128, 0, 0, 1, 1, 1, 3);   // i2t out_proj + bf16 residual -> fp32

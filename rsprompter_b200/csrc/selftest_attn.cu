@@ -1,4 +1,4 @@
-// Native self-test of the tcgen05 ViT attention kernel against the SIMT restatement.
+// Native self-test of the tensor-core ViT attention kernel against the SIMT restatement.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>

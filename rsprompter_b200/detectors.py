@@ -1,4 +1,4 @@
-"""RSPrompterAnchor / RSPrompterQuery detectors (M:53-272): orchestration of the B200 modules.
+"""RSPrompterAnchor / RSPrompterQuery detectors (M:53-272): orchestration of the H100 modules.
 
 ``predict(batch_inputs, batch_data_samples, rescale=True)`` keeps the reference contract
 (mmdet BaseDetector.forward mode='predict', detectors/base.py:58-99): it returns the data samples

@@ -1,4 +1,4 @@
-"""RSFPN neck on the B200 kernels: RSFeatureAggregator / PseudoFeatureAggregator -> RSSimpleFPN
+"""RSFPN neck on the H100 kernels: RSFeatureAggregator / PseudoFeatureAggregator -> RSSimpleFPN
 (M:917-1057, M:1277-1363), plus LN2d (M:32-50).
 
 All feature maps are channels-last bf16 inside the pipeline (``forward_nhwc``); every conv is a

@@ -1,4 +1,4 @@
-"""RSPrompter-query heads on the B200 kernels: MSDeformAttnPixelDecoder -> Mask2Former transformer decoder
+"""RSPrompter-query heads on the H100 kernels: MSDeformAttnPixelDecoder -> Mask2Former transformer decoder
 -> RSMask2FormerHead (SAM decoder prompted by the queries) -> RSMaskFormerFusionHead (M:274-715;
 mmdet/models/layers/msdeformattn_pixel_decoder.py:21-246; layers/transformer/mask2former_layers.py:9-135;
 seg_heads/panoptic_fusion_heads/maskformer_fusion_head.py:126-182).

@@ -4,7 +4,7 @@ The reference exposes its models through ``mmdet.registry.MODELS`` (mmdet/regist
 python config files resolved by ``mmengine.Config.fromfile`` (``_base_`` inheritance,
 ``_delete_`` keys, ``custom_imports``; configs/rsprompter/_base_/rsprompter_anchor.py:1-3).
 When mmengine/mmdet are importable the real registry is used and our classes are registered
-into it (``force=True``) so ``MODELS.build(cfg.model)`` returns the B200 implementation.
+into it (``force=True``) so ``MODELS.build(cfg.model)`` returns the H100 implementation.
 This container (and the GPU box) has neither, so a minimal work-alike is provided: same
 decorator, same ``build(dict(type=...))`` contract, same config-file semantics, same
 ``InstanceData`` / ``DetDataSample`` attribute containers the predict() methods fill in.

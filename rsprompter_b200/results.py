@@ -1,7 +1,7 @@
 """Fixed-size per-rank result records and their cross-rank gather.
 
 The inference path shards images across GPUs with no collective inside forward; the only exchange is ONE
-all-gather of a compact result record after predict (the B200 counterpart of mmengine's ``collect_results`` after
+all-gather of a compact result record after predict (the H100 counterpart of mmengine's ``collect_results`` after
 ``CocoMetric.process`` has encoded the masks, mmdet/evaluation/metrics/coco_metric.py:346-400, ``encode_mask_results``
 :365).  A record is one flat byte buffer per rank holding, for its B images with M instance slots each:
 

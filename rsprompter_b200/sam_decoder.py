@@ -1,4 +1,4 @@
-"""SAM mask decoder, positional embedding and prompt-encoder members on the B200 kernels.
+"""SAM mask decoder, positional embedding and prompt-encoder members on the H100 kernels.
 
 Registry types (M:744-759, 881-914): ``RSSamMaskDecoder``, ``RSSamPositionalEmbedding``,
 ``RSSamPromptEncoder``; parameter names are HF's (``mask_decoder.*`` etc.) so
@@ -90,7 +90,7 @@ class _ConvT(nn.Module):
 
 
 class SamMaskDecoderB200(nn.Module):
-    """HF ``SamMaskDecoder`` parameter tree; ``decode`` runs on the B200 kernels."""
+    """HF ``SamMaskDecoder`` parameter tree; ``decode`` runs on the H100 kernels."""
 
     def __init__(self, arch: SamDecoderArch | None = None):
         super().__init__()

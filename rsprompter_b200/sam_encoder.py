@@ -1,4 +1,4 @@
-"""SAM ViT image encoder on the B200 kernels.
+"""SAM ViT image encoder on the H100 kernels.
 
 Registry types (M:762-878): ``RSSamVisionEncoder`` (HF ``SamVisionEncoder`` semantics,
 HF:1020-1072) and ``MMPretrainSamVisionEncoder`` (``mmpretrain.ViTSAM`` semantics, VS:317-602).
@@ -117,7 +117,7 @@ def window_maps(batch: int, grid: int, window: int, device: torch.device) -> tup
 
 
 class SamVisionEncoderB200(nn.Module):
-    """HF ``SamVisionEncoder`` parameter tree with a forward made of B200 kernels."""
+    """HF ``SamVisionEncoder`` parameter tree with a forward made of H100 kernels."""
 
     def __init__(self, arch: SamVisionArch):
         super().__init__()
@@ -167,7 +167,7 @@ class SamVisionEncoderB200(nn.Module):
     def _prepare(self) -> dict:
         dev = self.pos_embed.device
         if dev.type != "cuda":
-            raise _lib.RspError("SamVisionEncoderB200 runs on CUDA only; move the module to a B200")
+            raise _lib.RspError("SamVisionEncoderB200 runs on CUDA only; move the module to a H100")
         bf = lambda t: t.detach().to(dtype=torch.bfloat16).contiguous()  # noqa: E731
         f32 = lambda t: t.detach().to(dtype=torch.float32).contiguous()  # noqa: E731
         a = self.arch

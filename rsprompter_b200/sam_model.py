@@ -1,4 +1,4 @@
-"""Box-prompted SAM on the B200 kernels: ``RSSamModel`` (M:718-741 over HF ``SamModel``, HF:1075-1300) and the
+"""Box-prompted SAM on the H100 kernels: ``RSSamModel`` (M:718-741 over HF ``SamModel``, HF:1075-1300) and the
 ``SAMDet`` detector that prompts it with another detector's boxes (M:1060-1215) - SURVEY 8(f4).
 
 ``RSSamModel.sam_model`` keeps HF ``SamModel``'s parameter tree (``vision_encoder.*``, ``prompt_encoder.*``,

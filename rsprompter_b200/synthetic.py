@@ -5,7 +5,7 @@ weights of the exact architecture (SURVEY.md appendix A; HF ``pytorch_model.bin`
 with the ``vision_encoder.`` prefix stripped as M:783 does).  Relative-position tables and the
 absolute position embedding are drawn non-zero (HF zero-initialises them, HF:1008-1014, which
 would hide every rel-pos bug).  The same dicts are loaded into the oracle (HF modules /
-restatement) and into the B200 modules, so parity compares arithmetic, not initialisation.
+restatement) and into the H100 modules, so parity compares arithmetic, not initialisation.
 """
 from __future__ import annotations
 

@@ -382,6 +382,22 @@ def main_necks():
     print("wrote", path, os.path.getsize(path), {k: list(v.keys()) for k, v in fx.items()})
 
 
+def main_configs():
+    """model / custom_imports of the reference's configs/rsprompter files, as the registry's Config resolves them
+    (reference_configs.pt, read by tests/test_reference_configs_cpu.py)."""
+    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+    from rsprompter_b200.registry import Config
+    names = ["rsprompter_anchor-nwpu.py", "rsprompter_anchor-nwpu-peft-512.py", "rsprompter_query-nwpu.py",
+             "rsprompter_query-nwpu-peft-512.py", "samdet-nwpu.py", "samseg-maskrcnn-nwpu.py", "samseg-mask2former-nwpu.py"]
+    fx = {}
+    for n in names:
+        d = Config.fromfile(os.path.join(REF, "configs", "rsprompter", n)).to_dict()
+        fx[n] = dict(model=d["model"], custom_imports=d.get("custom_imports"))
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_configs.pt")
+    torch.save(fx, path)
+    print("wrote", path, os.path.getsize(path))
+
+
 if __name__ == "__main__":
     if not os.path.isdir(REF):
         sys.exit("/root/reference not mounted")
@@ -391,5 +407,7 @@ if __name__ == "__main__":
         main_state_keys()
     elif "necks" in sys.argv[1:]:
         main_necks()
+    elif "configs" in sys.argv[1:]:
+        main_configs()
     else:
         main()

@@ -26,7 +26,7 @@ def test_global_attention_on_32x32_grid():
 
 @pytest.mark.parametrize("S,n_seq,H,hd", [(48, 2, 2, 64), (80, 1, 2, 80), (48, 1, 3, 80)])
 def test_other_grids_run_the_three_pass_tensor_core_path(S, n_seq, H, hd):
-    """768^2 / 1280^2 inputs (S = 48 / 80): Q K^T and P V as grouped tcgen05 GEMMs over all heads of an image,
+    """768^2 / 1280^2 inputs (S = 48 / 80): Q K^T and P V as grouped wgmma GEMMs over all heads of an image,
     Q [Rh; Rw]^T as a plain GEMM, the softmax + decomposed rel-pos row kernel in between (rsp_attn_softmax_bias);
     also checked against the CUDA-core kernel."""
     from oracle import restate

@@ -1,4 +1,4 @@
-"""SAM mask decoder on the B200 kernels vs the CPU oracle."""
+"""SAM mask decoder on the H100 kernels vs the CPU oracle."""
 import pytest
 import torch
 

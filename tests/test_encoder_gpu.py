@@ -1,4 +1,4 @@
-"""SAM ViT encoder on the B200 kernels vs the CPU oracle (same seeded weights, same input)."""
+"""SAM ViT encoder on the H100 kernels vs the CPU oracle (same seeded weights, same input)."""
 import pytest
 import torch
 

@@ -1,12 +1,19 @@
-"""The reference's own config files load unchanged through the registry surface and build the B200
-modules (skipped where /root/reference is not mounted, e.g. on the GPU box)."""
+"""The reference's own configs/rsprompter/*.py model configs build the H100 modules through the registry surface.
+tests/golden/reference_configs.pt holds each config's `model` (and `custom_imports`) as the registry's Config resolved
+it from the reference's files (_base_ inheritance, _delete_, merges); the loader itself is exercised on a small
+config tree of the same shape."""
+import copy
 import os
 
 import pytest
 import torch
 
-REF_CFG = "/root/reference/configs/rsprompter"
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF_CFG), reason="reference tree not mounted")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_configs.pt")
+
+
+def _ref_cfg(name):
+    """model / custom_imports of configs/rsprompter/<name> as the reference's files resolve."""
+    return copy.deepcopy(torch.load(GOLDEN, weights_only=False)[name])
 
 
 def _strip_init(cfg):
@@ -21,15 +28,34 @@ def _strip_init(cfg):
     return cfg
 
 
-def test_base_config_inheritance_and_delete():
+def test_base_config_inheritance_and_delete(tmp_path):
     from rsprompter_b200.registry import Config
-    cfg = Config.fromfile(os.path.join(REF_CFG, "rsprompter_anchor-nwpu-peft-512.py"))
+    c = _ref_cfg("rsprompter_anchor-nwpu-peft-512.py")
+    m = c["model"]
+    assert m["type"] == "RSPrompterAnchor"                                # from _base_
+    assert m["backbone"]["type"] == "MMPretrainSamVisionEncoder" and "extra_config" not in m["backbone"]  # _delete_
+    assert m["neck"]["feature_aggregator"]["type"] == "PseudoFeatureAggregator"
+    assert m["neck"]["feature_spliter"]["type"] == "RSSimpleFPN"          # merged, not replaced
+    assert m["roi_head"]["bbox_head"]["num_classes"] == 10
+    assert m["test_cfg"]["rcnn"]["max_per_img"] == 100
+    assert c["custom_imports"]["imports"] == ["mmdet.rsprompter"]
+    # the same three mechanisms on a config tree of the reference's shape
+    (tmp_path / "_base_").mkdir()
+    (tmp_path / "_base_" / "base.py").write_text(
+        "custom_imports = dict(imports=['mmdet.rsprompter'])\n"
+        "model = dict(type='RSPrompterAnchor', backbone=dict(type='RSSamVisionEncoder', extra_config=dict(a=1)),\n"
+        "             neck=dict(feature_aggregator=dict(type='RSFeatureAggregator'), feature_spliter=dict(type='RSSimpleFPN')),\n"
+        "             test_cfg=dict(rcnn=dict(max_per_img=100)))\n")
+    (tmp_path / "child.py").write_text(
+        "_base_ = ['_base_/base.py']\n"
+        "model = dict(backbone=dict(_delete_=True, type='MMPretrainSamVisionEncoder'),\n"
+        "             neck=dict(feature_aggregator=dict(_delete_=True, type='PseudoFeatureAggregator')))\n")
+    cfg = Config.fromfile(str(tmp_path / "child.py"))
     m = cfg.model
-    assert m.type == "RSPrompterAnchor"                                   # from _base_
-    assert m.backbone.type == "MMPretrainSamVisionEncoder" and "extra_config" not in m.backbone  # _delete_
+    assert m.type == "RSPrompterAnchor"
+    assert m.backbone.type == "MMPretrainSamVisionEncoder" and "extra_config" not in m.backbone
     assert m.neck.feature_aggregator.type == "PseudoFeatureAggregator"
-    assert m.neck.feature_spliter.type == "RSSimpleFPN"                   # merged, not replaced
-    assert m.roi_head.bbox_head.num_classes == 10
+    assert m.neck.feature_spliter.type == "RSSimpleFPN"
     assert m.test_cfg.rcnn.max_per_img == 100
     assert cfg.custom_imports["imports"] == ["mmdet.rsprompter"]
 
@@ -38,9 +64,8 @@ def test_base_config_inheritance_and_delete():
                                           ("rsprompter_anchor-nwpu-peft-512.py", "MMPretrainSamVisionEncoder")])
 def test_reference_anchor_configs_build(name, enc_cls):
     from rsprompter_b200 import synthetic
-    from rsprompter_b200.registry import MODELS, Config
-    cfg = Config.fromfile(os.path.join(REF_CFG, name))
-    model_cfg = _strip_init(cfg.to_dict()["model"])
+    from rsprompter_b200.registry import MODELS
+    model_cfg = _strip_init(_ref_cfg(name)["model"])
     model = MODELS.build(model_cfg)
     assert type(model).__name__ == "RSPrompterAnchor"
     assert type(model.backbone).__name__ == enc_cls
@@ -61,9 +86,8 @@ def test_reference_anchor_configs_build(name, enc_cls):
                                              ("rsprompter_query-nwpu-peft-512.py", "MMPretrainSamVisionEncoder", 70)])
 def test_reference_query_configs_build(name, enc_cls, nq):
     from rsprompter_b200 import synthetic
-    from rsprompter_b200.registry import MODELS, Config
-    cfg = Config.fromfile(os.path.join(REF_CFG, name))
-    model_cfg = _strip_init(cfg.to_dict()["model"])
+    from rsprompter_b200.registry import MODELS
+    model_cfg = _strip_init(_ref_cfg(name)["model"])
     model = MODELS.build(model_cfg)
     assert type(model).__name__ == "RSPrompterQuery" and type(model.backbone).__name__ == enc_cls
     head = model.panoptic_head
@@ -79,11 +103,10 @@ def test_reference_query_configs_build(name, enc_cls, nq):
 
 def test_reference_samdet_config_builds_the_segmentor():
     """configs/rsprompter/samdet-nwpu.py: type SAMDet with a stock mmdet FasterRCNN detector (outside this package) and
-    an RSSamModel segmentor (SURVEY 8(f4), M:718-741, 1060-1215): the segmentor entry builds the B200 SamModel
+    an RSSamModel segmentor (SURVEY 8(f4), M:718-741, 1060-1215): the segmentor entry builds the H100 SamModel
     (ViT-B: samdet-nwpu.py:25 points at sam_vit_base) with HF SamModel's parameter names; SAMDet is in the registry."""
-    from rsprompter_b200.registry import MODELS, Config
-    cfg = Config.fromfile(os.path.join(REF_CFG, "samdet-nwpu.py"))
-    m = cfg.to_dict()["model"]
+    from rsprompter_b200.registry import MODELS
+    m = _ref_cfg("samdet-nwpu.py")["model"]
     assert m["type"] == "SAMDet" and MODELS.get("SAMDet") is not None
     assert m["segmentor"]["type"] == "RSSamModel" and m["detector"]["type"] == "FasterRCNN"
     seg = MODELS.build(_strip_init(dict(m["segmentor"])))
@@ -102,9 +125,8 @@ def test_reference_samseg_maskrcnn_config_builds():
     StandardRoIHead / Shared2FCBBoxHead / FCNMaskHead builds from the reference's own config file and takes a state dict
     with mmdet's parameter names (fcn_mask_head.py:68-126: convs.N.conv, upsample, conv_logits)."""
     from rsprompter_b200 import synthetic
-    from rsprompter_b200.registry import MODELS, Config
-    cfg = Config.fromfile(os.path.join(REF_CFG, "samseg-maskrcnn-nwpu.py"))
-    model = MODELS.build(_strip_init(cfg.to_dict()["model"]))
+    from rsprompter_b200.registry import MODELS
+    model = MODELS.build(_strip_init(_ref_cfg("samseg-maskrcnn-nwpu.py")["model"]))
     assert type(model).__name__ == "SAMSegMaskRCNN" and type(model.roi_head).__name__ == "StandardRoIHead"
     assert type(model.roi_head.mask_head).__name__ == "FCNMaskHead" and model.roi_head.mask_head.num_classes == 10
     assert model.rpn_head.prior_generator.num_base_priors[0] == 3            # scales=[8] x 3 ratios
@@ -123,9 +145,8 @@ def test_reference_samseg_mask2former_config_builds():
     Mask2FormerHead (feat_channels 256, 9 decoder layers, FFN 2048) / MaskFormerFusionHead builds from the reference's
     own config file and takes a state dict with mmdet's parameter names."""
     from rsprompter_b200 import synthetic
-    from rsprompter_b200.registry import MODELS, Config
-    cfg = Config.fromfile(os.path.join(REF_CFG, "samseg-mask2former-nwpu.py"))
-    model = MODELS.build(_strip_init(cfg.to_dict()["model"]))
+    from rsprompter_b200.registry import MODELS
+    model = MODELS.build(_strip_init(_ref_cfg("samseg-mask2former-nwpu.py")["model"]))
     assert type(model).__name__ == "SAMSegMask2Former" and type(model.panoptic_head).__name__ == "Mask2FormerHead"
     assert type(model.panoptic_fusion_head).__name__ == "MaskFormerFusionHead"
     head = model.panoptic_head

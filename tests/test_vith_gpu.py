@@ -58,7 +58,7 @@ def test_vith_32_layer_encoder_matches_oracle():
 
 
 def test_lora_checkpoint_on_gpu_matches_unmerged_oracle():
-    """SURVEY 8(f3): a peft-LoRA checkpoint (M:785-797 key layout) loaded into the B200 encoder (adapter folded into
+    """SURVEY 8(f3): a peft-LoRA checkpoint (M:785-797 key layout) loaded into the H100 encoder (adapter folded into
     qkv.weight at load) against the oracle that keeps the adapter branch separate: y = Wx + b + (alpha/r) B(A x)."""
     from oracle import restate
     from rsprompter_b200 import synthetic
