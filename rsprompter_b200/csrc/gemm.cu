@@ -313,8 +313,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a,
       const int m_blk = tile / p.num_n_blocks;
       const int n_blk = tile % p.num_n_blocks;
       float acc[BN / 2];
-      wg_mainloop<BN, B_MN_MAJOR>(acc, smem_base, Cfg::STAGE_BYTES, A_STAGE_BYTES, STAGES, num_kb, wg, stage, phase,
-                                  bar_full, bar_empty);
+      wg_mainloop<BN, B_MN_MAJOR, STAGES>(acc, smem_base, Cfg::STAGE_BYTES, A_STAGE_BYTES, num_kb, wg, stage, phase,
+                                          bar_full, bar_empty);
       named_bar_sync(1, 256);   // the previous tile's epilogue has read the accumulator tile
       acc_store<BN>(acc, acc_base, Cfg::ACC_LD, wg, threadIdx.x & 127);
       named_bar_sync(1, 256);
@@ -515,7 +515,9 @@ int gemm_bf16(const GemmArgs& a, cudaStream_t stream) {
   }
   {
     static const bool force_v1 = getenv("RSP_GEMM_V1") != nullptr;
-    if ((!force_v1 || a.m_group_rows > 0) && gemm_v2_eligible(a)) return gemm_bf16_v2(a, bn, stream);
+    // the v2 kernel's standard epilogue runs tiles up to 128 wide; an explicit 256 stays on this one
+    if ((!force_v1 || a.m_group_rows > 0) && (bn <= 128 || a.m_group_rows > 0) && gemm_v2_eligible(a))
+      return gemm_bf16_v2(a, bn, stream);
   }
   switch (bn) {
     case 256: return launch_gemm<256, false>(a, stream);

@@ -208,6 +208,12 @@ int main(int argc, char** argv) {
     };
     for (const Case& c : cases) fails += run_case(c);
     if (bench) {
+      // ViT-H encoder linears at 1024^2, batch 8 (default tile width): qkv over 25 padded 14 x 14 windows per image,
+      // proj / lin1 / lin2 over 64 x 64 tokens per image
+      bench_gemm(39200, 3840, 1280, 0, 0, 0, 0);   // qkv: bias -> bf16
+      bench_gemm(32768, 1280, 1280, 0, 0, 1, 1);   // proj: bias + fp32 residual -> fp32
+      bench_gemm(32768, 5120, 1280, 0, 1, 0, 0);   // lin1: bias + GELU -> bf16
+      bench_gemm(32768, 1280, 5120, 0, 0, 1, 1);   // lin2: bias + fp32 residual -> fp32
       bench_gemm(32768, 2304, 768, 256, 0, 0, 0);
       bench_gemm(32768, 768, 768, 256, 0, 1, 1);
       bench_gemm(32768, 3072, 768, 256, 1, 0, 0);

@@ -64,18 +64,15 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar, uint32_t parity)
       : "memory");
   return ok;
 }
-// Bounded wait: a protocol bug must trap (launch error) instead of hanging the GPU box.
-// ~2^31 cycles (about a second) is far beyond any legitimate wait in this library.
+// Bounded wait: a protocol bug must trap (launch error) instead of hanging the GPU.
+// ~2^31 cycles (about a second) is far beyond any legitimate wait in this library.  No printf here: a function
+// call anywhere in a kernel makes ptxas serialise every wgmma of that kernel (warning C7510).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3ff) == 0 && clock64() - t0 > (1ll << 31)) {
-      printf("rsp: mbarrier timeout block %d thread %d bar 0x%x parity %u\n", (int)blockIdx.x,
-             (int)threadIdx.x, bar, parity);
-      __trap();
-    }
+    if ((++spins & 0x3ff) == 0 && clock64() - t0 > (1ll << 31)) __trap();
   }
 }
 
@@ -288,15 +285,28 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// Register budget of a warpgroup (setmaxnreg): every warp of the warpgroup executes the same one.  The producer gives
+// registers up, the MMA / epilogue roles take them; the block's total stays within what it was launched with.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // Consumer side of the GEMM ring: warpgroup wg accumulates rows [64 wg, 64 wg + 64) of a 128 x BN tile over num_kb
 // 64-deep k-blocks.  Stage s holds A (128 rows x 128 B, K-major) at base + s * stage_bytes and B at + a_bytes
 // (K-major BN rows, or MN-major: BN / 64 atoms of 64 K-rows x 128 B).  Each of the warpgroup's warps arrives once on
 // the stage's "empty" barrier (count 8 for two warpgroups) when its reads are done.
-template <int BN, bool B_MN>
-__device__ __forceinline__ void wg_mainloop(float (&d)[BN / 2], uint32_t base, int stage_bytes, int a_bytes, int stages,
+// One wgmma group stays in flight: k-block kb is committed, then the group of kb - 1 is retired and its stage
+// released, so the tensor cores never wait for the issuing warps between k-blocks.  The whole tile is retired
+// (wait_group 0) before the accumulators are returned.  With a single-stage ring the stage of kb must be released
+// before kb + 1 can be loaded, so there every group is retired at once.
+template <int BN, bool B_MN, int STAGES>
+__device__ __forceinline__ void wg_mainloop(float (&d)[BN / 2], uint32_t base, int stage_bytes, int a_bytes,
                                             int num_kb, int wg, int& stage, uint32_t& phase, uint64_t* bar_full,
                                             uint64_t* bar_empty) {
+  constexpr bool IN_FLIGHT = STAGES > 1;
   const int lane = threadIdx.x & 31;
+  int prev = 0;
 #pragma unroll 1
   for (int kb = 0; kb < num_kb; ++kb) {
     mbar_wait(smem_u32(&bar_full[stage]), phase);
@@ -311,11 +321,27 @@ __device__ __forceinline__ void wg_mainloop(float (&d)[BN / 2], uint32_t base, i
       Wgmma<BN>::template ss<B_MN ? 1 : 0>(d, adesc, bdesc, (kb | k) != 0);
     }
     wgmma_commit();
+    if constexpr (IN_FLIGHT) {
+      wgmma_wait<1>();
+      acc_fence(d);
+      if (kb > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&bar_empty[prev]));
+      }
+    } else {
+      wgmma_wait<0>();
+      acc_fence(d);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&bar_empty[stage]));
+    }
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  if constexpr (IN_FLIGHT) {
     wgmma_wait<0>();
     acc_fence(d);
     __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[stage]));
-    if (++stage == stages) { stage = 0; phase ^= 1; }
+    if (lane == 0 && num_kb > 0) mbar_arrive(smem_u32(&bar_empty[prev]));
   }
 }
 
