@@ -348,6 +348,25 @@ int rsp_mask_paste_boxes(const float* probs, const float* boxes, uint8_t* out, i
 int rsp_pack_mask_bits(const uint8_t* masks, uint8_t* bits, long long rows, int W, void* stream);
 int rsp_unpack_mask_bits(const uint8_t* bits, uint8_t* masks, long long rows, int W, void* stream);
 
+/* ---- COCO RLE of predicted masks on the device (SURVEY 8(f) rank 1, the RLE half).  Replaces the host encode of every
+ * predicted mask in CocoMetric.process: encode_mask_results(pred['masks'].detach().cpu().numpy())
+ * (coco_metric.py:365) -> pycocotools mask_util.encode per mask on a Fortran-order copy (mmdet/structures/mask/
+ * utils.py:37-53).  The output is pycocotools' compressed string (maskApi.c rleEncode + rleToString) byte for byte.
+ * Masks: desc int64 [n, 3] = (byte offset of mask i from src, H, W) in DEVICE memory and desc_host, the same values in
+ * host memory; every mask must have 1 .. 2^31 - 1 pixels (else RSP_ERR_INVALID, nothing launched).  packed = 0:
+ * uint8 [H, W] row-major, any nonzero byte is set (torch.bool masks); packed = 1: [H, ceil(W/8)] bytes, pixel x = bit
+ * x % 8 of byte x / 8 (the result-record payload).  One call covers masks of different sizes.  Two passes size the
+ * output exactly:
+ *   rsp_mask_rle_lengths  offsets int64 [n + 1]: offsets[i] = first char of mask i, offsets[n] = total chars
+ *   rsp_mask_rle_write    chars of mask i into pool[offsets[i], offsets[i + 1]) (pool: offsets[n] bytes) and
+ *                         lengths int32 [n] (-1: longer than INT32_MAX chars); src, packed, desc and offsets as
+ *                         given to / produced by rsp_mask_rle_lengths.  No write leaves a mask's range.
+ * No atomics: two calls give identical bytes. */
+int rsp_mask_rle_lengths(const uint8_t* src, int packed, const int64_t* desc, const int64_t* desc_host, int n,
+                         int64_t* offsets, void* stream);
+int rsp_mask_rle_write(const uint8_t* src, int packed, const int64_t* desc, int n, const int64_t* offsets, char* pool,
+                       int32_t* lengths, void* stream);
+
 /* ---- DetDataPreprocessor on the device (SURVEY 8(f2); data_preprocessor.py:110-148, ImgDataPreprocessor.forward,
  * BatchFixedSizePad :300).  mean3 / std3: HOST arrays of 3 floats in OUTPUT channel order. ---- */
 

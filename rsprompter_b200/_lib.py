@@ -104,6 +104,8 @@ _SIGNATURES = {
     "rsp_preprocess_u8": ([_vp, _i, _i, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp, _i, _i, _vp, _vp,
                            _i, _f, _vp], _i),
     "rsp_patchify16_u8": ([_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp], _i),
+    "rsp_mask_rle_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp], _i),
+    "rsp_mask_rle_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
 }
 
 
@@ -1093,4 +1095,52 @@ def patchify16_u8(img: torch.Tensor, mean, std, swap_rb: bool, out: torch.Tensor
     _check(_lib.rsp_patchify16_u8(_ptr(img), hwc, _ptr(out), B, H, W, _host_f3(mean), _host_f3(std), int(swap_rb),
                                   _stream()), "rsp_patchify16_u8")
     launch_count += 1
+    return out
+
+
+# ------------------------------------------------------------------------------ COCO RLE
+def mask_rle(groups: list, packed: bool) -> list:
+    """pycocotools compressed RLE strings (bytes, one per mask, in order) of every mask in ``groups`` = [(masks, W)]:
+    contiguous CUDA tensors [n, H, W] bool / uint8 (packed=False) or uint8 [n, H, ceil(W/8)] bit-packed rows
+    (packed=True), sizes free to differ between groups.  One batched encode: a length pass + offset scan, one
+    device->host read of the total, the write pass, one copy of the chars + lengths."""
+    global launch_count
+    groups = [(t, int(W)) for t, W in groups if t.shape[0] > 0]
+    if not groups:
+        return []
+    _require_cuda(*[t for t, _ in groups])
+    base = min(t.data_ptr() for t, _ in groups)        # descriptors address every mask from the lowest pointer
+    rows = []
+    for t, W in groups:
+        assert t.dtype in (torch.bool, torch.uint8) and t.dim() == 3 and t.is_contiguous()
+        n, H, ld = t.shape
+        assert ld == ((W + 7) // 8 if packed else W), "row length does not match W"
+        off = t.data_ptr() - base
+        rows += [(off + j * H * ld, H, W) for j in range(n)]
+    n = len(rows)
+    dev = groups[0][0].device
+    desc_host = torch.tensor(rows, dtype=torch.int64).pin_memory()
+    desc = desc_host.to(dev, non_blocking=True)
+    offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    _check(_lib.rsp_mask_rle_lengths(base, int(packed), _ptr(desc), _ptr(desc_host), n, _ptr(offsets), _stream()),
+           "rsp_mask_rle_lengths")
+    total = int(offsets[n].item())                       # host sync 1: the exact pool size
+    pool = torch.empty(total, dtype=torch.uint8, device=dev)
+    lengths = torch.empty(n, dtype=torch.int32, device=dev)
+    _check(_lib.rsp_mask_rle_write(base, int(packed), _ptr(desc), n, _ptr(offsets), _ptr(pool), _ptr(lengths),
+                                   _stream()), "rsp_mask_rle_write")
+    launch_count += 3
+    host_pool = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+    host_len = torch.empty(n, dtype=torch.int32, pin_memory=True)
+    host_pool.copy_(pool, non_blocking=True)
+    host_len.copy_(lengths, non_blocking=True)
+    torch.cuda.current_stream().synchronize()            # host sync 2: chars + lengths
+    lens = host_len.tolist()
+    if min(lens) < 0:
+        raise RspError("rsp_mask_rle_write: a mask's RLE string is longer than 2^31 - 1 chars")
+    buf = host_pool.numpy().tobytes()
+    out, p = [], 0
+    for ln in lens:
+        out.append(buf[p:p + ln])
+        p += ln
     return out

@@ -1,0 +1,247 @@
+// COCO compressed RLE of binary masks on the device (SURVEY 8(f) rank 1, the RLE half): the encode CocoMetric.process
+// runs on the host for every predicted mask (coco_metric.py:359-367 -> mask/utils.py:37-53 -> pycocotools maskApi.c
+// rleEncode + rleToString).  HBM / L2 bound, no tensor cores.
+//
+// Format (results.mask_to_coco_rle restates it): runs in column-major order (flat index x*H + y), the first run counts
+// zeros; count j is written in 5-bit groups with a continuation bit (0x20), offset 48, and for j > 2 as the
+// sign-extended difference to count j - 2.
+//
+// Boundaries: P[0] = 0, then every flat index p whose pixel differs from pixel p - 1 (pixel -1 counts as 0), then
+// H*W.  Count j = P[j+1] - P[j], so the chars of count j depend on P[j-2 .. j+1] only, and a scan with the
+// associative "boundaries so far + last three boundary positions" operator gives every column the context its first
+// counts need.
+//
+// One CTA per mask.  The mask is walked in tiles of kThreads columns; thread t owns column x0 + t and walks it top to
+// bottom (consecutive lanes read consecutive bytes of a row).  Per tile:
+//   walk 1  per column: boundary count, first and last three positions, and the chars of every count whose three
+//           preceding boundaries lie in the same column;
+//   scans   the context before each column -> the chars of its first (up to) three counts; an exclusive sum of the
+//           column chars -> the column's offset in the mask's string;
+//   walk 2  (write pass only) the column again, writing its chars there.
+// The length pass stores each mask's char count, a one-CTA scan turns them into offsets, and the write pass repeats
+// walk 1 + scans (same code, same result) before walk 2.  No atomics: the output is deterministic.  Every write is
+// bounded by the mask's [offsets[i], offsets[i+1]) range.
+#include <climits>
+
+#include <cub/block/block_scan.cuh>
+
+#include "rle.h"
+
+namespace rsp {
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kScanThreads = 256;
+
+struct RleCtx {
+  unsigned n;   // boundaries so far, P[0] included (<= H*W + 1 < 2^32)
+  int p[3];     // the last three boundary positions, p[2] the latest
+};
+
+// context of a run of columns a followed by b
+struct RleCtxOp {
+  __device__ __forceinline__ RleCtx operator()(const RleCtx& a, const RleCtx& b) const {
+    RleCtx r;
+    r.n = a.n + b.n;
+    r.p[2] = b.n >= 1 ? b.p[2] : a.p[2];
+    r.p[1] = b.n >= 2 ? b.p[1] : (b.n == 1 ? a.p[2] : a.p[1]);
+    r.p[0] = b.n >= 3 ? b.p[0] : (b.n == 2 ? a.p[2] : (b.n == 1 ? a.p[1] : a.p[0]));
+    return r;
+  }
+};
+
+// the value written for the count that ends at boundary `pos`, given the context before that boundary
+__device__ __forceinline__ int rle_value(const RleCtx& c, int pos) {
+  int v = pos - c.p[2];
+  if (c.n >= 4) v -= c.p[1] - c.p[0];   // count index c.n - 1 > 2
+  return v;
+}
+
+__device__ __forceinline__ void rle_push(RleCtx& c, int pos) {
+  c.p[0] = c.p[1];
+  c.p[1] = c.p[2];
+  c.p[2] = pos;
+  ++c.n;
+}
+
+__device__ __forceinline__ int rle_chars(int v) {
+  int k = 0;
+  bool more;
+  do {
+    const int ch = v & 0x1f;
+    v >>= 5;   // arithmetic shift: negative differences
+    more = (ch & 0x10) ? v != -1 : v != 0;
+    ++k;
+  } while (more);
+  return k;
+}
+
+// writes the chars of v from dst on, none at or past `end`; returns the position after them
+__device__ __forceinline__ char* rle_put(char* dst, const char* end, int v) {
+  bool more;
+  do {
+    int ch = v & 0x1f;
+    v >>= 5;
+    more = (ch & 0x10) ? v != -1 : v != 0;
+    if (more) ch |= 0x20;
+    if (dst < end) *dst = static_cast<char>(ch + 48);
+    ++dst;
+  } while (more);
+  return dst;
+}
+
+template <bool kPacked>
+struct MaskView {
+  const unsigned char* m;
+  int H, W, ld;   // ld = bytes per row
+  __device__ __forceinline__ unsigned at(int y, int x) const {
+    const unsigned char* row = m + static_cast<long long>(y) * ld;
+    if (kPacked) return (__ldg(row + (x >> 3)) >> (x & 7)) & 1u;
+    return __ldg(row + x) != 0 ? 1u : 0u;
+  }
+};
+
+// f(flat position) for every boundary inside column x, top to bottom; 16 rows are loaded before any is examined
+template <bool kPacked, typename F>
+__device__ __forceinline__ void for_each_boundary(const MaskView<kPacked>& mv, int x, F&& f) {
+  unsigned prev = x > 0 ? mv.at(mv.H - 1, x - 1) : 0u;
+  const int base = x * mv.H;
+  for (int y0 = 0; y0 < mv.H; y0 += 16) {
+    const int rows = min(16, mv.H - y0);
+    unsigned w = 0u;
+    if (rows == 16) {
+#pragma unroll
+      for (int k = 0; k < 16; ++k) w |= mv.at(y0 + k, x) << k;
+    } else {
+      for (int k = 0; k < rows; ++k) w |= mv.at(y0 + k, x) << k;
+    }
+    unsigned change = (w ^ ((w << 1) | prev)) & ((1u << rows) - 1u);
+    prev = (w >> (rows - 1)) & 1u;
+    while (change) {
+      const int k = __ffs(change) - 1;
+      change &= change - 1u;
+      f(base + y0 + k);
+    }
+  }
+}
+
+// kWrite = false: offsets[i + 1] = chars of mask i.  kWrite = true: the chars into pool[offsets[i], offsets[i+1]).
+template <bool kPacked, bool kWrite>
+__global__ void __launch_bounds__(kThreads) mask_rle_kernel(const unsigned char* __restrict__ src,
+                                                            const long long* __restrict__ desc, long long* offsets,
+                                                            char* __restrict__ pool, int* __restrict__ lengths) {
+  using CtxScan = cub::BlockScan<RleCtx, kThreads, cub::BLOCK_SCAN_WARP_SCANS>;
+  using SumScan = cub::BlockScan<long long, kThreads, cub::BLOCK_SCAN_WARP_SCANS>;
+  __shared__ union {
+    typename CtxScan::TempStorage ctx;
+    typename SumScan::TempStorage sum;
+  } tmp;
+  const int i = blockIdx.x;
+  const int H = static_cast<int>(desc[3 * i + 1]), W = static_cast<int>(desc[3 * i + 2]);
+  const MaskView<kPacked> mv{src + desc[3 * i], H, W, kPacked ? (W + 7) / 8 : W};
+  char* out = nullptr;
+  const char* end = nullptr;
+  if (kWrite) {
+    out = pool + offsets[i];
+    end = pool + offsets[i + 1];
+  }
+  RleCtx carry{1u, {0, 0, 0}};   // P[0] = 0
+  long long chars = 0;           // chars of the tiles before this one
+  for (int x0 = 0; x0 < W; x0 += kThreads) {
+    const int x = x0 + threadIdx.x;
+    RleCtx local{0u, {0, 0, 0}};
+    int first[3] = {0, 0, 0};
+    long long len = 0;
+    if (x < W) {
+      for_each_boundary(mv, x, [&](int pos) {
+        if (local.n >= 3) len += rle_chars((pos - local.p[2]) - (local.p[1] - local.p[0]));
+        else if (local.n == 0) first[0] = pos;
+        else if (local.n == 1) first[1] = pos;
+        else first[2] = pos;
+        rle_push(local, pos);
+      });
+    }
+    RleCtx pre, agg;
+    CtxScan(tmp.ctx).ExclusiveScan(local, pre, RleCtxOp{}, agg);
+    pre = threadIdx.x == 0 ? carry : RleCtxOp{}(carry, pre);
+    RleCtx c = pre;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      if (k < static_cast<int>(local.n)) {
+        len += rle_chars(rle_value(c, first[k]));
+        rle_push(c, first[k]);
+      }
+    }
+    __syncthreads();   // tmp is reused
+    long long off, tile_chars;
+    SumScan(tmp.sum).ExclusiveSum(len, off, tile_chars);
+    if (kWrite && x < W) {
+      char* dst = out + chars + off;
+      c = pre;
+      for_each_boundary(mv, x, [&](int pos) {
+        dst = rle_put(dst, end, rle_value(c, pos));
+        rle_push(c, pos);
+      });
+    }
+    carry = RleCtxOp{}(carry, agg);
+    chars += tile_chars;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {   // the last count ends at H*W
+    const int v = rle_value(carry, H * W);
+    if (kWrite) {
+      rle_put(out + chars, end, v);
+      const long long len = offsets[i + 1] - offsets[i];
+      lengths[i] = len <= INT_MAX ? static_cast<int>(len) : -1;
+    } else {
+      offsets[i + 1] = chars + rle_chars(v);
+    }
+  }
+}
+
+// offsets[1..n] = inclusive sum of the per-mask char counts stored there, offsets[0] = 0
+__global__ void __launch_bounds__(kScanThreads) rle_offsets_kernel(long long* offsets, int n) {
+  using Scan = cub::BlockScan<long long, kScanThreads, cub::BLOCK_SCAN_WARP_SCANS>;
+  __shared__ typename Scan::TempStorage tmp;
+  long long carry = 0;
+  for (int i0 = 0; i0 < n; i0 += kScanThreads) {
+    const int i = i0 + threadIdx.x;
+    long long v = i < n ? offsets[i + 1] : 0, inc, agg;
+    Scan(tmp).InclusiveSum(v, inc, agg);
+    if (i < n) offsets[i + 1] = carry + inc;
+    carry += agg;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) offsets[0] = 0;
+}
+
+}  // namespace
+
+int mask_rle_lengths(const unsigned char* src, int packed, const long long* desc, const long long* desc_host, int n,
+                     long long* offsets, cudaStream_t stream) {
+  RSP_CHECK_ARG(src && desc && desc_host && offsets && n > 0 && (packed == 0 || packed == 1), "mask_rle_lengths: bad args");
+  for (int i = 0; i < n; ++i) {
+    const long long off = desc_host[3 * i], H = desc_host[3 * i + 1], W = desc_host[3 * i + 2];
+    RSP_CHECK_ARG(off >= 0 && H >= 1 && W >= 1 && H <= INT_MAX && W <= INT_MAX && H * W <= INT_MAX,
+                  "mask_rle_lengths: mask %d is %lld x %lld at offset %lld (1 .. 2^31 - 1 pixels)", i, H, W, off);
+  }
+  if (packed) mask_rle_kernel<true, false><<<n, kThreads, 0, stream>>>(src, desc, offsets, nullptr, nullptr);
+  else mask_rle_kernel<false, false><<<n, kThreads, 0, stream>>>(src, desc, offsets, nullptr, nullptr);
+  RSP_CHECK_LAUNCH();
+  rle_offsets_kernel<<<1, kScanThreads, 0, stream>>>(offsets, n);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
+int mask_rle_write(const unsigned char* src, int packed, const long long* desc, int n, const long long* offsets,
+                   char* pool, int* lengths, cudaStream_t stream) {
+  RSP_CHECK_ARG(src && desc && offsets && pool && lengths && n > 0 && (packed == 0 || packed == 1),
+                "mask_rle_write: bad args");
+  long long* offs = const_cast<long long*>(offsets);   // only the length pass writes them
+  if (packed) mask_rle_kernel<true, true><<<n, kThreads, 0, stream>>>(src, desc, offs, pool, lengths);
+  else mask_rle_kernel<false, true><<<n, kThreads, 0, stream>>>(src, desc, offs, pool, lengths);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
+}  // namespace rsp

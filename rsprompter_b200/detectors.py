@@ -2,7 +2,8 @@
 
 ``predict(batch_inputs, batch_data_samples, rescale=True)`` keeps the reference contract
 (mmdet BaseDetector.forward mode='predict', detectors/base.py:58-99): it returns the data samples
-with ``pred_instances`` holding ``bboxes``, ``scores``, ``labels`` and boolean ``masks``.
+with ``pred_instances`` holding ``bboxes``, ``scores``, ``labels`` and boolean ``masks`` (COCO RLE dicts with
+``test_cfg.rle_masks``).
 Everything between the input tensor and the final per-image split runs on the device without
 host synchronisation; the one device->host read is the per-image detection count.
 """
@@ -13,7 +14,7 @@ import torch
 from . import _lib
 from .necks import PseudoFeatureAggregator
 from .registry import MODELS, BaseModule, ConfigDict, DetDataSample, InstanceData, make_data_samples
-from .results import ResultRecord
+from .results import ResultRecord, encode_mask_results
 from .sam_encoder import MMPretrainSamVisionEncoder, SamVisionEncoderOutput
 
 
@@ -158,6 +159,18 @@ class _SamDetectorBase(BaseModule):
             out.append(dict(ori_hw=ori, crop_hw=crop, scale_factor=sf))
         return hw, out
 
+    @staticmethod
+    def _rle_masks(test_cfg, batch_data_samples):
+        """With test_cfg.rle_masks, every pred_instances.masks becomes a list of COCO RLE dicts ({'size': [h, w],
+        'counts': bytes}, h, w = the mask's size) encoded on the device in one batched call.  CocoMetric.process passes
+        non-tensor masks through (coco_metric.py:364-367), so evaluation copies no mask pixel to the host."""
+        if test_cfg is None or not test_cfg.get("rle_masks", False):
+            return batch_data_samples
+        insts = [ds.pred_instances for ds in batch_data_samples]
+        for inst, rles in zip(insts, encode_mask_results([inst.masks for inst in insts])):
+            inst.masks = rles
+        return batch_data_samples
+
 
 @MODELS.register_module(force=True)
 class RSPrompterAnchor(_SamDetectorBase):
@@ -225,7 +238,7 @@ class RSPrompterAnchor(_SamDetectorBase):
                     crop = (min(int(ih * sf[1]), hw[0]), min(int(iw * sf[0]), hw[1]))
                 mk = _lib.mask_paste_rescale(logits[b * M:b * M + max(n, 1)], hw, crop, m["ori_hw"], thr)[:n]
             ds.pred_instances = InstanceData(bboxes=boxes, scores=r["scores"][b, :n], labels=r["labels"][b, :n], masks=mk)
-        return batch_data_samples
+        return self._rle_masks(self.test_cfg, batch_data_samples)
 
     @torch.no_grad()
     def predict_records(self, batch_inputs: torch.Tensor, record: ResultRecord | None = None) -> ResultRecord:
@@ -304,7 +317,7 @@ class RSPrompterQuery(_SamDetectorBase):
                 k = out["is_thing"][b]
                 inst = {n: v[k] for n, v in inst.items()}
             ds.pred_instances = InstanceData(**inst)
-        return batch_data_samples
+        return self._rle_masks(self.test_cfg, batch_data_samples)
 
     @torch.no_grad()
     def predict_records(self, batch_inputs: torch.Tensor, record: ResultRecord | None = None) -> ResultRecord:
@@ -410,7 +423,7 @@ class SAMSegMaskRCNN(_SamDetectorBase):
                 pb[:n] = boxes
                 mk = _lib.mask_paste_boxes(probs[b * M:b * M + max(n, 1)].contiguous(), pb, size, thr)[:n]
             ds.pred_instances = InstanceData(bboxes=boxes, scores=r["scores"][b, :n], labels=r["labels"][b, :n], masks=mk)
-        return batch_data_samples
+        return self._rle_masks(self.test_cfg, batch_data_samples)
 
     @torch.no_grad()
     def predict_records(self, batch_inputs: torch.Tensor, record: ResultRecord | None = None) -> ResultRecord:

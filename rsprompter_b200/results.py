@@ -84,7 +84,8 @@ class ResultRecord:
 # C extension absent from this image and from /root/reference; the two functions below restate its published format
 # (maskApi.c rleEncode / rleToString / rleFrString: column-major runs starting with a run of zeros; counts written as
 # 5-bit groups + continuation bit, offset 48, with every count from the fourth on stored as the difference to the count
-# two places back).  Host-side numpy on the bit-packed payload - evaluation itself stays outside this package.
+# two places back).  Host-side numpy on the bit-packed payload - evaluation itself stays outside this package.  The
+# device encoder (encode_mask_results, device records; csrc/rle.cu) is held to these bytes.
 def mask_to_coco_rle(mask) -> dict:
     """bool / uint8 [H, W] (numpy or CPU tensor) -> {'size': [H, W], 'counts': bytes}."""
     import numpy as np
@@ -140,22 +141,47 @@ def coco_rle_to_mask(rle: dict):
     return flat.reshape(w, h).T
 
 
+def encode_mask_results(masks) -> list:
+    """Device counterpart of mmdet's encode_mask_results (mmdet/structures/mask/utils.py:37-53, called from
+    CocoMetric.process, coco_metric.py:365): CUDA bool / uint8 masks [n, H, W] -> one {'size': [H, W], 'counts': bytes}
+    dict per mask, byte for byte what mask_to_coco_rle (pycocotools) gives.  A list of such tensors (sizes may differ,
+    e.g. one per image at its ori_shape) is encoded in one batched call and gives one list per tensor.  Only the RLE
+    strings leave the device."""
+    from . import _lib
+    single = isinstance(masks, torch.Tensor)
+    group = [m.contiguous() for m in ([masks] if single else masks)]
+    strs = _lib.mask_rle([(m, m.shape[-1]) for m in group], packed=False)
+    out, p = [], 0
+    for m in group:
+        n, h, w = m.shape
+        out.append([dict(size=[int(h), int(w)], counts=s) for s in strs[p:p + n]])
+        p += n
+    return out[0] if single else out
+
+
 def record_to_coco_results(rec: "ResultRecord", image_ids: list, label_to_cat=None) -> list:
-    """Host record -> the 'segm' result dicts CocoMetric.results2json writes (coco_metric.py:237-262): one dict per
-    valid slot with image_id, bbox (xywh), score, category_id and the RLE-encoded mask."""
+    """Record -> the 'segm' result dicts CocoMetric.results2json writes (coco_metric.py:237-262): one dict per valid
+    slot with image_id, bbox (xywh), score, category_id and the RLE-encoded mask.  A device record is encoded from its
+    bits on the GPU (only the RLE strings, rows and counts are copied to the host); a host record in numpy."""
     import numpy as np
-    assert not rec.buf.is_cuda, "copy the record to the host first (ResultRecord.to_host)"
     H, W = rec.hw
+    counts = rec.counts.tolist()
+    rows = rec.rows.cpu().numpy()
+    if rec.buf.is_cuda:
+        from . import _lib
+        strs = iter(_lib.mask_rle([(rec.mask_bits[b, :n], W) for b, n in enumerate(counts)], packed=True))
+        segm = [[dict(size=[int(H), int(W)], counts=next(strs)) for _ in range(n)] for n in counts]
+    else:
+        bits = rec.mask_bits.numpy()
+        masks = [np.unpackbits(bits[b, :n], axis=-1, bitorder="little")[..., :W].astype(bool) for b, n in enumerate(counts)]
+        segm = [[mask_to_coco_rle(m) for m in mk] for mk in masks]
     out = []
-    bits = rec.mask_bits.numpy()
-    rows = rec.rows.numpy()
-    for b, n in enumerate(rec.counts.tolist()):
-        masks = np.unpackbits(bits[b, :n], axis=-1, bitorder="little")[..., :W].astype(bool)
+    for b, n in enumerate(counts):
         for j in range(n):
             x1, y1, x2, y2, score, label = rows[b, j].tolist()
             cat = int(label) if label_to_cat is None else label_to_cat[int(label)]
             out.append(dict(image_id=image_ids[b], bbox=[x1, y1, x2 - x1, y2 - y1], score=float(score), category_id=cat,
-                            segmentation=mask_to_coco_rle(masks[j])))
+                            segmentation=segm[b][j]))
     return out
 
 

@@ -165,7 +165,8 @@ class SAMDet(BaseModule):
                 inst = ds.pred_instances
             inst.masks = self._segment(input_img, inst.bboxes.to(input_img.device), ds.metainfo)
             ds.pred_instances = inst
-        return batch_data_samples
+        from .detectors import _SamDetectorBase
+        return _SamDetectorBase._rle_masks(self.test_cfg, batch_data_samples)
 
     def forward(self, inputs, data_samples=None, mode: str = "predict"):
         if mode == "predict":
