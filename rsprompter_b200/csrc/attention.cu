@@ -4,16 +4,28 @@
 // (:803-831), get_rel_pos / get_decomposed_rel_pos (:729-801); mmpretrain vit_sam.py
 // Attention.forward (:202-221), add_decomposed_rel_pos (:117-157).
 //
-// Flash-style, everything in registers: one CTA = 64 query rows of one (sequence, head), 4 warps of 16 rows each.
-// Scores and the output accumulator are bf16 mma.sync m16n8k16 fragments with fp32 accumulation; the score fragment
-// of a 64-key tile becomes, after the online softmax, the A operand of P V without leaving the registers.  P V runs in
-// fp16 (P in [0, 1] keeps 11 mantissa bits instead of bf16's 8; each V tile is converted in shared memory, exactly for
-// |v| in fp16's normal range).  K / V tiles stream through a two-stage cp.async ring (rows padded by 16 bytes:
-// conflict-free ldmatrix).
+// Flash-style on wgmma.  Persistent: one CTA per SM works through query tiles of 128 rows of one (sequence, head),
+// 384 threads in three warpgroups:
+//   * warpgroup 0 gives its registers up (setmaxnreg).  Warp 0 is the TMA producer: the layer's two rel-pos tables
+//     once, then per query tile its Q (double-buffered where shared memory allows, so the next tile's Q lands during
+//     this one) and its 64-key K / V tiles through a four-stage mbarrier ring that runs on across query tiles.
+//     Warps 1-3 convert each landed V tile bf16 -> fp16 in place (exact for |v| in fp16's normal range), off the
+//     consumers' critical path.
+//   * warpgroups 1 and 2 own 64 query rows each.  S = Q K^T is an SS wgmma (bf16, fp32 accumulators); the online
+//     softmax runs on the accumulator fragment; P (fp16, which keeps 11 mantissa bits of a value in [0, 1] where bf16
+//     keeps 8) goes straight from those registers into the A operand of an RS wgmma against the fp16 V tile.
+//     Scores stay fp32 until the exp (reference: softmax in fp32).
+// Shared-memory layout of a [rows x hd] bf16 tile: columns 0-63 in the 128-byte-swizzled layout (rows of 128 bytes),
+// then, for hd = 80, columns 64-79 in the 32-byte-swizzled layout (rows of 32 bytes).  A head is 160 bytes, not a
+// multiple of one 128-byte swizzle row, so each tile is two TMA boxes (64 and 16 columns wide) from two tensor maps.
+// Q K^T is four k16 steps in the first part and one in the second; P V is an N = 64 wgmma on the first part plus an
+// N = 16 one on the second (both MN-major).  The fp16 V conversion keeps every element in place, so it needs no
+// layout of its own.
 // The decomposed relative-position bias is never materialised as a T x T tensor: a prologue runs Q x table^T for both
-// tables on the same tensor-core path (the reference's two einsums), scatters each row's S + S values (pre-multiplied
-// by log2 e) into shared memory, and the bias is added to the scores before the exp.  Scores stay fp32 until the exp
-// (reference: softmax in fp32).
+// tables on the same wgmma path (the reference's two einsums) and scatters each row's S + S values (pre-multiplied by
+// log2 e) into shared memory.  For S = 32 / 64 the key tile is a multiple of S, so each register of a thread's score
+// fragment always meets the same key column kw: the thread keeps its rel_w terms in registers and reads one rel_h
+// value per row and S-key block per tile.  For S = 14 both terms are read from shared memory per score.
 #include <cstdlib>
 
 #include "attention.h"
@@ -28,297 +40,394 @@ __device__ __forceinline__ float fast_exp2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-// d (+)= a[16 x 16] * b[16 x 8], bf16 (or fp16) in, fp32 accumulators (row.col)
-__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-      "{%0, %1, %2, %3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void mma_f16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-      "{%0, %1, %2, %3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
   __half2 v = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
+}
+__device__ __forceinline__ uint32_t bf16x2_to_f16x2(uint32_t w) {
+  return pack_f16x2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
 }
 
 template <int HD, int S>
 struct AttCfg {
   static constexpr int T = S * S;
-  static constexpr int HDP = HD + 8;                  // padded smem row (bf16): 16-byte rows shift banks
-  static constexpr int CH = HD / 8;                   // 16-byte chunks per row
-  static constexpr int NKT = (T + 63) / 64;           // 64-key tiles
-  static constexpr int NREL = 2 * S - 1;              // rel-pos table rows
-  static constexpr int NTG = (NREL + 63) / 64;        // 64-row groups of a table
-  static constexpr int SP = S + 4;                    // row stride of the gathered bias (floats)
-  static constexpr int Q_ELEMS = 64 * HDP;
-  static constexpr int KV_ELEMS = 128 * HDP;          // two 64-key stages (in the prologue: one whole table)
-  static constexpr int SMEM_BYTES = (Q_ELEMS + 2 * KV_ELEMS) * 2 + 2 * 64 * SP * 4;
+  static constexpr int BM = 128;                        // query rows per CTA: two consumer warpgroups of 64
+  static constexpr int BN = 64;                         // keys per K / V tile
+  static constexpr int NQT = (T + BM - 1) / BM;
+  static constexpr int NKT = (T + BN - 1) / BN;
+  static constexpr int NREL = 2 * S - 1;                // rel-pos table rows
+  static constexpr int NTAB = NREL <= 32 ? 32 : (NREL <= 64 ? 64 : 128);   // table rows loaded (N of the prologue)
+  static constexpr int TAIL = HD - 64;                  // columns in the 32-byte-swizzled part: 0 or 16
+  static constexpr int STAGES = 4;
+  static constexpr int SP = S + 4;                      // row stride of the gathered bias (floats)
+  __host__ __device__ static constexpr int tile_bytes(int rows) { return rows * (128 + 2 * TAIL); }
+  static constexpr int STAGE_BYTES = 2 * tile_bytes(BN);   // K, then V
+  static constexpr int smem_bytes(int qbuf) {                 // + 1024 bytes of slack to align the base
+    return qbuf * tile_bytes(BM) + STAGES * STAGE_BYTES + 2 * tile_bytes(NTAB) + 2 * BM * SP * 4 + 8 * 64 + 1024;
+  }
+  static constexpr int QBUF = smem_bytes(2) <= 227 * 1024 ? 2 : 1;   // Q buffers: the next tile's Q lands early
+  static constexpr int Q_OFF = 0;
+  static constexpr int KV_OFF = Q_OFF + QBUF * tile_bytes(BM);
+  static constexpr int TAB_OFF = KV_OFF + STAGES * STAGE_BYTES;
+  static constexpr int BIAS_OFF = TAB_OFF + 2 * tile_bytes(NTAB);
+  static constexpr int BAR_OFF = BIAS_OFF + 2 * BM * SP * 4;
+  static constexpr int SMEM_BYTES = smem_bytes(QBUF);
+  static constexpr int REG_PRODUCER = 40, REG_CONSUMER = 232;    // 128 x 40 + 256 x 232 <= 64K registers
+  static_assert(HD == 64 || HD == 80, "head dim");
   static_assert(NREL <= 128, "table rows");
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
 };
 
 struct AttDev {
-  const __nv_bfloat16* qkv;
-  const __nv_bfloat16* rel_h;
-  const __nv_bfloat16* rel_w;
   __nv_bfloat16* out;  // [M_tok, D]
+  const int* out_row_map;   // window_unpartition + crop fused into the store (HF:925-952), or null
   int H;
   int D;
-  int n_qt;            // 64-query tiles per sequence
+  int n_items;         // query tiles in all: n_seq * H * NQT
   float scale2;        // hd^-0.5 * log2(e)
-  const int* out_row_map;   // window_unpartition + crop fused into the store (HF:925-952), or null
 };
 
+// acc[64 x N] = (this warpgroup's 64 rows of Q) x B^T, B = the first N rows of a K-like tile of b_rows rows at b
+template <int N, int TAIL>
+__device__ __forceinline__ void qk_wgmma(float (&acc)[N / 2], uint32_t qa, uint32_t qtail, uint32_t b, int b_rows) {
+  acc_fence(acc);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    Wgmma<N>::template ss<0>(acc, make_gdesc(qa + 32 * k, 16, 1024), make_gdesc(b + 32 * k, 16, 1024), k);
+  if constexpr (TAIL > 0)
+    Wgmma<N>::template ss<0>(acc, make_gdesc_sw32(qtail, 16, 256), make_gdesc_sw32(b + b_rows * 128, 16, 256), 1);
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc_fence(acc);
+}
+
+// one [rows x HD] tile of a 3-D (column, token, sequence) tensor map pair: 64 columns 128B-swizzled, then the tail
+template <int TAIL>
+__device__ __forceinline__ void load_tile(uint32_t dst, int rows, const CUtensorMap* m, const CUtensorMap* mt,
+                                          uint32_t bar, int col, int row, int seq) {
+  tma_load_3d(dst, m, bar, col, row, seq);
+  if constexpr (TAIL > 0) tma_load_3d(dst + rows * 128, mt, bar, col + 64, row, seq);
+}
+
 template <int HD, int S>
-__global__ void __launch_bounds__(128)
-vit_attention_kernel(const AttDev p) {
+__global__ void __launch_bounds__(384, 1)
+vit_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_q_t,
+                     const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_kv_t,
+                     const __grid_constant__ CUtensorMap tm_rh, const __grid_constant__ CUtensorMap tm_rh_t,
+                     const __grid_constant__ CUtensorMap tm_rw, const __grid_constant__ CUtensorMap tm_rw_t,
+                     const AttDev p) {
   using C = AttCfg<HD, S>;
-  constexpr int T = C::T, HDP = C::HDP, CH = C::CH, SP = C::SP;
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_raw);
-  __nv_bfloat16* sK = sQ + C::Q_ELEMS;
-  __nv_bfloat16* sV = sK + C::KV_ELEMS;
-  float* relh = reinterpret_cast<float*>(sV + C::KV_ELEMS);   // [64][SP]: rel_h term of (row, key row kh)
-  float* relw = relh + 64 * SP;                               // [64][SP]: rel_w term of (row, key column kw)
+  constexpr int T = C::T, BM = C::BM, BN = C::BN, NKT = C::NKT, SP = C::SP, STAGES = C::STAGES, TAIL = C::TAIL;
+  constexpr int QBUF = C::QBUF;
+  constexpr uint32_t TILE_KV = C::tile_bytes(BN), TILE_TAB = C::tile_bytes(C::NTAB);
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const uint32_t sbase = smem_u32(smem);
+  float* relh = reinterpret_cast<float*>(smem + C::BIAS_OFF);   // [BM][SP]: rel_h term of (row, key row kh)
+  float* relw = relh + BM * SP;                                 // [BM][SP]: rel_w term of (row, key column kw)
+  uint64_t* bar_tab = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);   // both tables landed
+  uint64_t* bar_q = bar_tab + 1;            // per Q buffer: Q tile landed
+  uint64_t* bar_qe = bar_q + QBUF;          // per Q buffer: both consumer warpgroups are done with it
+  uint64_t* bar_k = bar_qe + QBUF;          // per stage: K tile landed
+  uint64_t* bar_v = bar_k + STAGES;         // per stage: V tile landed (bf16)
+  uint64_t* bar_vc = bar_v + STAGES;        // per stage: V tile converted to fp16 (one arrive per converter warp)
+  uint64_t* bar_e = bar_vc + STAGES;        // per stage: both consumer warpgroups are done with K and V
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  int bid = blockIdx.x;
-  const int qt = bid % p.n_qt; bid /= p.n_qt;
-  const int head = bid % p.H;
-  const int seq = bid / p.H;
-  const int q0 = qt * 64;
-  const size_t ld = static_cast<size_t>(3) * p.D;
-  const __nv_bfloat16* base = p.qkv + static_cast<size_t>(seq) * T * ld;
-  const int colq = head * HD, colk = p.D + head * HD, colv = 2 * p.D + head * HD;
-
-  // rows [r0, r0 + nrows) of a [*, ldr] bf16 matrix (columns col0 .. col0 + HD) -> padded smem; rows >= nvalid -> 0
-  auto load_rows = [&](__nv_bfloat16* dst, const __nv_bfloat16* src, size_t ldr, int col0, int r0, int nrows,
-                       int nvalid) {
-    for (int i = tid; i < nrows * CH; i += 128) {
-      const int r = i / CH, c = i - (i / CH) * CH;
-      const bool ok = r0 + r < nvalid;
-      const __nv_bfloat16* g = src + static_cast<size_t>(ok ? r0 + r : 0) * ldr + col0 + c * 8;
-      cp_async16(smem_u32(dst + r * HDP + c * 8), g, ok);
-    }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // Persistent: CTA b runs query tiles b, b + gridDim.x, ...  The query tiles of one (sequence, head) are adjacent
+  // numbers, so CTAs running at the same time share K / V through L2.
+  auto decode = [&](int item, int& q0, int& head, int& seq) {
+    q0 = (item % C::NQT) * BM;
+    item /= C::NQT;
+    head = item % p.H;
+    seq = item / p.H;
   };
-  load_rows(sQ, base, ld, colq, q0, 64, T);
-  load_rows(sK, p.rel_h, HD, 0, 0, C::NTG * 64, C::NREL);
-  load_rows(sV, p.rel_w, HD, 0, 0, C::NTG * 64, C::NREL);
-  cp_async_commit();
-  cp_async_wait<0>();
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tm_q);
+    tma_prefetch_desc(&tm_kv);
+    mbar_init(smem_u32(bar_tab), 1);
+    for (int b = 0; b < QBUF; ++b) {
+      mbar_init(smem_u32(&bar_q[b]), 1);
+      mbar_init(smem_u32(&bar_qe[b]), 8);
+    }
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(smem_u32(&bar_k[s]), 1);
+      mbar_init(smem_u32(&bar_v[s]), 1);
+      mbar_init(smem_u32(&bar_vc[s]), 3);
+      mbar_init(smem_u32(&bar_e[s]), 8);
+    }
+    fence_barrier_init();
+  }
   __syncthreads();
 
-  // this thread's fragment coordinates: rows rl + 8 i (i = 0, 1) of the warp's 16, columns 2 (lane % 4) + {0, 1}
-  const int rl = warp * 16 + (lane >> 2);
-  const int cq = 2 * (lane & 3);
-  uint32_t qf[HD / 16][4];
-#pragma unroll
-  for (int kk = 0; kk < HD / 16; ++kk)
-    ldsm_x4(smem_u32(sQ + (warp * 16 + (lane & 15)) * HDP + kk * 16 + (lane >> 4) * 8), qf[kk][0], qf[kk][1],
-            qf[kk][2], qf[kk][3]);
-  // B operand (x4: two 8-row blocks of K-like [rows][HD] smem at k-step kk)
-  const int b_row = (lane & 7) + ((lane >> 4) << 3), b_col = ((lane >> 3) & 1) * 8;
-
-  // ---- prologue: Q x table^T for both tables, gathered into relh / relw (this warp's 16 rows only)
-#pragma unroll 1
-  for (int tab = 0; tab < 2; ++tab) {
-    const __nv_bfloat16* tb = tab ? sV : sK;
-    float* dst = tab ? relw : relh;
-#pragma unroll 1
-    for (int g = 0; g < C::NTG; ++g) {
-      float acc[8][4];
-#pragma unroll
-      for (int nb = 0; nb < 8; ++nb) acc[nb][0] = acc[nb][1] = acc[nb][2] = acc[nb][3] = 0.f;
-#pragma unroll
-      for (int kk = 0; kk < HD / 16; ++kk) {
-#pragma unroll
-        for (int np = 0; np < 4; ++np) {
-          uint32_t b0, b1, b2, b3;
-          ldsm_x4(smem_u32(tb + (g * 64 + np * 16 + b_row) * HDP + kk * 16 + b_col), b0, b1, b2, b3);
-          mma_bf16(acc[2 * np], qf[kk], b0, b1);
-          mma_bf16(acc[2 * np + 1], qf[kk], b2, b3);
+  if (warp < 4) {
+    setmaxnreg_dec<C::REG_PRODUCER>();
+    if (warp == 0) {
+      if (lane == 0) {
+        // ------------------------------------------------------------ TMA producer
+        const uint32_t bq = smem_u32(bar_tab);   // the tables are the layer's: loaded once
+        mbar_expect_tx(bq, 2 * TILE_TAB);
+        tma_load_2d(sbase + C::TAB_OFF, &tm_rh, bq, 0, 0);
+        tma_load_2d(sbase + C::TAB_OFF + TILE_TAB, &tm_rw, bq, 0, 0);
+        if constexpr (TAIL > 0) {
+          tma_load_2d(sbase + C::TAB_OFF + C::NTAB * 128, &tm_rh_t, bq, 64, 0);
+          tma_load_2d(sbase + C::TAB_OFF + TILE_TAB + C::NTAB * 128, &tm_rw_t, bq, 64, 0);
         }
-      }
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int r = rl + 8 * i;
-        const int tq = q0 + r;
-        const int qc = tab ? tq % S : tq / S;   // query coordinate along the table's axis
-#pragma unroll
-        for (int nb = 0; nb < 8; ++nb) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int t = g * 64 + nb * 8 + cq + e;   // table index t = q - k + S - 1
-            const int k = qc + S - 1 - t;
-            if (t < C::NREL && k >= 0 && k < S) dst[r * SP + k] = acc[nb][2 * i + e] * LOG2E;
+        int g = 0;   // K / V tiles issued so far: ring position
+#pragma unroll 1
+        for (int item = blockIdx.x, it = 0; item < p.n_items; item += gridDim.x, ++it) {
+          int q0, head, seq;
+          decode(item, q0, head, seq);
+          const int colq = head * HD, colk = p.D + colq, colv = 2 * p.D + colq;
+          const int qb = it % QBUF;
+          mbar_wait(smem_u32(&bar_qe[qb]), ((it / QBUF) & 1) ^ 1);
+          mbar_expect_tx(smem_u32(&bar_q[qb]), C::tile_bytes(BM));
+          load_tile<TAIL>(sbase + C::Q_OFF + qb * C::tile_bytes(BM), BM, &tm_q, &tm_q_t, smem_u32(&bar_q[qb]),
+                          colq, q0, seq);
+#pragma unroll 1
+          for (int j = 0; j < NKT; ++j, ++g) {
+            const int s = g % STAGES;
+            mbar_wait(smem_u32(&bar_e[s]), ((g / STAGES) & 1) ^ 1);
+            const uint32_t kb = sbase + C::KV_OFF + s * C::STAGE_BYTES;
+            mbar_expect_tx(smem_u32(&bar_k[s]), TILE_KV);
+            load_tile<TAIL>(kb, BN, &tm_kv, &tm_kv_t, smem_u32(&bar_k[s]), colk, j * BN, seq);
+            mbar_expect_tx(smem_u32(&bar_v[s]), TILE_KV);
+            load_tile<TAIL>(kb + TILE_KV, BN, &tm_kv, &tm_kv_t, smem_u32(&bar_v[s]), colv, j * BN, seq);
           }
         }
       }
-    }
-  }
-  __syncthreads();   // the tables' smem becomes the K / V ring
-
-  auto load_kv = [&](int j) {
-    const int st = j & 1;
-    load_rows(sK + st * 64 * HDP, base, ld, colk, j * 64, 64, T);
-    load_rows(sV + st * 64 * HDP, base, ld, colv, j * 64, 64, T);
-    cp_async_commit();
-  };
-  load_kv(0);
-
-  float o[HD / 8][4];
-#pragma unroll
-  for (int nb = 0; nb < HD / 8; ++nb) o[nb][0] = o[nb][1] = o[nb][2] = o[nb][3] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-  const float scale2 = p.scale2;
-  const float* bh[2] = {relh + rl * SP, relh + (rl + 8) * SP};
-  const float* bw[2] = {relw + rl * SP, relw + (rl + 8) * SP};
-  // V operand (x4 trans: two 8-key halves of a 16-key step, two 8-column blocks)
-  const int v_row = (lane & 7) + ((lane >> 3) & 1) * 8, v_col = (lane >> 4) * 8;
-
-#pragma unroll 1
-  for (int j = 0; j < C::NKT; ++j) {
-    if (j + 1 < C::NKT) {
-      load_kv(j + 1);
-      cp_async_wait<1>();
     } else {
-      cp_async_wait<0>();
-    }
-    __syncthreads();
-    const __nv_bfloat16* Ks = sK + (j & 1) * 64 * HDP;
-    const __nv_bfloat16* Vs = sV + (j & 1) * 64 * HDP;
-    {   // V tile bf16 -> fp16 in place
-      uint32_t* v32 = reinterpret_cast<uint32_t*>(sV + (j & 1) * 64 * HDP);
-      for (int i = tid; i < 64 * HDP / 2; i += 128) {
-        const uint32_t w = v32[i];
-        v32[i] = pack_f16x2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
+      // ------------------------------------------------------------ V converters: bf16 -> fp16 in place
+      const int t = threadIdx.x - 32;
+      const int n_tiles = ((p.n_items - static_cast<int>(blockIdx.x) + gridDim.x - 1) / gridDim.x) * NKT;
+#pragma unroll 1
+      for (int g = 0; g < n_tiles; ++g) {
+        const int s = g % STAGES;
+        mbar_wait(smem_u32(&bar_v[s]), (g / STAGES) & 1);
+        uint4* v = reinterpret_cast<uint4*>(smem + C::KV_OFF + s * C::STAGE_BYTES + TILE_KV);
+#pragma unroll 2
+        for (int i = t; i < static_cast<int>(TILE_KV / 16); i += 96) {
+          uint4 w = v[i];
+          w.x = bf16x2_to_f16x2(w.x);
+          w.y = bf16x2_to_f16x2(w.y);
+          w.z = bf16x2_to_f16x2(w.z);
+          w.w = bf16x2_to_f16x2(w.w);
+          v[i] = w;
+        }
+        fence_proxy_async_smem();   // the generic-proxy writes become visible to wgmma
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&bar_vc[s]));
       }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------- consumers: rows [64 wg, 64 wg + 64) of the tile
+  setmaxnreg_inc<C::REG_CONSUMER>();
+  const int wg = (warp >> 2) - 1;
+  // this thread's fragment coordinates: rows r0 + 8 i (i = 0, 1) of the tile, columns 8 b + cq + {0, 1}
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  constexpr bool REG_W = BN % S == 0;
+  constexpr int CPS = REG_W ? S / 8 : 1;   // 8-column blocks per S keys
+  mbar_wait(smem_u32(bar_tab), 0);
+  int g = 0;   // K / V tiles consumed so far: ring position
+#pragma unroll 1
+  for (int item = blockIdx.x, it = 0; item < p.n_items; item += gridDim.x, ++it) {
+    int q0, head, seq;
+    decode(item, q0, head, seq);
+    const int qb = it % QBUF;
+    const uint32_t qbase = sbase + C::Q_OFF + qb * C::tile_bytes(BM);
+    const uint32_t qa = qbase + wg * 64 * 128;                 // this warpgroup's Q rows, columns 0-63
+    const uint32_t qtail = qbase + BM * 128 + wg * 64 * 32;    // columns 64-79
+
+    // ---- prologue: Q x table^T for both tables, gathered into relh / relw (this warpgroup's 64 rows only)
+    mbar_wait(smem_u32(&bar_q[qb]), (it / QBUF) & 1);
+    named_bar_sync(1 + wg, 128);   // the warpgroup is done reading the previous tile's bias
+#pragma unroll 1
+    for (int tab = 0; tab < 2; ++tab) {
+      float acc[C::NTAB / 2];
+      qk_wgmma<C::NTAB, TAIL>(acc, qa, qtail, sbase + C::TAB_OFF + tab * TILE_TAB, C::NTAB);
+      float* dst = tab ? relw : relh;
+#pragma unroll
+      for (int x = 0; x < C::NTAB / 2; ++x) {
+        const int r = r0 + 8 * ((x >> 1) & 1);
+        const int tq = q0 + r;
+        const int qc = tab ? tq % S : tq / S;          // query coordinate along the table's axis
+        const int t = 8 * (x >> 2) + cq + (x & 1);     // table index t = q - k + S - 1
+        const int k = qc + S - 1 - t;
+        if (t < C::NREL && k >= 0 && k < S) dst[r * SP + k] = acc[x] * LOG2E;
+      }
+    }
+    named_bar_sync(1 + wg, 128);
+
+    // S = 32 / 64: register x of the score fragment is key column kw = 8 ((x / 4) % CPS) + cq + x % 2 of every S-key
+    // block; the thread keeps those rel_w terms of its two rows in registers
+    float rw[2][2 * CPS];
+    if constexpr (REG_W) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int m = 0; m < 2 * CPS; ++m) rw[i][m] = relw[(r0 + 8 * i) * SP + 8 * (m >> 1) + cq + (m & 1)];
     }
 
-    float sc[8][4];
+    float om[32], ot[8];
 #pragma unroll
-    for (int nb = 0; nb < 8; ++nb) sc[nb][0] = sc[nb][1] = sc[nb][2] = sc[nb][3] = 0.f;
+    for (int y = 0; y < 32; ++y) om[y] = 0.f;
 #pragma unroll
-    for (int kk = 0; kk < HD / 16; ++kk) {
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4(smem_u32(Ks + (np * 16 + b_row) * HDP + kk * 16 + b_col), b0, b1, b2, b3);
-        mma_bf16(sc[2 * np], qf[kk], b0, b1);
-        mma_bf16(sc[2 * np + 1], qf[kk], b2, b3);
+    for (int y = 0; y < 8; ++y) ot[y] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    const float scale2 = p.scale2;
+
+#pragma unroll(REG_W ? 1 : NKT)
+    for (int j = 0; j < NKT; ++j, ++g) {
+      const int s = g % STAGES;
+      const uint32_t ph = (g / STAGES) & 1;
+      const uint32_t kb = sbase + C::KV_OFF + s * C::STAGE_BYTES, vb = kb + TILE_KV;
+      mbar_wait(smem_u32(&bar_k[s]), ph);
+      float sc[BN / 2];
+      qk_wgmma<BN, TAIL>(sc, qa, qtail, kb, BN);
+      if (j == NKT - 1) {   // the last Q K^T of this query tile has retired: its Q buffer may be refilled
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&bar_qe[qb]));
       }
-    }
-    // scores in the log2 domain with the bias; keys past T (last window tile) drop out
-    float mx[2] = {-INFINITY, -INFINITY};
+
+      // scores in the log2 domain with the bias; keys past T (last window tile) drop out
+      float mx[2] = {-INFINITY, -INFINITY};
+      if constexpr (REG_W) {
+        constexpr int NB = BN / S;   // S-key blocks per tile: one rel_h value per row and block
+        float bh[2][NB];
 #pragma unroll
-    for (int nb = 0; nb < 8; ++nb) {
+        for (int i = 0; i < 2; ++i)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = j * 64 + nb * 8 + cq + (e & 1);
-        const int i = e >> 1;
-        float t = -INFINITY;
-        if (T % 64 == 0 || key < T) {
-          const int kh = key / S, kw = key - kh * S;
-          t = fmaf(sc[nb][e], scale2, bh[i][kh] + bw[i][kw]);
+          for (int b = 0; b < NB; ++b) bh[i][b] = relh[(r0 + 8 * i) * SP + j * NB + b];
+#pragma unroll
+        for (int x = 0; x < BN / 2; ++x) {
+          const int i = (x >> 1) & 1;
+          const float t = fmaf(sc[x], scale2, bh[i][(x >> 2) / CPS] + rw[i][((x >> 2) % CPS) * 2 + (x & 1)]);
+          sc[x] = t;
+          mx[i] = fmaxf(mx[i], t);
         }
-        sc[nb][e] = t;
-        mx[i] = fmaxf(mx[i], t);
+      } else {
+#pragma unroll
+        for (int x = 0; x < BN / 2; ++x) {
+          const int i = (x >> 1) & 1;
+          const int key = j * BN + 8 * (x >> 2) + cq + (x & 1);
+          float t = -INFINITY;
+          if (T % BN == 0 || key < T) {
+            const int kh = key / S, kw = key - kh * S;
+            const int r = r0 + 8 * i;
+            t = fmaf(sc[x], scale2, relh[r * SP + kh] + relw[r * SP + kw]);
+          }
+          sc[x] = t;
+          mx[i] = fmaxf(mx[i], t);
+        }
       }
+      float alpha[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+        mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+        const float m_new = fmaxf(m_run[i], mx[i]);
+        alpha[i] = fast_exp2(m_run[i] - m_new);
+        m_run[i] = m_new;
+        l_run[i] *= alpha[i];
+      }
+#pragma unroll
+      for (int y = 0; y < 32; ++y) om[y] *= alpha[(y >> 1) & 1];
+#pragma unroll
+      for (int y = 0; y < 8; ++y) ot[y] *= alpha[(y >> 1) & 1];
+      // P = exp2(t - m) -> fp16 A fragments of P V: k16 step kk holds score registers 8 kk .. 8 kk + 7
+      uint32_t pa[BN / 16][4];
+#pragma unroll
+      for (int kk = 0; kk < BN / 16; ++kk) {
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+          const int x = 8 * kk + 2 * h, i = h & 1;
+          const float p0 = fast_exp2(sc[x] - m_run[i]), p1 = fast_exp2(sc[x + 1] - m_run[i]);
+          l_run[i] += p0 + p1;
+          pa[kk][h] = pack_f16x2(p0, p1);
+        }
+      }
+      mbar_wait(smem_u32(&bar_vc[s]), ph);
+      acc_fence(om);
+      acc_fence(ot);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BN / 16; ++kk) {
+        WgmmaRsF16<64>::rs(om, pa[kk], make_gdesc(vb + kk * 2048, BN * 128, 1024));
+        if constexpr (TAIL > 0) WgmmaRsF16<16>::rs(ot, pa[kk], make_gdesc_sw32(vb + BN * 128 + kk * 512, 256, 256));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(om);
+      acc_fence(ot);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&bar_e[s]));
     }
-    float alpha[2];
+
+    // ---- epilogue: O / l -> out[token, head*HD .. ]
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
-      const float m_new = fmaxf(m_run[i], mx[i]);
-      alpha[i] = fast_exp2(m_run[i] - m_new);
-      m_run[i] = m_new;
-      l_run[i] *= alpha[i];
-    }
+      float l = l_run[i];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      const float inv = 1.0f / l;
+      const int tq = q0 + r0 + 8 * i;
+      if (tq >= T) continue;
+      int dst = seq * T + tq;
+      if (p.out_row_map) dst = __ldg(p.out_row_map + dst);
+      if (dst < 0) continue;
+      __nv_bfloat16* orow = p.out + static_cast<size_t>(dst) * p.D + head * HD + cq;
 #pragma unroll
-    for (int nb = 0; nb < HD / 8; ++nb) {
-      o[nb][0] *= alpha[0]; o[nb][1] *= alpha[0];
-      o[nb][2] *= alpha[1]; o[nb][3] *= alpha[1];
-    }
-    // P = exp2(t - m) -> fp16 A fragments of P V
-    uint32_t pa[4][4];
+      for (int nb = 0; nb < 8; ++nb)
+        *reinterpret_cast<uint32_t*>(orow + nb * 8) = pack_bf16x2(om[4 * nb + 2 * i] * inv, om[4 * nb + 2 * i + 1] * inv);
+      if constexpr (TAIL > 0) {
 #pragma unroll
-    for (int nb = 0; nb < 8; ++nb) {
-      const float p0 = fast_exp2(sc[nb][0] - m_run[0]), p1 = fast_exp2(sc[nb][1] - m_run[0]);
-      const float p2 = fast_exp2(sc[nb][2] - m_run[1]), p3 = fast_exp2(sc[nb][3] - m_run[1]);
-      l_run[0] += p0 + p1;
-      l_run[1] += p2 + p3;
-      pa[nb >> 1][(nb & 1) * 2 + 0] = pack_f16x2(p0, p1);
-      pa[nb >> 1][(nb & 1) * 2 + 1] = pack_f16x2(p2, p3);
-    }
-    __syncthreads();   // the whole V tile is fp16
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-      for (int np = 0; np < HD / 16; ++np) {
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4_t(smem_u32(Vs + (kk * 16 + v_row) * HDP + np * 16 + v_col), b0, b1, b2, b3);
-        mma_f16(o[2 * np], pa[kk], b0, b1);
-        mma_f16(o[2 * np + 1], pa[kk], b2, b3);
+        for (int nb = 0; nb < 2; ++nb)
+          *reinterpret_cast<uint32_t*>(orow + 64 + nb * 8) =
+              pack_bf16x2(ot[4 * nb + 2 * i] * inv, ot[4 * nb + 2 * i + 1] * inv);
       }
     }
-    __syncthreads();   // this stage may be refilled by the next iteration's load
-  }
-
-  // ---- epilogue: O / l -> out[token, head*HD .. ]
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    float l = l_run[i];
-    l += __shfl_xor_sync(0xffffffffu, l, 1);
-    l += __shfl_xor_sync(0xffffffffu, l, 2);
-    const float inv = 1.0f / l;
-    const int tq = q0 + rl + 8 * i;
-    if (tq >= T) continue;
-    int dst = seq * T + tq;
-    if (p.out_row_map) dst = __ldg(p.out_row_map + dst);
-    if (dst < 0) continue;
-    __nv_bfloat16* orow = p.out + static_cast<size_t>(dst) * p.D + colq + cq;
-#pragma unroll
-    for (int nb = 0; nb < HD / 8; ++nb)
-      *reinterpret_cast<uint32_t*>(orow + nb * 8) = pack_bf16x2(o[nb][2 * i] * inv, o[nb][2 * i + 1] * inv);
   }
 }
 
 template <int HD, int S>
 static int launch_att(const AttentionArgs& a, cudaStream_t stream) {
   using C = AttCfg<HD, S>;
-  AttDev p;
-  p.qkv = static_cast<const __nv_bfloat16*>(a.qkv);
-  p.rel_h = static_cast<const __nv_bfloat16*>(a.rel_h);
-  p.rel_w = static_cast<const __nv_bfloat16*>(a.rel_w);
-  p.out = static_cast<__nv_bfloat16*>(a.out);
-  p.H = a.H; p.D = a.H * HD;
-  p.n_qt = (C::T + 63) / 64;
-  p.scale2 = (1.0f / sqrtf(static_cast<float>(HD))) * LOG2E;
-  p.out_row_map = a.out_row_map;
   RSP_CHECK_ARG((reinterpret_cast<uintptr_t>(a.qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.rel_h) & 15) == 0 &&
                 (reinterpret_cast<uintptr_t>(a.rel_w) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.out) & 3) == 0,
                 "attention: qkv / tables must be 16-byte aligned");
+  AttDev p;
+  p.out = static_cast<__nv_bfloat16*>(a.out);
+  p.out_row_map = a.out_row_map;
+  p.H = a.H; p.D = a.H * HD;
+  p.scale2 = (1.0f / sqrtf(static_cast<float>(HD))) * LOG2E;
+  // qkv as (column, token, sequence): a box never reads past its sequence (rows >= T of the last tile are zero)
+  const uint64_t ld = 3ull * p.D;
+  const uint64_t qdims[3] = {ld, static_cast<uint64_t>(C::T), static_cast<uint64_t>(a.n_seq)};
+  const uint64_t qstr[2] = {ld * 2, ld * 2 * C::T};
+  const uint64_t tdims[2] = {static_cast<uint64_t>(HD), static_cast<uint64_t>(C::NREL)};
+  const uint64_t tstr[1] = {static_cast<uint64_t>(HD) * 2};
+  // boxes: Q tiles of BM rows, K / V tiles of BN rows (the box is what each load's transaction bytes count)
+  const uint32_t qbox[3] = {64, C::BM, 1}, qbox_t[3] = {16, C::BM, 1};
+  const uint32_t kvbox[3] = {64, C::BN, 1}, kvbox_t[3] = {16, C::BN, 1};
+  const uint32_t tbox[2] = {64, static_cast<uint32_t>(C::NTAB)}, tbox_t[2] = {16, static_cast<uint32_t>(C::NTAB)};
+  CUtensorMap tq, tkv, th, tw, tq_t, tkv_t, th_t, tw_t;
+  RSP_TRY(make_tmap_swizzled(&tq, a.qkv, 3, qdims, qstr, qbox, 0, 128));
+  RSP_TRY(make_tmap_swizzled(&tkv, a.qkv, 3, qdims, qstr, kvbox, 0, 128));
+  RSP_TRY(make_tmap_swizzled(&th, a.rel_h, 2, tdims, tstr, tbox, 0, 128));
+  RSP_TRY(make_tmap_swizzled(&tw, a.rel_w, 2, tdims, tstr, tbox, 0, 128));
+  if (C::TAIL > 0) {
+    RSP_TRY(make_tmap_swizzled(&tq_t, a.qkv, 3, qdims, qstr, qbox_t, 0, 32));
+    RSP_TRY(make_tmap_swizzled(&tkv_t, a.qkv, 3, qdims, qstr, kvbox_t, 0, 32));
+    RSP_TRY(make_tmap_swizzled(&th_t, a.rel_h, 2, tdims, tstr, tbox_t, 0, 32));
+    RSP_TRY(make_tmap_swizzled(&tw_t, a.rel_w, 2, tdims, tstr, tbox_t, 0, 32));
+  } else {   // hd = 64 has no tail; the kernel never reads these
+    tq_t = tq; tkv_t = tkv; th_t = th; tw_t = tw;
+  }
   auto kern = vit_attention_kernel<HD, S>;
   static bool attr_set_dev[kMaxDevices] = {};   // the attribute is per device (one flag per ordinal)
   bool& attr_set = attr_set_dev[current_device()];
@@ -326,9 +435,11 @@ static int launch_att(const AttentionArgs& a, cudaStream_t stream) {
     RSP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr_set = true;
   }
-  const long long grid = static_cast<long long>(a.n_seq) * a.H * p.n_qt;
-  RSP_CHECK_ARG(grid > 0 && grid < (1ll << 31), "attention: grid %lld", grid);
-  kern<<<static_cast<unsigned>(grid), 128, C::SMEM_BYTES, stream>>>(p);
+  const long long items = static_cast<long long>(a.n_seq) * a.H * C::NQT;
+  RSP_CHECK_ARG(items > 0 && items < (1ll << 31), "attention: %lld query tiles", items);
+  p.n_items = static_cast<int>(items);
+  const int grid = static_cast<int>(items < num_sms() ? items : num_sms());   // one CTA per SM
+  kern<<<grid, 384, C::SMEM_BYTES, stream>>>(tq, tq_t, tkv, tkv_t, th, th_t, tw, tw_t, p);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
 }

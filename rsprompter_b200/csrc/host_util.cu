@@ -41,6 +41,11 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 
 int make_tmap(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
               const uint32_t* box, int is_f32) {
+  return make_tmap_swizzled(out, base, rank, dims, strides_bytes, box, is_f32, 128);
+}
+
+int make_tmap_swizzled(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                       const uint64_t* strides_bytes, const uint32_t* box, int is_f32, int swizzle_bytes) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
     set_last_error("cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
@@ -63,9 +68,14 @@ int make_tmap(CUtensorMap* out, const void* base, int rank, const uint64_t* dims
     RSP_CHECK_ARG((strides_bytes[i] & 15) == 0, "tensor map stride[%d]=%llu not 16B multiple", i,
                   (unsigned long long)strides_bytes[i]);
   }
-  RSP_CHECK_ARG(box[0] * (is_f32 ? 4 : 2) <= 128, "swizzle-128B inner box must be <= 128 bytes");
+  RSP_CHECK_ARG(swizzle_bytes == 32 || swizzle_bytes == 64 || swizzle_bytes == 128, "swizzle %d", swizzle_bytes);
+  RSP_CHECK_ARG(box[0] * (is_f32 ? 4 : 2) <= static_cast<uint32_t>(swizzle_bytes),
+                "swizzle-%dB inner box must be <= %d bytes", swizzle_bytes, swizzle_bytes);
+  const CUtensorMapSwizzle sw = swizzle_bytes == 128  ? CU_TENSOR_MAP_SWIZZLE_128B
+                                : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                      : CU_TENSOR_MAP_SWIZZLE_32B;
   CUresult r = fn(out, is_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base),
-                  gdim, gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  gdim, gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled failed: CUresult %d (rank %d dims %llu,%llu box %u,%u)",

@@ -52,6 +52,9 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 // same for bf16 (is_f32 = 0) or fp32 elements; also used for TMA stores (out-of-range box parts are clipped)
 int make_tmap(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
               const uint32_t* box, int is_f32);
+// same with a 32-, 64- or 128-byte swizzle (the inner box must fit in one swizzle span)
+int make_tmap_swizzled(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                       const uint64_t* strides_bytes, const uint32_t* box, int is_f32, int swizzle_bytes);
 
 inline int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                              uint64_t row_stride_bytes, uint32_t box_rows, uint32_t box_cols) {

@@ -1,4 +1,4 @@
-// Native self-test of the tensor-core ViT attention kernel against the SIMT restatement.
+// Native self-test of the wgmma ViT attention kernel against the SIMT restatement.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -128,6 +128,8 @@ int selftest_attention(int bench) {
   fails += attn_case("glob-hd64", 1, 64, 2, 64, 2.0f, 1.0f, 0);
   fails += attn_case("glob-hd80", 1, 64, 2, 80, 2.0f, 1.0f, 0);
   fails += attn_case("glob-hd64-sharp", 2, 64, 3, 64, 6.0f, 3.0f, 0);
+  fails += attn_case("glob32-hd80", 3, 32, 2, 80, 2.0f, 1.0f, 0);
+  fails += attn_case("win-hd80-sharp", 7, 14, 3, 80, 6.0f, 3.0f, 0);
   if (bench) {
     attn_case("vitb-window", 200, 14, 12, 64, 2.0f, 1.0f, 1);
     attn_case("vitb-global", 8, 64, 12, 64, 2.0f, 1.0f, 1);

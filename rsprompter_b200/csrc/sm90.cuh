@@ -137,6 +137,19 @@ __device__ __forceinline__ uint64_t make_gdesc(uint32_t saddr, uint32_t lbo_byte
   return d;
 }
 
+// Same with a 32-byte swizzle (layout type 3): one "row" = 32 bytes (16 elements), eight rows = one 256-byte atom,
+// the 16-byte chunk index of a row is XOR-ed with (row >> 2) & 1 (what TMA writes with CU_TENSOR_MAP_SWIZZLE_32B).
+//   K-major:  SBO = 256 (distance between 8-row groups); one k16 step covers the whole row.
+//   MN-major: SBO = 256 (distance between 8-row groups along K); LBO = distance between 16-wide atoms along M/N.
+__device__ __forceinline__ uint64_t make_gdesc_sw32(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((saddr & 0x3ffff) >> 4);
+  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fff) << 16;
+  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fff) << 32;
+  d |= 3ull << 62;
+  return d;
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -244,6 +257,40 @@ template <> struct Wgmma<256> {
           "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
           "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
         : "l"(a), "l"(b), "r"(acc), "n"(TB));
+  }
+};
+
+// D[64 x N] += A[64 x 16] * B[16 x N], fp16 in, fp32 accumulators; A from registers (four f16x2 per thread, the
+// m16n8k16 A-fragment layout per warp: rows 16 (t / 32) + (t % 32) / 4 (+ 8 for a1 / a3), columns 2 (t % 4) (+ 8 for
+// a2 / a3)), B MN-major from shared memory.
+template <int N>
+struct WgmmaRsF16;
+template <> struct WgmmaRsF16<16> {
+  __device__ __forceinline__ static void rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\n"
+        "setp.ne.b32 p, 1, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+  }
+};
+template <> struct WgmmaRsF16<64> {
+  __device__ __forceinline__ static void rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\n"
+        "setp.ne.b32 p, 1, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
   }
 };
 
