@@ -366,6 +366,16 @@ int rsp_mask_rle_lengths(const uint8_t* src, int packed, const int64_t* desc, co
                          int64_t* offsets, void* stream);
 int rsp_mask_rle_write(const uint8_t* src, int packed, const int64_t* desc, int n, const int64_t* offsets, char* pool,
                        int32_t* lengths, void* stream);
+/* ... of masks placed in larger canvases (a tile's mask in scene coordinates, sahi shift_masks followed by the encode:
+ * mmdet/utils/large_image.py:27-73).  desc int64 [n, 9] = (byte offset of the source mask from src, source row bytes,
+ * source rows, visible h, w, canvas H, W, origin y0, x0): the string of the H x W canvas that is zero except
+ * canvas[y0 + y, x0 + x] = mask[y, x] for y < h, x < w, without that canvas ever existing (the work is proportional to
+ * h x w).  RSP_ERR_INVALID, nothing launched, unless 1 <= H*W <= 2^31 - 1, 0 <= y0 < H, 0 <= x0 < W, 1 <= h <= H - y0,
+ * 1 <= w <= W - x0, h <= source rows and w <= source row bytes (x 8 when packed).  Pool, offsets and lengths as above. */
+int rsp_mask_rle_placed_lengths(const uint8_t* src, int packed, const int64_t* desc, const int64_t* desc_host, int n,
+                                int64_t* offsets, void* stream);
+int rsp_mask_rle_placed_write(const uint8_t* src, int packed, const int64_t* desc, int n, const int64_t* offsets,
+                              char* pool, int32_t* lengths, void* stream);
 
 /* ---- DetDataPreprocessor on the device (SURVEY 8(f2); data_preprocessor.py:110-148, ImgDataPreprocessor.forward,
  * BatchFixedSizePad :300).  mean3 / std3: HOST arrays of 3 floats in OUTPUT channel order. ---- */

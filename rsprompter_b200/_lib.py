@@ -106,6 +106,8 @@ _SIGNATURES = {
     "rsp_patchify16_u8": ([_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp], _i),
     "rsp_mask_rle_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp], _i),
     "rsp_mask_rle_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
+    "rsp_mask_rle_placed_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp], _i),
+    "rsp_mask_rle_placed_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
 }
 
 
@@ -1117,18 +1119,48 @@ def mask_rle(groups: list, packed: bool) -> list:
         assert ld == ((W + 7) // 8 if packed else W), "row length does not match W"
         off = t.data_ptr() - base
         rows += [(off + j * H * ld, H, W) for j in range(n)]
+    return _rle_strings(base, packed, rows, groups[0][0].device, placed=False)
+
+
+def mask_rle_placed(groups: list, packed: bool) -> list:
+    """pycocotools compressed RLE strings (bytes, in order) of canvases that hold one mask each, the canvas itself never
+    formed.  ``groups`` = [(src, placements)], src a contiguous CUDA tensor (bool / uint8 pixels, or bit-packed rows
+    with packed=True) and placements = [(byte offset in src, row bytes, rows, h, w, H, W, y0, x0)]: the H x W canvas is
+    zero but for canvas[y0:y0 + h, x0:x0 + w] = mask[:h, :w], the mask's rows of ``row bytes`` starting at that offset.
+    The work is proportional to h x w; host syncs and copies as mask_rle."""
+    groups = [(t, list(pl)) for t, pl in groups if len(pl) > 0]
+    if not groups:
+        return []
+    _require_cuda(*[t for t, _ in groups])
+    base = min(t.data_ptr() for t, _ in groups)
+    rows = []
+    for t, pl in groups:
+        assert t.is_contiguous() and t.dtype in (torch.bool, torch.uint8)
+        shift = t.data_ptr() - base
+        for p in pl:
+            off, ld, nrows, h, w, H, W, y0, x0 = (int(v) for v in p)
+            # the kernel reads rows [0, h) of the mask, from its offset on
+            assert 0 <= off and off + (h - 1) * ld + ((w + 7) // 8 if packed else w) <= t.numel(), "mask outside src"
+            rows.append((off + shift, ld, nrows, h, w, H, W, y0, x0))
+    return _rle_strings(base, packed, rows, groups[0][0].device, placed=True)
+
+
+def _rle_strings(base: int, packed: bool, rows: list, dev, placed: bool) -> list:
+    """The length pass + offset scan, one device->host read of the total, the write pass, one copy of the chars."""
+    global launch_count
     n = len(rows)
-    dev = groups[0][0].device
+    lengths_fn, write_fn = ((_lib.rsp_mask_rle_placed_lengths, _lib.rsp_mask_rle_placed_write) if placed else
+                            (_lib.rsp_mask_rle_lengths, _lib.rsp_mask_rle_write))
+    what = "rsp_mask_rle_placed" if placed else "rsp_mask_rle"
     desc_host = torch.tensor(rows, dtype=torch.int64).pin_memory()
     desc = desc_host.to(dev, non_blocking=True)
     offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
-    _check(_lib.rsp_mask_rle_lengths(base, int(packed), _ptr(desc), _ptr(desc_host), n, _ptr(offsets), _stream()),
-           "rsp_mask_rle_lengths")
+    _check(lengths_fn(base, int(packed), _ptr(desc), _ptr(desc_host), n, _ptr(offsets), _stream()), what + "_lengths")
     total = int(offsets[n].item())                       # host sync 1: the exact pool size
     pool = torch.empty(total, dtype=torch.uint8, device=dev)
     lengths = torch.empty(n, dtype=torch.int32, device=dev)
-    _check(_lib.rsp_mask_rle_write(base, int(packed), _ptr(desc), n, _ptr(offsets), _ptr(pool), _ptr(lengths),
-                                   _stream()), "rsp_mask_rle_write")
+    _check(write_fn(base, int(packed), _ptr(desc), n, _ptr(offsets), _ptr(pool), _ptr(lengths), _stream()),
+           what + "_write")
     launch_count += 3
     host_pool = torch.empty(total, dtype=torch.uint8, pin_memory=True)
     host_len = torch.empty(n, dtype=torch.int32, pin_memory=True)
@@ -1137,7 +1169,7 @@ def mask_rle(groups: list, packed: bool) -> list:
     torch.cuda.current_stream().synchronize()            # host sync 2: chars + lengths
     lens = host_len.tolist()
     if min(lens) < 0:
-        raise RspError("rsp_mask_rle_write: a mask's RLE string is longer than 2^31 - 1 chars")
+        raise RspError(what + "_write: a mask's RLE string is longer than 2^31 - 1 chars")
     buf = host_pool.numpy().tobytes()
     out, p = [], 0
     for ln in lens:

@@ -377,4 +377,17 @@ int rsp_mask_rle_write(const uint8_t* src, int packed, const int64_t* desc, int 
                         reinterpret_cast<const long long*>(offsets), pool, lengths, S(stream));
 }
 
+int rsp_mask_rle_placed_lengths(const uint8_t* src, int packed, const int64_t* desc, const int64_t* desc_host, int n,
+                                int64_t* offsets, void* stream) {
+  return mask_rle_placed_lengths(src, packed, reinterpret_cast<const long long*>(desc),
+                                 reinterpret_cast<const long long*>(desc_host), n, reinterpret_cast<long long*>(offsets),
+                                 S(stream));
+}
+
+int rsp_mask_rle_placed_write(const uint8_t* src, int packed, const int64_t* desc, int n, const int64_t* offsets,
+                              char* pool, int32_t* lengths, void* stream) {
+  return mask_rle_placed_write(src, packed, reinterpret_cast<const long long*>(desc), n,
+                               reinterpret_cast<const long long*>(offsets), pool, lengths, S(stream));
+}
+
 }  // extern "C"

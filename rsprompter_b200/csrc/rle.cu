@@ -93,7 +93,7 @@ __device__ __forceinline__ char* rle_put(char* dst, const char* end, int v) {
 template <bool kPacked>
 struct MaskView {
   const unsigned char* m;
-  int H, W, ld;   // ld = bytes per row
+  int ld;   // bytes per source row
   __device__ __forceinline__ unsigned at(int y, int x) const {
     const unsigned char* row = m + static_cast<long long>(y) * ld;
     if (kPacked) return (__ldg(row + (x >> 3)) >> (x & 7)) & 1u;
@@ -101,13 +101,28 @@ struct MaskView {
   }
 };
 
-// f(flat position) for every boundary inside column x, top to bottom; 16 rows are loaded before any is examined
-template <bool kPacked, typename F>
-__device__ __forceinline__ void for_each_boundary(const MaskView<kPacked>& mv, int x, F&& f) {
-  unsigned prev = x > 0 ? mv.at(mv.H - 1, x - 1) : 0u;
-  const int base = x * mv.H;
-  for (int y0 = 0; y0 < mv.H; y0 += 16) {
-    const int rows = min(16, mv.H - y0);
+// Where the h x w source mask lies in the H x W canvas whose runs are encoded: canvas[y0 + y, x0 + x] = mask[y, x],
+// zero elsewhere.  The plain mode is h = H, w = W at the origin.  Only the w source columns are walked; the zero
+// rows and columns around them enter through the boundary positions alone.
+struct Placement {
+  int h, w;     // visible extent
+  int H, W;     // canvas
+  int y0, x0;   // origin
+};
+
+// f(canvas flat position) for every boundary inside source column x, top to bottom; 16 rows are loaded before any
+// is examined.  With the mask spanning the canvas height (y0 = 0, h = H) runs cross columns: the pixel before row 0
+// is the previous source column's last one, and a run reaching the bottom ends in the next column's walk.
+// Otherwise the pixels above and below the mask are zero: a run that reaches the mask's last row ends one past it
+// (unless that is the end of the canvas, where the final count closes it).  A plain mask spans its canvas, so that
+// last boundary exists only for placed ones.
+template <bool kPlaced, bool kPacked, typename F>
+__device__ __forceinline__ void for_each_boundary(const MaskView<kPacked>& mv, const Placement& pl, int x, F&& f) {
+  const bool full_height = pl.y0 == 0 && pl.h == pl.H;
+  unsigned prev = full_height && x > 0 ? mv.at(pl.h - 1, x - 1) : 0u;
+  const int base = (pl.x0 + x) * pl.H + pl.y0;
+  for (int y0 = 0; y0 < pl.h; y0 += 16) {
+    const int rows = min(16, pl.h - y0);
     unsigned w = 0u;
     if (rows == 16) {
 #pragma unroll
@@ -123,10 +138,30 @@ __device__ __forceinline__ void for_each_boundary(const MaskView<kPacked>& mv, i
       f(base + y0 + k);
     }
   }
+  const int end = base + pl.h;   // canvas position after the mask's last row in this column
+  if (kPlaced && prev && !(full_height && x + 1 < pl.w) && end < pl.H * pl.W) f(end);
+}
+
+// Descriptor of mask i: plain (kPlaced = false) int64 [3] = (byte offset, H, W), the canvas is the mask; placed
+// int64 [9] = (byte offset, source row bytes, source rows, h, w, H, W, y0, x0).
+template <bool kPacked, bool kPlaced>
+__device__ __forceinline__ void load_desc(const long long* desc, int i, MaskView<kPacked>& mv, Placement& pl,
+                                          const unsigned char* src) {
+  if (kPlaced) {
+    const long long* d = desc + 9 * i;
+    mv = MaskView<kPacked>{src + d[0], static_cast<int>(d[1])};
+    pl = Placement{static_cast<int>(d[3]), static_cast<int>(d[4]), static_cast<int>(d[5]), static_cast<int>(d[6]),
+                   static_cast<int>(d[7]), static_cast<int>(d[8])};
+  } else {
+    const long long* d = desc + 3 * i;
+    const int H = static_cast<int>(d[1]), W = static_cast<int>(d[2]);
+    mv = MaskView<kPacked>{src + d[0], kPacked ? (W + 7) / 8 : W};
+    pl = Placement{H, W, H, W, 0, 0};
+  }
 }
 
 // kWrite = false: offsets[i + 1] = chars of mask i.  kWrite = true: the chars into pool[offsets[i], offsets[i+1]).
-template <bool kPacked, bool kWrite>
+template <bool kPacked, bool kWrite, bool kPlaced>
 __global__ void __launch_bounds__(kThreads) mask_rle_kernel(const unsigned char* __restrict__ src,
                                                             const long long* __restrict__ desc, long long* offsets,
                                                             char* __restrict__ pool, int* __restrict__ lengths) {
@@ -137,8 +172,9 @@ __global__ void __launch_bounds__(kThreads) mask_rle_kernel(const unsigned char*
     typename SumScan::TempStorage sum;
   } tmp;
   const int i = blockIdx.x;
-  const int H = static_cast<int>(desc[3 * i + 1]), W = static_cast<int>(desc[3 * i + 2]);
-  const MaskView<kPacked> mv{src + desc[3 * i], H, W, kPacked ? (W + 7) / 8 : W};
+  MaskView<kPacked> mv;
+  Placement pl;
+  load_desc<kPacked, kPlaced>(desc, i, mv, pl, src);
   char* out = nullptr;
   const char* end = nullptr;
   if (kWrite) {
@@ -147,13 +183,13 @@ __global__ void __launch_bounds__(kThreads) mask_rle_kernel(const unsigned char*
   }
   RleCtx carry{1u, {0, 0, 0}};   // P[0] = 0
   long long chars = 0;           // chars of the tiles before this one
-  for (int x0 = 0; x0 < W; x0 += kThreads) {
+  for (int x0 = 0; x0 < pl.w; x0 += kThreads) {
     const int x = x0 + threadIdx.x;
     RleCtx local{0u, {0, 0, 0}};
     int first[3] = {0, 0, 0};
     long long len = 0;
-    if (x < W) {
-      for_each_boundary(mv, x, [&](int pos) {
+    if (x < pl.w) {
+      for_each_boundary<kPlaced>(mv, pl, x, [&](int pos) {
         if (local.n >= 3) len += rle_chars((pos - local.p[2]) - (local.p[1] - local.p[0]));
         else if (local.n == 0) first[0] = pos;
         else if (local.n == 1) first[1] = pos;
@@ -175,10 +211,10 @@ __global__ void __launch_bounds__(kThreads) mask_rle_kernel(const unsigned char*
     __syncthreads();   // tmp is reused
     long long off, tile_chars;
     SumScan(tmp.sum).ExclusiveSum(len, off, tile_chars);
-    if (kWrite && x < W) {
+    if (kWrite && x < pl.w) {
       char* dst = out + chars + off;
       c = pre;
-      for_each_boundary(mv, x, [&](int pos) {
+      for_each_boundary<kPlaced>(mv, pl, x, [&](int pos) {
         dst = rle_put(dst, end, rle_value(c, pos));
         rle_push(c, pos);
       });
@@ -188,7 +224,7 @@ __global__ void __launch_bounds__(kThreads) mask_rle_kernel(const unsigned char*
     __syncthreads();
   }
   if (threadIdx.x == 0) {   // the last count ends at H*W
-    const int v = rle_value(carry, H * W);
+    const int v = rle_value(carry, pl.H * pl.W);
     if (kWrite) {
       rle_put(out + chars, end, v);
       const long long len = offsets[i + 1] - offsets[i];
@@ -217,6 +253,31 @@ __global__ void __launch_bounds__(kScanThreads) rle_offsets_kernel(long long* of
 
 }  // namespace
 
+namespace {
+
+template <bool kPlaced>
+int rle_lengths(const unsigned char* src, int packed, const long long* desc, int n, long long* offsets,
+                cudaStream_t stream) {
+  if (packed) mask_rle_kernel<true, false, kPlaced><<<n, kThreads, 0, stream>>>(src, desc, offsets, nullptr, nullptr);
+  else mask_rle_kernel<false, false, kPlaced><<<n, kThreads, 0, stream>>>(src, desc, offsets, nullptr, nullptr);
+  RSP_CHECK_LAUNCH();
+  rle_offsets_kernel<<<1, kScanThreads, 0, stream>>>(offsets, n);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
+template <bool kPlaced>
+int rle_write(const unsigned char* src, int packed, const long long* desc, int n, const long long* offsets, char* pool,
+              int* lengths, cudaStream_t stream) {
+  long long* offs = const_cast<long long*>(offsets);   // only the length pass writes them
+  if (packed) mask_rle_kernel<true, true, kPlaced><<<n, kThreads, 0, stream>>>(src, desc, offs, pool, lengths);
+  else mask_rle_kernel<false, true, kPlaced><<<n, kThreads, 0, stream>>>(src, desc, offs, pool, lengths);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
+}  // namespace
+
 int mask_rle_lengths(const unsigned char* src, int packed, const long long* desc, const long long* desc_host, int n,
                      long long* offsets, cudaStream_t stream) {
   RSP_CHECK_ARG(src && desc && desc_host && offsets && n > 0 && (packed == 0 || packed == 1), "mask_rle_lengths: bad args");
@@ -225,23 +286,42 @@ int mask_rle_lengths(const unsigned char* src, int packed, const long long* desc
     RSP_CHECK_ARG(off >= 0 && H >= 1 && W >= 1 && H <= INT_MAX && W <= INT_MAX && H * W <= INT_MAX,
                   "mask_rle_lengths: mask %d is %lld x %lld at offset %lld (1 .. 2^31 - 1 pixels)", i, H, W, off);
   }
-  if (packed) mask_rle_kernel<true, false><<<n, kThreads, 0, stream>>>(src, desc, offsets, nullptr, nullptr);
-  else mask_rle_kernel<false, false><<<n, kThreads, 0, stream>>>(src, desc, offsets, nullptr, nullptr);
-  RSP_CHECK_LAUNCH();
-  rle_offsets_kernel<<<1, kScanThreads, 0, stream>>>(offsets, n);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
+  return rle_lengths<false>(src, packed, desc, n, offsets, stream);
 }
 
 int mask_rle_write(const unsigned char* src, int packed, const long long* desc, int n, const long long* offsets,
                    char* pool, int* lengths, cudaStream_t stream) {
   RSP_CHECK_ARG(src && desc && offsets && pool && lengths && n > 0 && (packed == 0 || packed == 1),
                 "mask_rle_write: bad args");
-  long long* offs = const_cast<long long*>(offsets);   // only the length pass writes them
-  if (packed) mask_rle_kernel<true, true><<<n, kThreads, 0, stream>>>(src, desc, offs, pool, lengths);
-  else mask_rle_kernel<false, true><<<n, kThreads, 0, stream>>>(src, desc, offs, pool, lengths);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
+  return rle_write<false>(src, packed, desc, n, offsets, pool, lengths, stream);
+}
+
+int mask_rle_placed_lengths(const unsigned char* src, int packed, const long long* desc, const long long* desc_host,
+                            int n, long long* offsets, cudaStream_t stream) {
+  RSP_CHECK_ARG(src && desc && desc_host && offsets && n > 0 && (packed == 0 || packed == 1),
+                "mask_rle_placed_lengths: bad args");
+  for (int i = 0; i < n; ++i) {
+    const long long* d = desc_host + 9 * i;
+    const long long off = d[0], ld = d[1], rows = d[2], h = d[3], w = d[4], H = d[5], W = d[6], y0 = d[7], x0 = d[8];
+    RSP_CHECK_ARG(H >= 1 && W >= 1 && H <= INT_MAX && W <= INT_MAX && H * W <= INT_MAX,
+                  "mask_rle_placed_lengths: mask %d: canvas %lld x %lld (1 .. 2^31 - 1 pixels)", i, H, W);
+    RSP_CHECK_ARG(y0 >= 0 && x0 >= 0 && y0 < H && x0 < W,
+                  "mask_rle_placed_lengths: mask %d: origin (%lld, %lld) outside the %lld x %lld canvas", i, y0, x0, H, W);
+    RSP_CHECK_ARG(h >= 1 && w >= 1 && h <= H - y0 && w <= W - x0,
+                  "mask_rle_placed_lengths: mask %d: %lld x %lld at (%lld, %lld) leaves the %lld x %lld canvas", i, h, w,
+                  y0, x0, H, W);
+    RSP_CHECK_ARG(off >= 0 && ld <= INT_MAX && h <= rows && w <= (packed ? 8 * ld : ld),
+                  "mask_rle_placed_lengths: mask %d: visible %lld x %lld exceeds the source (%lld rows of %lld bytes, "
+                  "offset %lld)", i, h, w, rows, ld, off);
+  }
+  return rle_lengths<true>(src, packed, desc, n, offsets, stream);
+}
+
+int mask_rle_placed_write(const unsigned char* src, int packed, const long long* desc, int n, const long long* offsets,
+                          char* pool, int* lengths, cudaStream_t stream) {
+  RSP_CHECK_ARG(src && desc && offsets && pool && lengths && n > 0 && (packed == 0 || packed == 1),
+                "mask_rle_placed_write: bad args");
+  return rle_write<true>(src, packed, desc, n, offsets, pool, lengths, stream);
 }
 
 }  // namespace rsp

@@ -1,0 +1,281 @@
+"""Whole remote-sensing scenes through the detectors: sliced inference, a cross-tile merge and scene-size RLE masks.
+
+The counterpart of the reference's large-image demo (demo/large_image_demo.py:141-262 over
+mmdet/utils/large_image.py:27-104): the scene is cut into overlapping model-size windows (sahi ``slice_image`` with
+``auto_slice_resolution=False``), every window is detected, the results are shifted into scene coordinates and
+merged with one class-aware NMS (``merge_results_by_nms``).  Here all of it stays on the device:
+
+  * tiles are copied out of the scene in batches and normalised by the detector's own DetDataPreprocessor path
+    (the fused uint8 patch-embed loader, or ``rsp_preprocess_u8`` for tiles that overhang a scene smaller than
+    the patch, padded with 0 after normalisation as BatchFixedSizePad pads);
+  * every batch leaves ``predict_records`` as one ResultRecord, resident until the merge;
+  * the merge is ``rsp_nms_batched`` + ``rsp_compact_keep`` over every valid slot of every tile (mmcv
+    ``batched_nms`` semantics, label offset included);
+  * the kept masks are encoded as COCO RLE of the whole scene by ``rsp_mask_rle_placed_*`` straight from the
+    records' bits: the full-scene bool mask sahi's ``shift_masks`` builds for every instance never exists.
+
+The merge's NMS is dense: at most 393 216 candidates (tiles x slots), with an n^2 / 8-byte workspace.
+
+``python -m rsprompter_b200.large_image CONFIG IMAGE`` writes the COCO result dicts of one scene."""
+from __future__ import annotations
+
+import argparse
+import json
+import math
+
+import torch
+
+from . import _lib
+from .detectors import RSPrompterAnchor, RSPrompterQuery, SAMSegMaskRCNN
+from .registry import DetDataSample, InstanceData
+from .results import ResultRecord, _align16
+
+# rsp_nms_batched keeps one 64-candidate word per candidate and word column in shared memory (48 KB)
+MAX_MERGE_CANDIDATES = 48 * 1024 // 8 * 64
+
+
+def slice_origins(hw: tuple, patch: int, overlap_ratio: float) -> list:
+    """Top-left corners (x0, y0) of the patch x patch windows sahi's slice_image(..., auto_slice_resolution=False)
+    cuts from an H x W scene, row-major.  Windows step by patch - int(overlap_ratio * patch); the last one of a row
+    or column is shifted inward to end at the scene's edge, so a window overhangs the scene only where the scene is
+    smaller than the patch."""
+    H, W = int(hw[0]), int(hw[1])
+    patch = int(patch)
+    ov = int(overlap_ratio * patch)
+    out = []
+    y_min = y_max = 0
+    while y_max < H:
+        x_min = x_max = 0
+        y_max = y_min + patch
+        while x_max < W:
+            x_max = x_min + patch
+            if y_max > H or x_max > W:
+                out.append((max(0, min(W, x_max) - patch), max(0, min(H, y_max) - patch)))
+            else:
+                out.append((x_min, y_min))
+            x_min = x_max - ov
+        y_min = y_max - ov
+    return out
+
+
+def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_thr: float = 0.25,
+                       score_thr: float = 0.0) -> dict:
+    """Class-aware NMS of every valid slot of every tile, in scene coordinates.
+
+    ``records`` are ResultRecords of tiles (one image per tile; records of one call share slots and device) and
+    ``origins[r]`` lists the (x0, y0) of the first len(origins[r]) images of record r; later images are ignored (the
+    padding of a last partial batch).  Each box is shifted by its tile's origin (the fp32 add of sahi's
+    shift_bboxes) and clipped to the tile's window intersected with the scene, a no-op for a box inside its tile.
+    The candidates are sorted by score, ties by (tile, slot), and merged as mmcv batched_nms(boxes, scores, labels,
+    iou_threshold=merge_iou_thr).  Candidates below ``score_thr`` are dropped first; greedy NMS lets a box suppress
+    only lower-scored boxes, so that is exactly the unfiltered result restricted to score >= score_thr.
+
+    Returns dict(bboxes fp32 [k, 4], scores [k], labels int64 [k] on the device, in descending score order, and
+    source int64 [k, 3] on the host: (record, image, slot) of each kept row).  One host synchronisation."""
+    H, W = int(scene_hw[0]), int(scene_hw[1])
+    assert len(records) == len(origins) and records, "one origin list per record"
+    M = records[0].slots
+    rows, counts, win, src = [], [], [], []
+    for r, (rec, org) in enumerate(zip(records, origins)):
+        assert rec.slots == M and 0 < len(org) <= rec.batch, "records of one merge share their slot count"
+        n = len(org)
+        rows.append(rec.rows[:n])
+        counts.append(rec.counts[:n])
+        ph, pw = rec.hw
+        for b, (x0, y0) in enumerate(org):
+            win.append((x0, y0, min(x0 + pw, W), min(y0 + ph, H)))
+            src.append((r, b))
+    T = len(src)
+    N = T * M
+    if N > MAX_MERGE_CANDIDATES:
+        raise ValueError(f"{T} tiles x {M} slots = {N} merge candidates; the dense NMS takes at most "
+                         f"{MAX_MERGE_CANDIDATES}")
+    rows = torch.cat(rows)                                        # [T, M, 6]
+    counts = torch.cat(counts)
+    dev = rows.device
+    win = torch.tensor(win, dtype=torch.float32).pin_memory().to(dev, non_blocking=True)
+    lo, hi = win[:, None, [0, 1, 0, 1]], win[:, None, [2, 3, 2, 3]]
+    boxes = torch.minimum(torch.maximum(rows[..., :4] + lo, lo), hi)
+    scores = rows[..., 4]
+    valid = torch.arange(M, device=dev)[None, :] < counts[:, None]
+    if score_thr > 0:
+        valid &= scores >= score_thr
+    key = torch.where(valid, scores, torch.full_like(scores, -math.inf)).reshape(N)
+    _, order = torch.sort(key, descending=True, stable=True)     # invalid slots last; ties by (tile, slot)
+    nvalid = valid.sum().to(torch.int32).view(1)
+    boxes_s = boxes.reshape(N, 4)[order].contiguous()
+    scores_s = scores.reshape(N)[order].contiguous()
+    labels_s = rows[..., 5].reshape(N)[order].long().contiguous()
+    keep = _lib.nms_batched(boxes_s[None], labels_s[None], nvalid, merge_iou_thr)
+    ob, os_, ol, oi, cnt = _lib.compact_keep(keep, boxes_s[None], scores_s[None], labels_s[None], N)
+    flat = order[oi[0].clamp(min=0).long()]
+    host = torch.cat([cnt.long(), flat]).cpu()                   # the one host sync: count + sources
+    k = int(host[0])
+    flat = host[1:1 + k]
+    tile, slot = flat // M, flat % M
+    src = torch.tensor(src, dtype=torch.int64).view(-1, 2)
+    return dict(bboxes=ob[0, :k], scores=os_[0, :k], labels=ol[0, :k],
+                source=torch.cat([src[tile], slot[:, None]], dim=1))
+
+
+def _slots(model) -> int:
+    if isinstance(model, RSPrompterQuery):
+        return int(model.test_cfg.get("max_per_image", 100))
+    return int(model.test_cfg.rcnn.get("max_per_img", 100))
+
+
+def _record_nbytes(B: int, M: int, P: int) -> int:
+    return _align16(B * M * P * (P // 8)) + _align16(B * M * 24) + _align16(B * 4)
+
+
+@torch.no_grad()
+def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr: float = 0.25,
+                        score_thr: float = 0.0, batch_size: int = 8) -> DetDataSample:
+    """Detect a whole scene: slice, run the tiles in batches, merge across tiles, encode the kept masks.
+
+    ``image`` is the scene as mmcv.imread decodes it, uint8 [H, W, 3] BGR: a numpy array or a tensor on the host
+    (copied to the device once, pinned) or on the model's device.  Tiles are model-size (``image_size``) windows,
+    never resized.  The last partial batch repeats a tile whose slots are ignored, so every batch has one shape and
+    enable_cuda_graphs() replays one graph.  No host synchronisation happens per tile or per batch; the merge reads
+    the kept rows once and the RLE encode synchronises twice.
+
+    Returns a DetDataSample with ori_shape = img_shape = (H, W), scale_factor (1, 1) and pred_instances: bboxes,
+    scores, labels on the device in descending score order, masks a list of {'size': [H, W], 'counts': bytes} (the
+    test_cfg.rle_masks convention, passed through by CocoMetric.process)."""
+    records, batches = run_tiles(model, image, overlap_ratio, batch_size)
+    H, W = int(image.shape[0]), int(image.shape[1])
+    merged = merge_tile_records(records, batches, (H, W), merge_iou_thr=merge_iou_thr, score_thr=score_thr)
+    masks = encode_kept_masks(records, batches, merged["source"], (H, W))
+    ds = DetDataSample(metainfo=dict(ori_shape=(H, W), img_shape=(H, W), scale_factor=(1.0, 1.0)))
+    ds.pred_instances = InstanceData(bboxes=merged["bboxes"], scores=merged["scores"], labels=merged["labels"],
+                                     masks=masks)
+    return ds
+
+
+@torch.no_grad()
+def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8):
+    """The tile stage of predict_large_image -> (records, origins per record), everything left on the device."""
+    if not isinstance(model, (RSPrompterAnchor, RSPrompterQuery, SAMSegMaskRCNN)):
+        raise NotImplementedError(f"large-scene inference needs a detector with per-tile result records "
+                                  f"(RSPrompterAnchor, RSPrompterQuery, SAMSegMaskRCNN), not {type(model).__name__}")
+    if batch_size < 1:
+        raise ValueError("batch_size must be >= 1")
+    dev = next(model.parameters()).device
+    img = torch.from_numpy(image) if not isinstance(image, torch.Tensor) else image
+    if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3:
+        raise ValueError(f"the scene must be uint8 [H, W, 3] (BGR, as mmcv.imread decodes it), got "
+                         f"{img.dtype} {tuple(img.shape)}")
+    H, W = int(img.shape[0]), int(img.shape[1])
+    P = int(model.backbone.vision_encoder.arch.image_size)
+    origins = slice_origins((H, W), P, overlap_ratio)
+    B = min(batch_size, len(origins))
+    batches = [origins[i:i + B] for i in range(0, len(origins), B)]
+    M = _slots(model)
+
+    # everything that stays resident until the merge, checked before any tile runs
+    N = len(origins) * M
+    if N > MAX_MERGE_CANDIDATES:
+        raise ValueError(f"{len(origins)} tiles x {M} slots = {N} merge candidates; the dense NMS takes at most "
+                         f"{MAX_MERGE_CANDIDATES}")
+    need = (len(batches) * _record_nbytes(B, M, P) + (0 if img.is_cuda else H * W * 3)
+            + N * ((N + 63) // 64) * 8)
+    free, _ = torch.cuda.mem_get_info(dev)
+    free += torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+    if need > free:
+        raise RuntimeError(f"a {H} x {W} scene needs {need / 2**30:.2f} GiB resident on {dev} ({len(origins)} tiles "
+                           f"of {P}^2 in {len(batches)} result records, the scene and the merge workspace); "
+                           f"{free / 2**30:.2f} GiB are free")
+
+    scene = img.to(dev) if img.is_cuda else img.pin_memory().to(dev, non_blocking=True)
+    dp = model.data_preprocessor
+    mean, std, swap = dp._norm3() if dp is not None else ((0.0,) * 3, (1.0,) * 3, False)
+    overhang = H < P or W < P
+    if overhang:    # every window overhangs: normalised fp32 tiles padded with 0, clipped to their in-scene extent
+        buf = torch.empty(B, 3, P, P, dtype=torch.float32, device=dev)
+        hv, wv = min(P, H), min(P, W)
+        shapes = torch.tensor([[hv, wv]] * B, dtype=torch.float32).pin_memory().to(dev, non_blocking=True)
+    else:           # uint8 HWC tiles: the normalisation is fused into the patch-embed loader
+        buf = torch.empty(B, P, P, 3, dtype=torch.uint8, device=dev)
+    records = []
+    for org in batches:
+        tiles = org + [org[-1]] * (B - len(org))
+        for i, (x0, y0) in enumerate(tiles):
+            view = scene[y0:y0 + P, x0:x0 + P]
+            if overhang:
+                _lib.preprocess_u8(view.permute(2, 0, 1), buf[i], mean, std, swap, 0.0)
+            else:
+                buf[i].copy_(view)
+        if overhang:
+            batch = buf
+            batch.rsp_img_shapes = shapes
+        else:
+            batch = buf.permute(0, 3, 1, 2)
+            batch.rsp_norm = (mean, std, swap)
+        records.append(model.predict_records(batch, record=ResultRecord(B, M, (P, P), device=dev)))
+    return records, batches
+
+
+def encode_kept_masks(records: list, origins: list, source: torch.Tensor, scene_hw: tuple) -> list:
+    """COCO RLE dicts of the kept masks (``source`` rows (record, image, slot) from merge_tile_records) as masks of
+    the whole H x W scene, encoded from the records' bits; two host synchronisations."""
+    H, W = int(scene_hw[0]), int(scene_hw[1])
+    groups = []
+    for r, b, s in source.tolist():
+        rec = records[r]
+        P, M = rec.hw[0], rec.slots
+        ld = rec.hw[1] // 8
+        x0, y0 = origins[r][b]
+        groups.append((rec.buf, [((b * M + s) * P * ld, ld, P, min(P, H - y0), min(rec.hw[1], W - x0), H, W, y0, x0)]))
+    return [dict(size=[H, W], counts=c) for c in _lib.mask_rle_placed(groups, packed=True)]
+
+
+def coco_results(ds: DetDataSample, image_id=0, label_to_cat=None) -> list:
+    """COCO result dicts of one scene, as CocoMetric.results2json writes them: xywh bbox, score, category_id and the
+    RLE segmentation with ``counts`` as str."""
+    p = ds.pred_instances
+    out = []
+    for (x1, y1, x2, y2), score, label, m in zip(p.bboxes.tolist(), p.scores.tolist(), p.labels.tolist(), p.masks):
+        cat = int(label) if label_to_cat is None else label_to_cat[int(label)]
+        out.append(dict(image_id=image_id, bbox=[x1, y1, x2 - x1, y2 - y1], score=float(score), category_id=cat,
+                        segmentation=dict(size=m["size"], counts=m["counts"].decode())))
+    return out
+
+
+def main(argv=None) -> list:
+    ap = argparse.ArgumentParser(description="Detect one large scene: sliced inference, merge, COCO RLE masks")
+    ap.add_argument("config")
+    ap.add_argument("image")
+    ap.add_argument("--checkpoint", default=None)
+    ap.add_argument("--patch-overlap-ratio", type=float, default=0.25)
+    ap.add_argument("--merge-iou-thr", type=float, default=0.25)
+    ap.add_argument("--score-thr", type=float, default=0.0)
+    ap.add_argument("--batch-size", type=int, default=8)
+    ap.add_argument("--out", default=None, help="JSON file for the result dicts (default: stdout)")
+    args = ap.parse_args(argv)
+
+    import cv2
+
+    from .registry import MODELS, Config
+    cfg = Config.fromfile(args.config)
+    model = MODELS.build(cfg.model)
+    if args.checkpoint:
+        sd = torch.load(args.checkpoint, map_location="cpu")
+        model.load_state_dict(sd.get("state_dict", sd), strict=True)
+    model = model.cuda().eval()
+    img = cv2.imread(args.image, cv2.IMREAD_COLOR)
+    if img is None:
+        raise FileNotFoundError(args.image)
+    ds = predict_large_image(model, img, overlap_ratio=args.patch_overlap_ratio, merge_iou_thr=args.merge_iou_thr,
+                             score_thr=args.score_thr, batch_size=args.batch_size)
+    res = coco_results(ds)
+    text = json.dumps(res)
+    if args.out:
+        with open(args.out, "w") as f:
+            f.write(text)
+    else:
+        print(text)
+    return res
+
+
+if __name__ == "__main__":
+    main()
