@@ -149,6 +149,23 @@ int rsp_t2i_attention(const void* q, const void* K, const void* V, int ldkv, con
 int rsp_i2t_attention(const void* Q, const int32_t* q_block, const void* ktok, const void* vtok,
                       void* out, int N, int Tq, int HW, void* stream);
 
+/* t2i with the k | v projection of per-prompt image tokens fused in: out = t2i(q, K, V) with
+ * [K | V] = bf16((keys Wkv^T + kvb) + pe_kv[row % HW]), keys bf16 [N*HW, 256] (row stride ldk), Wkv bf16 [256, 256]
+ * (k_proj rows, then v_proj rows), kvb fp32 [256], pe_kv bf16 [HW, 256], q / out bf16 [N, Tq, 128].  K and V never
+ * reach global memory; the bytes equal rsp_gemm_bf16 (residual = pe_kv, res_mod = HW) followed by rsp_t2i_attention. */
+int rsp_t2i_fused(const void* keys, int ldk, const void* kvw, const float* kvb, const void* pe_kv, const void* q,
+                  void* out, int N, int Tq, int HW, void* stream);
+
+/* The image -> token step of a two-way layer for per-prompt keys, fused:
+ *   out = LN((i2t(Q, ktok, vtok) Wo^T + ob) + keys),  Q = bf16((keys Wq^T + qb) + pe_q[row % HW])
+ * keys bf16 [N*HW, 256] (row stride ldk; also the residual), Wq bf16 [128, 256], qb fp32 [128], pe_q bf16 [HW, 128],
+ * ktok / vtok bf16 [N, Tq, 128], Wo bf16 [256, 128], ob / ln_g / ln_b fp32 [256], out bf16 [N*HW, 256]; HW % 64 == 0.
+ * Q and the attention output never reach global memory; the bytes equal rsp_gemm_bf16 (Qimg) ->
+ * rsp_i2t_attention -> rsp_gemm_bf16_ex (epi_mode 1, residual = keys). */
+int rsp_i2t_fused(const void* keys, int ldk, const void* wq, const float* qb, const void* pe_q, const void* ktok,
+                  const void* vtok, const void* wo, const float* ob, const float* ln_g, const float* ln_b, float eps,
+                  void* out, int N, int Tq, int HW, void* stream);
+
 /* ---- detection side of the anchor variant: batched over B images with fixed-size padded
  * candidate lists (score -1 = filtered / padding), so RPN -> RoI head -> mask head runs without
  * host synchronisation.  All arithmetic that decides indices is fp32 without FMA contraction. ---- */

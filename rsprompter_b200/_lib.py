@@ -66,6 +66,8 @@ _SIGNATURES = {
     "rsp_token_self_attention": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp], _i),
     "rsp_t2i_attention": ([_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp], _i),
     "rsp_i2t_attention": ([_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp], _i),
+    "rsp_t2i_fused": ([_vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp], _i),
+    "rsp_i2t_fused": ([_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp], _i),
     "rsp_rpn_decode": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _f, _f, _f, _i, _i, _vp, _vp, _vp], _i),
     "rsp_bbox_cls_decode": ([_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _f, _f, _f, _vp, _vp, _vp, _vp], _i),
     "rsp_rpn_decode_shapes": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp], _i),
@@ -342,6 +344,54 @@ def t2i_attention(q: torch.Tensor, K: torch.Tensor, V: torch.Tensor, hw: int,
     _check(_lib.rsp_t2i_attention(_ptr(q), _ptr(K), _ptr(V), K.stride(0), _ptr(kv_block), _ptr(out), N, Tq, hw, _stream()),
            "rsp_t2i_attention")
     launch_count += 1
+    return out
+
+
+def t2i_fused(q: torch.Tensor, keys: torch.Tensor, kvw: torch.Tensor, kvb: torch.Tensor, pe_kv: torch.Tensor,
+              hw: int) -> torch.Tensor:
+    """t2i_attention(q, K, V, hw) with [K | V] = gemm(keys, kvw, kvb, residual=pe_kv, res_mod=hw) computed on chip.
+
+    q bf16 [N, Tq, 128]; keys bf16 [N*hw, 256] (row stride may exceed 256); kvw bf16 [256, 256]; kvb fp32 [256];
+    pe_kv bf16 [hw, 256] -> bf16 [N, Tq, 128], the same bytes as the two-call chain."""
+    global launch_count
+    _require_cuda(q, keys, kvw, kvb, pe_kv)
+    N, Tq, C = q.shape
+    assert C == 128 and q.dtype == torch.bfloat16 and q.is_contiguous()
+    assert keys.dtype == torch.bfloat16 and keys.dim() == 2 and keys.stride(1) == 1 and keys.shape == (N * hw, 256)
+    assert kvw.dtype == torch.bfloat16 and kvw.shape == (256, 256) and kvw.is_contiguous()
+    assert kvb.dtype == torch.float32 and kvb.numel() == 256 and kvb.is_contiguous()
+    assert pe_kv.dtype == torch.bfloat16 and pe_kv.shape == (hw, 256) and pe_kv.is_contiguous()
+    out = torch.empty_like(q)
+    _check(_lib.rsp_t2i_fused(_ptr(keys), keys.stride(0), _ptr(kvw), _ptr(kvb), _ptr(pe_kv), _ptr(q), _ptr(out), N, Tq,
+                              hw, _stream()), "rsp_t2i_fused")
+    launch_count += 1
+    _log("gemm", 2.0 * N * hw * 256 * 256)
+    return out
+
+
+def i2t_fused(keys: torch.Tensor, wq: torch.Tensor, qb: torch.Tensor, pe_q: torch.Tensor, ktok: torch.Tensor,
+              vtok: torch.Tensor, wo: torch.Tensor, ob: torch.Tensor, ln: tuple, hw: int) -> torch.Tensor:
+    """LN((i2t(Q, ktok, vtok) @ wo.T + ob) + keys) with Q = gemm(keys, wq, qb, residual=pe_q, res_mod=hw), on chip.
+
+    keys bf16 [N*hw, 256] (row stride may exceed 256; also the residual); wq bf16 [128, 256]; qb fp32 [128];
+    pe_q bf16 [hw, 128]; ktok, vtok bf16 [N, Tq, 128]; wo bf16 [256, 128]; ob fp32 [256]; ln = (gamma, beta, eps);
+    hw % 64 == 0 -> bf16 [N*hw, 256], the same bytes as the three-call chain."""
+    global launch_count
+    g, b, eps = ln
+    _require_cuda(keys, wq, qb, pe_q, ktok, vtok, wo, ob, g, b)
+    N, Tq, C = ktok.shape
+    assert C == 128 and hw % 64 == 0
+    assert keys.dtype == torch.bfloat16 and keys.dim() == 2 and keys.stride(1) == 1 and keys.shape == (N * hw, 256)
+    for t, shape in ((wq, (128, 256)), (pe_q, (hw, 128)), (ktok, (N, Tq, 128)), (vtok, (N, Tq, 128)), (wo, (256, 128))):
+        assert t.dtype == torch.bfloat16 and t.shape == shape and t.is_contiguous()
+    for t, n in ((qb, 128), (ob, 256), (g, 256), (b, 256)):
+        assert t.dtype == torch.float32 and t.numel() == n and t.is_contiguous()
+    out = torch.empty((N * hw, 256), device=keys.device, dtype=torch.bfloat16)
+    _check(_lib.rsp_i2t_fused(_ptr(keys), keys.stride(0), _ptr(wq), _ptr(qb), _ptr(pe_q), _ptr(ktok), _ptr(vtok),
+                              _ptr(wo), _ptr(ob), _ptr(g), _ptr(b), float(eps), _ptr(out), N, Tq, hw, _stream()),
+           "rsp_i2t_fused")
+    launch_count += 1
+    _log("gemm", 2.0 * N * hw * 256 * 256)
     return out
 
 

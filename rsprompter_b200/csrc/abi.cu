@@ -174,6 +174,17 @@ int rsp_i2t_attention(const void* Q, const int32_t* q_block, const void* ktok, c
   return i2t_attention(Q, q_block, ktok, vtok, out, N, Tq, HW, S(stream));
 }
 
+int rsp_t2i_fused(const void* keys, int ldk, const void* kvw, const float* kvb, const void* pe_kv, const void* q,
+                  void* out, int N, int Tq, int HW, void* stream) {
+  return t2i_fused(keys, ldk, kvw, kvb, pe_kv, q, out, N, Tq, HW, S(stream));
+}
+
+int rsp_i2t_fused(const void* keys, int ldk, const void* wq, const float* qb, const void* pe_q, const void* ktok,
+                  const void* vtok, const void* wo, const float* ob, const float* ln_g, const float* ln_b, float eps,
+                  void* out, int N, int Tq, int HW, void* stream) {
+  return i2t_fused(keys, ldk, wq, qb, pe_q, ktok, vtok, wo, ob, ln_g, ln_b, eps, out, N, Tq, HW, S(stream));
+}
+
 }  // extern "C"
 
 #include "detect.h"

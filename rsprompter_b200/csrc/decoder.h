@@ -9,7 +9,12 @@ int token_self_attention(const void* q, const void* k, const void* v, void* out,
                          int heads, int c, cudaStream_t stream);
 int t2i_attention(const void* q, const void* K, const void* V, int ldkv, const int* kv_block, void* out, int N,
                   int Tq, int HW, cudaStream_t stream);
+int t2i_fused(const void* keys, int ldk, const void* kvw, const float* kvb, const void* pe_kv, const void* q,
+              void* out, int N, int Tq, int HW, cudaStream_t stream);
 int i2t_attention(const void* Q, const int* q_block, const void* ktok, const void* vtok, void* out,
                   int N, int Tq, int HW, cudaStream_t stream);
+int i2t_fused(const void* keys, int ldk, const void* wq, const float* qb, const void* pe_q, const void* ktok,
+              const void* vtok, const void* wo, const float* ob, const float* ln_g, const float* ln_b, float eps,
+              void* out, int N, int Tq, int HW, cudaStream_t stream);
 
 }  // namespace rsp

@@ -13,6 +13,10 @@ Decoder data flow (HF:461-543 over HF:306-405), N prompts, Tt = 5 + P tokens, HW
   * prompts of one image share its embedding through block maps (``res_block_map`` /
     ``kv_block`` / ``q_block``) instead of the ``repeat_interleave`` copies of M:367-368,1682-1683
     (3 x N x 4 MB in the reference);
+  * per-prompt image tokens (every layer after a shared first one, all of a per-prompt call) take two
+    passes per two-way layer: ``t2i_fused`` (k | v projection + tokens -> image attention) and
+    ``i2t_fused`` (q projection + image -> tokens attention + out_proj + LN4); the projections and the
+    attention output stay on chip, and the bytes equal the GEMM + attention chains they replace;
   * upscaling: conv-transpose 1 + LayerNorm2d + GELU is one GEMM (epi_mode 2), conv-transpose 2
     + GELU + the hypernetwork product is another (epi_mode 3): the (N, 32, 4h, 4w) upscaled
     embedding is never materialised.
@@ -233,9 +237,12 @@ class SamMaskDecoderB200(nn.Module):
         def t2i(layer: dict, queries: torch.Tensor, keys_b: torch.Tensor, pos_kv: torch.Tensor, kv_blk, ln):
             qin = _lib.add_cast_bf16(queries, tokens)
             q = _lib.gemm(qin, layer["qw"], layer["qb"])
-            KV = _lib.gemm(keys_b, layer["kvw"], layer["kvb"], residual=pos_kv, res_mod=HW)   # [rows, k | v]
-            n_k = layer["kw"].shape[0]
-            att = _lib.t2i_attention(q.view(N, Tt, -1), KV[:, :n_k], KV[:, n_k:], HW, kv_block=kv_blk)
+            if kv_blk is None:   # per-prompt keys: the k | v projection runs inside the attention kernel
+                att = _lib.t2i_fused(q.view(N, Tt, -1), keys_b, layer["kvw"], layer["kvb"], pos_kv, HW)
+            else:                # prompts share an image's keys: project each image's rows once
+                KV = _lib.gemm(keys_b, layer["kvw"], layer["kvb"], residual=pos_kv, res_mod=HW)   # [rows, k | v]
+                n_k = layer["kw"].shape[0]
+                att = _lib.t2i_attention(q.view(N, Tt, -1), KV[:, :n_k], KV[:, n_k:], HW, kv_block=kv_blk)
             return _lib.gemm(att.view(N * Tt, -1), layer["ow"], layer["ob"], residual=queries,
                              out_dtype=torch.float32, ln=ln)
 
@@ -270,13 +277,19 @@ class SamMaskDecoderB200(nn.Module):
             qin = _lib.add_cast_bf16(queries, tokens)
             ktok = _lib.gemm(qin, i2t["kw"], i2t["kb"])
             vtok = _lib.gemm(_lib.cast_bf16(queries), i2t["vw"], i2t["vb"])
-            Qimg = _lib.gemm(keys_b, i2t["qw"], i2t["qb"], residual=pt["q"][li], res_mod=HW)
-            att = _lib.i2t_attention(Qimg, ktok.view(N, Tt, -1), vtok.view(N, Tt, -1), HW, q_block=kblk)
-            # keys = LN4(keys + out_proj(attn)) (HF:346-347) in the out_proj GEMM's epilogue: the residual slab
-            # (block-mapped prompt -> image in the first layer) arrives by TMA, the row statistics are taken on
-            # the fp32 accumulator, and only the normalised bf16 keys are written
-            keys_b = _lib.gemm(att, i2t["ow"], i2t["ob"], residual=keys_res, ln=(*L["ln4"], a.layer_norm_eps),
-                               res_block_map=kblk, res_block_rows=HW if kblk is not None else 0)
+            if kblk is None and HW % 64 == 0:
+                # per-prompt keys: Qimg, the attention and keys = LN4(keys + out_proj(attn)) (HF:340-347) in one
+                # kernel; Qimg and the attention output stay on chip
+                keys_b = _lib.i2t_fused(keys_b, i2t["qw"], i2t["qb"], pt["q"][li], ktok.view(N, Tt, -1),
+                                        vtok.view(N, Tt, -1), i2t["ow"], i2t["ob"], (*L["ln4"], a.layer_norm_eps), HW)
+            else:
+                Qimg = _lib.gemm(keys_b, i2t["qw"], i2t["qb"], residual=pt["q"][li], res_mod=HW)
+                att = _lib.i2t_attention(Qimg, ktok.view(N, Tt, -1), vtok.view(N, Tt, -1), HW, q_block=kblk)
+                # keys = LN4(keys + out_proj(attn)) (HF:346-347) in the out_proj GEMM's epilogue: the residual slab
+                # (block-mapped prompt -> image in the first layer) arrives by TMA, the row statistics are taken on
+                # the fp32 accumulator, and only the normalised bf16 keys are written
+                keys_b = _lib.gemm(att, i2t["ow"], i2t["ob"], residual=keys_res, ln=(*L["ln4"], a.layer_norm_eps),
+                                   res_block_map=kblk, res_block_rows=HW if kblk is not None else 0)
             keys_res, kblk = keys_b, None
         queries = t2i(p["final"], queries, keys_b, pt["kv"][-1], None, (*p["lnf"], 1e-5))
         qv = queries.view(N, Tt, C)
