@@ -123,7 +123,12 @@ int rsp_nhwc_to_nchw(const void* in, int in_fp32, float* out, int B, int HW, int
  *               hypernetwork product (HF:521-531); `out` is unused
  * res_block_map (int32 [M / res_block_rows]) redirects the residual of row r to row
  * map[r / res_block_rows] * res_block_rows + r % res_block_rows: prompts of one image share its
- * embedding without the repeat_interleave copies of M:367-368 / M:1682-1683. */
+ * embedding without the repeat_interleave copies of M:367-368 / M:1682-1683.
+ * Alignment (a call that breaks it returns RSP_ERR_INVALID, nothing launched):
+ *   epi_mode 1  out, residual, bias, ln_gamma, ln_beta 16-byte aligned; ldo, ldr % 8 == 0
+ *   epi_mode 2  N % 128 == 0 with out 8-byte aligned and ldo % 4 == 0: bias, ln_gamma, ln_beta 16-byte aligned;
+ *               otherwise out 16-byte aligned and ldo % 8 == 0
+ *   epi_mode 3  hyper 16-byte aligned, mask_out 8-byte aligned; bias 16-byte aligned when grid_w is even */
 int rsp_gemm_bf16_ex(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M, int N,
                      int K, const float* bias, const void* residual, int ldr, int res_fp32, int res_mod,
                      const int32_t* row_map, int act, int out_fp32, int epi_mode, const float* ln_gamma,

@@ -471,21 +471,31 @@ int gemm_bf16(const GemmArgs& a, cudaStream_t stream) {
   RSP_CHECK_ARG(a.lda % 8 == 0 && a.ldw % 8 == 0, "gemm: lda/ldw must be multiples of 8 bf16");
   RSP_CHECK_ARG(a.act >= 0 && a.act <= 2, "gemm: act %d", a.act);
   if (a.res_block_map) RSP_CHECK_ARG(a.res_block_rows > 0, "gemm: res_block_rows");
+  auto al = [](const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; };
+  // The fused epilogues make vector accesses (16-byte rows, float4 / float2 loads and stores) whose alignment is
+  // checked here, before any kernel is chosen: a misaligned pointer is rejected, never handed to a fallback.
   if (a.epi_mode == EPI_LN_ROW) {
     RSP_CHECK_ARG(a.N % 32 == 0 && a.N <= 256 && a.ln_gamma && a.ln_beta && !a.w_is_kn && !a.row_map,
                   "gemm: row-LN epilogue needs N %% 32 == 0, N <= 256, gamma/beta");
-    RSP_CHECK_ARG(a.ldo % 8 == 0 && (!a.residual || a.ldr % 8 == 0), "gemm: row-LN epilogue alignment");
+    // both kernels move 16 bytes at a time through out, residual, bias, gamma and beta
+    RSP_CHECK_ARG(a.ldo % 8 == 0 && (!a.residual || a.ldr % 8 == 0) && al(a.out, 16) && al(a.residual, 16) &&
+                  al(a.bias, 16) && al(a.ln_gamma, 16) && al(a.ln_beta, 16), "gemm: row-LN epilogue alignment");
     if (gemm_v2_ln_row_eligible(a)) return gemm_bf16_v2_ln_row(a, stream);
     if (a.N > 128) return launch_gemm<256, false>(a, stream);
     if (a.N > 64) return launch_gemm<128, false>(a, stream);
     return launch_gemm<64, false>(a, stream);
   }
   if (a.epi_mode == EPI_LN64_GELU) {
-    RSP_CHECK_ARG(a.N % 64 == 0 && a.bias && a.ln_gamma && a.ln_beta && !a.out_fp32 && !a.w_is_kn &&
-                  !a.row_map && a.ldo % 8 == 0, "gemm: LN64+GELU epilogue needs N %% 64 == 0, bias, bf16 out");
+    RSP_CHECK_ARG(a.N % 64 == 0 && a.bias && a.ln_gamma && a.ln_beta && !a.out_fp32 && !a.w_is_kn && !a.row_map,
+                  "gemm: LN64+GELU epilogue needs N %% 64 == 0, bias, bf16 out");
     static const bool v1 = getenv("RSP_GEMM_V1") != nullptr;
-    if (!v1 && a.N % 128 == 0 && (reinterpret_cast<uintptr_t>(a.out) & 7) == 0 && a.ldo % 4 == 0)
+    if (!v1 && a.N % 128 == 0 && al(a.out, 8) && a.ldo % 4 == 0) {
+      // float4 bias / gamma / beta loads; out is a TMA store (16-byte aligned rows) or 8-byte stores
+      RSP_CHECK_ARG(al(a.bias, 16) && al(a.ln_gamma, 16) && al(a.ln_beta, 16), "gemm: LN64+GELU epilogue alignment");
       return gemm_bf16_v2_ln64_gelu(a, stream);
+    }
+    // 16-byte stores of 8 bf16 per row
+    RSP_CHECK_ARG(al(a.out, 16) && a.ldo % 8 == 0, "gemm: LN64+GELU epilogue output alignment");
     if (a.N % 128 == 0) return launch_gemm<128, false>(a, stream);
     return launch_gemm<64, false>(a, stream);
   }
@@ -493,8 +503,13 @@ int gemm_bf16(const GemmArgs& a, cudaStream_t stream) {
     RSP_CHECK_ARG(a.N == 128 && a.bias && a.hyper && a.mask_out && a.grid_h > 0 && a.grid_w > 0 &&
                   a.M % (4 * a.grid_h * a.grid_w) == 0 && !a.w_is_kn,
                   "gemm: GELU+hyper epilogue needs N == 128 and M = prompts * 4 * h * w");
+    // float4 hyper loads, float2 mask stores (at even columns of rows 4 * grid_w wide)
+    RSP_CHECK_ARG(al(a.hyper, 16) && al(a.mask_out, 8), "gemm: GELU+hyper epilogue alignment");
     static const bool v1h = getenv("RSP_GEMM_V1") != nullptr;
-    if (!v1h && a.grid_w % 2 == 0) return gemm_bf16_v2_gelu_hyper(a, stream);
+    if (!v1h && a.grid_w % 2 == 0) {
+      RSP_CHECK_ARG(al(a.bias, 16), "gemm: GELU+hyper epilogue bias alignment");   // float4 bias loads
+      return gemm_bf16_v2_gelu_hyper(a, stream);
+    }
     return launch_gemm<128, false>(a, stream);
   }
   RSP_CHECK_ARG(a.epi_mode == EPI_STD, "gemm: epi_mode %d", a.epi_mode);
