@@ -358,6 +358,20 @@ int rsp_query_postprocess_bits(const float* logits, const int32_t* sel, const fl
  * (anchor variant, M:1758-1780 when ori_shape == batch shape). */
 int rsp_mask_paste_bits(const float* maps, uint8_t* bits, int n, int hm, int wm, float thr, int mode, void* stream);
 
+/* rsp_mask_paste_rescale (the two resizes and the threshold, M:1763-1777) with bit-packed output into record slots of
+ * Hr x Wr (H <= Hr, W <= Wr, Wr % 16 == 0): bits uint8 [n, Hr, Wr/8]; the (H, W) = ori_shape mask at the slot's
+ * top-left, every other pixel 0.  With (Hr, Wr) = (H, W) the bits are rsp_pack_mask_bits of rsp_mask_paste_rescale's
+ * output exactly (predict_records of resized images). */
+int rsp_mask_paste_rescale_bits(const float* maps, uint8_t* bits, int n, int hm, int wm, int Hb, int Wb, int crop_h,
+                                int crop_w, int H, int W, int Hr, int Wr, float thr, int mode, void* stream);
+
+/* rsp_query_postprocess_rescale (M:652-656 + 679-691) with the masks bit-packed as above; scores and boxes are
+ * bit-identical to it.  part_ws fp32 [n_inst, ceil(Hr/16), 6]; Wr <= 16384. */
+int rsp_query_postprocess_rescale_bits(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst,
+                                       int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr,
+                                       int Wr, uint8_t* bits, float* part_ws, float* scores, float* boxes,
+                                       void* stream);
+
 /* FCNMaskHead mask paste (SAMSegMaskRCNN; fcn_mask_head.py:_do_paste_mask + threshold :388-392): activated RoI masks
  * probs fp32 [n, hm, wm] are sampled with F.grid_sample(bilinear, align_corners=False, zero padding) semantics at the
  * image pixel centres mapped into boxes fp32 [n, 4] (x1, y1, x2, y2) -> out uint8 [n, H, W] = (value >= thr); packed != 0 (W % 16 == 0): the
@@ -408,6 +422,21 @@ int rsp_mask_rle_placed_write(const uint8_t* src, int packed, const int64_t* des
 int rsp_preprocess_u8(const uint8_t* img, int h, int w, long long stride_c, long long stride_y, long long stride_x,
                       float* out, int H, int W, const float* mean3, const float* std3, int swap_rb, float pad_value,
                       void* stream);
+
+/* The test pipeline's keep-ratio Resize + Pad + DetDataPreprocessor for a batch of images of different sizes, one
+ * launch.  Replaces, per image, mmcv Resize(keep_ratio=True) -> imrescale -> cv2.resize(float32, INTER_LINEAR)
+ * (mmcv/image/geometric.py rescale_size / imresize; cv2 imgproc/src/resize.cpp resizeGeneric, HResizeLinear,
+ * VResizeLinear), mmcv Pad(size, pad_val) (mmcv/transforms/processing.py Pad.transform) and data_preprocessor.py:110-148
+ * (the configs' test_pipeline, configs/rsprompter/_base_/rsprompter_anchor.py, rsprompter_query.py,
+ * samseg-maskrcnn.py, samseg-mask2former.py).  desc / desc_host int64 [B, 8], the same values in DEVICE and HOST
+ * memory, per image: (source address, byte strides c, y, x, h, w, new_h, new_w); sources are uint8 CHW planes or HWC
+ * views read in place, new_h <= Hp, new_w <= Wp.  out fp32 [B, 3, Hp, Wp]: channel c from input channel
+ * (swap_rb ? 2 - c : c), bilinear with cv2's coefficients (computed in double, rounded to float; borders clamped;
+ * horizontal pass first), then (x - mean[c]) / std[c] with true fp32 division; outside (new_h, new_w) the raw pad3
+ * (HOST, 3 floats in INPUT channel order) normalised the same way.  new == source size reproduces
+ * rsp_preprocess_u8 bit for bit. */
+int rsp_resize_pad_u8(const int64_t* desc, const int64_t* desc_host, int B, float* out, int Hp, int Wp,
+                      const float* mean3, const float* std3, int swap_rb, const float* pad3, void* stream);
 
 /* The same arithmetic fused into the patch-embed operand loader: uint8 batch [B, 3, H, W] (hwc = 0) or [B, H, W, 3]
  * (hwc = 1), contiguous, 16-byte aligned, H, W % 16 == 0 -> bf16 patch rows [B*(H/16)*(W/16), 768] in (c, ky, kx)

@@ -106,6 +106,10 @@ _SIGNATURES = {
     "rsp_preprocess_u8": ([_vp, _i, _i, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp, _i, _i, _vp, _vp,
                            _i, _f, _vp], _i),
     "rsp_patchify16_u8": ([_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp], _i),
+    "rsp_resize_pad_u8": ([_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _vp], _i),
+    "rsp_mask_paste_rescale_bits": ([_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp], _i),
+    "rsp_query_postprocess_rescale_bits": ([_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp,
+                                            _vp, _vp], _i),
     "rsp_mask_rle_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp], _i),
     "rsp_mask_rle_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
     "rsp_mask_rle_placed_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp], _i),
@@ -1077,6 +1081,56 @@ def mask_paste_bits(logits: torch.Tensor, thr: float, mode: int, bits: torch.Ten
     return bits
 
 
+def mask_paste_rescale_bits(logits: torch.Tensor, batch_hw: tuple, crop_hw: tuple, ori_hw: tuple, thr: float,
+                            bits: torch.Tensor, raw: bool = False) -> torch.Tensor:
+    """mask_paste_rescale written bit-packed into ``bits`` uint8 [n, Hr, Wr/8] (record slots, Wr % 16 == 0): the
+    ori_hw mask at each slot's top-left, 0 elsewhere."""
+    global launch_count
+    _require_cuda(logits, bits)
+    n, hm, wm = logits.shape
+    assert logits.dtype == torch.float32 and logits.is_contiguous() and n > 0
+    assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.dim() == 3 and bits.shape[0] == n
+    Hr, Wr = bits.shape[1], bits.shape[2] * 8
+    act = logits
+    if not raw:
+        act = torch.empty_like(logits)
+        _check(_lib.rsp_sigmoid_f32(_ptr(logits), _ptr(act), logits.numel(), _stream()), "rsp_sigmoid_f32")
+        launch_count += 1
+    _check(_lib.rsp_mask_paste_rescale_bits(_ptr(act), _ptr(bits), n, hm, wm, batch_hw[0], batch_hw[1], crop_hw[0],
+                                            crop_hw[1], ori_hw[0], ori_hw[1], Hr, Wr, float(thr), 1 if raw else 2,
+                                            _stream()), "rsp_mask_paste_rescale_bits")
+    launch_count += 1
+    return bits
+
+
+def query_postprocess_rescale_bits(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch.Tensor, batch_hw: tuple,
+                                   crop_hw: tuple, out_hw: tuple, bits: torch.Tensor, scores: torch.Tensor | None = None,
+                                   boxes: torch.Tensor | None = None):
+    """query_postprocess_rescale with the masks written bit-packed into ``bits`` uint8 [n, Hr, Wr/8] (out_hw mask at
+    each slot's top-left) -> (bits, scores [n], boxes [n, 4]); scores / boxes may be views of a result record."""
+    global launch_count
+    _require_cuda(logits, sel, cls_scores, bits, scores, boxes)
+    n = sel.numel()
+    _, hm, wm = logits.shape
+    H, W = out_hw
+    assert logits.dtype == torch.float32 and logits.is_contiguous() and sel.dtype == torch.int32 and cls_scores.dtype == torch.float32
+    assert sel.is_contiguous() and cls_scores.is_contiguous() and cls_scores.numel() == n
+    assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.dim() == 3 and bits.shape[0] == n
+    Hr, Wr = bits.shape[1], bits.shape[2] * 8
+    if scores is None:
+        scores = torch.empty(n, device=logits.device, dtype=torch.float32)
+    if boxes is None:
+        boxes = torch.empty(n, 4, device=logits.device, dtype=torch.float32)
+    assert scores.is_contiguous() and boxes.is_contiguous() and scores.numel() == n and boxes.numel() == 4 * n
+    part = torch.empty(n * ((Hr + 15) // 16) * 6, device=logits.device, dtype=torch.float32)
+    _check(_lib.rsp_query_postprocess_rescale_bits(_ptr(logits), _ptr(sel), _ptr(cls_scores), n, hm, wm, batch_hw[0],
+                                                   batch_hw[1], crop_hw[0], crop_hw[1], H, W, Hr, Wr, _ptr(bits),
+                                                   _ptr(part), _ptr(scores), _ptr(boxes), _stream()),
+           "rsp_query_postprocess_rescale_bits")
+    launch_count += 2
+    return bits, scores, boxes
+
+
 def pack_mask_bits(masks: torch.Tensor, bits: torch.Tensor | None = None) -> torch.Tensor:
     """bool / uint8 [..., W] -> uint8 [..., ceil(W/8)], pixel x = bit x % 8 of byte x // 8."""
     global launch_count
@@ -1124,6 +1178,28 @@ def preprocess_u8(img: torch.Tensor, out: torch.Tensor, mean, std, swap_rb: bool
     sc, sy, sx = img.stride()
     _check(_lib.rsp_preprocess_u8(_ptr(img), h, w, sc, sy, sx, _ptr(out), out.shape[1], out.shape[2], _host_f3(mean),
                                   _host_f3(std), int(swap_rb), float(pad_value), _stream()), "rsp_preprocess_u8")
+    launch_count += 1
+    return out
+
+
+def resize_pad_u8(imgs: list, sizes: list, out: torch.Tensor, mean, std, swap_rb: bool, pad) -> torch.Tensor:
+    """The keep-ratio Resize + Pad + normalisation of a batch in one launch: imgs = uint8 [3, h, w] device views (any
+    strides: CHW planes, permuted HWC arrays, tile views of a scene), sizes = (new_h, new_w) per image, out fp32
+    [B, 3, Hp, Wp]; pad = 3 raw pad values in input channel order."""
+    global launch_count
+    _require_cuda(out, *imgs)
+    B = len(imgs)
+    assert B == len(sizes) == out.shape[0] and B > 0
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.dim() == 4 and out.shape[1] == 3
+    rows = []
+    for t, (nh, nw) in zip(imgs, sizes):
+        assert t.dtype == torch.uint8 and t.dim() == 3 and t.shape[0] == 3
+        rows.append([t.data_ptr(), *t.stride(), t.shape[1], t.shape[2], int(nh), int(nw)])
+    host = torch.tensor(rows, dtype=torch.int64).pin_memory()
+    desc = host.to(out.device, non_blocking=True)
+    _check(_lib.rsp_resize_pad_u8(_ptr(desc), host.data_ptr(), B, _ptr(out), out.shape[2], out.shape[3],
+                                  _host_f3(mean), _host_f3(std), int(swap_rb), _host_f3(pad), _stream()),
+           "rsp_resize_pad_u8")
     launch_count += 1
     return out
 

@@ -344,6 +344,19 @@ int rsp_mask_paste_bits(const float* maps, uint8_t* bits, int n, int hm, int wm,
   return mask_paste_bits(maps, bits, n, hm, wm, thr, mode, S(stream));
 }
 
+int rsp_mask_paste_rescale_bits(const float* maps, uint8_t* bits, int n, int hm, int wm, int Hb, int Wb, int crop_h,
+                                int crop_w, int H, int W, int Hr, int Wr, float thr, int mode, void* stream) {
+  return mask_paste_rescale_bits(maps, bits, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, Hr, Wr, thr, mode, S(stream));
+}
+
+int rsp_query_postprocess_rescale_bits(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst,
+                                       int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr,
+                                       int Wr, uint8_t* bits, float* part_ws, float* scores, float* boxes,
+                                       void* stream) {
+  return query_postprocess_rescale_bits(logits, sel, cls_scores, n_inst, hm, wm, Hb, Wb, crop_h, crop_w, H, W, Hr, Wr,
+                                        bits, part_ws, scores, boxes, S(stream));
+}
+
 }  // extern "C"
 
 #include "records.h"
@@ -362,6 +375,12 @@ int rsp_preprocess_u8(const uint8_t* img, int h, int w, long long stride_c, long
                       float* out, int H, int W, const float* mean3, const float* std3, int swap_rb, float pad_value,
                       void* stream) {
   return preprocess_u8(img, h, w, stride_c, stride_y, stride_x, out, H, W, mean3, std3, swap_rb, pad_value, S(stream));
+}
+
+int rsp_resize_pad_u8(const int64_t* desc, const int64_t* desc_host, int B, float* out, int Hp, int Wp,
+                      const float* mean3, const float* std3, int swap_rb, const float* pad3, void* stream) {
+  return resize_pad_u8(reinterpret_cast<const long long*>(desc), reinterpret_cast<const long long*>(desc_host), B, out,
+                       Hp, Wp, mean3, std3, swap_rb, pad3, S(stream));
 }
 
 int rsp_patchify16_u8(const uint8_t* img, int hwc, void* out, int B, int H, int W, const float* mean3, const float* std3,

@@ -553,6 +553,47 @@ int mask_paste_rescale(const float* maps, unsigned char* out, int n, int hm, int
   return RSP_OK;
 }
 
+// ... bit-packed into record slots of Hr x Wr (Wr % 16 == 0): thread = 16 pixels of one row, one uint16 store; the
+// (H, W) mask sits at the slot's top-left, pixels outside it are 0.  Per pixel the value is resize2_at, as above.
+template <int MODE>
+__global__ void mask_paste_rescale_bits_kernel(const float* __restrict__ maps, unsigned char* __restrict__ bits, int n,
+                                               Resize2 g, int Hr, int Wr, float thr) {
+  const int w16 = Wr / 16;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= static_cast<long long>(n) * Hr * w16) return;
+  const int xb = static_cast<int>(idx % w16);
+  long long t = idx / w16;
+  const int y = static_cast<int>(t % Hr);
+  const int m = static_cast<int>(t / Hr);
+  const float* src = maps + static_cast<size_t>(m) * g.hm * g.wm;
+  uint32_t word = 0u;
+  if (y < g.H) {
+#pragma unroll 4
+    for (int k = 0; k < 16; ++k) {
+      const int x = 16 * xb + k;
+      if (x >= g.W) break;
+      const float v = resize2_at(src, g, y, x);
+      word |= ((MODE == 1 ? (v > thr) : (v >= thr)) ? 1u : 0u) << k;
+    }
+  }
+  *reinterpret_cast<uint16_t*>(bits + (static_cast<size_t>(m) * Hr + y) * (Wr / 8) + 2 * xb) = static_cast<uint16_t>(word);
+}
+
+int mask_paste_rescale_bits(const float* maps, unsigned char* bits, int n, int hm, int wm, int Hb, int Wb, int crop_h,
+                            int crop_w, int H, int W, int Hr, int Wr, float thr, int mode, cudaStream_t stream) {
+  RSP_CHECK_ARG(maps && bits && n > 0 && hm > 0 && wm > 0 && Hb > 0 && Wb > 0 && crop_h > 0 && crop_w > 0 &&
+                crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 && H <= Hr && W <= Wr && Wr % 16 == 0 &&
+                (reinterpret_cast<uintptr_t>(bits) & 1) == 0 && (mode == 1 || mode == 2),
+                "mask_paste_rescale_bits: bad args (H <= Hr, W <= Wr, Wr % 16 == 0, 2-byte aligned bits; mode 1 or 2)");
+  Resize2 g{hm, wm, Hb, Wb, crop_h, crop_w, H, W};
+  const long long total = static_cast<long long>(n) * Hr * (Wr / 16);
+  const unsigned blocks = static_cast<unsigned>((total + 255) / 256);
+  if (mode == 1) mask_paste_rescale_bits_kernel<1><<<blocks, 256, 0, stream>>>(maps, bits, n, g, Hr, Wr, thr);
+  else mask_paste_rescale_bits_kernel<2><<<blocks, 256, 0, stream>>>(maps, bits, n, g, Hr, Wr, thr);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
 // FCNMaskHead paste (fcn_mask_head.py:_do_paste_mask + the threshold of _predict_by_feat_single :388-392): the
 // activated RoI mask probs fp32 [n, hm, wm] of detection i are sampled bilinearly (F.grid_sample, align_corners=False,
 // zero padding) at every image pixel centre mapped into its box, then compared with thr.  thread = 16 output pixels of

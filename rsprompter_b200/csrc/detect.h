@@ -22,6 +22,8 @@ int roi_align_nhwc(const void* const* feats, const float* const* pes, const int*
                    float finest_scale, void* out, cudaStream_t stream);
 int mask_paste_rescale(const float* maps, unsigned char* out, int n, int hm, int wm, int Hb, int Wb, int crop_h,
                        int crop_w, int H, int W, float thr, int mode, cudaStream_t stream);
+int mask_paste_rescale_bits(const float* maps, unsigned char* bits, int n, int hm, int wm, int Hb, int Wb, int crop_h,
+                            int crop_w, int H, int W, int Hr, int Wr, float thr, int mode, cudaStream_t stream);
 int mask_paste(const float* logits, unsigned char* out, int n, int hm, int wm, int H, int W, float thr,
                int mode, cudaStream_t stream);
 int mask_paste_bits(const float* maps, unsigned char* bits, int n, int hm, int wm, float thr, int mode,

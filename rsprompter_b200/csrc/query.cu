@@ -918,6 +918,65 @@ __global__ void query_mask_rescale_kernel(const float* __restrict__ logits, cons
   }
 }
 
+// ... bit-packed into record slots of Hr x Wr (Wr % 16 == 0), the (H, W) mask at the slot's top-left and 0 elsewhere.
+// The pixel -> thread assignment and the reductions are those of query_mask_rescale_kernel, so scores and boxes are
+// bit-identical to it; the bits of the block's 16 rows collect in a shared bitmap (16 x Wr/32 words) and leave as
+// one uint16 store per 16 pixels.
+__global__ void query_mask_rescale_bits_kernel(const float* __restrict__ logits, const int* __restrict__ sel, Resize2 g,
+                                               int Hr, int Wr, unsigned char* __restrict__ bits,
+                                               float* __restrict__ part) {
+  extern __shared__ uint32_t s_bits[];                 // [QP_ROWS][Wr / 32]
+  const int words = Wr / 32 + (Wr % 32 ? 1 : 0);
+  for (int i = threadIdx.x; i < QP_ROWS * words; i += blockDim.x) s_bits[i] = 0u;
+  __syncthreads();
+  const int inst = blockIdx.y;
+  const float* src = logits + static_cast<size_t>(sel[inst]) * g.hm * g.wm;
+  float sum = 0.f;
+  int cnt = 0, minx = g.W, maxx = -1, miny = g.H, maxy = -1;
+  const int y_base = blockIdx.x * QP_ROWS;
+  for (int i = threadIdx.x; i < QP_ROWS * g.W; i += blockDim.x) {
+    const int y = y_base + i / g.W, x = i % g.W;
+    if (y >= g.H) break;
+    const float v = resize2_at(src, g, y, x);
+    if (v > 0.f) {
+      atomicOr(&s_bits[(y - y_base) * words + (x >> 5)], 1u << (x & 31));
+      sum += __fdividef(1.f, 1.f + __expf(-v));   // fast sigmoid: ~2 ulp, the sum is an average over >= 1e3 pixels
+      ++cnt;
+      minx = min(minx, x); maxx = max(maxx, x); miny = min(miny, y); maxy = max(maxy, y);
+    }
+  }
+  __shared__ float s_sum[256];
+  __shared__ int s_i[256][5];
+  s_sum[threadIdx.x] = sum;
+  s_i[threadIdx.x][0] = cnt; s_i[threadIdx.x][1] = minx; s_i[threadIdx.x][2] = maxx;
+  s_i[threadIdx.x][3] = miny; s_i[threadIdx.x][4] = maxy;
+  __syncthreads();
+  for (int i = threadIdx.x; i < QP_ROWS * (Wr / 16); i += blockDim.x) {
+    const int r = i / (Wr / 16), k = i % (Wr / 16);
+    const int y = y_base + r;
+    if (y >= Hr) break;
+    const uint32_t w = s_bits[r * words + (k >> 1)];
+    *reinterpret_cast<uint16_t*>(bits + (static_cast<size_t>(inst) * Hr + y) * (Wr / 8) + 2 * k) =
+        static_cast<uint16_t>(k & 1 ? w >> 16 : w);
+  }
+  for (int s = blockDim.x / 2; s > 0; s >>= 1) {
+    if (threadIdx.x < s) {
+      s_sum[threadIdx.x] += s_sum[threadIdx.x + s];
+      s_i[threadIdx.x][0] += s_i[threadIdx.x + s][0];
+      s_i[threadIdx.x][1] = min(s_i[threadIdx.x][1], s_i[threadIdx.x + s][1]);
+      s_i[threadIdx.x][2] = max(s_i[threadIdx.x][2], s_i[threadIdx.x + s][2]);
+      s_i[threadIdx.x][3] = min(s_i[threadIdx.x][3], s_i[threadIdx.x + s][3]);
+      s_i[threadIdx.x][4] = max(s_i[threadIdx.x][4], s_i[threadIdx.x + s][4]);
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    float* o = part + (static_cast<size_t>(inst) * gridDim.x + blockIdx.x) * 6;
+    o[0] = s_sum[0]; o[1] = static_cast<float>(s_i[0][0]); o[2] = static_cast<float>(s_i[0][1]);
+    o[3] = static_cast<float>(s_i[0][2]); o[4] = static_cast<float>(s_i[0][3]); o[5] = static_cast<float>(s_i[0][4]);
+  }
+}
+
 __global__ void query_finalize_kernel(const float* __restrict__ part, int nblk, const float* __restrict__ cls_scores,
                                       int n_inst, int W, int H, float* __restrict__ scores, float* __restrict__ boxes) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -974,6 +1033,27 @@ int query_postprocess_rescale(const float* logits, const int* sel, const float* 
   const int nblk = (H + QP_ROWS - 1) / QP_ROWS;
   dim3 grid(nblk, n_inst);
   query_mask_rescale_kernel<<<grid, 256, 0, stream>>>(logits, sel, g, masks, part_ws);
+  RSP_CHECK_LAUNCH();
+  query_finalize_kernel<<<(n_inst + 127) / 128, 128, 0, stream>>>(part_ws, nblk, cls_scores, n_inst, W, H, scores, boxes);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
+int query_postprocess_rescale_bits(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm,
+                                   int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr, int Wr,
+                                   unsigned char* bits, float* part_ws, float* scores, float* boxes,
+                                   cudaStream_t stream) {
+  RSP_CHECK_ARG(logits && sel && cls_scores && bits && part_ws && scores && boxes && n_inst > 0 && crop_h > 0 &&
+                crop_w > 0 && crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 && H <= Hr && W <= Wr &&
+                Wr % 16 == 0 && Wr <= 16384 && (reinterpret_cast<uintptr_t>(bits) & 1) == 0,
+                "query_postprocess_rescale_bits: bad args (H <= Hr, W <= Wr, Wr % 16 == 0, Wr <= 16384, 2-byte "
+                "aligned bits)");
+  Resize2 g{hm, wm, Hb, Wb, crop_h, crop_w, H, W};
+  // blocks past row H contribute empty partials (+0 to the sums): scores equal query_postprocess_rescale's
+  const int nblk = (Hr + QP_ROWS - 1) / QP_ROWS;
+  dim3 grid(nblk, n_inst);
+  const size_t smem = QP_ROWS * ((Wr + 31) / 32) * sizeof(uint32_t);
+  query_mask_rescale_bits_kernel<<<grid, 256, smem, stream>>>(logits, sel, g, Hr, Wr, bits, part_ws);
   RSP_CHECK_LAUNCH();
   query_finalize_kernel<<<(n_inst + 127) / 128, 128, 0, stream>>>(part_ws, nblk, cls_scores, n_inst, W, H, scores, boxes);
   RSP_CHECK_LAUNCH();

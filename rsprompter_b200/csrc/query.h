@@ -21,5 +21,9 @@ int query_postprocess_bits(const float* logits, const int* sel, const float* cls
 int query_postprocess_rescale(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm,
                               int Hb, int Wb, int crop_h, int crop_w, int H, int W, unsigned char* masks, float* part_ws,
                               float* scores, float* boxes, cudaStream_t stream);
+int query_postprocess_rescale_bits(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm,
+                                   int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr, int Wr,
+                                   unsigned char* bits, float* part_ws, float* scores, float* boxes,
+                                   cudaStream_t stream);
 
 }  // namespace rsp

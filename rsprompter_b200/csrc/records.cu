@@ -117,6 +117,79 @@ int preprocess_u8(const unsigned char* img, int h, int w, long long stride_c, lo
   return RSP_OK;
 }
 
+// cv::resize INTER_LINEAR source tap of output index d along one axis (imgproc/src/resize.cpp, resizeGeneric's
+// coefficient loop): f = (float)((d + 0.5) * scale - 0.5) with scale = 1 / (new / old) in double, i = floor(f),
+// a = f - i; at either border the tap is clamped to (0, 0) / (old - 1, 0).  Explicit _rn intrinsics: no contraction.
+__device__ __forceinline__ void cv_linear_tap(int d, int n_new, int n_old, int& i, float& a) {
+  const double scale = __ddiv_rn(1.0, __ddiv_rn(static_cast<double>(n_new), static_cast<double>(n_old)));
+  const float f = __double2float_rn(__dsub_rn(__dmul_rn(static_cast<double>(d) + 0.5, scale), 0.5));
+  const float fl = floorf(f);
+  i = static_cast<int>(fl);
+  a = __fsub_rn(f, fl);
+  if (i < 0) { i = 0; a = 0.f; }
+  if (i >= n_old - 1) { i = n_old - 1; a = 0.f; }
+}
+
+// grid (pixels of the padded plane / 256, images); desc int64 [B, 8] per image = (source address, byte strides c, y,
+// x, h, w, new_h, new_w).  thread = one output pixel, 3 channel planes written.  Horizontal pass then vertical pass,
+// (1 - a) * p[i] + a * p[i + 1] in fp32, as cv2's HResizeLinear / VResizeLinear compute it for float images; then the
+// normalisation of preprocess_u8.  Outside (new_h, new_w): pad3 (input channel order) normalised the same way.
+__global__ void resize_pad_u8_kernel(const long long* __restrict__ desc, float* __restrict__ out, int Hp, int Wp,
+                                     Norm3 nm, int swap_rb, Norm3 pad) {
+  const long long plane = static_cast<long long>(Hp) * Wp;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= plane) return;
+  const long long* d = desc + static_cast<size_t>(blockIdx.y) * 8;
+  const int x = static_cast<int>(idx % Wp), y = static_cast<int>(idx / Wp);
+  const int h = static_cast<int>(d[4]), w = static_cast<int>(d[5]), nh = static_cast<int>(d[6]),
+            nw = static_cast<int>(d[7]);
+  float v[3];
+  if (y < nh && x < nw) {
+    const unsigned char* img = reinterpret_cast<const unsigned char*>(d[0]);
+    const long long sc = d[1], sy = d[2], sx = d[3];
+    int ix, iy;
+    float ax, ay;
+    cv_linear_tap(x, nw, w, ix, ax);
+    cv_linear_tap(y, nh, h, iy, ay);
+    const int ix1 = min(ix + 1, w - 1), iy1 = min(iy + 1, h - 1);
+    const float bx = __fsub_rn(1.f, ax), by = __fsub_rn(1.f, ay);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const unsigned char* p = img + (swap_rb ? 2 - c : c) * sc;
+      const unsigned char* r0 = p + iy * sy;
+      const unsigned char* r1 = p + iy1 * sy;
+      const float h0 = __fadd_rn(__fmul_rn(static_cast<float>(r0[ix * sx]), bx), __fmul_rn(static_cast<float>(r0[ix1 * sx]), ax));
+      const float h1 = __fadd_rn(__fmul_rn(static_cast<float>(r1[ix * sx]), bx), __fmul_rn(static_cast<float>(r1[ix1 * sx]), ax));
+      const float u = __fadd_rn(__fmul_rn(h0, by), __fmul_rn(h1, ay));
+      v[c] = __fdiv_rn(__fsub_rn(u, nm.mean[c]), nm.stdv[c]);
+    }
+  } else {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = __fdiv_rn(__fsub_rn(pad.mean[swap_rb ? 2 - c : c], nm.mean[c]), nm.stdv[c]);
+  }
+  float* o = out + static_cast<size_t>(blockIdx.y) * 3 * plane + idx;
+  o[0] = v[0]; o[plane] = v[1]; o[2 * plane] = v[2];
+}
+
+int resize_pad_u8(const long long* desc, const long long* desc_host, int B, float* out, int Hp, int Wp,
+                  const float* mean3, const float* std3, int swap_rb, const float* pad3, cudaStream_t stream) {
+  RSP_CHECK_ARG(desc && desc_host && out && mean3 && std3 && pad3 && B > 0 && B <= 65535 && Hp > 0 && Wp > 0,
+                "resize_pad_u8: bad args");
+  for (int b = 0; b < B; ++b) {
+    const long long* d = desc_host + static_cast<size_t>(b) * 8;
+    RSP_CHECK_ARG(d[0] != 0 && d[1] > 0 && d[2] > 0 && d[3] > 0 && d[4] > 0 && d[5] > 0 && d[6] > 0 && d[7] > 0 &&
+                  d[6] <= Hp && d[7] <= Wp && d[4] < (1LL << 31) && d[5] < (1LL << 31),
+                  "resize_pad_u8: bad descriptor (positive strides and sizes, the resized image inside the pad size)");
+  }
+  Norm3 nm{{mean3[0], mean3[1], mean3[2]}, {std3[0], std3[1], std3[2]}};
+  Norm3 pad{{pad3[0], pad3[1], pad3[2]}, {0.f, 0.f, 0.f}};
+  const long long plane = static_cast<long long>(Hp) * Wp;
+  dim3 grid(static_cast<unsigned>((plane + 255) / 256), static_cast<unsigned>(B));
+  resize_pad_u8_kernel<<<grid, 256, 0, stream>>>(desc, out, Hp, Wp, nm, swap_rb, pad);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
 __device__ __forceinline__ void store_patch_seg(__nv_bfloat16* dst, const float f[16]) {
   reinterpret_cast<uint4*>(dst)[0] = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]),
                                                 pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));

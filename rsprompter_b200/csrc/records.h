@@ -8,6 +8,8 @@ int unpack_mask_bits(const unsigned char* bits, unsigned char* masks, long long 
 int preprocess_u8(const unsigned char* img, int h, int w, long long stride_c, long long stride_y, long long stride_x,
                   float* out, int H, int W, const float* mean3, const float* std3, int swap_rb, float pad_value,
                   cudaStream_t stream);
+int resize_pad_u8(const long long* desc, const long long* desc_host, int B, float* out, int Hp, int Wp,
+                  const float* mean3, const float* std3, int swap_rb, const float* pad3, cudaStream_t stream);
 int patchify16_u8(const unsigned char* img, int hwc, void* out, int B, int H, int W, const float* mean3,
                   const float* std3, int swap_rb, cudaStream_t stream);
 

@@ -159,6 +159,35 @@ class _SamDetectorBase(BaseModule):
             out.append(dict(ori_hw=ori, crop_hw=crop, scale_factor=sf))
         return hw, out
 
+    def _record_metas(self, batch_data_samples, batch_inputs, record):
+        """predict_records with data samples -> (batch_inputs, metas, record hw).  metas is None when every image is at
+        the batch shape with scale 1 (the batch-shape record path); otherwise the per-image _metas of resized images
+        that all share one ori_shape, whose masks the record holds at its slots' top-left: record.hw must cover
+        ori_shape (a new record is ori_shape with the width rounded up to 16, the bit kernels' store width)."""
+        if batch_data_samples is None:
+            return batch_inputs, None, None
+        hw, metas = self._metas(batch_data_samples, batch_inputs)
+        batch_inputs = self._attach_img_shapes(batch_data_samples, batch_inputs)
+        if all(m is None for m in metas):
+            return batch_inputs, None, None
+        oris = {hw if m is None else m["ori_hw"] for m in metas}
+        if len(oris) != 1:
+            raise ValueError(f"predict_records writes one record shape: every image must share one ori_shape, got "
+                             f"{sorted(oris)}")
+        metas = [m or dict(ori_hw=hw, crop_hw=hw, scale_factor=(1.0, 1.0)) for m in metas]
+        ori = metas[0]["ori_hw"]
+        rhw = tuple(record.hw) if record is not None else (ori[0], (ori[1] + 15) // 16 * 16)
+        if ori[0] > rhw[0] or ori[1] > rhw[1] or rhw[1] % 16:
+            raise ValueError(f"a record of {rhw} cannot hold masks of ori_shape {ori} (needs H, W >= ori_shape and "
+                             f"W % 16 == 0)")
+        return batch_inputs, metas, rhw
+
+    @staticmethod
+    def _rescaled_boxes(boxes: torch.Tensor, metas: list) -> torch.Tensor:
+        """boxes [B, M, 4] / scale_factor per image, the fp32 division predict(rescale=True) does."""
+        sf = torch.tensor([list(m["scale_factor"]) * 2 for m in metas], dtype=torch.float32)
+        return boxes / sf.to(boxes.device, non_blocking=True)[:, None, :]
+
     @staticmethod
     def _rle_masks(test_cfg, batch_data_samples):
         """With test_cfg.rle_masks, every pred_instances.masks becomes a list of COCO RLE dicts ({'size': [h, w],
@@ -241,16 +270,28 @@ class RSPrompterAnchor(_SamDetectorBase):
         return self._rle_masks(self.test_cfg, batch_data_samples)
 
     @torch.no_grad()
-    def predict_records(self, batch_inputs: torch.Tensor, record: ResultRecord | None = None) -> ResultRecord:
-        """predict() for images at the batch shape with the result left on the device as one ResultRecord
-        (bit-packed masks + rows + counts): what a distributed test loop gathers / copies to the host."""
+    def predict_records(self, batch_inputs: torch.Tensor, record: ResultRecord | None = None,
+                        batch_data_samples=None) -> ResultRecord:
+        """predict() with the result left on the device as one ResultRecord (bit-packed masks + rows + counts): what a
+        distributed test loop gathers / copies to the host.  Without samples the images are at the batch shape; with
+        samples of resized images (one shared ori_shape) the rows and masks are in original-image coordinates, as
+        predict(rescale=True) returns them."""
+        batch_inputs, metas, rhw = self._record_metas(batch_data_samples, batch_inputs, record)
         r = self._raw(batch_inputs)
         hw = tuple(int(v) for v in batch_inputs.shape[-2:])
         B, M = r["scores"].shape
-        rec = record or self._new_record(B, M, hw, r["scores"].device)
+        rec = record or self._new_record(B, M, rhw or hw, r["scores"].device)
         thr = float(self.test_cfg.rcnn.get("mask_thr_binary", 0.5))
-        _lib.mask_paste_bits(r["mask_logits"][:, 0].contiguous(), thr, 0, bits=rec.mask_bits)
-        torch.cat([r["bboxes"], r["scores"][..., None], r["labels"].to(torch.float32)[..., None]], dim=2, out=rec.rows)
+        boxes = r["bboxes"]
+        if metas is None:
+            _lib.mask_paste_bits(r["mask_logits"][:, 0].contiguous(), thr, 0, bits=rec.mask_bits)
+        else:
+            logits = r["mask_logits"][:, 0].contiguous()
+            for b, m in enumerate(metas):
+                _lib.mask_paste_rescale_bits(logits[b * M:(b + 1) * M], hw, m["crop_hw"], m["ori_hw"], thr,
+                                             bits=rec.mask_bits.view(B * M, *rec.mask_bits.shape[2:])[b * M:(b + 1) * M])
+            boxes = self._rescaled_boxes(boxes, metas)
+        torch.cat([boxes, r["scores"][..., None], r["labels"].to(torch.float32)[..., None]], dim=2, out=rec.rows)
         rec.counts.copy_(r["counts"])
         return rec
 
@@ -320,14 +361,17 @@ class RSPrompterQuery(_SamDetectorBase):
         return self._rle_masks(self.test_cfg, batch_data_samples)
 
     @torch.no_grad()
-    def predict_records(self, batch_inputs: torch.Tensor, record: ResultRecord | None = None) -> ResultRecord:
-        """predict() for images at the batch shape with the result left on the device as one ResultRecord."""
+    def predict_records(self, batch_inputs: torch.Tensor, record: ResultRecord | None = None,
+                        batch_data_samples=None) -> ResultRecord:
+        """predict() with the result left on the device as one ResultRecord; images at the batch shape, or with
+        samples of resized images (one shared ori_shape) in original-image coordinates (RSPrompterAnchor's)."""
+        batch_inputs, metas, rhw = self._record_metas(batch_data_samples, batch_inputs, record)
         r = self._raw(batch_inputs)
         hw = tuple(int(v) for v in batch_inputs.shape[-2:])
         B = r["cls"].shape[0]
         K = int(self.test_cfg.get("max_per_image", 100))
-        rec = record or self._new_record(B, K, hw, r["cls"].device)
-        self.panoptic_fusion_head.instance_postprocess_record(r["cls"], r["mask_logits"], rec)
+        rec = record or self._new_record(B, K, rhw or hw, r["cls"].device)
+        self.panoptic_fusion_head.instance_postprocess_record(r["cls"], r["mask_logits"], rec, metas=metas, size=hw)
         return rec
 
     def forward(self, inputs, data_samples=None, mode: str = "predict"):
@@ -426,15 +470,22 @@ class SAMSegMaskRCNN(_SamDetectorBase):
         return self._rle_masks(self.test_cfg, batch_data_samples)
 
     @torch.no_grad()
-    def predict_records(self, batch_inputs: torch.Tensor, record: ResultRecord | None = None) -> ResultRecord:
-        """predict() for images at the batch shape, left on the device as one ResultRecord."""
+    def predict_records(self, batch_inputs: torch.Tensor, record: ResultRecord | None = None,
+                        batch_data_samples=None) -> ResultRecord:
+        """predict() left on the device as one ResultRecord; images at the batch shape, or with samples of resized
+        images (one shared ori_shape) in original-image coordinates: the RoI masks are pasted into the rescaled boxes
+        on the record's canvas (fcn_mask_head.py:333-343), which agrees with predict() on ori_shape."""
+        batch_inputs, metas, rhw = self._record_metas(batch_data_samples, batch_inputs, record)
         r = self._raw(batch_inputs)
         hw = tuple(int(v) for v in batch_inputs.shape[-2:])
         B, M = r["scores"].shape
-        rec = record or self._new_record(B, M, hw, r["scores"].device)
+        rec = record or self._new_record(B, M, rhw or hw, r["scores"].device)
         thr = float(self.test_cfg.rcnn.get("mask_thr_binary", 0.5))
-        _lib.mask_paste_boxes(r["mask_probs"], r["bboxes"].reshape(B * M, 4), hw, thr, bits=rec.mask_bits)
-        torch.cat([r["bboxes"], r["scores"][..., None], r["labels"].to(torch.float32)[..., None]], dim=2, out=rec.rows)
+        boxes = r["bboxes"]
+        if metas is not None:
+            boxes = self._rescaled_boxes(boxes, metas)
+        _lib.mask_paste_boxes(r["mask_probs"], boxes.reshape(B * M, 4).contiguous(), rec.hw, thr, bits=rec.mask_bits)
+        torch.cat([boxes, r["scores"][..., None], r["labels"].to(torch.float32)[..., None]], dim=2, out=rec.rows)
         rec.counts.copy_(r["counts"])
         return rec
 

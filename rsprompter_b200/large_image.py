@@ -7,7 +7,9 @@ merged with one class-aware NMS (``merge_results_by_nms``).  Here all of it stay
 
   * tiles are copied out of the scene in batches and normalised by the detector's own DetDataPreprocessor path
     (the fused uint8 patch-embed loader, or ``rsp_preprocess_u8`` for tiles that overhang a scene smaller than
-    the patch, padded with 0 after normalisation as BatchFixedSizePad pads);
+    the patch, padded with 0 after normalisation as BatchFixedSizePad pads); with an explicit patch size
+    (the demo's ``--patch-size``) every window is resized to the model size by ``rsp_resize_pad_u8`` straight
+    from the scene, as the test pipeline's keep-ratio Resize + Pad does;
   * every batch leaves ``predict_records`` as one ResultRecord, resident until the merge;
   * the merge is ``rsp_nms_batched`` + ``rsp_compact_keep`` over every valid slot of every tile (mmcv
     ``batched_nms`` semantics, label offset included);
@@ -59,7 +61,7 @@ def slice_origins(hw: tuple, patch: int, overlap_ratio: float) -> list:
 
 
 def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_thr: float = 0.25,
-                       score_thr: float = 0.0) -> dict:
+                       score_thr: float = 0.0, window: tuple | None = None) -> dict:
     """Class-aware NMS of every valid slot of every tile, in scene coordinates.
 
     ``records`` are ResultRecords of tiles (one image per tile; records of one call share slots and device) and
@@ -68,7 +70,9 @@ def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_
     shift_bboxes) and clipped to the tile's window intersected with the scene, a no-op for a box inside its tile.
     The candidates are sorted by score, ties by (tile, slot), and merged as mmcv batched_nms(boxes, scores, labels,
     iou_threshold=merge_iou_thr).  Candidates below ``score_thr`` are dropped first; greedy NMS lets a box suppress
-    only lower-scored boxes, so that is exactly the unfiltered result restricted to score >= score_thr.
+    only lower-scored boxes, so that is exactly the unfiltered result restricted to score >= score_thr.  ``window``
+    (h, w) is the tile size when it differs from the records' canvas (resized patches: the canvas width is rounded
+    up to 16).
 
     Returns dict(bboxes fp32 [k, 4], scores [k], labels int64 [k] on the device, in descending score order, and
     source int64 [k, 3] on the host: (record, image, slot) of each kept row).  One host synchronisation."""
@@ -81,7 +85,7 @@ def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_
         n = len(org)
         rows.append(rec.rows[:n])
         counts.append(rec.counts[:n])
-        ph, pw = rec.hw
+        ph, pw = window or rec.hw
         for b, (x0, y0) in enumerate(org):
             win.append((x0, y0, min(x0 + pw, W), min(y0 + ph, H)))
             src.append((r, b))
@@ -124,28 +128,34 @@ def _slots(model) -> int:
     return int(model.test_cfg.rcnn.get("max_per_img", 100))
 
 
-def _record_nbytes(B: int, M: int, P: int) -> int:
-    return _align16(B * M * P * (P // 8)) + _align16(B * M * 24) + _align16(B * 4)
+def _record_nbytes(B: int, M: int, hw: tuple) -> int:
+    return _align16(B * M * hw[0] * (hw[1] // 8)) + _align16(B * M * 24) + _align16(B * 4)
 
 
 @torch.no_grad()
 def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr: float = 0.25,
-                        score_thr: float = 0.0, batch_size: int = 8) -> DetDataSample:
+                        score_thr: float = 0.0, batch_size: int = 8, patch_size: int | None = None) -> DetDataSample:
     """Detect a whole scene: slice, run the tiles in batches, merge across tiles, encode the kept masks.
 
     ``image`` is the scene as mmcv.imread decodes it, uint8 [H, W, 3] BGR: a numpy array or a tensor on the host
-    (copied to the device once, pinned) or on the model's device.  Tiles are model-size (``image_size``) windows,
-    never resized.  The last partial batch repeats a tile whose slots are ignored, so every batch has one shape and
-    enable_cuda_graphs() replays one graph.  No host synchronisation happens per tile or per batch; the merge reads
-    the kept rows once and the RLE encode synchronises twice.
+    (copied to the device once, pinned) or on the model's device.  With ``patch_size=None`` tiles are model-size
+    (``image_size``) windows, never resized.  An explicit ``patch_size`` P cuts P x P windows and resizes each (its
+    in-scene part when the scene is smaller than P) to the model size the way the test pipeline's keep-ratio Resize
+    + Pad does (the reference demo's ``--patch-size``, whose inference_detector runs every slice through that
+    pipeline); P = image_size on a scene at least that large is the unresized path.  The last partial batch repeats
+    a tile whose slots are ignored, so every batch has one shape and enable_cuda_graphs() replays one graph.  No
+    host synchronisation happens per tile or per batch; the merge reads the kept rows once and the RLE encode
+    synchronises twice.
 
     Returns a DetDataSample with ori_shape = img_shape = (H, W), scale_factor (1, 1) and pred_instances: bboxes,
     scores, labels on the device in descending score order, masks a list of {'size': [H, W], 'counts': bytes} (the
     test_cfg.rle_masks convention, passed through by CocoMetric.process)."""
-    records, batches = run_tiles(model, image, overlap_ratio, batch_size)
+    records, batches = run_tiles(model, image, overlap_ratio, batch_size, patch_size=patch_size)
     H, W = int(image.shape[0]), int(image.shape[1])
-    merged = merge_tile_records(records, batches, (H, W), merge_iou_thr=merge_iou_thr, score_thr=score_thr)
-    masks = encode_kept_masks(records, batches, merged["source"], (H, W))
+    window = None if patch_size is None else (int(patch_size), int(patch_size))
+    merged = merge_tile_records(records, batches, (H, W), merge_iou_thr=merge_iou_thr, score_thr=score_thr,
+                                window=window)
+    masks = encode_kept_masks(records, batches, merged["source"], (H, W), window=window)
     ds = DetDataSample(metainfo=dict(ori_shape=(H, W), img_shape=(H, W), scale_factor=(1.0, 1.0)))
     ds.pred_instances = InstanceData(bboxes=merged["bboxes"], scores=merged["scores"], labels=merged["labels"],
                                      masks=masks)
@@ -153,8 +163,10 @@ def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr
 
 
 @torch.no_grad()
-def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8):
-    """The tile stage of predict_large_image -> (records, origins per record), everything left on the device."""
+def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8, patch_size: int | None = None):
+    """The tile stage of predict_large_image -> (records, origins per record), everything left on the device.
+    Records of resized patches hold each tile's result in P x P window coordinates on a canvas of
+    (P, P rounded up to 16)."""
     if not isinstance(model, (RSPrompterAnchor, RSPrompterQuery, SAMSegMaskRCNN)):
         raise NotImplementedError(f"large-scene inference needs a detector with per-tile result records "
                                   f"(RSPrompterAnchor, RSPrompterQuery, SAMSegMaskRCNN), not {type(model).__name__}")
@@ -166,19 +178,24 @@ def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8):
         raise ValueError(f"the scene must be uint8 [H, W, 3] (BGR, as mmcv.imread decodes it), got "
                          f"{img.dtype} {tuple(img.shape)}")
     H, W = int(img.shape[0]), int(img.shape[1])
-    P = int(model.backbone.vision_encoder.arch.image_size)
+    S = int(model.backbone.vision_encoder.arch.image_size)
+    P = S if patch_size is None else int(patch_size)
+    if P < 1:
+        raise ValueError("patch_size must be >= 1")
+    resize = patch_size is not None and (P != S or H < P or W < P)
     origins = slice_origins((H, W), P, overlap_ratio)
     B = min(batch_size, len(origins))
     batches = [origins[i:i + B] for i in range(0, len(origins), B)]
     M = _slots(model)
+    rec_hw = (P, (P + 15) // 16 * 16) if resize else (P, P)
 
     # everything that stays resident until the merge, checked before any tile runs
     N = len(origins) * M
     if N > MAX_MERGE_CANDIDATES:
         raise ValueError(f"{len(origins)} tiles x {M} slots = {N} merge candidates; the dense NMS takes at most "
                          f"{MAX_MERGE_CANDIDATES}")
-    need = (len(batches) * _record_nbytes(B, M, P) + (0 if img.is_cuda else H * W * 3)
-            + N * ((N + 63) // 64) * 8)
+    need = (len(batches) * _record_nbytes(B, M, rec_hw) + (0 if img.is_cuda else H * W * 3)
+            + N * ((N + 63) // 64) * 8 + (B * 3 * S * S * 4 if resize else 0))
     free, _ = torch.cuda.mem_get_info(dev)
     free += torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
     if need > free:
@@ -189,6 +206,8 @@ def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8):
     scene = img.to(dev) if img.is_cuda else img.pin_memory().to(dev, non_blocking=True)
     dp = model.data_preprocessor
     mean, std, swap = dp._norm3() if dp is not None else ((0.0,) * 3, (1.0,) * 3, False)
+    if resize:
+        return _run_resized_tiles(model, scene, batches, B, M, S, P, rec_hw, (mean, std, swap)), batches
     overhang = H < P or W < P
     if overhang:    # every window overhangs: normalised fp32 tiles padded with 0, clipped to their in-scene extent
         buf = torch.empty(B, 3, P, P, dtype=torch.float32, device=dev)
@@ -215,17 +234,42 @@ def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8):
     return records, batches
 
 
-def encode_kept_masks(records: list, origins: list, source: torch.Tensor, scene_hw: tuple) -> list:
+def _run_resized_tiles(model, scene, batches, B, M, S, P, rec_hw, norm):
+    """Tiles of P x P resized to the model size S by rsp_resize_pad_u8 straight from the device scene (one launch per
+    batch), then predict_records with the samples Resize + Pad would write: records in window coordinates."""
+    from .preprocess import rescale_size, resize_metainfo
+    H, W = int(scene.shape[0]), int(scene.shape[1])
+    hv, wv = min(P, H), min(P, W)                  # a window's in-scene part (sahi slices it so)
+    new_hw = rescale_size((hv, wv), (S, S))
+    meta = dict(resize_metainfo((hv, wv), new_hw, (S, S)), batch_input_shape=(S, S), pad_shape=(S, S))
+    samples = [DetDataSample(metainfo=dict(meta)) for _ in range(B)]
+    mean, std, swap = norm
+    pad = tuple(reversed(mean)) if swap else tuple(mean)    # the configs pad with the mean: 0 after normalisation
+    buf = torch.empty(B, 3, S, S, dtype=torch.float32, device=scene.device)
+    records = []
+    for org in batches:
+        tiles = org + [org[-1]] * (B - len(org))
+        views = [scene[y0:y0 + hv, x0:x0 + wv].permute(2, 0, 1) for x0, y0 in tiles]
+        _lib.resize_pad_u8(views, [new_hw] * B, buf, mean, std, swap, pad)
+        records.append(model.predict_records(buf, record=ResultRecord(B, M, rec_hw, device=scene.device),
+                                             batch_data_samples=samples))
+    return records
+
+
+def encode_kept_masks(records: list, origins: list, source: torch.Tensor, scene_hw: tuple,
+                      window: tuple | None = None) -> list:
     """COCO RLE dicts of the kept masks (``source`` rows (record, image, slot) from merge_tile_records) as masks of
-    the whole H x W scene, encoded from the records' bits; two host synchronisations."""
+    the whole H x W scene, encoded from the records' bits; two host synchronisations.  ``window`` as in
+    merge_tile_records."""
     H, W = int(scene_hw[0]), int(scene_hw[1])
     groups = []
     for r, b, s in source.tolist():
         rec = records[r]
         P, M = rec.hw[0], rec.slots
+        ph, pw = window or rec.hw
         ld = rec.hw[1] // 8
         x0, y0 = origins[r][b]
-        groups.append((rec.buf, [((b * M + s) * P * ld, ld, P, min(P, H - y0), min(rec.hw[1], W - x0), H, W, y0, x0)]))
+        groups.append((rec.buf, [((b * M + s) * P * ld, ld, P, min(ph, H - y0), min(pw, W - x0), H, W, y0, x0)]))
     return [dict(size=[H, W], counts=c) for c in _lib.mask_rle_placed(groups, packed=True)]
 
 
@@ -250,6 +294,9 @@ def main(argv=None) -> list:
     ap.add_argument("--merge-iou-thr", type=float, default=0.25)
     ap.add_argument("--score-thr", type=float, default=0.0)
     ap.add_argument("--batch-size", type=int, default=8)
+    ap.add_argument("--patch-size", type=int, default=None,
+                    help="window size; each window is resized to the model size (default: model-size windows, "
+                         "not resized)")
     ap.add_argument("--out", default=None, help="JSON file for the result dicts (default: stdout)")
     args = ap.parse_args(argv)
 
@@ -266,7 +313,7 @@ def main(argv=None) -> list:
     if img is None:
         raise FileNotFoundError(args.image)
     ds = predict_large_image(model, img, overlap_ratio=args.patch_overlap_ratio, merge_iou_thr=args.merge_iou_thr,
-                             score_thr=args.score_thr, batch_size=args.batch_size)
+                             score_thr=args.score_thr, batch_size=args.batch_size, patch_size=args.patch_size)
     res = coco_results(ds)
     text = json.dumps(res)
     if args.out:

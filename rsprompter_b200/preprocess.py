@@ -9,7 +9,14 @@ detectors (``fuse_patch_embed=True``) and the images already have the batch shap
 over with the normalisation attached (``tensor.rsp_norm``): ``rsp_patchify16_u8`` then applies it inside the
 patch-embed operand loader and the fp32 image never exists.  Float inputs keep the round-1 torch expression.
 Training-time batch augmentations (``BatchFixedSizePad`` ...) are ignored: the reference applies them only when
-``training=True`` (data_preprocessor.py:145-147)."""
+``training=True`` (data_preprocessor.py:145-147).
+
+``device_transforms=[dict(type='Resize', scale=..., keep_ratio=True), dict(type='Pad', size=..., pad_val=...)]``
+moves the test pipeline's keep-ratio Resize and Pad here: the two dicts are taken from ``test_pipeline`` unchanged
+(and ``to_float32`` dropped from LoadImageFromFile), so the original uint8 bytes of images of any size are uploaded
+with one pinned copy and resized, padded, flipped and normalised by one ``rsp_resize_pad_u8`` launch.  The resize is
+cv2's float32 INTER_LINEAR (what ``to_float32=True`` pipelines compute); the metainfo is what Resize and Pad write
+(``rescale_size`` / ``resize_metainfo`` below, the one place this rule lives)."""
 from __future__ import annotations
 
 import math
@@ -21,17 +28,67 @@ from . import _lib
 from .registry import MODELS, BaseModule, DetDataSample
 
 
+def rescale_size(hw, scale) -> tuple:
+    """mmcv rescale_size + _scale_size for Resize(scale, keep_ratio=True): (h, w) -> (new_h, new_w) with
+    s = min(max(scale) / max(h, w), min(scale) / min(h, w)) and new = int(old * s + 0.5)."""
+    h, w = int(hw[0]), int(hw[1])
+    s = min(max(scale) / max(h, w), min(scale) / min(h, w))
+    return int(h * float(s) + 0.5), int(w * float(s) + 0.5)
+
+
+def resize_metainfo(hw, new_hw, pad_hw) -> dict:
+    """What Resize + Pad write: ori_shape, scale_factor = (new_w / w, new_h / h) as Python floats, and img_shape = the
+    padded size (mmcv Pad overwrites it, mmdet transforms.py:719-724)."""
+    h, w = int(hw[0]), int(hw[1])
+    return dict(ori_shape=(h, w), scale_factor=(new_hw[1] / w, new_hw[0] / h),
+                img_shape=(int(pad_hw[0]), int(pad_hw[1])))
+
+
+def _parse_device_transforms(cfg, pad_size_divisor: int):
+    """-> (scale, (Hp, Wp), raw pad value per input channel) of [Resize(keep_ratio=True), Pad(size=...)]."""
+    cfg = [dict(t) for t in cfg]
+    kinds = [str(t.get("type", "")).split(".")[-1] for t in cfg]
+    if kinds != ["Resize", "Pad"]:
+        raise ValueError(f"device_transforms supports exactly [Resize, Pad] (the configs' test pipeline), got {kinds}")
+    rs, pd = cfg
+    extra = set(rs) - {"type", "scale", "keep_ratio", "backend", "interpolation", "clip_object_border"}
+    if extra or rs.get("scale") is None or not rs.get("keep_ratio", False):
+        raise ValueError(f"device_transforms Resize needs scale= and keep_ratio=True (no {sorted(extra) or 'other'} "
+                         f"options): {rs}")
+    if rs.get("interpolation", "bilinear") != "bilinear" or rs.get("backend", "cv2") != "cv2":
+        raise ValueError(f"device_transforms Resize reproduces cv2 bilinear only: {rs}")
+    scale = rs["scale"]
+    scale = (int(scale), int(scale)) if isinstance(scale, (int, float)) else tuple(int(s) for s in scale)
+    extra = set(pd) - {"type", "size", "pad_val", "padding_mode"}
+    if extra or pd.get("size") is None or pd.get("padding_mode", "constant") != "constant":
+        raise ValueError(f"device_transforms Pad needs size= with constant padding (no size_divisor / "
+                         f"pad_to_square): {pd}")
+    size = pd["size"]
+    Wp, Hp = (int(size), int(size)) if isinstance(size, (int, float)) else (int(size[0]), int(size[1]))
+    if Hp % pad_size_divisor or Wp % pad_size_divisor:
+        raise ValueError(f"device_transforms Pad size {size} must be a multiple of pad_size_divisor {pad_size_divisor}")
+    pv = pd.get("pad_val", 0)
+    pv = pv.get("img", 0) if isinstance(pv, dict) else pv
+    pv = tuple(float(v) for v in pv) if isinstance(pv, (tuple, list)) else (float(pv),) * 3
+    if len(pv) != 3:
+        raise ValueError(f"device_transforms Pad pad_val must be one value or three: {pd}")
+    return scale, (Hp, Wp), pv
+
+
 @MODELS.register_module(force=True)
 class DetDataPreprocessor(BaseModule):
     def __init__(self, mean=None, std=None, pad_size_divisor: int = 1, pad_value: float = 0, pad_mask: bool = False,
                  mask_pad_value: int = 0, pad_seg: bool = False, seg_pad_value: int = 255, bgr_to_rgb: bool = False,
                  rgb_to_bgr: bool = False, boxtype2tensor: bool = True, non_blocking: bool = False,
-                 batch_augments=None, init_cfg=None, **kwargs):
+                 batch_augments=None, device_transforms=None, init_cfg=None, **kwargs):
         BaseModule.__init__(self, init_cfg=None)
         assert not (bgr_to_rgb and rgb_to_bgr), "bgr_to_rgb and rgb_to_bgr cannot both be set"
         assert (mean is None) == (std is None), "mean and std come together"
         self.channel_conversion = bool(bgr_to_rgb or rgb_to_bgr)
         self.pad_size_divisor, self.pad_value = int(pad_size_divisor), float(pad_value)
+        self.device_transforms = None
+        if device_transforms:
+            self.device_transforms = _parse_device_transforms(device_transforms, self.pad_size_divisor)
         self._enable_normalize = mean is not None
         self._mean3 = self._std3 = None
         if self._enable_normalize:
@@ -63,6 +120,8 @@ class DetDataPreprocessor(BaseModule):
         if training:
             raise NotImplementedError("rsprompter_b200 implements the inference path only")
         inputs, samples = data["inputs"], data.get("data_samples")
+        if self.device_transforms is not None:
+            return self._resize_pad(inputs, samples)
         d = self.pad_size_divisor
         if isinstance(inputs, torch.Tensor):          # default_collate: already a batch [N, C, H, W]
             assert inputs.dim() == 4, "inputs must be NCHW or a list of CHW tensors"
@@ -98,5 +157,44 @@ class DetDataPreprocessor(BaseModule):
             ds.set_metainfo(dict(batch_input_shape=(H, W), pad_shape=ps))
         return dict(inputs=batch, data_samples=samples)
 
+    def _resize_pad(self, inputs, samples) -> dict:
+        """device_transforms: uint8 CHW images of any sizes -> fp32 [B, 3, Hp, Wp] by one rsp_resize_pad_u8 launch,
+        the metainfo of Resize + Pad written into the samples."""
+        scale, (Hp, Wp), pad = self.device_transforms
+        imgs = [inputs[i] for i in range(inputs.shape[0])] if isinstance(inputs, torch.Tensor) else list(inputs)
+        for t in imgs:
+            if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[0] != 3:
+                raise ValueError("device_transforms take uint8 [3, h, w] images (LoadImageFromFile without "
+                                 f"to_float32), got {getattr(t, 'dtype', type(t))} {tuple(getattr(t, 'shape', ()))}")
+        if self.device.type != "cuda":
+            raise RuntimeError("device_transforms run on the GPU: move the preprocessor to a CUDA device")
+        sizes = [rescale_size(t.shape[1:], scale) for t in imgs]
+        for t, (nh, nw) in zip(imgs, sizes):
+            if nh > Hp or nw > Wp:
+                raise ValueError(f"a {tuple(t.shape[1:])} image resized by scale {scale} is {nh} x {nw}, larger than "
+                                 f"the Pad size {Hp} x {Wp}")
+        if all(t.is_cuda for t in imgs):
+            dev = [t.to(self.device) for t in imgs]
+        else:   # the original bytes of the whole batch in one pinned host -> device copy
+            counts = [t.numel() for t in imgs]
+            host = torch.empty(sum(counts), dtype=torch.uint8, pin_memory=True)
+            offs = [0]
+            for t, n in zip(imgs, counts):
+                host[offs[-1]:offs[-1] + n].view(t.shape).copy_(t)
+                offs.append(offs[-1] + n)
+            flat = host.to(self.device, non_blocking=True)
+            dev = [flat[o:o + n].view(t.shape) for t, o, n in zip(imgs, offs, counts)]
+        batch = torch.empty((len(imgs), 3, Hp, Wp), dtype=torch.float32, device=self.device)
+        mean, std, swap = self._norm3()
+        _lib.resize_pad_u8(dev, sizes, batch, mean, std, swap, pad)
+        if samples is None:
+            samples = [DetDataSample(metainfo={}) for _ in imgs]
+        for ds, t, s in zip(samples, imgs, sizes):
+            meta = resize_metainfo(t.shape[1:], s, (Hp, Wp))
+            if "ori_shape" in ds.metainfo:
+                meta.pop("ori_shape")
+            ds.set_metainfo(dict(meta, batch_input_shape=(Hp, Wp), pad_shape=(Hp, Wp)))
+        return dict(inputs=batch, data_samples=samples)
 
-__all__ = ["DetDataPreprocessor"]
+
+__all__ = ["DetDataPreprocessor", "rescale_size", "resize_metainfo"]

@@ -445,9 +445,12 @@ class RSMaskFormerFusionHead(BaseModule):
         return dict(masks=ms, scores=ds, bboxes=bs, labels=labels, query=query, is_thing=keep_thing)
 
     @torch.no_grad()
-    def instance_postprocess_record(self, cls: torch.Tensor, mask_pred: torch.Tensor, rec) -> None:
+    def instance_postprocess_record(self, cls: torch.Tensor, mask_pred: torch.Tensor, rec, metas: list | None = None,
+                                    size: tuple | None = None) -> None:
         """instance_postprocess for images at the batch shape (4x the logit size), written into a ResultRecord: the
-        masks go out bit-packed, rows = (tight box, cls * mask score, label) (maskformer_fusion_head.py:149-182)."""
+        masks go out bit-packed, rows = (tight box, cls * mask score, label) (maskformer_fusion_head.py:149-182).
+        With ``metas`` (per-image dict(ori_hw, crop_hw) of resized images, batch shape ``size``) the masks, scores and
+        boxes are those of instance_postprocess_batched(rescale=True), written at ori_hw."""
         B, nq, _ = cls.shape
         C = self.num_classes
         K = rec.slots
@@ -456,6 +459,16 @@ class RSMaskFormerFusionHead(BaseModule):
         sc, top = scores.topk(K, dim=1, sorted=False)
         labels, query = top % C, top // C
         sel = (query + torch.arange(B, device=cls.device).view(B, 1) * nq).to(torch.int32).contiguous()
+        if metas is not None:
+            bits = rec.mask_bits.view(B * K, *rec.mask_bits.shape[2:])
+            det = torch.empty(B, K, device=cls.device, dtype=torch.float32)
+            boxes = torch.empty(B, K, 4, device=cls.device, dtype=torch.float32)
+            for b, m in enumerate(metas):
+                _lib.query_postprocess_rescale_bits(mask_pred, sel[b].contiguous(), sc[b].contiguous(), size,
+                                                    m["crop_hw"], m["ori_hw"], bits[b * K:(b + 1) * K], det[b], boxes[b])
+            torch.cat([boxes, det[..., None], labels.to(torch.float32)[..., None]], dim=2, out=rec.rows)
+            rec.counts.fill_(K)
+            return
         _, det, boxes = _lib.query_postprocess_bits(mask_pred, sel.reshape(-1), sc.reshape(-1).contiguous(),
                                                     bits=rec.mask_bits.view(B * K, rec.hw[0], rec.hw[1] // 8))
         torch.cat([boxes.view(B, K, 4), det.view(B, K, 1), labels.to(torch.float32)[..., None]], dim=2, out=rec.rows)
