@@ -223,6 +223,23 @@ int rsp_compact_keep(const uint8_t* keep, const float* boxes, const float* score
                      int B, int n, int K, float* out_boxes, float* out_scores, int64_t* out_labels,
                      int32_t* out_index, int32_t* counts, void* stream);
 
+/* mmcv.ops.batched_nms with nms_cfg type='soft_nms' (mmcv.ops.soft_nms, softnms_cpu in mmcv/ops/csrc/pytorch/cpu/nms.cpp;
+ * rpn_head.py:285-291, bbox_nms.py:95-103, mmdet/utils/large_image.py:76-104).  Candidates in the caller's input order
+ * (that order breaks ties): boxes fp32 [B, n, 4], scores fp32 [B, n], ids int64 [B, n] in [0, G), nvalid int32 [B] =
+ * length of the valid prefix.  Boxes are offset by id * (max_coord + 1) as mmcv does; below split_thr valid candidates
+ * one soft-NMS runs (output in selection order), otherwise one per id, merged by decayed score (ties: lower id, then
+ * selection order; mmcv's sort leaves them unordered).  method 0 naive, 1 linear, 2 gaussian; offset 0.  Arithmetic is
+ * fp32 without contraction in softnms_cpu's order; gaussian's exp runs in double on the fp32 argument, rounded once.
+ * Outputs as rsp_compact_keep: the first K selections, boxes un-offset, scores decayed, zero padded, index -1 past
+ * counts; out_labels / out_index may be NULL.  The loop stops after K selections per problem, so K = max_per_img
+ * costs K steps.  ws: *bytes from rsp_soft_nms_workspace_bytes(B, n, G, bytes) of device memory, O(B * n + B * G).
+ * 1 <= G <= 1024. */
+int rsp_soft_nms_workspace_bytes(int B, int n, int G, size_t* bytes);
+int rsp_soft_nms_batched(const float* boxes, const float* scores, const int64_t* ids, const int32_t* nvalid, int B,
+                         int n, int G, float iou_thr, float sigma, float min_score, int method, int split_thr, int K,
+                         void* ws, size_t ws_bytes, float* out_boxes, float* out_scores, int64_t* out_labels,
+                         int32_t* out_index, int32_t* counts, void* stream);
+
 /* SingleRoIExtractor + mmcv RoIAlign(output_size=P, sampling_ratio=0, aligned=True, avg)
  * (single_level_roi_extractor.py:55-119, base_roi_extractor.py:58-67) on up to 4 channels-last bf16
  * levels: feats[l] [B, Hs[l], Ws[l], C]; rois fp32 [n, 5] = (batch, x1, y1, x2, y2); level =

@@ -75,6 +75,9 @@ _SIGNATURES = {
     "rsp_bbox_cls_decode_shapes": ([_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp], _i),
     "rsp_nms_batched": ([_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp], _i),
     "rsp_compact_keep": ([_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp], _i),
+    "rsp_soft_nms_workspace_bytes": ([_i, _i, _i, _vp], _i),
+    "rsp_soft_nms_batched": ([_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _f, _i, _i, _i, _vp, ctypes.c_size_t, _vp, _vp,
+                              _vp, _vp, _vp, _vp], _i),
     "rsp_roi_align_nhwc": ([_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _f, _vp, _vp], _i),
     "rsp_mask_paste": ([_vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp], _i),
     "rsp_pool2_nhwc": ([_vp, _vp, _i, _i, _i, _i, _i, _vp], _i),
@@ -725,6 +728,50 @@ def compact_keep(keep: torch.Tensor, boxes: torch.Tensor, scores: torch.Tensor, 
     _check(_lib.rsp_compact_keep(_ptr(keep), _ptr(boxes), _ptr(scores), _ptr(labels), B, n, K, _ptr(ob),
                                  _ptr(os_), _ptr(ol), _ptr(oi), _ptr(cnt), _stream()), "rsp_compact_keep")
     launch_count += 1
+    return ob, os_, ol, oi, cnt
+
+
+SOFT_NMS_METHODS = {"naive": 0, "linear": 1, "gaussian": 2}   # mmcv soft_nms method_dict
+
+
+def soft_nms_workspace_bytes(B: int, n: int, G: int) -> int:
+    """Device workspace of soft_nms_batched for B images of n candidates in G id groups (O(B * n))."""
+    out = ctypes.c_size_t(0)
+    _check(_lib.rsp_soft_nms_workspace_bytes(int(B), int(n), int(G), ctypes.addressof(out)),
+           "rsp_soft_nms_workspace_bytes")
+    return int(out.value)
+
+
+def soft_nms_batched(boxes: torch.Tensor, scores: torch.Tensor, ids: torch.Tensor, nvalid: torch.Tensor,
+                     num_groups: int, iou_thr: float, sigma: float = 0.5, min_score: float = 1e-3,
+                     method: str = "linear", K: int = 0, split_thr: int = 10000):
+    """mmcv batched_nms(..., dict(type='soft_nms', ...)) per image on candidates in input order (see
+    rsp_soft_nms_batched).  boxes fp32 [B, n, 4], scores fp32 [B, n], ids int64 [B, n] in [0, num_groups), nvalid
+    int32 [B] (valid prefix).  K > 0: the first K selections (the loop stops there); K = 0: all n.
+    -> boxes [B, K, 4], decayed scores [B, K], labels = ids [B, K], input index int32 [B, K], counts int32 [B]."""
+    global launch_count
+    _require_cuda(boxes, scores, ids, nvalid)
+    B, n, _ = boxes.shape
+    assert boxes.dtype == torch.float32 and boxes.is_contiguous()
+    assert scores.dtype == torch.float32 and scores.is_contiguous() and scores.shape == (B, n)
+    assert ids.dtype == torch.int64 and ids.is_contiguous() and ids.shape == (B, n)
+    assert nvalid.dtype == torch.int32 and nvalid.is_contiguous() and nvalid.numel() == B
+    if method not in SOFT_NMS_METHODS:
+        raise ValueError(f"soft_nms method must be one of {sorted(SOFT_NMS_METHODS)}, got {method!r}")
+    K = int(K) if K > 0 else n
+    dev = boxes.device
+    nbytes = soft_nms_workspace_bytes(B, n, num_groups)
+    ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+    ob = torch.empty(B, K, 4, device=dev, dtype=torch.float32)
+    os_ = torch.empty(B, K, device=dev, dtype=torch.float32)
+    ol = torch.empty(B, K, device=dev, dtype=torch.int64)
+    oi = torch.empty(B, K, device=dev, dtype=torch.int32)
+    cnt = torch.empty(B, device=dev, dtype=torch.int32)
+    _check(_lib.rsp_soft_nms_batched(_ptr(boxes), _ptr(scores), _ptr(ids), _ptr(nvalid), B, n, int(num_groups),
+                                     float(iou_thr), float(sigma), float(min_score), SOFT_NMS_METHODS[method],
+                                     int(split_thr), K, _ptr(ws), nbytes, _ptr(ob), _ptr(os_), _ptr(ol), _ptr(oi),
+                                     _ptr(cnt), _stream()), "rsp_soft_nms_batched")
+    launch_count += 3
     return ob, os_, ol, oi, cnt
 
 

@@ -34,6 +34,56 @@ def _cfg(d) -> ConfigDict:
     return d if isinstance(d, ConfigDict) else ConfigDict(d or {})
 
 
+# keys of an mmcv batched_nms config this package runs, per type; a key outside these raises instead of being ignored.
+# offset, class_agnostic and split_thr are accepted at their mmcv defaults only.
+_NMS_KEYS = {"nms": ("iou_threshold",), "soft_nms": ("iou_threshold", "sigma", "min_score", "method")}
+_NMS_DEFAULTS = dict(offset=0, class_agnostic=False, split_thr=10000)
+
+
+def parse_nms_cfg(nms) -> dict:
+    """Validate a test_cfg ``nms`` dict (mmcv batched_nms nms_cfg) -> dict(type, iou_threshold[, sigma, min_score,
+    method]) with mmcv's defaults filled in.  Raises ValueError naming an unsupported type, key or method."""
+    d = dict(nms or {})
+    typ = d.pop("type", "nms")
+    if typ not in _NMS_KEYS:
+        raise ValueError(f"nms type {typ!r} is not supported (supported: {', '.join(_NMS_KEYS)})")
+    for k, v in _NMS_DEFAULTS.items():
+        if k in d and d.pop(k) != v:
+            raise ValueError(f"nms {k}={nms[k]!r} is not supported (only {v!r})")
+    extra = sorted(set(d) - set(_NMS_KEYS[typ]))
+    if extra:
+        raise ValueError(f"nms key(s) {extra} not supported for type {typ!r}")
+    out = dict(type=typ)
+    if "iou_threshold" in d:
+        out["iou_threshold"] = float(d["iou_threshold"])
+    if typ == "soft_nms":
+        method = d.get("method", "linear")
+        if method not in _lib.SOFT_NMS_METHODS:
+            raise ValueError(f"soft_nms method {method!r} is not supported (supported: "
+                             f"{', '.join(_lib.SOFT_NMS_METHODS)})")
+        out.update(iou_threshold=float(d.get("iou_threshold", 0.3)), sigma=float(d.get("sigma", 0.5)),
+                   min_score=float(d.get("min_score", 1e-3)), method=method)
+        if method == "gaussian" and not out["sigma"] > 0:
+            raise ValueError(f"soft_nms sigma must be > 0 for method 'gaussian', got {out['sigma']}")
+    return out
+
+
+def _soft_nms_input_order(scores: torch.Tensor, boxes: torch.Tensor, ids: torch.Tensor, K: int, num_groups: int,
+                          nms: dict):
+    """Soft-NMS of each image's valid candidates (score >= 0) in their array order, which is mmcv's input order
+    (ties and the serial loop's swaps depend on it): the valid ones are moved to the front, order kept, on the
+    device.  -> boxes [B, K, 4], decayed scores [B, K], ids [B, K], counts int32 [B]."""
+    invalid = (scores < 0).to(torch.uint8)
+    _, order = torch.sort(invalid, dim=1, stable=True)
+    s = torch.gather(scores, 1, order).contiguous()
+    b = torch.gather(boxes, 1, order[:, :, None].expand(-1, -1, 4)).contiguous()
+    i = torch.gather(ids, 1, order).contiguous()
+    nvalid = (invalid == 0).sum(dim=1).to(torch.int32)
+    ob, os_, ol, _, cnt = _lib.soft_nms_batched(b, s, i, nvalid, num_groups, nms["iou_threshold"], nms["sigma"],
+                                                nms["min_score"], nms["method"], K=K)
+    return ob, os_, ol, cnt
+
+
 # ------------------------------------------------------------------------------ small registry types
 @MODELS.register_module(force=True)
 class AnchorGenerator:
@@ -112,6 +162,7 @@ class RPNHead(_PrepMixin, BaseModule):
         self.prior_generator = MODELS.build(anchor_generator)
         self.bbox_coder = MODELS.build(bbox_coder)
         self.test_cfg = _cfg(test_cfg)
+        self._nms = parse_nms_cfg(self.test_cfg.get("nms"))
         A = self.prior_generator.num_base_priors[0]
         self.num_base_priors = A
         self.rpn_conv = _conv(feat_channels, in_channels, 3)
@@ -138,7 +189,7 @@ class RPNHead(_PrepMixin, BaseModule):
         """feats: bf16 NHWC levels -> proposals fp32 [B, K, 4], scores [B, K], counts int32 [B].
         img_shapes: device fp32 [B, 2] per-image (h, w) the boxes are clipped to (img_meta['img_shape'],
         rpn_head.py:208-215); None = the batch shape img_hw for every image.
-        capture (tests): receives the raw per-level head outputs."""
+        capture (tests): receives the raw per-level head outputs (and, with soft_nms, the NMS candidates)."""
         p = self._prep or self._prepare()
         cfg = self.test_cfg
         nms_pre, K = int(cfg.get("nms_pre", 1000)), int(cfg.get("max_per_img", 1000))
@@ -169,6 +220,11 @@ class RPNHead(_PrepMixin, BaseModule):
                             stds=self.bbox_coder.stds, img_shapes=img_shapes)
             ids[:, off:off + k] = l
             off += k
+        if self._nms["type"] == "soft_nms":   # candidates in level order, each level's top-k in descending order
+            if capture is not None:
+                capture["candidates"] = (boxes, scores, ids)
+            pb, ps, _, cnt = _soft_nms_input_order(scores, boxes, ids, K, len(feats), self._nms)
+            return pb, ps, cnt
         # batched_nms sorts by score internally; filtered boxes (score -1) sink to the end
         s_sorted, order = torch.sort(scores, dim=1, descending=True, stable=True)
         b_sorted = torch.gather(boxes, 1, order[:, :, None].expand(-1, -1, 4)).contiguous()
@@ -305,7 +361,8 @@ def _predict_bboxes(head, feats: list, proposals: torch.Tensor, prop_counts: tor
                     pes: list | None = None, capture: dict | None = None, img_shapes: torch.Tensor | None = None):
     """StandardRoIHead.predict_bbox (standard_roi_head.py:292-345) + BBoxHead._predict_by_feat_single
     (bbox_head.py:505-571) + multiclass_nms (bbox_nms.py:13-105), batched over the B images.
-    -> detections bboxes fp32 [B, M, 4], scores [B, M], labels int64 [B, M], counts int32 [B]."""
+    -> detections bboxes fp32 [B, M, 4], scores [B, M], labels int64 [B, M], counts int32 [B].
+    nms type 'soft_nms': the scores are the decayed ones and the rows are in selection order."""
     cfg = head.test_cfg
     B, K, _ = proposals.shape
     dev = proposals.device
@@ -321,6 +378,10 @@ def _predict_bboxes(head, feats: list, proposals: torch.Tensor, prop_counts: tor
                                      stds=head.bbox_head.bbox_coder.stds, img_shapes=img_shapes)
     n = K * C
     s, b, lab = s.view(B, n), b.view(B, n, 4), lab.view(B, n)
+    if head._nms["type"] == "soft_nms":   # candidates (RoI, class) with score > score_thr, RoI-major
+        if capture is not None:
+            capture["candidates"] = (b, s, lab)
+        return _soft_nms_input_order(s, b, lab, int(cfg.get("max_per_img", 100)), C, head._nms)
     s_sorted, order = torch.sort(s, dim=1, descending=True, stable=True)
     b_sorted = torch.gather(b, 1, order[:, :, None].expand(-1, -1, 4)).contiguous()
     l_sorted = torch.gather(lab, 1, order).contiguous()
@@ -366,6 +427,7 @@ class RSPrompterAnchorRoIPromptHead(BaseModule):
         self.mask_roi_extractor = MODELS.build(mask_roi_extractor)
         self.mask_head = MODELS.build(mask_head)
         self.test_cfg = _cfg(test_cfg)
+        self._nms = parse_nms_cfg(self.test_cfg.get("nms"))
         self.with_extra_pe = with_extra_pe
         self._pe_cache: dict = {}
 
@@ -510,6 +572,7 @@ class StandardRoIHead(BaseModule):
             self.mask_roi_extractor = MODELS.build(mask_roi_extractor) if mask_roi_extractor is not None else None
             self.mask_head = MODELS.build(mask_head)
         self.test_cfg = _cfg(test_cfg)
+        self._nms = parse_nms_cfg(self.test_cfg.get("nms"))
 
     def init_weights(self):
         pass
@@ -532,5 +595,5 @@ class StandardRoIHead(BaseModule):
         return out
 
 
-__all__ = ["FCNMaskHead", "StandardRoIHead", "AnchorGenerator", "DeltaXYWHBBoxCoder", "RoIAlign", "SingleRoIExtractor", "RPNHead",
+__all__ = ["parse_nms_cfg", "FCNMaskHead", "StandardRoIHead", "AnchorGenerator", "DeltaXYWHBBoxCoder", "RoIAlign", "SingleRoIExtractor", "RPNHead",
            "Shared2FCBBoxHead", "RSPrompterAnchorMaskHead", "RSPrompterAnchorRoIPromptHead", "sine_pe_rows"]

@@ -240,6 +240,21 @@ int rsp_compact_keep(const uint8_t* keep, const float* boxes, const float* score
                       out_scores, reinterpret_cast<long long*>(out_labels), out_index, counts, S(stream));
 }
 
+int rsp_soft_nms_workspace_bytes(int B, int n, int G, size_t* bytes) {
+  RSP_CHECK_ARG(bytes && B > 0 && n > 0 && G >= 1, "soft_nms_workspace_bytes: bad args");
+  *bytes = soft_nms_workspace_bytes(B, n, G);
+  return RSP_OK;
+}
+
+int rsp_soft_nms_batched(const float* boxes, const float* scores, const int64_t* ids, const int32_t* nvalid, int B,
+                         int n, int G, float iou_thr, float sigma, float min_score, int method, int split_thr, int K,
+                         void* ws, size_t ws_bytes, float* out_boxes, float* out_scores, int64_t* out_labels,
+                         int32_t* out_index, int32_t* counts, void* stream) {
+  return soft_nms_batched(boxes, scores, reinterpret_cast<const long long*>(ids), nvalid, B, n, G, iou_thr, sigma,
+                          min_score, method, split_thr, K, ws, ws_bytes, out_boxes, out_scores,
+                          reinterpret_cast<long long*>(out_labels), out_index, counts, S(stream));
+}
+
 int rsp_roi_align_nhwc(const void* const* feats, const float* const* pes, const int32_t* Hs,
                        const int32_t* Ws, const float* scales, int num_levels, const float* rois, int n,
                        int C, int P, float finest_scale, void* out, void* stream) {

@@ -18,6 +18,8 @@
 #include "sm90.cuh"
 #include "upsample4.cuh"
 
+#include <climits>
+
 namespace rsp {
 
 // exact-rounding helpers: no FMA contraction, so IoU / box arithmetic matches the fp32 reference
@@ -330,6 +332,355 @@ int compact_keep(const unsigned char* keep, const float* boxes, const float* sco
                 "compact_keep: bad args");
   compact_keep_kernel<<<B, 32, 0, stream>>>(keep, boxes, scores, labels, n, K, out_boxes, out_scores,
                                             out_labels, out_index, counts);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// Soft-NMS: mmcv.ops.batched_nms with nms_cfg type='soft_nms' (softnms_cpu of mmcv/ops/csrc/pytorch/cpu/nms.cpp).
+// Candidates are taken in input order (ties go to the lower position, and the serial loop's swaps move positions,
+// so the order is part of the answer).  Per image: boxes offset by id * (max + 1) as in nms_batched; below split_thr
+// valid candidates one problem, otherwise one problem per id, merged by decayed score.  One CTA per (id, image)
+// problem, state in the O(n) workspace: per candidate the offset box, area, running score and input index, plus a
+// position -> candidate permutation.  A step is
+//   argmax over positions [i, live) (larger score, then lower position; a NaN never replaces the running max, and a
+//   NaN at i itself is selected, as the serial scan does) -> swap with i -> decay every position in (i, live) once
+//   -> removal of the ones below min_score.
+// The serial removal loop (the last live candidate moves into a removed one's slot, which is re-examined) leaves
+// the m survivors of (i, live) as: survivors below i + 1 + m in place, and each removed slot below that end filled by
+// a survivor from above it, lowest slot first, highest survivor first.  A step is therefore two block scans.
+// A selection is final once made and selected scores do not increase, so K selections per problem suffice.
+constexpr int SN_THREADS = 1024;
+constexpr int SN_MAX_GROUPS = 1024;
+
+struct SoftNmsWs {
+  float *x1, *y1, *x2, *y2, *area, *score;   // [B, n] per candidate, segment-local order
+  int *orig, *perm, *holes;                  // [B, n] input index, position -> candidate, removed slots
+  float* sel_score;                          // [B, n] selections of segment g at seg_off[g]
+  int* sel_idx;
+  int *seg_off, *seg_cnt, *sel_cnt;          // [B, G]
+  float* max_coord;                          // [B]
+  int* per_class;                            // [B]
+};
+
+inline size_t sn_align(size_t x) { return (x + 255) & ~static_cast<size_t>(255); }
+
+inline SoftNmsWs sn_carve(void* base, int B, int n, int G, size_t* bytes) {
+  char* p = static_cast<char*>(base);
+  size_t off = 0;
+  const size_t bn = static_cast<size_t>(B) * n * 4, bg = static_cast<size_t>(B) * G * 4, b1 = static_cast<size_t>(B) * 4;
+  auto take = [&](size_t sz) { char* r = p + off; off += sn_align(sz); return r; };
+  SoftNmsWs w;
+  w.x1 = reinterpret_cast<float*>(take(bn)); w.y1 = reinterpret_cast<float*>(take(bn));
+  w.x2 = reinterpret_cast<float*>(take(bn)); w.y2 = reinterpret_cast<float*>(take(bn));
+  w.area = reinterpret_cast<float*>(take(bn)); w.score = reinterpret_cast<float*>(take(bn));
+  w.orig = reinterpret_cast<int*>(take(bn)); w.perm = reinterpret_cast<int*>(take(bn));
+  w.holes = reinterpret_cast<int*>(take(bn));
+  w.sel_score = reinterpret_cast<float*>(take(bn)); w.sel_idx = reinterpret_cast<int*>(take(bn));
+  w.seg_off = reinterpret_cast<int*>(take(bg)); w.seg_cnt = reinterpret_cast<int*>(take(bg));
+  w.sel_cnt = reinterpret_cast<int*>(take(bg));
+  w.max_coord = reinterpret_cast<float*>(take(b1)); w.per_class = reinterpret_cast<int*>(take(b1));
+  if (bytes) *bytes = off;
+  return w;
+}
+
+size_t soft_nms_workspace_bytes(int B, int n, int G) {
+  size_t bytes = 0;
+  sn_carve(nullptr, B, n, G, &bytes);
+  return bytes;
+}
+
+// The three comparisons of softnms_cpu, in one place:
+//   selection:  the running max is replaced only when  max < sc[pos]   (first position of the largest score wins)
+//   decay:      naive / linear act when               ovr >= iou_threshold   (gaussian always)
+//   removal:    a candidate is dropped when           sc[pos] < min_score
+__device__ __forceinline__ bool sn_removed(float s, float min_score) { return s < min_score; }
+
+__device__ __forceinline__ void sn_better(float& s, int& p, float s2, int p2) {
+  if (s2 > s || (s2 == s && p2 < p)) { s = s2; p = p2; }
+}
+
+__device__ __forceinline__ float sn_weight(float ovr, float thr, float sigma, int method) {
+  if (method == 0) return ovr >= thr ? 0.f : 1.f;
+  if (method == 1) return ovr >= thr ? fsub(1.f, ovr) : 1.f;
+  const float arg = __fdiv_rn(-fmul(ovr, ovr), sigma);       // -(ovr * ovr) / sigma in fp32
+  return __double2float_rn(exp(static_cast<double>(arg)));   // exp in double, rounded once to fp32
+}
+
+// block-wide helpers for SN_THREADS threads; each ends with every thread holding the result
+__device__ __forceinline__ void sn_block_argmax(float& s, int& p, float* rs, int* rp) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const float s2 = __shfl_xor_sync(0xffffffffu, s, o);
+    const int p2 = __shfl_xor_sync(0xffffffffu, p, o);
+    sn_better(s, p, s2, p2);
+  }
+  __syncthreads();
+  if (lane == 0) { rs[warp] = s; rp[warp] = p; }
+  __syncthreads();
+  s = rs[0]; p = rp[0];
+  for (int w = 1; w < SN_THREADS / 32; ++w) sn_better(s, p, rs[w], rp[w]);
+}
+
+// exclusive scan of two counters over the block; totals in ta / tb
+__device__ __forceinline__ void sn_block_exscan2(int& a, int& b, int& ta, int& tb, int2* red) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int ia = a, ib = b;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int xa = __shfl_up_sync(0xffffffffu, ia, o), xb = __shfl_up_sync(0xffffffffu, ib, o);
+    if (lane >= o) { ia += xa; ib += xb; }
+  }
+  __syncthreads();
+  if (lane == 31) red[warp] = make_int2(ia, ib);
+  __syncthreads();
+  int pa = 0, pb = 0;
+  ta = 0; tb = 0;
+  for (int w = 0; w < SN_THREADS / 32; ++w) {
+    const int2 v = red[w];
+    if (w < warp) { pa += v.x; pb += v.y; }
+    ta += v.x; tb += v.y;
+  }
+  a = pa + ia - a; b = pb + ib - b;
+}
+
+// per image: max coordinate of the valid boxes, the regime, and the per-id segments of the workspace
+__global__ void __launch_bounds__(SN_THREADS)
+soft_nms_prep_kernel(const float* __restrict__ boxes, const long long* __restrict__ ids, const int* __restrict__ nvalid,
+                     int n, int G, int split_thr, SoftNmsWs ws) {
+  __shared__ float red[SN_THREADS / 32];
+  __shared__ int hist[SN_MAX_GROUPS];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int nv = min(max(nvalid[b], 0), n);
+  const bool per_class = nv >= split_thr;
+  float m = -INFINITY;
+  for (int i = tid; i < nv * 4; i += SN_THREADS) m = fmaxf(m, boxes[static_cast<size_t>(b) * n * 4 + i]);
+#pragma unroll
+  for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  for (int g = tid; g < G; g += SN_THREADS) hist[g] = 0;
+  if ((tid & 31) == 0) red[tid >> 5] = m;
+  __syncthreads();
+  if (per_class) {
+    for (int i = tid; i < nv; i += SN_THREADS) {
+      const long long id = ids[static_cast<size_t>(b) * n + i];
+      if (id >= 0 && id < G) atomicAdd(&hist[id], 1);
+    }
+  } else if (tid == 0) {
+    hist[0] = nv;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float mm = red[0];
+    for (int w = 1; w < SN_THREADS / 32; ++w) mm = fmaxf(mm, red[w]);
+    ws.max_coord[b] = mm;
+    ws.per_class[b] = per_class ? 1 : 0;
+    int off = 0;
+    for (int g = 0; g < G; ++g) {
+      ws.seg_off[b * G + g] = off;
+      ws.seg_cnt[b * G + g] = hist[g];
+      off += hist[g];
+    }
+  }
+}
+
+// one CTA per (id group, image): gather the group's candidates in input order, then run the serial loop's steps
+__global__ void __launch_bounds__(SN_THREADS)
+soft_nms_kernel(const float* __restrict__ boxes, const float* __restrict__ scores, const long long* __restrict__ ids,
+                const int* __restrict__ nvalid, int n, int G, float thr, float sigma, float min_score, int method,
+                int K, SoftNmsWs ws) {
+  __shared__ float rs[SN_THREADS / 32];
+  __shared__ int rp[SN_THREADS / 32];
+  __shared__ int2 red2[SN_THREADS / 32];
+  __shared__ int s_sel;
+  const int g = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  const int cnt = ws.seg_cnt[b * G + g];
+  if (cnt == 0) {
+    if (tid == 0) ws.sel_cnt[b * G + g] = 0;
+    return;
+  }
+  const size_t base = static_cast<size_t>(b) * n + ws.seg_off[b * G + g];
+  float *x1 = ws.x1 + base, *y1 = ws.y1 + base, *x2 = ws.x2 + base, *y2 = ws.y2 + base;
+  float *area = ws.area + base, *sc = ws.score + base;
+  int *orig = ws.orig + base, *perm = ws.perm + base, *holes = ws.holes + base;
+  const int nv = min(max(nvalid[b], 0), n);
+  const bool per_class = ws.per_class[b] != 0;
+  const float off1 = fadd(ws.max_coord[b], 1.0f);
+
+  // gather (order-preserving compaction of this group's candidates)
+  int run = 0;
+  for (int j0 = 0; j0 < nv; j0 += SN_THREADS) {
+    const int j = j0 + tid;
+    const size_t gj = static_cast<size_t>(b) * n + j;
+    const bool mine = j < nv && (!per_class || ids[gj] == g);
+    int r = mine ? 1 : 0, z = 0, tot, tz;
+    sn_block_exscan2(r, z, tot, tz, red2);
+    if (mine) {
+      const int k = run + r;
+      const float off = fmul(static_cast<float>(ids[gj]), off1);
+      const float a0 = fadd(boxes[gj * 4], off), a1 = fadd(boxes[gj * 4 + 1], off);
+      const float a2 = fadd(boxes[gj * 4 + 2], off), a3 = fadd(boxes[gj * 4 + 3], off);
+      x1[k] = a0; y1[k] = a1; x2[k] = a2; y2[k] = a3;
+      area[k] = fmul(fsub(a2, a0), fsub(a3, a1));
+      sc[k] = scores[gj];
+      orig[k] = j;
+      perm[k] = k;
+    }
+    run += tot;
+  }
+  __syncthreads();
+
+  // first argmax over all positions
+  float bs = -INFINITY;
+  int bp = INT_MAX;
+  for (int q = tid; q < cnt; q += SN_THREADS) sn_better(bs, bp, sc[q], q);
+  sn_block_argmax(bs, bp, rs, rp);
+
+  int live = cnt, i = 0;
+  for (; i < live && i < K; ++i) {
+    if (tid == 0) {
+      const int p = isnan(sc[perm[i]]) ? i : bp;
+      const int c = perm[p];
+      perm[p] = perm[i];
+      perm[i] = c;
+      ws.sel_score[base + i] = sc[c];
+      ws.sel_idx[base + i] = orig[c];
+      s_sel = c;
+    }
+    __syncthreads();
+    const int c = s_sel;
+    const float ix1 = x1[c], iy1 = y1[c], ix2 = x2[c], iy2 = y2[c], iarea = area[c];
+    const int lo0 = i + 1, len = live - lo0;
+    if (len <= 0) { ++i; break; }
+    const int L = (len + SN_THREADS - 1) / SN_THREADS;
+    const int lo = min(lo0 + tid * L, live), hi = min(lo + L, live);
+    // decay each of (i, live) once
+    int alive = 0, zero = 0;
+    for (int q = lo; q < hi; ++q) {
+      const int d = perm[q];
+      const float w = fmaxf(fsub(fminf(ix2, x2[d]), fmaxf(ix1, x1[d])), 0.f);
+      const float h = fmaxf(fsub(fminf(iy2, y2[d]), fmaxf(iy1, y1[d])), 0.f);
+      const float inter = fmul(w, h);
+      const float ovr = __fdiv_rn(inter, fsub(fadd(iarea, area[d]), inter));
+      const float s = fmul(sc[d], sn_weight(ovr, thr, sigma, method));
+      sc[d] = s;
+      alive += sn_removed(s, min_score) ? 0 : 1;
+    }
+    int m, unused;
+    sn_block_exscan2(alive, zero, m, unused, red2);
+    const int end = lo0 + m;
+    // removed slots below the new end, survivors at or above it
+    int nh = 0, ns = 0;
+    for (int q = lo; q < hi; ++q) {
+      const bool dead = sn_removed(sc[perm[q]], min_score);
+      if (q < end) nh += dead ? 1 : 0;
+      else ns += dead ? 0 : 1;
+    }
+    int th, ts;
+    sn_block_exscan2(nh, ns, th, ts, red2);
+    bs = -INFINITY; bp = INT_MAX;
+    for (int q = lo; q < min(hi, end); ++q) {
+      const float s = sc[perm[q]];
+      if (sn_removed(s, min_score)) holes[nh++] = q;
+      else sn_better(bs, bp, s, q);
+    }
+    __syncthreads();
+    for (int q = max(lo, end); q < hi; ++q) {
+      const int d = perm[q];
+      const float s = sc[d];
+      if (!sn_removed(s, min_score)) {
+        const int dst = holes[ts - 1 - ns];   // highest survivor fills the lowest slot
+        ++ns;
+        perm[dst] = d;
+        sn_better(bs, bp, s, dst);
+      }
+    }
+    sn_block_argmax(bs, bp, rs, rp);
+    live = end;
+  }
+  if (tid == 0) ws.sel_cnt[b * G + g] = i;
+}
+
+// entries of a non-increasing list before value s: v > s, or v >= s when ties rank first
+__device__ __forceinline__ int sn_count_before(const float* v, int len, float s, bool ties_first) {
+  int lo = 0, hi = len;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    const float x = v[mid];
+    if (ties_first ? x >= s : x > s) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// selections -> [B, K] outputs: entry k of group g goes to rank k + (entries of the other groups ranked before it);
+// in the per-id regime that is a merge by decayed score (ties: lower id first), otherwise the selection order.
+__global__ void soft_nms_finish_kernel(const float* __restrict__ boxes, const long long* __restrict__ ids, int n,
+                                       int G, int K, SoftNmsWs ws, float* __restrict__ out_boxes,
+                                       float* __restrict__ out_scores, long long* __restrict__ out_labels,
+                                       int* __restrict__ out_index, int* __restrict__ counts) {
+  const int b = blockIdx.y;
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  const int* soff = ws.seg_off + b * G;
+  const int* scnt = ws.seg_cnt + b * G;
+  const int* selc = ws.sel_cnt + b * G;
+  int total = 0;
+  for (int h = 0; h < G; ++h) total += selc[h];
+  const int kout = min(total, K);
+  if (e < n) {
+    int g = -1;
+    for (int h = 0; h < G; ++h)
+      if (scnt[h] > 0 && e >= soff[h] && e < soff[h] + scnt[h]) { g = h; break; }
+    const int k = g >= 0 ? e - soff[g] : 0;
+    if (g >= 0 && k < selc[g]) {
+      const float* sel = ws.sel_score + static_cast<size_t>(b) * n;
+      const float s = sel[e];
+      int rank = k;
+      for (int h = 0; h < G && rank < K; ++h)
+        if (h != g && selc[h] > 0) rank += sn_count_before(sel + soff[h], selc[h], s, h < g);
+      if (rank < K) {
+        const int j = ws.sel_idx[static_cast<size_t>(b) * n + e];
+        const size_t src = static_cast<size_t>(b) * n + j, dst = static_cast<size_t>(b) * K + rank;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) out_boxes[dst * 4 + c] = boxes[src * 4 + c];
+        out_scores[dst] = s;
+        if (out_labels) out_labels[dst] = ids[src];
+        if (out_index) out_index[dst] = j;
+      }
+    }
+  }
+  if (e >= kout && e < K) {
+    const size_t dst = static_cast<size_t>(b) * K + e;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) out_boxes[dst * 4 + c] = 0.f;
+    out_scores[dst] = 0.f;
+    if (out_labels) out_labels[dst] = 0;
+    if (out_index) out_index[dst] = -1;
+  }
+  if (e == 0) counts[b] = kout;
+}
+
+int soft_nms_batched(const float* boxes, const float* scores, const long long* ids, const int* nvalid, int B, int n,
+                     int G, float iou_thr, float sigma, float min_score, int method, int split_thr, int K, void* ws,
+                     size_t ws_bytes, float* out_boxes, float* out_scores, long long* out_labels, int* out_index,
+                     int* counts, cudaStream_t stream) {
+  RSP_CHECK_ARG(boxes && scores && ids && nvalid && ws && out_boxes && out_scores && counts && B > 0 && B <= 65535 &&
+                n > 0 && K > 0, "soft_nms_batched: bad args");
+  RSP_CHECK_ARG(G >= 1 && G <= SN_MAX_GROUPS, "soft_nms_batched: 1 <= G <= %d id groups", SN_MAX_GROUPS);
+  RSP_CHECK_ARG(method >= 0 && method <= 2, "soft_nms_batched: method 0 naive, 1 linear, 2 gaussian");
+  RSP_CHECK_ARG(method != 2 || sigma > 0.f, "soft_nms_batched: gaussian needs sigma > 0");
+  RSP_CHECK_ARG(static_cast<long long>(B) * n <= 0x7fffffffLL, "soft_nms_batched: B * n must fit in int32");
+  size_t need = 0;
+  SoftNmsWs w = sn_carve(ws, B, n, G, &need);
+  RSP_CHECK_ARG(ws_bytes >= need, "soft_nms_batched: workspace of %zu bytes, %zu needed", ws_bytes, need);
+  soft_nms_prep_kernel<<<B, SN_THREADS, 0, stream>>>(boxes, ids, nvalid, n, G, split_thr, w);
+  RSP_CHECK_LAUNCH();
+  soft_nms_kernel<<<dim3(G, B), SN_THREADS, 0, stream>>>(boxes, scores, ids, nvalid, n, G, iou_thr, sigma, min_score,
+                                                         method, K, w);
+  RSP_CHECK_LAUNCH();
+  const int span = max(n, K);
+  soft_nms_finish_kernel<<<dim3((span + 255) / 256, B), 256, 0, stream>>>(boxes, ids, n, G, K, w, out_boxes,
+                                                                          out_scores, out_labels, out_index, counts);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
 }

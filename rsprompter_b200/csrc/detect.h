@@ -17,6 +17,11 @@ int nms_batched(const float* boxes, const long long* ids, const int* nvalid, int
 int compact_keep(const unsigned char* keep, const float* boxes, const float* scores, const long long* labels,
                  int B, int n, int K, float* out_boxes, float* out_scores, long long* out_labels,
                  int* out_index, int* counts, cudaStream_t stream);
+size_t soft_nms_workspace_bytes(int B, int n, int G);
+int soft_nms_batched(const float* boxes, const float* scores, const long long* ids, const int* nvalid, int B, int n,
+                     int G, float iou_thr, float sigma, float min_score, int method, int split_thr, int K, void* ws,
+                     size_t ws_bytes, float* out_boxes, float* out_scores, long long* out_labels, int* out_index,
+                     int* counts, cudaStream_t stream);
 int roi_align_nhwc(const void* const* feats, const float* const* pes, const int* Hs, const int* Ws,
                    const float* scales, int num_levels, const float* rois, int n, int C, int P,
                    float finest_scale, void* out, cudaStream_t stream);

@@ -12,11 +12,13 @@ merged with one class-aware NMS (``merge_results_by_nms``).  Here all of it stay
     from the scene, as the test pipeline's keep-ratio Resize + Pad does;
   * every batch leaves ``predict_records`` as one ResultRecord, resident until the merge;
   * the merge is ``rsp_nms_batched`` + ``rsp_compact_keep`` over every valid slot of every tile (mmcv
-    ``batched_nms`` semantics, label offset included);
+    ``batched_nms`` semantics, label offset included), or ``rsp_soft_nms_batched`` with ``merge_nms_type='soft_nms'``
+    (the demo's ``--merge-nms-type``);
   * the kept masks are encoded as COCO RLE of the whole scene by ``rsp_mask_rle_placed_*`` straight from the
     records' bits: the full-scene bool mask sahi's ``shift_masks`` builds for every instance never exists.
 
-The merge's NMS is dense: at most 393 216 candidates (tiles x slots), with an n^2 / 8-byte workspace.
+The merge's hard NMS is dense: at most 393 216 candidates (tiles x slots), with an n^2 / 8-byte workspace.  The soft
+merge takes the same number of candidates with an O(n) workspace.
 
 ``python -m rsprompter_b200.large_image CONFIG IMAGE`` writes the COCO result dicts of one scene."""
 from __future__ import annotations
@@ -60,8 +62,11 @@ def slice_origins(hw: tuple, patch: int, overlap_ratio: float) -> list:
     return out
 
 
+MERGE_NMS_TYPES = ("nms", "soft_nms")
+
+
 def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_thr: float = 0.25,
-                       score_thr: float = 0.0, window: tuple | None = None) -> dict:
+                       score_thr: float = 0.0, window: tuple | None = None, nms_type: str = "nms") -> dict:
     """Class-aware NMS of every valid slot of every tile, in scene coordinates.
 
     ``records`` are ResultRecords of tiles (one image per tile; records of one call share slots and device) and
@@ -74,8 +79,18 @@ def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_
     (h, w) is the tile size when it differs from the records' canvas (resized patches: the canvas width is rounded
     up to 16).
 
-    Returns dict(bboxes fp32 [k, 4], scores [k], labels int64 [k] on the device, in descending score order, and
-    source int64 [k, 3] on the host: (record, image, slot) of each kept row).  One host synchronisation."""
+    ``nms_type='soft_nms'`` merges as mmcv batched_nms(..., dict(type='soft_nms', iou_threshold=merge_iou_thr)) with
+    soft_nms's defaults (sigma 0.5, min_score 1e-3, linear), on the valid slots in (tile, slot) order, which is the
+    order InstanceData.cat leaves them in and the tie-break of soft-NMS.  As the reference's merge_results_by_nms does
+    (``_, keeps = batched_nms(...)``), the kept rows keep their original scores, in keep order: selection order below
+    10 000 candidates, by decayed score at or above it.  ``score_thr`` then drops kept rows scored below it.  Filtering
+    before a soft merge would not be the same: a low-scored box can be selected early and decay others.
+
+    Returns dict(bboxes fp32 [k, 4], scores [k], labels int64 [k] on the device, in descending score order (soft: keep
+    order), and source int64 [k, 3] on the host: (record, image, slot) of each kept row).  One host synchronisation
+    (two for soft_nms: the number of label groups is read first)."""
+    if nms_type not in MERGE_NMS_TYPES:
+        raise ValueError(f"merge nms type {nms_type!r} is not supported (supported: {', '.join(MERGE_NMS_TYPES)})")
     H, W = int(scene_hw[0]), int(scene_hw[1])
     assert len(records) == len(origins) and records, "one origin list per record"
     M = records[0].slots
@@ -102,6 +117,10 @@ def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_
     boxes = torch.minimum(torch.maximum(rows[..., :4] + lo, lo), hi)
     scores = rows[..., 4]
     valid = torch.arange(M, device=dev)[None, :] < counts[:, None]
+    src = torch.tensor(src, dtype=torch.int64).view(-1, 2)
+    if nms_type == "soft_nms":
+        return _soft_merge(boxes.reshape(N, 4), scores.reshape(N), rows[..., 5].reshape(N).long(), valid.reshape(N),
+                           merge_iou_thr, score_thr, src, M)
     if score_thr > 0:
         valid &= scores >= score_thr
     key = torch.where(valid, scores, torch.full_like(scores, -math.inf)).reshape(N)
@@ -117,8 +136,32 @@ def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_
     k = int(host[0])
     flat = host[1:1 + k]
     tile, slot = flat // M, flat % M
-    src = torch.tensor(src, dtype=torch.int64).view(-1, 2)
     return dict(bboxes=ob[0, :k], scores=os_[0, :k], labels=ol[0, :k],
+                source=torch.cat([src[tile], slot[:, None]], dim=1))
+
+
+def _soft_merge(boxes, scores, labels, valid, iou_thr, score_thr, src, M) -> dict:
+    """The soft_nms branch of merge_tile_records over the N = tiles x slots candidates (flat, valid flags)."""
+    _, order = torch.sort((~valid).to(torch.uint8), stable=True)       # valid slots first, (tile, slot) order kept
+    nvalid = valid.sum().to(torch.int32).view(1)
+    b = boxes[order].contiguous()
+    lab = labels[order].contiguous()
+    groups = int(torch.where(valid, labels, torch.zeros_like(labels)).max()) + 1   # host sync 1: label groups
+    if groups > 1024:
+        raise ValueError(f"soft-NMS merge takes labels below 1024, got {groups - 1}")
+    ob, _, ol, oi, cnt = _lib.soft_nms_batched(b[None], scores[order].contiguous()[None], lab[None], nvalid, groups,
+                                               iou_thr)
+    flat_d = order[oi[0].clamp(min=0).long()]
+    os_ = scores[flat_d]                                               # the kept rows' original scores
+    n = int(boxes.shape[0])
+    keep = (torch.arange(n, device=boxes.device) < cnt[0]) & (os_ >= score_thr)
+    host = torch.cat([keep.long(), flat_d]).cpu()                       # host sync 2: kept rows + sources
+    sel = host[:n].bool()
+    idx = torch.nonzero(sel).view(-1)
+    flat = host[n:][sel]
+    tile, slot = flat // M, flat % M
+    idx_d = idx.to(boxes.device, non_blocking=True)
+    return dict(bboxes=ob[0, idx_d], scores=os_[idx_d], labels=ol[0, idx_d],
                 source=torch.cat([src[tile], slot[:, None]], dim=1))
 
 
@@ -134,7 +177,8 @@ def _record_nbytes(B: int, M: int, hw: tuple) -> int:
 
 @torch.no_grad()
 def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr: float = 0.25,
-                        score_thr: float = 0.0, batch_size: int = 8, patch_size: int | None = None) -> DetDataSample:
+                        score_thr: float = 0.0, batch_size: int = 8, patch_size: int | None = None,
+                        merge_nms_type: str = "nms") -> DetDataSample:
     """Detect a whole scene: slice, run the tiles in batches, merge across tiles, encode the kept masks.
 
     ``image`` is the scene as mmcv.imread decodes it, uint8 [H, W, 3] BGR: a numpy array or a tensor on the host
@@ -147,14 +191,20 @@ def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr
     host synchronisation happens per tile or per batch; the merge reads the kept rows once and the RLE encode
     synchronises twice.
 
+    ``merge_nms_type`` ('nms' or 'soft_nms', the demo's ``--merge-nms-type``) selects the cross-tile merge; see
+    merge_tile_records for what soft_nms returns and how ``score_thr`` applies to it.
+
     Returns a DetDataSample with ori_shape = img_shape = (H, W), scale_factor (1, 1) and pred_instances: bboxes,
     scores, labels on the device in descending score order, masks a list of {'size': [H, W], 'counts': bytes} (the
     test_cfg.rle_masks convention, passed through by CocoMetric.process)."""
-    records, batches = run_tiles(model, image, overlap_ratio, batch_size, patch_size=patch_size)
+    if merge_nms_type not in MERGE_NMS_TYPES:
+        raise ValueError(f"merge nms type {merge_nms_type!r} is not supported (supported: {', '.join(MERGE_NMS_TYPES)})")
+    records, batches = run_tiles(model, image, overlap_ratio, batch_size, patch_size=patch_size,
+                                 merge_nms_type=merge_nms_type)
     H, W = int(image.shape[0]), int(image.shape[1])
     window = None if patch_size is None else (int(patch_size), int(patch_size))
     merged = merge_tile_records(records, batches, (H, W), merge_iou_thr=merge_iou_thr, score_thr=score_thr,
-                                window=window)
+                                window=window, nms_type=merge_nms_type)
     masks = encode_kept_masks(records, batches, merged["source"], (H, W), window=window)
     ds = DetDataSample(metainfo=dict(ori_shape=(H, W), img_shape=(H, W), scale_factor=(1.0, 1.0)))
     ds.pred_instances = InstanceData(bboxes=merged["bboxes"], scores=merged["scores"], labels=merged["labels"],
@@ -163,7 +213,8 @@ def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr
 
 
 @torch.no_grad()
-def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8, patch_size: int | None = None):
+def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8, patch_size: int | None = None,
+              merge_nms_type: str = "nms"):
     """The tile stage of predict_large_image -> (records, origins per record), everything left on the device.
     Records of resized patches hold each tile's result in P x P window coordinates on a canvas of
     (P, P rounded up to 16)."""
@@ -194,8 +245,10 @@ def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8, pa
     if N > MAX_MERGE_CANDIDATES:
         raise ValueError(f"{len(origins)} tiles x {M} slots = {N} merge candidates; the dense NMS takes at most "
                          f"{MAX_MERGE_CANDIDATES}")
+    merge_ws = (_lib.soft_nms_workspace_bytes(1, N, 1024) + N * 64 if merge_nms_type == "soft_nms"   # O(N) + gathers
+                else N * ((N + 63) // 64) * 8)
     need = (len(batches) * _record_nbytes(B, M, rec_hw) + (0 if img.is_cuda else H * W * 3)
-            + N * ((N + 63) // 64) * 8 + (B * 3 * S * S * 4 if resize else 0))
+            + merge_ws + (B * 3 * S * S * 4 if resize else 0))
     free, _ = torch.cuda.mem_get_info(dev)
     free += torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
     if need > free:
@@ -293,6 +346,8 @@ def main(argv=None) -> list:
     ap.add_argument("--patch-overlap-ratio", type=float, default=0.25)
     ap.add_argument("--merge-iou-thr", type=float, default=0.25)
     ap.add_argument("--score-thr", type=float, default=0.0)
+    ap.add_argument("--merge-nms-type", default="nms", choices=MERGE_NMS_TYPES,
+                    help="NMS type of the cross-tile merge (soft_nms: linear, sigma 0.5, min_score 1e-3)")
     ap.add_argument("--batch-size", type=int, default=8)
     ap.add_argument("--patch-size", type=int, default=None,
                     help="window size; each window is resized to the model size (default: model-size windows, "
@@ -313,7 +368,8 @@ def main(argv=None) -> list:
     if img is None:
         raise FileNotFoundError(args.image)
     ds = predict_large_image(model, img, overlap_ratio=args.patch_overlap_ratio, merge_iou_thr=args.merge_iou_thr,
-                             score_thr=args.score_thr, batch_size=args.batch_size, patch_size=args.patch_size)
+                             score_thr=args.score_thr, batch_size=args.batch_size, patch_size=args.patch_size,
+                             merge_nms_type=args.merge_nms_type)
     res = coco_results(ds)
     text = json.dumps(res)
     if args.out:
