@@ -136,6 +136,14 @@ int rsp_gemm_bf16_ex(const void* A, int lda, const void* W, int ldw, void* out, 
                      int res_block_rows, const float* hyper, float* mask_out, int grid_h, int grid_w,
                      void* stream);
 
+/* epi_mode 3 for n_out (1..3) hypernetwork vectors per prompt in one GEMM: A bf16 [M, K] up1 rows (prompt, y, x,
+ * tap1), W bf16 [128, K], hyper fp32 [prompts, n_out, 32] -> mask_out fp32 [prompts, n_out, 4*grid_h, 4*grid_w].
+ * The multimask_output upscale of SamMaskDecoder (HF:521-531, mask_slice 1:): each accumulator tile of
+ * upscale_conv2 feeds all n_out products, so the up1 rows are read once.  Output o has the bytes of
+ * rsp_gemm_bf16_ex(epi_mode 3) with hyper[:, o].  grid_w even; hyper, bias 16-byte and mask_out 8-byte aligned. */
+int rsp_gemm_upscale_masks(const void* A, int lda, const void* W, int ldw, int M, int K, const float* bias,
+                           const float* hyper, int n_out, float* mask_out, int grid_h, int grid_w, void* stream);
+
 /* out = bf16(a + b[i % b_mod]) over n fp32 elements (b NULL = plain cast; n, b_mod % 4 == 0):
  * "queries + query_point_embedding" before a projection (HF:318,325,338). */
 int rsp_add_cast_bf16(const float* a, const float* b, void* out, long long n, long long b_mod,
@@ -317,6 +325,12 @@ int rsp_resize_bilinear_nhwc(const void* x, int B, int H, int W, int C, int h, i
  * ln2 g,b, conv3 w,b).  emb fp32 [imgs*h*w, 256], pos fp32 [h*w, 256], mpp fp32 [N, 4h, 4w]. */
 int rsp_mask_embed_src(const float* mpp, const float* const* wts, const float* emb, const float* pos, int N,
                        int n_per_img, int hm, int wm, int h, int w, float eps, void* src, void* src_pe, void* stream);
+
+/* SamMaskEmbedding.forward (HF:583-593) alone: masks fp32 [B, 4h, 4w] (a low-res mask prompt) -> dense fp32
+ * [B*h*w, 256] channels-last rows, the dense_embeddings of SamPromptEncoder.forward with input_masks (HF:691-692).
+ * wts as in rsp_mask_embed_src; dense 8-byte aligned. */
+int rsp_sam_mask_embed(const float* masks, const float* const* wts, int B, int hm, int wm, int h, int w, float eps,
+                       float* dense, void* stream);
 
 /* Mask resize of RSPrompterAnchorMaskHead._predict_by_feat_single for resized / padded images (M:1763-1777): maps
  * fp32 [n, hm, wm] (mode 2: already sigmoid-activated, >= thr; mode 1: raw, > thr) -> bilinear to (Hb, Wb) =

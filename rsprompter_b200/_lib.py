@@ -117,6 +117,8 @@ _SIGNATURES = {
     "rsp_mask_rle_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
     "rsp_mask_rle_placed_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp], _i),
     "rsp_mask_rle_placed_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
+    "rsp_gemm_upscale_masks": ([_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _i, _vp], _i),
+    "rsp_sam_mask_embed": ([_vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp], _i),
 }
 
 
@@ -300,6 +302,49 @@ def gemm_upscale_mask(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, hype
     launch_count += 1
     _log("gemm", 2.0 * M * 128 * K)
     return out
+
+
+def gemm_upscale_masks(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, hyper: torch.Tensor,
+                       grid_h: int, grid_w: int, out: torch.Tensor | None = None) -> torch.Tensor:
+    """gemm_upscale_mask for n_out <= 3 hypernetwork vectors per prompt in one GEMM (rsp_gemm_upscale_masks).
+
+    a: bf16 [P*4*h*w, 64]; hyper fp32 [P, n_out, 32] -> fp32 masks [P, n_out, 4h, 4w]; mask o equals
+    gemm_upscale_mask(a, w, bias, hyper[:, o]) byte for byte.  grid_w must be even."""
+    global launch_count
+    _require_cuda(a, w, bias, hyper, out)
+    M, K = a.shape
+    P = M // (4 * grid_h * grid_w)
+    assert a.dtype == torch.bfloat16 and a.stride(1) == 1 and w.dtype == torch.bfloat16 and w.shape == (128, K)
+    assert hyper.dtype == torch.float32 and hyper.dim() == 3 and hyper.shape[0] == P and hyper.shape[2] == 32
+    assert hyper.is_contiguous() and bias.dtype == torch.float32 and bias.numel() == 128 and bias.is_contiguous()
+    n_out = hyper.shape[1]
+    if out is None:
+        out = torch.empty((P, n_out, 4 * grid_h, 4 * grid_w), device=a.device, dtype=torch.float32)
+    assert out.is_contiguous() and out.dtype == torch.float32 and out.shape == (P, n_out, 4 * grid_h, 4 * grid_w)
+    st = _lib.rsp_gemm_upscale_masks(_ptr(a), a.stride(0), _ptr(w), w.stride(0), M, K, _ptr(bias), _ptr(hyper), n_out,
+                                     _ptr(out), grid_h, grid_w, _stream())
+    _check(st, "rsp_gemm_upscale_masks")
+    launch_count += 1
+    _log("gemm", 2.0 * M * 128 * K)
+    return out
+
+
+def sam_mask_embed(masks: torch.Tensor, weights: list, eps: float = 1e-6) -> torch.Tensor:
+    """SamMaskEmbedding: masks fp32 [B, 4h, 4w] -> dense fp32 [B*h*w, 256] channels-last rows (rsp_sam_mask_embed).
+    weights = 10 fp32 tensors (conv1 w,b, ln1 g,b, conv2 w,b, ln2 g,b, conv3 w,b)."""
+    global launch_count
+    _require_cuda(masks, *weights)
+    B, hm, wm = masks.shape
+    assert masks.dtype == torch.float32 and masks.is_contiguous() and len(weights) == 10
+    for t in weights:
+        assert t.dtype == torch.float32 and t.is_contiguous()
+    h, w = hm // 4, wm // 4
+    wp = (ctypes.c_void_p * 10)(*[t.data_ptr() for t in weights])
+    dense = torch.empty(B * h * w, 256, device=masks.device, dtype=torch.float32)
+    _check(_lib.rsp_sam_mask_embed(_ptr(masks), ctypes.cast(wp, _vp), B, hm, wm, h, w, float(eps), _ptr(dense),
+                                   _stream()), "rsp_sam_mask_embed")
+    launch_count += 1
+    return dense
 
 
 def add_cast_bf16(a: torch.Tensor, b: torch.Tensor | None = None, out: torch.Tensor | None = None) -> torch.Tensor:

@@ -154,6 +154,13 @@ int rsp_gemm_bf16_ex(const void* A, int lda, const void* W, int ldw, void* out, 
   return gemm_bf16(a, S(stream));
 }
 
+int rsp_gemm_upscale_masks(const void* A, int lda, const void* W, int ldw, int M, int K, const float* bias,
+                           const float* hyper, int n_out, float* mask_out, int grid_h, int grid_w, void* stream) {
+  GemmArgs a = make_gemm_args(A, lda, W, ldw, nullptr, 0, M, 128, K, bias, nullptr, 0, 1, 0, nullptr, 0, 0);
+  a.epi_mode = 3; a.hyper = hyper; a.mask_out = mask_out; a.grid_h = grid_h; a.grid_w = grid_w;
+  return gemm_upscale_masks(a, n_out, S(stream));
+}
+
 int rsp_add_cast_bf16(const float* a, const float* b, void* out, long long n, long long b_mod,
                       void* stream) {
   return add_cast_bf16(a, b, out, n, b_mod, S(stream));
@@ -326,6 +333,11 @@ int rsp_resize_bilinear_nhwc(const void* x, int B, int H, int W, int C, int h, i
 int rsp_mask_embed_src(const float* mpp, const float* const* wts, const float* emb, const float* pos, int N,
                        int n_per_img, int hm, int wm, int h, int w, float eps, void* src, void* src_pe, void* stream) {
   return mask_embed_src(mpp, wts, emb, pos, N, n_per_img, hm, wm, h, w, eps, src, src_pe, S(stream));
+}
+
+int rsp_sam_mask_embed(const float* masks, const float* const* wts, int B, int hm, int wm, int h, int w, float eps,
+                       float* dense, void* stream) {
+  return sam_mask_embed(masks, wts, B, hm, wm, h, w, eps, dense, S(stream));
 }
 
 int rsp_mask_paste_rescale(const float* maps, uint8_t* out, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w,

@@ -465,6 +465,18 @@ static int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   return RSP_OK;
 }
 
+int gemm_upscale_masks(const GemmArgs& a, int n_out, cudaStream_t stream) {
+  RSP_CHECK_ARG(a.A && a.W && a.bias && a.hyper && a.mask_out, "gemm_upscale_masks: null pointer");
+  RSP_CHECK_ARG(n_out >= 1 && n_out <= 3, "gemm_upscale_masks: n_out %d (1 to 3)", n_out);
+  RSP_CHECK_ARG(a.M > 0 && a.K > 0 && a.N == 128 && a.lda % 8 == 0 && a.ldw % 8 == 0 && a.grid_h > 0 &&
+                a.grid_w > 0 && a.grid_w % 2 == 0 && a.M % (4 * a.grid_h * a.grid_w) == 0,
+                "gemm_upscale_masks: needs N == 128, an even grid_w and M = prompts * 4 * h * w");
+  auto al = [](const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; };
+  // float4 hyper and bias loads, float2 mask stores
+  RSP_CHECK_ARG(al(a.hyper, 16) && al(a.bias, 16) && al(a.mask_out, 8), "gemm_upscale_masks: alignment");
+  return gemm_bf16_v2_gelu_hyper_multi(a, n_out, stream);
+}
+
 int gemm_bf16(const GemmArgs& a, cudaStream_t stream) {
   RSP_CHECK_ARG(a.A && a.W && (a.out || a.mask_out), "gemm: null pointer");
   RSP_CHECK_ARG(a.M > 0 && a.N > 0 && a.K > 0, "gemm: bad shape %d %d %d", a.M, a.N, a.K);

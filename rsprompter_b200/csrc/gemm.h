@@ -50,5 +50,9 @@ bool gemm_v2_ln_row_eligible(const GemmArgs& a);
 int gemm_bf16_v2_ln_row(const GemmArgs& a, cudaStream_t stream);             // N == 256, bf16 residual / out
 int gemm_bf16_v2_ln64_gelu(const GemmArgs& a, cudaStream_t stream);     // N % 128 == 0
 int gemm_bf16_v2_gelu_hyper(const GemmArgs& a, cudaStream_t stream);    // N == 128
+// N == 128, hyper [prompts, n_out, 32], mask_out [prompts, n_out, 4*grid_h, 4*grid_w], 1 <= n_out <= 3
+int gemm_bf16_v2_gelu_hyper_multi(const GemmArgs& a, int n_out, cudaStream_t stream);
+// checked entry of the multi-output upscale (epi_mode 3 arguments + n_out; grid_w even)
+int gemm_upscale_masks(const GemmArgs& a, int n_out, cudaStream_t stream);
 
 }  // namespace rsp

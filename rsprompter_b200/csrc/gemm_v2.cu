@@ -35,7 +35,11 @@ constexpr int STG_WARP = 32 * STG_ROW;
 constexpr int BAR_BYTES = 256;
 constexpr int SMEM_MAX = 227 * 1024;
 
-enum { EPI_STD = 0, EPI_LN_ROW = 1, EPI_LN64_GELU = 2, EPI_GELU_HYPER = 3 };
+// EPI_GELU_HYPER2 / 3: EPI_GELU_HYPER with 2 / 3 hypernetwork vectors per prompt (multimask_output); the output count
+// is part of the instantiation, so the single-output kernel is compiled exactly as before
+enum { EPI_STD = 0, EPI_LN_ROW = 1, EPI_LN64_GELU = 2, EPI_GELU_HYPER = 3, EPI_GELU_HYPER2 = 4, EPI_GELU_HYPER3 = 5 };
+
+__host__ __device__ constexpr int hyper_outputs(int epi) { return epi == EPI_GELU_HYPER3 ? 3 : epi == EPI_GELU_HYPER2 ? 2 : 1; }
 
 template <int BN, int EPI>
 struct Cfg {
@@ -164,6 +168,64 @@ __device__ __forceinline__ void epilogue_tile(const Dev& p, const CUtensorMap& t
       const int Y = 4 * y + 2 * (tap1 >> 1) + hf, X = 4 * x + 2 * (tap1 & 1);
       *reinterpret_cast<float2*>(p.mask_out + (static_cast<size_t>(n) * 4 * p.grid_h + Y) * W4 + X) =
           make_float2(m2[0], m2[1]);
+    }
+  } else if constexpr (EPI == EPI_GELU_HYPER2 || EPI == EPI_GELU_HYPER3) {
+    // the EPI_GELU_HYPER tile for NO outputs: hyper [prompt, NO, 32], mask_out [prompt, NO, 4h, 4w].  GELU(acc + bias)
+    // is evaluated once per element and feeds NO sums; each sum takes its terms in the single-output order, so output
+    // o has the bytes of an EPI_GELU_HYPER launch with hyper[:, o], and the up1 rows are read once instead of NO times
+    constexpr int NO = hyper_outputs(EPI);
+    const int row = m_blk * BM + q * 32 + lane;
+    const bool valid = row < p.M;
+    const int rows_per_prompt = p.grid_h * p.grid_w * 4;
+    const int n = valid ? row / rows_per_prompt : 0;
+    const int rem = row - n * rows_per_prompt;
+    const int tap1 = rem & 3, pix = rem >> 2;
+    const int y = pix / p.grid_w, x = pix - y * p.grid_w;
+    float hyp[NO][32];
+#pragma unroll
+    for (int o = 0; o < NO; ++o) {
+      const float4* h4 = reinterpret_cast<const float4*>(p.hyper + (static_cast<size_t>(n) * NO + o) * 32);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float4 h = __ldg(h4 + i);
+        hyp[o][4 * i] = h.x; hyp[o][4 * i + 1] = h.y; hyp[o][4 * i + 2] = h.z; hyp[o][4 * i + 3] = h.w;
+      }
+    }
+    const uint32_t t_row = acc_row(acc_base, C::ACC_LD, q * 32 + lane) + 4 * hf * 64;
+    float m2[NO][2];
+#pragma unroll
+    for (int t = 0; t < 2; ++t) {
+      uint32_t r[32];
+      acc_ld32(t_row + (t * 32) * 4, r);
+      const float4* b4 = reinterpret_cast<const float4*>(p.bias + hf * 64 + t * 32);
+      float acc[NO];
+#pragma unroll
+      for (int o = 0; o < NO; ++o) acc[o] = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float4 b = __ldg(b4 + i);
+        const float g0 = gelu_fast(__uint_as_float(r[4 * i]) + b.x);
+        const float g1 = gelu_fast(__uint_as_float(r[4 * i + 1]) + b.y);
+        const float g2 = gelu_fast(__uint_as_float(r[4 * i + 2]) + b.z);
+        const float g3 = gelu_fast(__uint_as_float(r[4 * i + 3]) + b.w);
+#pragma unroll
+        for (int o = 0; o < NO; ++o) {
+          acc[o] += g0 * hyp[o][4 * i];
+          acc[o] += g1 * hyp[o][4 * i + 1];
+          acc[o] += g2 * hyp[o][4 * i + 2];
+          acc[o] += g3 * hyp[o][4 * i + 3];
+        }
+      }
+#pragma unroll
+      for (int o = 0; o < NO; ++o) m2[o][t] = acc[o];
+    }
+    if (valid) {
+      const int W4 = 4 * p.grid_w;
+      const int Y = 4 * y + 2 * (tap1 >> 1) + hf, X = 4 * x + 2 * (tap1 & 1);
+#pragma unroll
+      for (int o = 0; o < NO; ++o)
+        *reinterpret_cast<float2*>(p.mask_out + ((static_cast<size_t>(n) * NO + o) * 4 * p.grid_h + Y) * W4 + X) =
+            make_float2(m2[o][0], m2[o][1]);
     }
   } else if constexpr (EPI == EPI_LN_ROW) {
     // out = LayerNorm_256(acc + bias + residual), bf16 (N == BN == 256: the tile holds whole rows).  Two warps
@@ -930,6 +992,15 @@ int gemm_bf16_v2_ln64_gelu(const GemmArgs& a, cudaStream_t stream) {
 
 int gemm_bf16_v2_gelu_hyper(const GemmArgs& a, cudaStream_t stream) {
   return v2::launch<128, v2::EPI_GELU_HYPER>(a, stream);
+}
+
+int gemm_bf16_v2_gelu_hyper_multi(const GemmArgs& a, int n_out, cudaStream_t stream) {
+  switch (n_out) {
+    case 1: return v2::launch<128, v2::EPI_GELU_HYPER>(a, stream);
+    case 2: return v2::launch<128, v2::EPI_GELU_HYPER2>(a, stream);
+    case 3: return v2::launch<128, v2::EPI_GELU_HYPER3>(a, stream);
+    default: set_last_error("gemm_v2: %d hypernetwork outputs (1 to 3)", n_out); return RSP_ERR_INVALID;
+  }
 }
 
 }  // namespace rsp

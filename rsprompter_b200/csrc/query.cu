@@ -745,6 +745,96 @@ int mask_embed_src(const float* mpp, const float* const* wts, const float* emb, 
   return RSP_OK;
 }
 
+// SamMaskEmbedding alone, fp32 out: the dense prompt embedding of HF SamPromptEncoder.forward (HF:691-692) as
+// channels-last rows [B*h*w, 256].  A kernel of its own (the two above feed the query head and stay as they are):
+// block = 32 pixels of one mask; thread = pixel for the two stride-2 convs, then thread = 2 output channels for the 1x1.
+__global__ void sam_mask_embed_kernel(const float* __restrict__ masks, MaskEmbedW W, int hm, int wm, int h, int w,
+                                      float eps, float* __restrict__ dense) {
+  constexpr int PP = 32;
+  __shared__ __align__(16) float hid[PP][16];
+  const int b = blockIdx.y;
+  const int p0 = blockIdx.x * PP;
+  const int HW = h * w;
+  if (threadIdx.x < PP && p0 + threadIdx.x < HW) {
+    const int pix = p0 + threadIdx.x, y = pix / w, x = pix - y * w;
+    const float* in = masks + (static_cast<size_t>(b) * hm + 4 * y) * wm + 4 * x;
+    float h1[2][2][4];
+#pragma unroll
+    for (int py = 0; py < 2; ++py)
+#pragma unroll
+      for (int px = 0; px < 2; ++px) {
+        float a[4], mean = 0.f;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          float s = W.b1[c];
+#pragma unroll
+          for (int ky = 0; ky < 2; ++ky)
+#pragma unroll
+            for (int kx = 0; kx < 2; ++kx) s += W.w1[c * 4 + ky * 2 + kx] * in[(2 * py + ky) * wm + 2 * px + kx];
+          a[c] = s; mean += s;
+        }
+        mean *= 0.25f;
+        float var = 0.f;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) var += (a[c] - mean) * (a[c] - mean);
+        const float rstd = rsqrtf(var * 0.25f + eps);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) h1[py][px][c] = gelu_erf((a[c] - mean) * rstd * W.g1[c] + W.be1[c]);
+      }
+    float a2[16], mean = 0.f;
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+      float s = W.b2[c];
+#pragma unroll
+      for (int ci = 0; ci < 4; ++ci)
+#pragma unroll
+        for (int ky = 0; ky < 2; ++ky)
+#pragma unroll
+          for (int kx = 0; kx < 2; ++kx) s += W.w2[((c * 4 + ci) * 2 + ky) * 2 + kx] * h1[ky][kx][ci];
+      a2[c] = s; mean += s;
+    }
+    mean *= (1.0f / 16.0f);
+    float var = 0.f;
+#pragma unroll
+    for (int c = 0; c < 16; ++c) var += (a2[c] - mean) * (a2[c] - mean);
+    const float rstd = rsqrtf(var * (1.0f / 16.0f) + eps);
+#pragma unroll
+    for (int c = 0; c < 16; ++c) hid[threadIdx.x][c] = gelu_erf((a2[c] - mean) * rstd * W.g2[c] + W.be2[c]);
+  }
+  __syncthreads();
+  const int c = 2 * threadIdx.x;
+  float wa[16], wb[16];
+#pragma unroll
+  for (int k = 0; k < 16; ++k) { wa[k] = W.w3[c * 16 + k]; wb[k] = W.w3[(c + 1) * 16 + k]; }
+  const float ba = W.b3[c], bb = W.b3[c + 1];
+  const int npix = min(PP, HW - p0);
+#pragma unroll 4
+  for (int pp = 0; pp < npix; ++pp) {
+    float hv[16];
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4) {
+      const float4 v = *reinterpret_cast<const float4*>(&hid[pp][4 * k4]);
+      hv[4 * k4] = v.x; hv[4 * k4 + 1] = v.y; hv[4 * k4 + 2] = v.z; hv[4 * k4 + 3] = v.w;
+    }
+    float sa = ba, sb = bb;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) { sa = fmaf(wa[k], hv[k], sa); sb = fmaf(wb[k], hv[k], sb); }
+    *reinterpret_cast<float2*>(dense + (static_cast<size_t>(b) * HW + p0 + pp) * 256 + c) = make_float2(sa, sb);
+  }
+}
+
+int sam_mask_embed(const float* masks, const float* const* wts, int B, int hm, int wm, int h, int w, float eps,
+                   float* dense, cudaStream_t stream) {
+  RSP_CHECK_ARG(masks && wts && dense && B > 0 && h > 0 && w > 0 && hm == 4 * h && wm == 4 * w,
+                "sam_mask_embed: bad args");
+  RSP_CHECK_ARG((reinterpret_cast<uintptr_t>(dense) & 7) == 0, "sam_mask_embed: dense must be 8-byte aligned");
+  MaskEmbedW W{wts[0], wts[1], wts[2], wts[3], wts[4], wts[5], wts[6], wts[7], wts[8], wts[9]};
+  dim3 grid((h * w + 31) / 32, B);
+  sam_mask_embed_kernel<<<grid, 128, 0, stream>>>(masks, W, hm, wm, h, w, eps, dense);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
 // ------------------------------------------------------------------------------------ query post-process
 // grid (rows / ROWS, instances); logits fp32 [n_maps, hm, wm]; sel int32 [n_inst] map index of each instance.
 // Writes the boolean mask and per-block partials (sum sigmoid over positives, count, bbox) reduced by

@@ -13,6 +13,8 @@ int attn_mask_bits(const float* logits, int ld, int rows, int nk, unsigned long 
 int resize_bilinear_nhwc(const void* x, int B, int H, int W, int C, int h, int w, void* out, cudaStream_t stream);
 int mask_embed_src(const float* mpp, const float* const* wts, const float* emb, const float* pos, int N, int n_per_img,
                    int hm, int wm, int h, int w, float eps, void* src, void* src_pe, cudaStream_t stream);
+int sam_mask_embed(const float* masks, const float* const* wts, int B, int hm, int wm, int h, int w, float eps,
+                   float* dense, cudaStream_t stream);
 int query_postprocess(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm, int H,
                       int W, unsigned char* masks, float* part_ws, float* scores, float* boxes, cudaStream_t stream);
 

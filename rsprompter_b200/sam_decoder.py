@@ -197,11 +197,13 @@ class SamMaskDecoderB200(nn.Module):
     def decode(self, emb_rows: torch.Tensor, pos_rows: torch.Tensor, sparse: torch.Tensor,
                hw: tuple[int, int], prompt_img: torch.Tensor | None = None,
                dense_vec: torch.Tensor | None = None, dense_rows: torch.Tensor | None = None,
-               multimask_output: bool = False, src_pair: tuple | None = None):
+               multimask_output: bool = False, src_pair: tuple | None = None,
+               dense_img_rows: torch.Tensor | None = None):
         """emb_rows fp32 [Bi*HW, C] channels-last image embeddings (Bi images, or N when
         prompt_img is None); pos_rows fp32 [HW, C]; sparse fp32 [N, P, C]; prompt_img int32 [N]
         image of each prompt; dense_vec fp32 [C] (no_mask_embed broadcast, M:1680) or dense_rows
-        fp32 [N*HW, C] per-prompt dense embeddings (M:362).
+        fp32 [N*HW, C] per-prompt dense embeddings (M:362) or dense_img_rows fp32 [Bi*HW, C] per-image
+        dense embeddings (a mask prompt, HF:499-500), added once per image and shared by its prompts.
         -> masks fp32 [N, n_out, 4h, 4w], iou fp32 [N, n_out]."""
         p = self._prep or self._prepare()
         a = self.arch
@@ -224,6 +226,10 @@ class SamMaskDecoderB200(nn.Module):
                 emb_rows = emb_rows.view(-1, HW, C)[prompt_img.long()].reshape(N * HW, C)
             src32 = emb_rows + dense_rows
             blk = None
+        elif dense_img_rows is not None:
+            # one dense term per image: src = emb + dense on the image's rows, and the prompts keep sharing them
+            src32 = emb_rows + dense_img_rows
+            blk = prompt_img if shared else None
         else:
             src32 = emb_rows if dense_vec is None else emb_rows + dense_vec.view(1, C)
             blk = prompt_img if shared else None
@@ -299,6 +305,12 @@ class SamMaskDecoderB200(nn.Module):
         up1 = _lib.gemm(keys_b, p["up1_w"], p["up1_b"], ln64_gelu=(*p["up_ln"], 1e-6))   # [N*HW, 4*64]
         up1 = up1.view(N * HW * 4, -1)
         sel = range(1, self.num_mask_tokens) if multimask_output else range(0, 1)
+        if len(sel) > 1 and w % 2 == 0:
+            # every output mask from one pass over up1: [N, n_out, 32] hypernetwork vectors, one GEMM, the masks
+            # written in place ([N, n_out, 4h, 4w]); each equals its single-output launch byte for byte
+            hyper = torch.stack([self._ff(_lib.cast_bf16(qv[:, 1 + i].contiguous()), p["hyper"][i]) for i in sel], dim=1)
+            masks = _lib.gemm_upscale_masks(up1, p["up2_w"], p["up2_b"], hyper, h, w)
+            return masks, iou[:, 1:]
         masks = []
         for i in sel:
             mt = _lib.cast_bf16(qv[:, 1 + i].contiguous())
@@ -312,15 +324,33 @@ class SamMaskDecoderB200(nn.Module):
                 dense_prompt_embeddings, multimask_output, attention_similarity=None,
                 target_embedding=None, output_attentions=None):
         """Reference signature (HF:461-470 + the 3-tuple of transformers 4.38 the callers unpack,
-        M:369, M:1685).  Per-prompt NCHW inputs; point_batch_size must be 1."""
+        M:369, M:1685).  NCHW image_embeddings / dense [B, C, h, w], sparse [B, point_batch, P, C] (or None: no sparse
+        tokens).  point_batch 1 is the RSPrompter heads' per-prompt call; with point_batch > 1 the point_batch prompts
+        of an image share its embedding (HF:499-501) through the block map instead of repeat_interleave copies.
+        -> (masks [B, point_batch, n_out, 4h, 4w], iou [B, point_batch, n_out], None)."""
         if attention_similarity is not None or target_embedding is not None:
             raise NotImplementedError("attention_similarity / target_embedding are not used by RSPrompter")
         N, C, h, w = image_embeddings.shape
-        assert sparse_prompt_embeddings.shape[1] == 1, "point_batch_size must be 1"
+        if sparse_prompt_embeddings is None:
+            sparse_prompt_embeddings = image_embeddings.new_zeros(N, 1, 0, C)
+        if sparse_prompt_embeddings.dim() != 4 or sparse_prompt_embeddings.shape[0] != N:
+            raise ValueError(f"sparse_prompt_embeddings must be [batch, point_batch, P, C] with batch {N}, "
+                             f"got {tuple(sparse_prompt_embeddings.shape)}")
+        check_sparse_tokens(sparse_prompt_embeddings.shape[2], self.num_mask_tokens)
         to_rows = lambda t: t.to(torch.float32).permute(0, 2, 3, 1).reshape(-1, C).contiguous()  # noqa: E731
         pos_rows = to_rows(image_positional_embeddings[:1])
+        pb = sparse_prompt_embeddings.shape[1]
+        if pb > 1:
+            dense = dense_prompt_embeddings.expand(N, -1, -1, -1)
+            prompt_img = torch.arange(N, device=image_embeddings.device, dtype=torch.int32).repeat_interleave(pb)
+            P = sparse_prompt_embeddings.shape[2]
+            masks, iou = self.decode(to_rows(image_embeddings), pos_rows,
+                                     sparse_prompt_embeddings.reshape(N * pb, P, C).contiguous(), (h, w),
+                                     prompt_img=prompt_img.contiguous(), dense_img_rows=to_rows(dense),
+                                     multimask_output=multimask_output)
+            return masks.view(N, pb, *masks.shape[1:]), iou.view(N, pb, -1), None
         masks, iou = self.decode(to_rows(image_embeddings), pos_rows, sparse_prompt_embeddings[:, 0],
-                                 (h, w), dense_rows=to_rows(dense_prompt_embeddings),
+                                 (h, w), dense_rows=to_rows(dense_prompt_embeddings.expand(N, -1, -1, -1)),
                                  multimask_output=multimask_output)
         return masks.unsqueeze(1), iou.unsqueeze(1), None
 
@@ -404,13 +434,63 @@ class _MaskEmbed(nn.Module):
         self.layer_norm2 = _Affine((mc,))
 
 
+    def kernel_weights(self) -> list:
+        """The 10 fp32 tensors of rsp_sam_mask_embed / rsp_mask_embed_src (conv1 w,b, ln1 g,b, conv2 w,b, ln2 g,b,
+        conv3 w,b)."""
+        f32 = lambda t: t.detach().to(torch.float32).contiguous()  # noqa: E731
+        return [f32(t) for t in (self.conv1.weight, self.conv1.bias, self.layer_norm1.weight, self.layer_norm1.bias,
+                                 self.conv2.weight, self.conv2.bias, self.layer_norm2.weight, self.layer_norm2.bias,
+                                 self.conv3.weight.reshape(self.conv3.weight.shape[0], -1), self.conv3.bias)]
+
+    @torch.no_grad()
+    def dense_rows(self, masks: torch.Tensor, eps: float) -> torch.Tensor:
+        """SamMaskEmbedding(masks) for masks [B, 1, 4h, 4w] -> fp32 [B*h*w, C] channels-last rows on the device."""
+        if masks.dim() != 4 or masks.shape[1] != 1:
+            raise ValueError(f"input_masks must be [batch, 1, 4h, 4w], got {tuple(masks.shape)}")
+        dev = self.conv1.weight.device
+        return _lib.sam_mask_embed(masks[:, 0].to(dev, torch.float32).contiguous(), self.kernel_weights(), eps)
+
+
+# token kernels of the mask decoder: T = 1 + num_mask_tokens + P <= 16 tokens per prompt
+MAX_TOKENS = 16
+
+
+def check_sparse_tokens(P: int, num_mask_tokens: int = 4) -> None:
+    """Raise ValueError when P sparse tokens per prompt exceed what the decoder's token kernels take."""
+    limit = MAX_TOKENS - 1 - num_mask_tokens
+    if P > limit:
+        raise ValueError(f"{P} sparse prompt tokens per prompt (points + pad point + 2 per box): the mask decoder's "
+                         f"token kernels take at most {limit} ({MAX_TOKENS} tokens with the iou and mask tokens)")
+
+
 class SamPromptEncoderB200(nn.Module):
-    """The members of HF SamPromptEncoder the RSPrompter heads touch (M:305-307, M:1635)."""
+    """HF SamPromptEncoder as RSSamPromptEncoder builds it (M:893): ``SamPromptEncoder(config,
+    shared_patch_embedding=None)`` of transformers 4.38, i.e. the parameter tree without ``shared_embedding``."""
 
     def __init__(self, a: SamDecoderArch):
         super().__init__()
+        self.arch = a
         self.no_mask_embed = _Embedding(1, a.hidden_size)
         self.mask_embed = _MaskEmbed(a)
+        self.point_embed = nn.ModuleList(_Embedding(1, a.hidden_size) for _ in range(4))
+        self.not_a_point_embed = _Embedding(1, a.hidden_size)
+        self.image_embedding_size = 64     # SamPromptEncoderConfig: image_size 1024 / patch_size 16
+
+    @torch.no_grad()
+    def forward(self, input_points=None, input_labels=None, input_boxes=None, input_masks=None):
+        """SamPromptEncoder.forward (HF:658-698) -> (sparse None, dense [B, C, h, w]).  Points and boxes need the
+        positional embedding this module does not have (shared_patch_embedding=None), so they raise, as in the
+        reference; SamModel.get_prompt_embeddings embeds them."""
+        if input_points is not None or input_boxes is not None:
+            raise ValueError("RSSamPromptEncoder has no positional embedding (built with shared_patch_embedding=None, "
+                             "M:893), so it cannot embed points or boxes: use RSSamModel.get_prompt_embeddings")
+        C = self.no_mask_embed.weight.shape[1]
+        if input_masks is not None:
+            rows = self.mask_embed.dense_rows(input_masks, self.arch.layer_norm_eps)
+            B, _, hm, wm = input_masks.shape
+            return None, rows.view(B, hm // 4, wm // 4, C).permute(0, 3, 1, 2)
+        g = self.image_embedding_size
+        return None, self.no_mask_embed.weight.reshape(1, -1, 1, 1).expand(1, -1, g, g)
 
 
 @MODELS.register_module(force=True)
@@ -425,6 +505,9 @@ class RSSamPromptEncoder(BaseModule):
     def init_weights(self):
         pass
 
+    def forward(self, *args, **kwargs):
+        return self.prompt_encoder(*args, **kwargs)
+
 
 __all__ = ["SamMaskDecoderB200", "RSSamMaskDecoder", "RSSamPositionalEmbedding", "RSSamPromptEncoder",
-           "SamPositionalEmbeddingB200", "SamPromptEncoderB200"]
+           "SamPositionalEmbeddingB200", "SamPromptEncoderB200", "MAX_TOKENS", "check_sparse_tokens"]

@@ -17,7 +17,7 @@ from torch import nn
 from . import _lib
 from .registry import MODELS, BaseModule, ConfigDict, InstanceData
 from .sam_config import decoder_arch, vision_arch
-from .sam_decoder import SamMaskDecoderB200, SamPositionalEmbeddingB200, _Embedding, _MaskEmbed
+from .sam_decoder import SamMaskDecoderB200, SamPositionalEmbeddingB200, _Embedding, _MaskEmbed, check_sparse_tokens
 from .sam_encoder import SamVisionEncoderB200, _load_pretrained
 
 
@@ -71,36 +71,171 @@ class SamModelB200(nn.Module):
         corner = torch.stack([pe.point_embed[2].weight[0], pe.point_embed[3].weight[0]]).to(emb.dtype)
         return emb + corner.view(1, 1, 2, -1)
 
+    def embed_points(self, points: torch.Tensor, labels: torch.Tensor, pad: bool) -> torch.Tensor:
+        """HF SamPromptEncoder._embed_points (HF:613-645): [B, pb, n, 2] image-space xy and [B, pb, n] labels ->
+        sparse embeddings [B, pb, n (+1 with pad), C].  Label -1: not_a_point_embed; -10: zero; 0 / 1: + point_embed[0
+        / 1]; any other label keeps the bare positional embedding."""
+        pe = self.prompt_encoder
+        S = self.varch.image_size
+        coords = points.to(torch.float32) + 0.5
+        if pad:
+            coords = torch.cat([coords, coords.new_zeros(*coords.shape[:2], 1, 2)], dim=2)
+            labels = torch.cat([labels, labels.new_full((*labels.shape[:2], 1), -1)], dim=2)
+        emb = pe.shared_embedding(coords, (S, S))
+        lab = labels[..., None]
+        emb = torch.where(lab == -1, pe.not_a_point_embed.weight[0].to(emb.dtype), emb)
+        emb = torch.where(lab != -10, emb, torch.zeros_like(emb))
+        emb = torch.where(lab == 0, emb + pe.point_embed[0].weight[0].to(emb.dtype), emb)
+        return torch.where(lab == 1, emb + pe.point_embed[1].weight[0].to(emb.dtype), emb)
+
+    def _check_prompts(self, n_images, input_points, input_labels, input_boxes, input_masks, grid: int) -> tuple:
+        """HF SamModel.forward's shape rules (HF:1286-1334) plus the token bound of the decoder kernels, all before any
+        device work.  -> (point_batch, sparse tokens per prompt)."""
+        if input_points is not None and input_points.dim() != 4:
+            raise ValueError("The input_points must be a 4D tensor. Of shape `batch_size`, `point_batch_size`, "
+                             f"`nb_points_per_image`, `2`. got {tuple(input_points.shape)}.")
+        if input_points is not None and input_points.shape[-1] != 2:
+            raise ValueError(f"input_points must hold (x, y) pairs, got last dimension {input_points.shape[-1]}")
+        if input_boxes is not None and (input_boxes.dim() != 3 or input_boxes.shape[-1] != 4):
+            raise ValueError("The input_boxes must be a 3D tensor. Of shape `batch_size`, `nb_boxes`, `4`. "
+                             f"got {tuple(input_boxes.shape)}.")
+        if input_points is not None and input_boxes is not None and input_points.shape[1] != input_boxes.shape[1]:
+            raise ValueError("You should provide as many bounding boxes as input points per box. "
+                             f"Got {input_points.shape[1]} and {input_boxes.shape[1]}.")
+        for name, t in (("input points", input_points), ("input boxes", input_boxes)):
+            if t is not None and t.shape[0] != n_images:
+                raise ValueError(f"The batch size of the image embeddings and the {name} must be the same. "
+                                 f"Got {n_images} and {t.shape[0]} respectively.")
+        if input_labels is not None and input_points is not None and tuple(input_labels.shape) != tuple(input_points.shape[:3]):
+            raise ValueError(f"input_labels must be [batch, point_batch, n_points] like input_points[..., 0], got "
+                             f"{tuple(input_labels.shape)}")
+        if input_masks is not None and tuple(input_masks.shape) != (n_images, 1, 4 * grid, 4 * grid):
+            raise ValueError(f"input_masks must be [{n_images}, 1, {4 * grid}, {4 * grid}], got {tuple(input_masks.shape)}")
+        pb, P = 1, 0
+        if input_points is not None:
+            pb, P = input_points.shape[1], input_points.shape[2] + (1 if input_boxes is None else 0)
+        if input_boxes is not None:
+            pb, P = input_boxes.shape[1], P + 2
+        check_sparse_tokens(P, self.mask_decoder.num_mask_tokens)
+        return pb, P
+
+    def _sparse(self, input_points, input_labels, input_boxes, dev) -> torch.Tensor | None:
+        """sparse = cat([points (no pad point when boxes are given), box corners], dim=2) (HF:676-690)."""
+        parts = []
+        if input_points is not None:
+            if input_labels is None:
+                input_labels = torch.ones(input_points.shape[:3], dtype=torch.int32)
+            parts.append(self.embed_points(input_points.to(dev), input_labels.to(dev), pad=input_boxes is None))
+        if input_boxes is not None:
+            parts.append(self.embed_boxes(input_boxes.to(dev)))
+        if not parts:
+            return None
+        return parts[0] if len(parts) == 1 else torch.cat(parts, dim=2)
+
+    def _encode(self, pixel_values) -> torch.Tensor:
+        _, _, emb_nhwc = self.vision_encoder.encode(pixel_values, want_hidden=False)
+        return emb_nhwc
+
+    @torch.no_grad()
+    def get_image_embeddings(self, pixel_values) -> torch.Tensor:
+        """HF SamModel.get_image_embeddings (HF:1142-1155): fp32 [B, 256, g, g].  Passing them back as
+        forward(image_embeddings=...) gives the bytes of forward(pixel_values=...)."""
+        return self._encode(pixel_values).permute(0, 3, 1, 2)
+
+    @torch.no_grad()
+    def get_prompt_embeddings(self, input_points=None, input_labels=None, input_boxes=None, input_masks=None):
+        """HF SamModel.get_prompt_embeddings (HF:1158-1191) -> (sparse [B, pb, P, 256] or None, dense [B, 256, g, g]);
+        without a mask prompt dense is no_mask_embed broadcast over the batch of the sparse prompts (1 if none)."""
+        if input_points is not None and input_labels is None:
+            raise ValueError("If points are provided, labels must also be provided.")
+        g = self.varch.grid
+        n = next((t.shape[0] for t in (input_points, input_boxes, input_masks) if t is not None), 1)
+        self._check_prompts(n, input_points, input_labels, input_boxes, input_masks, g)
+        dev = self.prompt_encoder.no_mask_embed.weight.device
+        sparse = self._sparse(input_points, input_labels, input_boxes, dev)
+        C = self.darch.hidden_size
+        if input_masks is not None:
+            rows = self.prompt_encoder.mask_embed.dense_rows(input_masks, self.darch.layer_norm_eps)
+            return sparse, rows.view(n, g, g, C).permute(0, 3, 1, 2)
+        return sparse, self.prompt_encoder.no_mask_embed.weight.reshape(1, -1, 1, 1).expand(n, -1, g, g)
+
     @torch.no_grad()
     def forward(self, pixel_values=None, input_points=None, input_labels=None, input_boxes=None, input_masks=None,
                 image_embeddings=None, multimask_output: bool = True, attention_similarity=None, target_embedding=None,
                 **kwargs):
+        """HF SamModel.forward (HF:1193-1358): points [B, pb, n, 2] with labels [B, pb, n] (None: all 1), boxes
+        [B, pb, 4], points and boxes together, a low-res mask prompt [B, 1, 4g, 4g], pixel_values or image_embeddings.
+        -> iou_scores [B, pb, n_out], pred_masks [B, pb, n_out, 4g, 4g]."""
         if pixel_values is None and image_embeddings is None:
             raise ValueError("Either pixel_values or image_embeddings must be provided.")
         if pixel_values is not None and image_embeddings is not None:
             raise ValueError("Only one of pixel_values and image_embeddings can be provided.")
-        if input_boxes is None or input_points is not None or input_masks is not None:
-            raise NotImplementedError("rsprompter_b200 RSSamModel implements the box-prompted path SAMDet uses (M:1120-1131)")
-        if input_boxes.dim() != 3:
-            raise ValueError(f"The input_points must be a 3D tensor. Of shape `batch_size`, `nb_boxes`, `4`. got {input_boxes.shape}.")
         if attention_similarity is not None or target_embedding is not None:
             raise NotImplementedError("attention_similarity / target_embedding are not used by RSPrompter")
+        n_images = pixel_values.shape[0] if pixel_values is not None else image_embeddings.shape[0]
+        grid = self.varch.grid if pixel_values is not None else image_embeddings.shape[-1]
+        pb, _ = self._check_prompts(n_images, input_points, input_labels, input_boxes, input_masks, grid)
         C = self.darch.hidden_size
         if pixel_values is not None:
-            _, _, emb_nhwc = self.vision_encoder.encode(pixel_values, want_hidden=False)
+            emb_nhwc = self._encode(pixel_values)
         else:
             emb_nhwc = image_embeddings.to(torch.float32).permute(0, 2, 3, 1).contiguous()
         B, g = emb_nhwc.shape[0], emb_nhwc.shape[1]
-        nb = input_boxes.shape[1]
-        assert input_boxes.shape[0] == B
-        sparse = self.embed_boxes(input_boxes.to(emb_nhwc.device)).reshape(B * nb, 2, C).contiguous()
-        prompt_img = torch.arange(B, device=emb_nhwc.device, dtype=torch.int32).repeat_interleave(nb).contiguous()
+        dev = emb_nhwc.device
+        if input_points is None and input_masks is None and input_boxes is not None:
+            # boxes only (SAMDet, M:1120-1131)
+            nb = input_boxes.shape[1]
+            sparse = self.embed_boxes(input_boxes.to(dev)).reshape(B * nb, 2, C).contiguous()
+            prompt_img = torch.arange(B, device=dev, dtype=torch.int32).repeat_interleave(nb).contiguous()
+            pos_rows = self.shared_image_embedding.image_wide_rows(g)
+            dense = self.prompt_encoder.no_mask_embed.weight[0].to(torch.float32).contiguous()
+            masks, iou = self.mask_decoder.decode(emb_nhwc.reshape(B * g * g, C), pos_rows, sparse, (g, g),
+                                                  prompt_img=prompt_img, dense_vec=dense,
+                                                  multimask_output=multimask_output)
+            return SamImageSegmentationOutput(iou_scores=iou.view(B, nb, -1),
+                                              pred_masks=masks.view(B, nb, masks.shape[1], *masks.shape[-2:]))
+        sparse = self._sparse(input_points, input_labels, input_boxes, dev)
+        if sparse is None:                 # no sparse prompt: the 5 output tokens alone (HF:487-495)
+            sparse = emb_nhwc.new_zeros(B, 1, 0, C)
+        P = sparse.shape[2]
+        sparse = sparse.reshape(B * pb, P, C).contiguous()
+        prompt_img = torch.arange(B, device=dev, dtype=torch.int32).repeat_interleave(pb).contiguous()
         pos_rows = self.shared_image_embedding.image_wide_rows(g)
-        dense = self.prompt_encoder.no_mask_embed.weight[0].to(torch.float32).contiguous()
-        masks, iou = self.mask_decoder.decode(emb_nhwc.reshape(B * g * g, C), pos_rows, sparse, (g, g),
-                                              prompt_img=prompt_img, dense_vec=dense, multimask_output=multimask_output)
-        return SamImageSegmentationOutput(iou_scores=iou.view(B, nb, -1),
-                                          pred_masks=masks.view(B, nb, masks.shape[1], *masks.shape[-2:]))
+        emb_rows = emb_nhwc.reshape(B * g * g, C)
+        if input_masks is not None:        # one dense term per image (HF:499-500), shared by its prompts
+            dense_img = self.prompt_encoder.mask_embed.dense_rows(input_masks, self.darch.layer_norm_eps)
+            masks, iou = self.mask_decoder.decode(emb_rows, pos_rows, sparse, (g, g), prompt_img=prompt_img,
+                                                  dense_img_rows=dense_img, multimask_output=multimask_output)
+        else:
+            dense = self.prompt_encoder.no_mask_embed.weight[0].to(torch.float32).contiguous()
+            masks, iou = self.mask_decoder.decode(emb_rows, pos_rows, sparse, (g, g), prompt_img=prompt_img,
+                                                  dense_vec=dense, multimask_output=multimask_output)
+        return SamImageSegmentationOutput(iou_scores=iou.view(B, pb, -1),
+                                          pred_masks=masks.view(B, pb, masks.shape[1], *masks.shape[-2:]))
+
+
+@torch.no_grad()
+def post_process_masks(masks, original_sizes, reshaped_input_sizes, mask_threshold: float = 0.0,
+                       binarize: bool = True, pad_size=(1024, 1024)) -> list:
+    """HF SamProcessor.post_process_masks on the device: per image, low-res logits [pb, n_out, h, w] -> bilinear to
+    pad_size -> crop to the reshaped (resized, unpadded) input size -> bilinear to the original size -> > threshold, in
+    one fused kernel (rsp_mask_paste_rescale, the SAMDet path).  -> list of bool [pb, n_out, H, W]."""
+    if not binarize:
+        raise ValueError("post_process_masks computes binary masks only (binarize=False is not supported)")
+    if len(original_sizes) != len(masks) or len(reshaped_input_sizes) != len(masks):
+        raise ValueError("masks, original_sizes and reshaped_input_sizes need one entry per image")
+    out = []
+    for m, ori, rs in zip(masks, original_sizes, reshaped_input_sizes):
+        ori = tuple(int(v) for v in ori)
+        rs = tuple(int(v) for v in rs)
+        lead = m.shape[:-2]
+        logits = m.reshape(-1, *m.shape[-2:]).to(torch.float32).contiguous()
+        if logits.shape[0] == 0:
+            out.append(torch.zeros(*lead, *ori, dtype=torch.bool, device=m.device))
+            continue
+        bits = _lib.mask_paste_rescale(logits, tuple(int(v) for v in pad_size), rs, ori, float(mask_threshold), raw=True)
+        out.append(bits.view(*lead, *ori))
+    return out
 
 
 @MODELS.register_module(force=True)
@@ -119,6 +254,12 @@ class RSSamModel(BaseModule):
 
     def forward(self, *args, **kwargs):
         return self.sam_model(*args, **kwargs)
+
+    def get_image_embeddings(self, pixel_values):
+        return self.sam_model.get_image_embeddings(pixel_values)
+
+    def get_prompt_embeddings(self, input_points=None, input_labels=None, input_boxes=None, input_masks=None):
+        return self.sam_model.get_prompt_embeddings(input_points, input_labels, input_boxes, input_masks)
 
 
 @MODELS.register_module(force=True)
@@ -179,4 +320,4 @@ class SAMDet(BaseModule):
         return self.predict(data["inputs"], data.get("data_samples"))
 
 
-__all__ = ["SamModelB200", "RSSamModel", "SAMDet", "SamImageSegmentationOutput"]
+__all__ = ["SamModelB200", "RSSamModel", "SAMDet", "SamImageSegmentationOutput", "post_process_masks"]

@@ -104,7 +104,8 @@ def mask_decoder_state_dict(arch: SamDecoderArch | None = None, seed: int = 1) -
 
 
 def prompt_encoder_state_dict(arch: SamDecoderArch | None = None, seed: int = 2) -> dict[str, torch.Tensor]:
-    """The members of HF ``SamPromptEncoder`` the path uses (M:305-307,1635): no_mask_embed, mask_embed."""
+    """HF ``SamPromptEncoder`` as RSSamPromptEncoder builds it (no shared_embedding): no_mask_embed, mask_embed, then
+    point_embed.{0..3} and not_a_point_embed, drawn after the others so the earlier tensors keep their values."""
     arch = arch or SamDecoderArch()
     gen = torch.Generator().manual_seed(seed)
     C, mc = arch.hidden_size, arch.mask_input_channels
@@ -118,6 +119,9 @@ def prompt_encoder_state_dict(arch: SamDecoderArch | None = None, seed: int = 2)
     _norm(sd, gen, "mask_embed.layer_norm2", mc)
     sd["mask_embed.conv3.weight"] = _randn(gen, C, mc, 1, 1, std=0.25)
     sd["mask_embed.conv3.bias"] = _randn(gen, C, std=0.1)
+    for i in range(4):
+        sd[f"point_embed.{i}.weight"] = _randn(gen, 1, C, std=0.5)
+    sd["not_a_point_embed.weight"] = _randn(gen, 1, C, std=0.5)
     return sd
 
 
