@@ -15,8 +15,9 @@ m = (torch.rand(3, 5, 100, generator=g) > 0.5).to(dev)
 bits = _lib.pack_mask_bits(m)
 assert torch.equal(_lib.unpack_mask_bits(bits, 100), m)
 logits = (torch.randn(4, 16, 16, generator=g) * 3).to(dev)
-_lib.mask_paste_bits(logits, 0.5, 0)
-_lib.query_postprocess_bits(logits, torch.tensor([1, 3], dtype=torch.int32, device=dev), torch.rand(2, device=dev))
+_lib.mask_paste(logits, 0.5, raw=False, bits=torch.empty(4, 64, 8, dtype=torch.uint8, device=dev))
+_lib.query_postprocess(logits, torch.tensor([1, 3], dtype=torch.int32, device=dev), torch.rand(2, device=dev),
+                       bits=torch.empty(2, 64, 8, dtype=torch.uint8, device=dev))
 # uint8 preprocessing
 img = torch.randint(0, 256, (3, 45, 70), generator=g, dtype=torch.uint8).to(dev)
 _lib.preprocess_u8(img, torch.empty(3, 64, 96, device=dev), [1., 2., 3.], [4., 5., 6.], True, 0.0)

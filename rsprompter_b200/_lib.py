@@ -849,24 +849,50 @@ def roi_align_nhwc(feats: list, rois: torch.Tensor, P: int, strides: list, pes: 
     return out
 
 
-def mask_paste(logits: torch.Tensor, size: tuple, thr: float, mode: int) -> torch.Tensor:
-    """fp32 [n, hm, wm] -> bool [n, H, W]; mode 0 sigmoid+bilinear >= thr, mode 1 bilinear > thr."""
+def mask_paste(logits: torch.Tensor, thr: float, *, raw: bool, size: tuple | None = None,
+               rescale: tuple | None = None, bits: torch.Tensor | None = None) -> torch.Tensor:
+    """Mask logits fp32 [n, hm, wm], resized bilinearly and thresholded: raw=False sigmoid, then >= thr (M:1763-1777);
+    raw=True > thr on the resized logits (SAMDet, M:1133-1152).  size = (H, W): one resize; rescale = (batch_hw,
+    crop_hw, ori_hw) for a resized / padded image: to batch_hw -> crop -> to ori_hw.  -> bool [n, H, W], or with
+    ``bits`` the masks bit-packed into it: record slots uint8 [n, Hr, Wr/8] (Wr % 16 == 0, the mask at each slot's
+    top-left, 0 elsewhere) with rescale, uint8 [n, 4hm, 4wm/8] (the x4 resize) without."""
     global launch_count
-    _require_cuda(logits)
+    _require_cuda(logits, bits)
     assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.dim() == 3
+    assert size is None or rescale is None
     n, hm, wm = logits.shape
-    out = torch.empty(n, size[0], size[1], device=logits.device, dtype=torch.uint8)
-    if n > 0:
-        src = logits
-        if mode == 0 and logits.numel() % 4 == 0:   # activate once per low-res pixel, then paste
-            src = torch.empty_like(logits)
-            _check(_lib.rsp_sigmoid_f32(_ptr(logits), _ptr(src), logits.numel(), _stream()), "rsp_sigmoid_f32")
-            launch_count += 1
-            mode = 2
-        _check(_lib.rsp_mask_paste(_ptr(src), _ptr(out), n, hm, wm, size[0], size[1], float(thr), mode, _stream()),
+    if rescale is not None:
+        assert n > 0
+        (Hb, Wb), (ch, cw), (H, W) = rescale
+    if bits is None:
+        out = torch.empty(n, *(size if rescale is None else (H, W)), device=logits.device, dtype=torch.uint8)
+    elif rescale is None:
+        assert size is None or tuple(size) == (4 * hm, 4 * wm)
+        assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.numel() == n * 4 * hm * (wm // 2)
+    else:
+        assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.dim() == 3 and bits.shape[0] == n
+    if n == 0:
+        return out.view(torch.bool) if bits is None else bits
+    mode = 1 if raw else 2
+    if not raw and rescale is None and bits is None and logits.numel() % 4:
+        mode = 0   # rsp_sigmoid_f32 takes numel % 4 == 0; rsp_mask_paste's mode 0 activates the taps instead
+    elif not raw:
+        logits = sigmoid_f32(logits)   # activate once per low-res pixel, then paste
+    if rescale is None and bits is None:
+        _check(_lib.rsp_mask_paste(_ptr(logits), _ptr(out), n, hm, wm, size[0], size[1], float(thr), mode, _stream()),
                "rsp_mask_paste")
-        launch_count += 1
-    return out.view(torch.bool)
+    elif rescale is None:
+        _check(_lib.rsp_mask_paste_bits(_ptr(logits), _ptr(bits), n, hm, wm, float(thr), mode, _stream()),
+               "rsp_mask_paste_bits")
+    elif bits is None:
+        _check(_lib.rsp_mask_paste_rescale(_ptr(logits), _ptr(out), n, hm, wm, Hb, Wb, ch, cw, H, W, float(thr), mode,
+                                           _stream()), "rsp_mask_paste_rescale")
+    else:
+        _check(_lib.rsp_mask_paste_rescale_bits(_ptr(logits), _ptr(bits), n, hm, wm, Hb, Wb, ch, cw, H, W, bits.shape[1],
+                                                bits.shape[2] * 8, float(thr), mode, _stream()),
+               "rsp_mask_paste_rescale_bits")
+    launch_count += 1
+    return out.view(torch.bool) if bits is None else bits
 
 
 def sigmoid_f32(x: torch.Tensor) -> torch.Tensor:
@@ -902,27 +928,6 @@ def mask_paste_boxes(probs: torch.Tensor, boxes: torch.Tensor, size: tuple, thr:
                                          0 if bits is None else 1, _stream()), "rsp_mask_paste_boxes")
         launch_count += 1
     return out if bits is not None else out.view(torch.bool)
-
-
-def mask_paste_rescale(logits: torch.Tensor, batch_hw: tuple, crop_hw: tuple, ori_hw: tuple, thr: float,
-                       raw: bool = False) -> torch.Tensor:
-    """M:1763-1777 for a resized / padded image: sigmoid -> bilinear to batch_hw -> crop -> bilinear to ori_hw -> >= thr.
-    raw=True: no sigmoid, > thr on the resized logits (SAMDet, M:1133-1152).
-    logits fp32 [n, hm, wm] -> bool [n, ori_h, ori_w]."""
-    global launch_count
-    _require_cuda(logits)
-    n, hm, wm = logits.shape
-    assert logits.dtype == torch.float32 and logits.is_contiguous() and n > 0
-    act = logits
-    if not raw:
-        act = torch.empty_like(logits)
-        _check(_lib.rsp_sigmoid_f32(_ptr(logits), _ptr(act), logits.numel(), _stream()), "rsp_sigmoid_f32")
-        launch_count += 1
-    out = torch.empty(n, ori_hw[0], ori_hw[1], device=logits.device, dtype=torch.uint8)
-    _check(_lib.rsp_mask_paste_rescale(_ptr(act), _ptr(out), n, hm, wm, batch_hw[0], batch_hw[1], crop_hw[0], crop_hw[1],
-                                       ori_hw[0], ori_hw[1], float(thr), 1 if raw else 2, _stream()), "rsp_mask_paste_rescale")
-    launch_count += 1
-    return out.view(torch.bool)
 
 
 def zero_border_nhwc(x: torch.Tensor) -> torch.Tensor:
@@ -1086,143 +1091,60 @@ def mask_embed_src(mpp: torch.Tensor, weights: list, emb_rows: torch.Tensor, pos
     return src, src_pe
 
 
-def query_postprocess_rescale(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch.Tensor, batch_hw: tuple,
-                              crop_hw: tuple, out_hw: tuple):
-    """query_postprocess for a resized / padded image: logits -> batch_hw -> crop -> out_hw, then mask / score / box."""
-    global launch_count
-    _require_cuda(logits, sel, cls_scores)
-    n = sel.numel()
-    _, hm, wm = logits.shape
-    H, W = out_hw
-    assert logits.dtype == torch.float32 and logits.is_contiguous() and sel.dtype == torch.int32 and cls_scores.dtype == torch.float32
-    masks = torch.empty(n, H, W, device=logits.device, dtype=torch.uint8)
-    part = torch.empty(n * ((H + 15) // 16) * 6, device=logits.device, dtype=torch.float32)
-    scores = torch.empty(n, device=logits.device, dtype=torch.float32)
-    boxes = torch.empty(n, 4, device=logits.device, dtype=torch.float32)
-    _check(_lib.rsp_query_postprocess_rescale(_ptr(logits), _ptr(sel), _ptr(cls_scores), n, hm, wm, batch_hw[0], batch_hw[1],
-                                              crop_hw[0], crop_hw[1], H, W, _ptr(masks), _ptr(part), _ptr(scores),
-                                              _ptr(boxes), _stream()), "rsp_query_postprocess_rescale")
-    launch_count += 2
-    return masks.view(torch.bool), scores, boxes
-
-
-def query_postprocess(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch.Tensor, size: tuple):
-    """logits fp32 [n_maps, hm, wm]; sel int32 [n]; cls_scores fp32 [n] -> (masks bool [n,H,W], scores [n], boxes [n,4])."""
-    global launch_count
-    _require_cuda(logits, sel, cls_scores)
-    n = sel.numel()
-    _, hm, wm = logits.shape
-    H, W = size
-    assert logits.dtype == torch.float32 and logits.is_contiguous() and sel.dtype == torch.int32 and cls_scores.dtype == torch.float32
-    masks = torch.empty(n, H, W, device=logits.device, dtype=torch.uint8)
-    part = torch.empty(n * ((H + 15) // 16) * 6, device=logits.device, dtype=torch.float32)
-    scores = torch.empty(n, device=logits.device, dtype=torch.float32)
-    boxes = torch.empty(n, 4, device=logits.device, dtype=torch.float32)
-    _check(_lib.rsp_query_postprocess(_ptr(logits), _ptr(sel), _ptr(cls_scores), n, hm, wm, H, W, _ptr(masks), _ptr(part),
-                                      _ptr(scores), _ptr(boxes), _stream()), "rsp_query_postprocess")
-    launch_count += 2
-    return masks.view(torch.bool), scores, boxes
-
-
-# ------------------------------------------------------------------------------ result-record payload
-def query_postprocess_bits(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch.Tensor, bits: torch.Tensor | None = None,
-                           scores: torch.Tensor | None = None, boxes: torch.Tensor | None = None):
-    """query_postprocess at 4x the logit size with bit-packed masks: -> (bits uint8 [n, 4hm, 4wm/8], scores [n], boxes [n,4]).
-    Outputs may be preallocated views of a result record."""
+def query_postprocess(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch.Tensor, size: tuple | None = None, *,
+                      rescale: tuple | None = None, bits: torch.Tensor | None = None, scores: torch.Tensor | None = None,
+                      boxes: torch.Tensor | None = None):
+    """logits fp32 [n_maps, hm, wm]; sel int32 [n] map of each instance; cls_scores fp32 [n] -> (masks, scores [n],
+    boxes [n, 4]) of the selected maps resized bilinearly: size = (H, W), one resize; rescale = (batch_hw, crop_hw,
+    out_hw) for a resized / padded image: to batch_hw -> crop -> to out_hw.  masks bool [n, H, W], or with ``bits``
+    bit-packed into it: record slots uint8 [n, Hr, Wr/8] (out_hw mask at each slot's top-left) with rescale, uint8
+    [n, 4hm, 4wm/8] (the x4 resize) without.  scores / boxes may be views of a result record."""
     global launch_count
     _require_cuda(logits, sel, cls_scores, bits, scores, boxes)
     n = sel.numel()
     _, hm, wm = logits.shape
-    H, W = 4 * hm, 4 * wm
     assert logits.dtype == torch.float32 and logits.is_contiguous() and sel.dtype == torch.int32 and cls_scores.dtype == torch.float32
-    assert sel.is_contiguous() and cls_scores.is_contiguous() and cls_scores.numel() == n
+    assert size is None or rescale is None
+    if rescale is not None:
+        (Hb, Wb), (ch, cw), (H, W) = rescale
+    elif bits is not None:
+        assert size is None or tuple(size) == (4 * hm, 4 * wm)
+        H, W = 4 * hm, 4 * wm
+    else:
+        H, W = size
+    Hr = H
     if bits is None:
-        bits = torch.empty(n, H, W // 8, device=logits.device, dtype=torch.uint8)
-    if scores is None:
-        scores = torch.empty(n, device=logits.device, dtype=torch.float32)
-    if boxes is None:
-        boxes = torch.empty(n, 4, device=logits.device, dtype=torch.float32)
-    assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.numel() == n * H * W // 8
-    assert scores.is_contiguous() and boxes.is_contiguous() and scores.numel() == n and boxes.numel() == 4 * n
-    part = torch.empty(n * ((H + 15) // 16) * 6, device=logits.device, dtype=torch.float32)
-    _check(_lib.rsp_query_postprocess_bits(_ptr(logits), _ptr(sel), _ptr(cls_scores), n, hm, wm, _ptr(bits), _ptr(part),
-                                           _ptr(scores), _ptr(boxes), _stream()), "rsp_query_postprocess_bits")
-    launch_count += 2
-    return bits, scores, boxes
-
-
-def mask_paste_bits(logits: torch.Tensor, thr: float, mode: int, bits: torch.Tensor | None = None) -> torch.Tensor:
-    """fp32 [n, hm, wm] -> bit-packed uint8 [n, 4hm, 4wm/8]; mode 0 sigmoid+bilinear >= thr, mode 1 bilinear > thr."""
-    global launch_count
-    _require_cuda(logits, bits)
-    assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.dim() == 3
-    n, hm, wm = logits.shape
-    if bits is None:
-        bits = torch.empty(n, 4 * hm, wm // 2, device=logits.device, dtype=torch.uint8)
-    assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.numel() == n * 4 * hm * (wm // 2)
-    if n == 0:
-        return bits
-    src = logits
-    if mode == 0:
-        src = torch.empty_like(logits)
-        _check(_lib.rsp_sigmoid_f32(_ptr(logits), _ptr(src), logits.numel(), _stream()), "rsp_sigmoid_f32")
-        launch_count += 1
-        mode = 2
-    _check(_lib.rsp_mask_paste_bits(_ptr(src), _ptr(bits), n, hm, wm, float(thr), mode, _stream()), "rsp_mask_paste_bits")
-    launch_count += 1
-    return bits
-
-
-def mask_paste_rescale_bits(logits: torch.Tensor, batch_hw: tuple, crop_hw: tuple, ori_hw: tuple, thr: float,
-                            bits: torch.Tensor, raw: bool = False) -> torch.Tensor:
-    """mask_paste_rescale written bit-packed into ``bits`` uint8 [n, Hr, Wr/8] (record slots, Wr % 16 == 0): the
-    ori_hw mask at each slot's top-left, 0 elsewhere."""
-    global launch_count
-    _require_cuda(logits, bits)
-    n, hm, wm = logits.shape
-    assert logits.dtype == torch.float32 and logits.is_contiguous() and n > 0
-    assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.dim() == 3 and bits.shape[0] == n
-    Hr, Wr = bits.shape[1], bits.shape[2] * 8
-    act = logits
-    if not raw:
-        act = torch.empty_like(logits)
-        _check(_lib.rsp_sigmoid_f32(_ptr(logits), _ptr(act), logits.numel(), _stream()), "rsp_sigmoid_f32")
-        launch_count += 1
-    _check(_lib.rsp_mask_paste_rescale_bits(_ptr(act), _ptr(bits), n, hm, wm, batch_hw[0], batch_hw[1], crop_hw[0],
-                                            crop_hw[1], ori_hw[0], ori_hw[1], Hr, Wr, float(thr), 1 if raw else 2,
-                                            _stream()), "rsp_mask_paste_rescale_bits")
-    launch_count += 1
-    return bits
-
-
-def query_postprocess_rescale_bits(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch.Tensor, batch_hw: tuple,
-                                   crop_hw: tuple, out_hw: tuple, bits: torch.Tensor, scores: torch.Tensor | None = None,
-                                   boxes: torch.Tensor | None = None):
-    """query_postprocess_rescale with the masks written bit-packed into ``bits`` uint8 [n, Hr, Wr/8] (out_hw mask at
-    each slot's top-left) -> (bits, scores [n], boxes [n, 4]); scores / boxes may be views of a result record."""
-    global launch_count
-    _require_cuda(logits, sel, cls_scores, bits, scores, boxes)
-    n = sel.numel()
-    _, hm, wm = logits.shape
-    H, W = out_hw
-    assert logits.dtype == torch.float32 and logits.is_contiguous() and sel.dtype == torch.int32 and cls_scores.dtype == torch.float32
-    assert sel.is_contiguous() and cls_scores.is_contiguous() and cls_scores.numel() == n
-    assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.dim() == 3 and bits.shape[0] == n
-    Hr, Wr = bits.shape[1], bits.shape[2] * 8
+        masks = torch.empty(n, H, W, device=logits.device, dtype=torch.uint8)
+    else:
+        assert sel.is_contiguous() and cls_scores.is_contiguous() and cls_scores.numel() == n
+        assert bits.dtype == torch.uint8 and bits.is_contiguous()
+        if rescale is None:
+            assert bits.numel() == n * H * W // 8
+        else:
+            assert bits.dim() == 3 and bits.shape[0] == n
+            Hr = bits.shape[1]
     if scores is None:
         scores = torch.empty(n, device=logits.device, dtype=torch.float32)
     if boxes is None:
         boxes = torch.empty(n, 4, device=logits.device, dtype=torch.float32)
     assert scores.is_contiguous() and boxes.is_contiguous() and scores.numel() == n and boxes.numel() == 4 * n
     part = torch.empty(n * ((Hr + 15) // 16) * 6, device=logits.device, dtype=torch.float32)
-    _check(_lib.rsp_query_postprocess_rescale_bits(_ptr(logits), _ptr(sel), _ptr(cls_scores), n, hm, wm, batch_hw[0],
-                                                   batch_hw[1], crop_hw[0], crop_hw[1], H, W, Hr, Wr, _ptr(bits),
-                                                   _ptr(part), _ptr(scores), _ptr(boxes), _stream()),
-           "rsp_query_postprocess_rescale_bits")
+    args = (_ptr(logits), _ptr(sel), _ptr(cls_scores), n, hm, wm)
+    tail = (_ptr(masks if bits is None else bits), _ptr(part), _ptr(scores), _ptr(boxes), _stream())
+    if rescale is None and bits is None:
+        _check(_lib.rsp_query_postprocess(*args, H, W, *tail), "rsp_query_postprocess")
+    elif rescale is None:
+        _check(_lib.rsp_query_postprocess_bits(*args, *tail), "rsp_query_postprocess_bits")
+    elif bits is None:
+        _check(_lib.rsp_query_postprocess_rescale(*args, Hb, Wb, ch, cw, H, W, *tail), "rsp_query_postprocess_rescale")
+    else:
+        _check(_lib.rsp_query_postprocess_rescale_bits(*args, Hb, Wb, ch, cw, H, W, Hr, bits.shape[2] * 8, *tail),
+               "rsp_query_postprocess_rescale_bits")
     launch_count += 2
-    return bits, scores, boxes
+    return (masks.view(torch.bool) if bits is None else bits), scores, boxes
 
 
+# ------------------------------------------------------------------------------ result-record payload
 def pack_mask_bits(masks: torch.Tensor, bits: torch.Tensor | None = None) -> torch.Tensor:
     """bool / uint8 [..., W] -> uint8 [..., ceil(W/8)], pixel x = bit x % 8 of byte x // 8."""
     global launch_count

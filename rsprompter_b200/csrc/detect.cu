@@ -796,44 +796,10 @@ int roi_align_nhwc(const void* const* feats, const float* const* pes, const int*
 }
 
 // ---------------------------------------------------------------------------------------
-// logits fp32 [n, hm, wm] -> uint8 [n, H, W].  mode 0: (bilinear(sigmoid(x)) >= thr);
-// mode 1: (bilinear(x) > thr).  PyTorch align_corners=False source index rule.
-__global__ void mask_paste_kernel(const float* __restrict__ logits, unsigned char* __restrict__ out, int n,
-                                  int hm, int wm, int H, int W, float thr, int mode) {
-  // thread = 16 consecutive output pixels of one row (one 16-byte store)
-  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const int w16 = W / 16;
-  const long long total = static_cast<long long>(n) * H * w16;
-  if (idx >= total) return;
-  const int xb = static_cast<int>(idx % w16);
-  long long t = idx / w16;
-  const int y = static_cast<int>(t % H);
-  const int m = static_cast<int>(t / H);
-  const float sy = fmaxf((y + 0.5f) * (static_cast<float>(hm) / H) - 0.5f, 0.f);
-  const int y0 = static_cast<int>(sy), y1 = min(y0 + 1, hm - 1);
-  const float ly = sy - y0;
-  const float* r0 = logits + (static_cast<size_t>(m) * hm + y0) * wm;
-  const float* r1 = logits + (static_cast<size_t>(m) * hm + y1) * wm;
-  const float sxs = static_cast<float>(wm) / W;
-  uint32_t packed[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-  for (int k = 0; k < 16; ++k) {
-    const int x = xb * 16 + k;
-    const float sx = fmaxf((x + 0.5f) * sxs - 0.5f, 0.f);
-    const int x0 = static_cast<int>(sx), x1 = min(x0 + 1, wm - 1);
-    const float lx = sx - x0;
-    float v00 = __ldg(r0 + x0), v01 = __ldg(r0 + x1), v10 = __ldg(r1 + x0), v11 = __ldg(r1 + x1);
-    if (mode == 0) {
-      v00 = 1.f / (1.f + expf(-v00)); v01 = 1.f / (1.f + expf(-v01));
-      v10 = 1.f / (1.f + expf(-v10)); v11 = 1.f / (1.f + expf(-v11));
-    }
-    const float v = (1.f - ly) * ((1.f - lx) * v00 + lx * v01) + ly * ((1.f - lx) * v10 + lx * v11);
-    const uint32_t bit = (mode == 1 ? (v > thr) : (v >= thr)) ? 1u : 0u;   // mode 2: input already activated
-    packed[k >> 2] |= bit << ((k & 3) * 8);
-  }
-  *reinterpret_cast<uint4*>(out + (static_cast<size_t>(m) * H + y) * W + xb * 16) =
-      make_uint4(packed[0], packed[1], packed[2], packed[3]);
-}
+// Mask paste: low-resolution maps [n, hm, wm] -> thresholded masks, bytes or bits.  Two kernel families: the x4 tile
+// kernel below for the mask decoder's image / 4 logits, and mask_paste_px_kernel, which takes each pixel's value from
+// a sampler (OneResize, TwoResizes, BoxSample).  MODE 1: v > thr; 0 and 2: v >= thr (mode 0 is OneResize<true>, which
+// activates the taps; mode 2 takes maps that rsp_sigmoid_f32 activated once).
 
 // x4 fast path (the mask decoder's logits are always image / 4): thread = 4 output rows x 16 columns
 // PACKED: out holds W/8 bytes per row, pixel x = bit x%8 of byte x/8 (the result-record payload)
@@ -868,26 +834,98 @@ __global__ void mask_paste_x4_kernel(const float* __restrict__ logits, unsigned 
   }
 }
 
-// general case: resized / padded images (two chained resizes with a crop); thread = 4 output pixels of one row
-template <int MODE>
-__global__ void mask_paste_rescale_kernel(const float* __restrict__ maps, unsigned char* __restrict__ out, int n,
-                                          Resize2 g, float thr) {
-  const int w4 = (g.W + 3) / 4;
-  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (idx >= static_cast<long long>(n) * g.H * w4) return;
-  const int xb = static_cast<int>(idx % w4);
-  long long t = idx / w4;
-  const int y = static_cast<int>(t % g.H);
-  const int m = static_cast<int>(t / g.H);
-  const float* src = maps + static_cast<size_t>(m) * g.hm * g.wm;
-  unsigned char* o = out + (static_cast<size_t>(m) * g.H + y) * g.W;
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int x = 4 * xb + k;
-    if (x >= g.W) break;
-    const float v = resize2_at(src, g, y, x);
-    o[x] = (MODE == 1 ? (v > thr) : (v >= thr)) ? 1 : 0;
+// FCNMaskHead paste (fcn_mask_head.py:_do_paste_mask + the threshold of _predict_by_feat_single :388-392): the
+// activated RoI mask probs fp32 [n, hm, wm] of detection m are sampled bilinearly (F.grid_sample, align_corners=False,
+// zero padding) at every image pixel centre mapped into its box, in the reference's rounding order.  row() reports
+// rows whose taps all fall outside the RoI grid.
+struct BoxSample {
+  const float* probs;
+  const float* boxes;
+  int hm, wm;
+  const float* p;
+  float bx0, bx1, iy, fy;
+  int yi0, yi1;
+  bool vy0, vy1;
+
+  __device__ __forceinline__ bool row(int m, int y) {
+    const float by0 = boxes[m * 4 + 1], by1 = boxes[m * 4 + 3];
+    bx0 = boxes[m * 4];
+    bx1 = boxes[m * 4 + 2];
+    // normalised grid coordinate in [-1, 1] (inf from a degenerate box becomes 0, as the reference does)
+    float gy = __fsub_rn(__fmul_rn(__fdiv_rn(__fsub_rn(y + 0.5f, by0), __fsub_rn(by1, by0)), 2.f), 1.f);
+    if (isinf(gy)) gy = 0.f;
+    iy = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), static_cast<float>(hm)), 1.f), 0.5f);
+    fy = floorf(iy);
+    yi0 = static_cast<int>(fy);
+    yi1 = yi0 + 1;
+    vy0 = yi0 >= 0 && yi0 < hm;
+    vy1 = yi1 >= 0 && yi1 < hm;
+    p = probs + static_cast<size_t>(m) * hm * wm;
+    return vy0 || vy1;
   }
+
+  __device__ __forceinline__ float at(int x) const {
+    float gx = __fsub_rn(__fmul_rn(__fdiv_rn(__fsub_rn(x + 0.5f, bx0), __fsub_rn(bx1, bx0)), 2.f), 1.f);
+    if (isinf(gx)) gx = 0.f;
+    const float ix = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), static_cast<float>(wm)), 1.f), 0.5f);
+    const float fx = floorf(ix);
+    const int xi0 = static_cast<int>(fx), xi1 = xi0 + 1;
+    const bool vx0 = xi0 >= 0 && xi0 < wm, vx1 = xi1 >= 0 && xi1 < wm;
+    const float v00 = (vy0 && vx0) ? __ldg(p + yi0 * wm + xi0) : 0.f, v01 = (vy0 && vx1) ? __ldg(p + yi0 * wm + xi1) : 0.f;
+    const float v10 = (vy1 && vx0) ? __ldg(p + yi1 * wm + xi0) : 0.f, v11 = (vy1 && vx1) ? __ldg(p + yi1 * wm + xi1) : 0.f;
+    // grid_sample weights in ATen's form: (x_se - ix)(y_se - iy), (ix - x_nw)(y_se - iy), (x_se - ix)(iy - y_nw), ...
+    const float wx0 = (fx + 1.f) - ix, wx1 = ix - fx, wy0 = (fy + 1.f) - iy, wy1 = iy - fy;
+    return v00 * (wx0 * wy0) + v01 * (wx1 * wy0) + v10 * (wx0 * wy1) + v11 * (wx1 * wy1);
+  }
+};
+
+// thread = 16 consecutive pixels of one output row.  BITS: record slots [n, Hr, Wr/8] (Wr % 16 == 0), pixel x = bit
+// x % 8 of byte x / 8, one uint16 per thread, the (H, W) mask at the slot's top-left and 0 elsewhere.  Otherwise bytes
+// [n, H, W] (Hr = H, Wr = W): one 16-byte store where the row segment is whole and 16-byte aligned, byte stores
+// elsewhere.  Rows the sampler reports empty store zeros without loads.
+template <class Sampler, int MODE, bool BITS>
+__global__ void mask_paste_px_kernel(Sampler s, unsigned char* __restrict__ out, int n, int H, int W, int Hr, int Wr,
+                                     float thr) {
+  const int w16 = (Wr + 15) / 16;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= static_cast<long long>(n) * Hr * w16) return;
+  const int xb = static_cast<int>(idx % w16);
+  const long long t = idx / w16;
+  const int y = static_cast<int>(t % Hr);
+  const int m = static_cast<int>(t / Hr);
+  uint32_t packed[4] = {0u, 0u, 0u, 0u};
+  uint32_t bits = 0u;
+  if (y < H && s.row(m, y)) {
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+      const int x = 16 * xb + k;
+      if (x >= W) break;
+      const float v = s.at(x);
+      const uint32_t bit = (MODE == 1 ? (v > thr) : (v >= thr)) ? 1u : 0u;
+      if (BITS) bits |= bit << k;
+      else packed[k >> 2] |= bit << ((k & 3) * 8);
+    }
+  }
+  if (BITS) {
+    *reinterpret_cast<uint16_t*>(out + (static_cast<size_t>(m) * Hr + y) * (Wr / 8) + 2 * xb) = static_cast<uint16_t>(bits);
+    return;
+  }
+  unsigned char* dst = out + (static_cast<size_t>(m) * H + y) * W + 16 * xb;
+  if (16 * xb + 16 <= W && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+    *reinterpret_cast<uint4*>(dst) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
+  } else {
+    for (int k = 0; k < 16 && 16 * xb + k < W; ++k) dst[k] = static_cast<unsigned char>((packed[k >> 2] >> ((k & 3) * 8)) & 1u);
+  }
+}
+
+template <int MODE, bool BITS, class Sampler>
+static int paste_px(const Sampler& s, unsigned char* out, int n, int H, int W, int Hr, int Wr, float thr,
+                    cudaStream_t stream) {
+  const long long total = static_cast<long long>(n) * Hr * ((Wr + 15) / 16);
+  mask_paste_px_kernel<Sampler, MODE, BITS><<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
+      s, out, n, H, W, Hr, Wr, thr);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
 }
 
 int mask_paste_rescale(const float* maps, unsigned char* out, int n, int hm, int wm, int Hb, int Wb, int crop_h,
@@ -895,39 +933,9 @@ int mask_paste_rescale(const float* maps, unsigned char* out, int n, int hm, int
   RSP_CHECK_ARG(maps && out && n > 0 && hm > 0 && wm > 0 && Hb > 0 && Wb > 0 && crop_h > 0 && crop_w > 0 &&
                 crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 && (mode == 1 || mode == 2),
                 "mask_paste_rescale: bad args (mode 1: > thr on raw maps, 2: >= thr on activated maps)");
-  Resize2 g{hm, wm, Hb, Wb, crop_h, crop_w, H, W};
-  const long long total = static_cast<long long>(n) * H * ((W + 3) / 4);
-  const unsigned blocks = static_cast<unsigned>((total + 255) / 256);
-  if (mode == 1) mask_paste_rescale_kernel<1><<<blocks, 256, 0, stream>>>(maps, out, n, g, thr);
-  else mask_paste_rescale_kernel<2><<<blocks, 256, 0, stream>>>(maps, out, n, g, thr);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
-}
-
-// ... bit-packed into record slots of Hr x Wr (Wr % 16 == 0): thread = 16 pixels of one row, one uint16 store; the
-// (H, W) mask sits at the slot's top-left, pixels outside it are 0.  Per pixel the value is resize2_at, as above.
-template <int MODE>
-__global__ void mask_paste_rescale_bits_kernel(const float* __restrict__ maps, unsigned char* __restrict__ bits, int n,
-                                               Resize2 g, int Hr, int Wr, float thr) {
-  const int w16 = Wr / 16;
-  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (idx >= static_cast<long long>(n) * Hr * w16) return;
-  const int xb = static_cast<int>(idx % w16);
-  long long t = idx / w16;
-  const int y = static_cast<int>(t % Hr);
-  const int m = static_cast<int>(t / Hr);
-  const float* src = maps + static_cast<size_t>(m) * g.hm * g.wm;
-  uint32_t word = 0u;
-  if (y < g.H) {
-#pragma unroll 4
-    for (int k = 0; k < 16; ++k) {
-      const int x = 16 * xb + k;
-      if (x >= g.W) break;
-      const float v = resize2_at(src, g, y, x);
-      word |= ((MODE == 1 ? (v > thr) : (v >= thr)) ? 1u : 0u) << k;
-    }
-  }
-  *reinterpret_cast<uint16_t*>(bits + (static_cast<size_t>(m) * Hr + y) * (Wr / 8) + 2 * xb) = static_cast<uint16_t>(word);
+  const TwoResizes s{maps, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
+  return mode == 1 ? paste_px<1, false>(s, out, n, H, W, H, W, thr, stream)
+                   : paste_px<2, false>(s, out, n, H, W, H, W, thr, stream);
 }
 
 int mask_paste_rescale_bits(const float* maps, unsigned char* bits, int n, int hm, int wm, int Hb, int Wb, int crop_h,
@@ -936,82 +944,18 @@ int mask_paste_rescale_bits(const float* maps, unsigned char* bits, int n, int h
                 crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 && H <= Hr && W <= Wr && Wr % 16 == 0 &&
                 (reinterpret_cast<uintptr_t>(bits) & 1) == 0 && (mode == 1 || mode == 2),
                 "mask_paste_rescale_bits: bad args (H <= Hr, W <= Wr, Wr % 16 == 0, 2-byte aligned bits; mode 1 or 2)");
-  Resize2 g{hm, wm, Hb, Wb, crop_h, crop_w, H, W};
-  const long long total = static_cast<long long>(n) * Hr * (Wr / 16);
-  const unsigned blocks = static_cast<unsigned>((total + 255) / 256);
-  if (mode == 1) mask_paste_rescale_bits_kernel<1><<<blocks, 256, 0, stream>>>(maps, bits, n, g, Hr, Wr, thr);
-  else mask_paste_rescale_bits_kernel<2><<<blocks, 256, 0, stream>>>(maps, bits, n, g, Hr, Wr, thr);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
-}
-
-// FCNMaskHead paste (fcn_mask_head.py:_do_paste_mask + the threshold of _predict_by_feat_single :388-392): the
-// activated RoI mask probs fp32 [n, hm, wm] of detection i are sampled bilinearly (F.grid_sample, align_corners=False,
-// zero padding) at every image pixel centre mapped into its box, then compared with thr.  thread = 16 output pixels of
-// one row (one 16-byte store); rows / columns whose taps all fall outside the RoI grid write zeros without loads.
-__global__ void mask_paste_boxes_kernel(const float* __restrict__ probs, const float* __restrict__ boxes,
-                                        unsigned char* __restrict__ out, int n, int hm, int wm, int H, int W, float thr,
-                                        int packed) {
-  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const int w16 = (W + 15) / 16;
-  if (idx >= static_cast<long long>(n) * H * w16) return;
-  const int xb = static_cast<int>(idx % w16);
-  long long t = idx / w16;
-  const int y = static_cast<int>(t % H);
-  const int m = static_cast<int>(t / H);
-  const float x0 = boxes[m * 4], y0 = boxes[m * 4 + 1], x1 = boxes[m * 4 + 2], y1 = boxes[m * 4 + 3];
-  // normalised grid coordinate in [-1, 1] (inf from a degenerate box becomes 0, as the reference does)
-  float gy = __fsub_rn(__fmul_rn(__fdiv_rn(__fsub_rn(y + 0.5f, y0), __fsub_rn(y1, y0)), 2.f), 1.f);
-  if (isinf(gy)) gy = 0.f;
-  const float iy = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), static_cast<float>(hm)), 1.f), 0.5f);
-  const float fy = floorf(iy);
-  const int yi0 = static_cast<int>(fy), yi1 = yi0 + 1;
-  const bool vy0 = yi0 >= 0 && yi0 < hm, vy1 = yi1 >= 0 && yi1 < hm;
-  const float* p = probs + static_cast<size_t>(m) * hm * wm;
-  uint32_t pk[4] = {0u, 0u, 0u, 0u};
-  if (vy0 || vy1) {
-#pragma unroll
-    for (int k = 0; k < 16; ++k) {
-      const int x = xb * 16 + k;
-      float gx = __fsub_rn(__fmul_rn(__fdiv_rn(__fsub_rn(x + 0.5f, x0), __fsub_rn(x1, x0)), 2.f), 1.f);
-      if (isinf(gx)) gx = 0.f;
-      const float ix = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), static_cast<float>(wm)), 1.f), 0.5f);
-      const float fx = floorf(ix);
-      const int xi0 = static_cast<int>(fx), xi1 = xi0 + 1;
-      const bool vx0 = xi0 >= 0 && xi0 < wm, vx1 = xi1 >= 0 && xi1 < wm;
-      const float v00 = (vy0 && vx0) ? __ldg(p + yi0 * wm + xi0) : 0.f, v01 = (vy0 && vx1) ? __ldg(p + yi0 * wm + xi1) : 0.f;
-      const float v10 = (vy1 && vx0) ? __ldg(p + yi1 * wm + xi0) : 0.f, v11 = (vy1 && vx1) ? __ldg(p + yi1 * wm + xi1) : 0.f;
-      // grid_sample weights in ATen's form: (x_se - ix)(y_se - iy), (ix - x_nw)(y_se - iy), (x_se - ix)(iy - y_nw), ...
-      const float wx0 = (fx + 1.f) - ix, wx1 = ix - fx, wy0 = (fy + 1.f) - iy, wy1 = iy - fy;
-      const float v = v00 * (wx0 * wy0) + v01 * (wx1 * wy0) + v10 * (wx0 * wy1) + v11 * (wx1 * wy1);
-      pk[k >> 2] |= (v >= thr ? 1u : 0u) << ((k & 3) * 8);
-    }
-  }
-  if (packed) {   // result-record layout: pixel x = bit x % 8 of byte x / 8 (W % 16 == 0)
-    uint32_t bits = 0;
-#pragma unroll
-    for (int k = 0; k < 16; ++k) bits |= ((pk[k >> 2] >> ((k & 3) * 8)) & 1u) << k;
-    *reinterpret_cast<unsigned short*>(out + (static_cast<size_t>(m) * H + y) * (W / 8) + xb * 2) =
-        static_cast<unsigned short>(bits);
-    return;
-  }
-  unsigned char* dst = out + (static_cast<size_t>(m) * H + y) * W + xb * 16;
-  if ((W & 15) == 0) {
-    *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-  } else {   // original-image canvases of any width: byte stores
-    for (int k = 0; k < 16 && xb * 16 + k < W; ++k) dst[k] = static_cast<unsigned char>((pk[k >> 2] >> ((k & 3) * 8)) & 1u);
-  }
+  const TwoResizes s{maps, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
+  return mode == 1 ? paste_px<1, true>(s, bits, n, H, W, Hr, Wr, thr, stream)
+                   : paste_px<2, true>(s, bits, n, H, W, Hr, Wr, thr, stream);
 }
 
 int mask_paste_boxes(const float* probs, const float* boxes, unsigned char* out, int n, int hm, int wm, int H, int W,
                      float thr, int packed, cudaStream_t stream) {
   RSP_CHECK_ARG(probs && boxes && out && n > 0 && hm > 0 && wm > 0 && H > 0 && W > 0, "mask_paste_boxes: bad arguments");
   RSP_CHECK_ARG(!packed || W % 16 == 0, "mask_paste_boxes: bit-packed output needs W % 16 == 0");
-  const long long total = static_cast<long long>(n) * H * ((W + 15) / 16);
-  mask_paste_boxes_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(probs, boxes, out, n, hm, wm, H, W,
-                                                                                         thr, packed);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
+  const BoxSample s{probs, boxes, hm, wm};
+  return packed ? paste_px<2, true>(s, out, n, H, W, H, W, thr, stream)
+                : paste_px<2, false>(s, out, n, H, W, H, W, thr, stream);
 }
 
 __global__ void sigmoid_f32_kernel(const float4* __restrict__ in, float4* __restrict__ out, long long n4) {
@@ -1054,11 +998,10 @@ int mask_paste(const float* logits, unsigned char* out, int n, int hm, int wm, i
     RSP_CHECK_LAUNCH();
     return RSP_OK;
   }
-  const long long total = static_cast<long long>(n) * H * (W / 16);
-  mask_paste_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(logits, out, n, hm, wm, H, W,
-                                                                                   thr, mode);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
+  if (mode == 0) return paste_px<0, false>(OneResize<true, false>{logits, hm, wm, H, W}, out, n, H, W, H, W, thr, stream);
+  const OneResize<false, false> s{logits, hm, wm, H, W};
+  return mode == 1 ? paste_px<1, false>(s, out, n, H, W, H, W, thr, stream)
+                   : paste_px<2, false>(s, out, n, H, W, H, W, thr, stream);
 }
 
 // ---------------------------------------------------------------------------------------

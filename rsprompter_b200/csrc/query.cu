@@ -836,44 +836,16 @@ int sam_mask_embed(const float* masks, const float* const* wts, int B, int hm, i
 }
 
 // ------------------------------------------------------------------------------------ query post-process
-// grid (rows / ROWS, instances); logits fp32 [n_maps, hm, wm]; sel int32 [n_inst] map index of each instance.
-// Writes the boolean mask and per-block partials (sum sigmoid over positives, count, bbox) reduced by
-// query_finalize_kernel in a fixed order (deterministic).
+// grid (rows / QP_ROWS, instances); logits fp32 [n_maps, hm, wm]; sel int32 [n_inst] map index of each instance.
+// The mask kernels write the boolean mask and per-block partials (sum sigmoid over positives, count, bbox) reduced by
+// query_finalize_kernel in a fixed order (deterministic).  Two families: the x4 tile kernel for the mask decoder's
+// image / 4 logits, and query_mask_px_kernel, which takes each pixel's value from OneResize or TwoResizes.
 constexpr int QP_ROWS = 16;
-__global__ void query_mask_kernel(const float* __restrict__ logits, const int* __restrict__ sel, int hm, int wm, int H,
-                                  int W, unsigned char* __restrict__ masks, float* __restrict__ part) {
-  const int inst = blockIdx.y;
-  const float* src = logits + static_cast<size_t>(sel[inst]) * hm * wm;
-  const float sy_s = static_cast<float>(hm) / H, sx_s = static_cast<float>(wm) / W;
-  float sum = 0.f;
-  int cnt = 0, minx = W, maxx = -1, miny = H, maxy = -1;
-  const int y_base = blockIdx.x * QP_ROWS;
-  for (int i = threadIdx.x; i < QP_ROWS * (W / 4); i += blockDim.x) {
-    const int y = y_base + i / (W / 4), x4 = i % (W / 4);
-    if (y >= H) break;
-    const float sy = fmaxf((y + 0.5f) * sy_s - 0.5f, 0.f);
-    const int y0 = static_cast<int>(sy), y1 = min(y0 + 1, hm - 1);
-    const float ly = sy - y0;
-    unsigned char r[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int x = x4 * 4 + k;
-      const float sx = fmaxf((x + 0.5f) * sx_s - 0.5f, 0.f);
-      const int x0 = static_cast<int>(sx), x1 = min(x0 + 1, wm - 1);
-      const float lx = sx - x0;
-      const float v = (1.f - ly) * ((1.f - lx) * src[y0 * wm + x0] + lx * src[y0 * wm + x1]) +
-                      ly * ((1.f - lx) * src[y1 * wm + x0] + lx * src[y1 * wm + x1]);
-      const bool on = v > 0.f;
-      r[k] = on;
-      if (on) {
-        sum += __fdividef(1.f, 1.f + __expf(-v));   // fast sigmoid: ~2 ulp, the sum is an average over >= 1e3 pixels
-        ++cnt;
-        minx = min(minx, x); maxx = max(maxx, x); miny = min(miny, y); maxy = max(maxy, y);
-      }
-    }
-    *reinterpret_cast<uchar4*>(masks + (static_cast<size_t>(inst) * H + y) * W + x4 * 4) = make_uchar4(r[0], r[1], r[2], r[3]);
-  }
-  // block reduction (fixed tree -> deterministic)
+
+// The block's (sum, count, min / max x, min / max y) over a fixed tree (deterministic) -> its 6-float partial.  Every
+// thread of the block calls it; blockDim.x <= 256.
+__device__ __forceinline__ void qp_block_partial(float sum, int cnt, int minx, int maxx, int miny, int maxy,
+                                                 float* __restrict__ part) {
   __shared__ float s_sum[256];
   __shared__ int s_i[256][5];
   s_sum[threadIdx.x] = sum;
@@ -892,13 +864,69 @@ __global__ void query_mask_kernel(const float* __restrict__ logits, const int* _
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    float* o = part + (static_cast<size_t>(inst) * gridDim.x + blockIdx.x) * 6;
+    float* o = part + (static_cast<size_t>(blockIdx.y) * gridDim.x + blockIdx.x) * 6;
     o[0] = s_sum[0]; o[1] = static_cast<float>(s_i[0][0]); o[2] = static_cast<float>(s_i[0][1]);
     o[3] = static_cast<float>(s_i[0][2]); o[4] = static_cast<float>(s_i[0][3]); o[5] = static_cast<float>(s_i[0][4]);
   }
 }
 
-// x4 fast path: block = 16 output rows of one instance (same partial layout as above); thread = 4 x 16 tile
+// Block = QP_ROWS rows of the (H, W) mask of instance blockIdx.y; a thread takes PX consecutive pixels of a row per
+// step (PX = 4: one uchar4 store, W % 4 == 0).  The pixel -> thread order fixes each thread's fast-sigmoid sum, so
+// it decides the scores' bits.  BITS: the mask goes bit-packed into record slots [n, Hr, Wr/8] (Wr % 16 == 0), the
+// (H, W) mask at the slot's top-left and 0 elsewhere: the block's rows collect in a shared bitmap (QP_ROWS x Wr/32
+// words) and leave as one uint16 store per 16 pixels.  Otherwise bytes [n, H, W] (Hr = H, Wr = W).
+template <class Sampler, int PX, bool BITS>
+__global__ void query_mask_px_kernel(Sampler s, const int* __restrict__ sel, int H, int W, int Hr, int Wr,
+                                     unsigned char* __restrict__ out, float* __restrict__ part) {
+  extern __shared__ uint32_t s_bits[];
+  const int words = (Wr + 31) / 32;
+  if (BITS) {
+    for (int i = threadIdx.x; i < QP_ROWS * words; i += blockDim.x) s_bits[i] = 0u;
+    __syncthreads();
+  }
+  const int inst = blockIdx.y, m = sel[inst];
+  float sum = 0.f;
+  int cnt = 0, minx = W, maxx = -1, miny = H, maxy = -1;
+  const int y_base = blockIdx.x * QP_ROWS, wp = W / PX;
+  for (int i = threadIdx.x; i < QP_ROWS * wp; i += blockDim.x) {
+    const int y = y_base + i / wp, xp = i % wp;
+    if (y >= H) break;
+    s.row(m, y);
+    unsigned char r[4];
+#pragma unroll
+    for (int k = 0; k < PX; ++k) {
+      const int x = PX * xp + k;
+      const float v = s.at(x);
+      const bool on = v > 0.f;
+      r[k] = on;
+      if (on) {
+        if (BITS) atomicOr(&s_bits[(y - y_base) * words + (x >> 5)], 1u << (x & 31));
+        sum += __fdividef(1.f, 1.f + __expf(-v));   // fast sigmoid: ~2 ulp, the sum is an average over >= 1e3 pixels
+        ++cnt;
+        minx = min(minx, x); maxx = max(maxx, x); miny = min(miny, y); maxy = max(maxy, y);
+      }
+    }
+    if (!BITS) {
+      unsigned char* o = out + (static_cast<size_t>(inst) * H + y) * W + PX * xp;
+      if (PX == 4) *reinterpret_cast<uchar4*>(o) = make_uchar4(r[0], r[1], r[2], r[3]);
+      else *o = r[0];
+    }
+  }
+  if (BITS) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < QP_ROWS * (Wr / 16); i += blockDim.x) {
+      const int rr = i / (Wr / 16), k = i % (Wr / 16);
+      const int y = y_base + rr;
+      if (y >= Hr) break;
+      const uint32_t w = s_bits[rr * words + (k >> 1)];
+      *reinterpret_cast<uint16_t*>(out + (static_cast<size_t>(inst) * Hr + y) * (Wr / 8) + 2 * k) =
+          static_cast<uint16_t>(k & 1 ? w >> 16 : w);
+    }
+  }
+  qp_block_partial(sum, cnt, minx, maxx, miny, maxy, part);
+}
+
+// x4 fast path: block = 16 output rows of one instance (see query_mask_px_kernel for the partials); thread = 4 x 16 tile
 // PACKED: masks is the bit-packed record payload (H rows of W/8 bytes, pixel x = bit x%8 of byte x/8, i.e.
 // numpy packbits(bitorder='little')); a thread writes its 16 pixels of a row as one uint16.
 template <bool PACKED>
@@ -940,131 +968,7 @@ __global__ void query_mask_x4_kernel(const float* __restrict__ logits, const int
       }
     }
   }
-  __shared__ float s_sum[256];
-  __shared__ int s_i[256][5];
-  s_sum[threadIdx.x] = sum;
-  s_i[threadIdx.x][0] = cnt; s_i[threadIdx.x][1] = minx; s_i[threadIdx.x][2] = maxx;
-  s_i[threadIdx.x][3] = miny; s_i[threadIdx.x][4] = maxy;
-  __syncthreads();
-  for (int s = blockDim.x / 2; s > 0; s >>= 1) {
-    if (threadIdx.x < s) {
-      s_sum[threadIdx.x] += s_sum[threadIdx.x + s];
-      s_i[threadIdx.x][0] += s_i[threadIdx.x + s][0];
-      s_i[threadIdx.x][1] = min(s_i[threadIdx.x][1], s_i[threadIdx.x + s][1]);
-      s_i[threadIdx.x][2] = max(s_i[threadIdx.x][2], s_i[threadIdx.x + s][2]);
-      s_i[threadIdx.x][3] = min(s_i[threadIdx.x][3], s_i[threadIdx.x + s][3]);
-      s_i[threadIdx.x][4] = max(s_i[threadIdx.x][4], s_i[threadIdx.x + s][4]);
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    float* o = part + (static_cast<size_t>(inst) * gridDim.x + blockIdx.x) * 6;
-    o[0] = s_sum[0]; o[1] = static_cast<float>(s_i[0][0]); o[2] = static_cast<float>(s_i[0][1]);
-    o[3] = static_cast<float>(s_i[0][2]); o[4] = static_cast<float>(s_i[0][3]); o[5] = static_cast<float>(s_i[0][4]);
-  }
-}
-
-// general case (resized / padded images): same partial layout, two chained resizes per pixel
-__global__ void query_mask_rescale_kernel(const float* __restrict__ logits, const int* __restrict__ sel, Resize2 g,
-                                          unsigned char* __restrict__ masks, float* __restrict__ part) {
-  const int inst = blockIdx.y;
-  const float* src = logits + static_cast<size_t>(sel[inst]) * g.hm * g.wm;
-  float sum = 0.f;
-  int cnt = 0, minx = g.W, maxx = -1, miny = g.H, maxy = -1;
-  const int y_base = blockIdx.x * QP_ROWS;
-  for (int i = threadIdx.x; i < QP_ROWS * g.W; i += blockDim.x) {
-    const int y = y_base + i / g.W, x = i % g.W;
-    if (y >= g.H) break;
-    const float v = resize2_at(src, g, y, x);
-    const bool on = v > 0.f;
-    masks[(static_cast<size_t>(inst) * g.H + y) * g.W + x] = on;
-    if (on) {
-      sum += __fdividef(1.f, 1.f + __expf(-v));   // fast sigmoid: ~2 ulp, the sum is an average over >= 1e3 pixels
-      ++cnt;
-      minx = min(minx, x); maxx = max(maxx, x); miny = min(miny, y); maxy = max(maxy, y);
-    }
-  }
-  __shared__ float s_sum[256];
-  __shared__ int s_i[256][5];
-  s_sum[threadIdx.x] = sum;
-  s_i[threadIdx.x][0] = cnt; s_i[threadIdx.x][1] = minx; s_i[threadIdx.x][2] = maxx;
-  s_i[threadIdx.x][3] = miny; s_i[threadIdx.x][4] = maxy;
-  __syncthreads();
-  for (int s = blockDim.x / 2; s > 0; s >>= 1) {
-    if (threadIdx.x < s) {
-      s_sum[threadIdx.x] += s_sum[threadIdx.x + s];
-      s_i[threadIdx.x][0] += s_i[threadIdx.x + s][0];
-      s_i[threadIdx.x][1] = min(s_i[threadIdx.x][1], s_i[threadIdx.x + s][1]);
-      s_i[threadIdx.x][2] = max(s_i[threadIdx.x][2], s_i[threadIdx.x + s][2]);
-      s_i[threadIdx.x][3] = min(s_i[threadIdx.x][3], s_i[threadIdx.x + s][3]);
-      s_i[threadIdx.x][4] = max(s_i[threadIdx.x][4], s_i[threadIdx.x + s][4]);
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    float* o = part + (static_cast<size_t>(inst) * gridDim.x + blockIdx.x) * 6;
-    o[0] = s_sum[0]; o[1] = static_cast<float>(s_i[0][0]); o[2] = static_cast<float>(s_i[0][1]);
-    o[3] = static_cast<float>(s_i[0][2]); o[4] = static_cast<float>(s_i[0][3]); o[5] = static_cast<float>(s_i[0][4]);
-  }
-}
-
-// ... bit-packed into record slots of Hr x Wr (Wr % 16 == 0), the (H, W) mask at the slot's top-left and 0 elsewhere.
-// The pixel -> thread assignment and the reductions are those of query_mask_rescale_kernel, so scores and boxes are
-// bit-identical to it; the bits of the block's 16 rows collect in a shared bitmap (16 x Wr/32 words) and leave as
-// one uint16 store per 16 pixels.
-__global__ void query_mask_rescale_bits_kernel(const float* __restrict__ logits, const int* __restrict__ sel, Resize2 g,
-                                               int Hr, int Wr, unsigned char* __restrict__ bits,
-                                               float* __restrict__ part) {
-  extern __shared__ uint32_t s_bits[];                 // [QP_ROWS][Wr / 32]
-  const int words = Wr / 32 + (Wr % 32 ? 1 : 0);
-  for (int i = threadIdx.x; i < QP_ROWS * words; i += blockDim.x) s_bits[i] = 0u;
-  __syncthreads();
-  const int inst = blockIdx.y;
-  const float* src = logits + static_cast<size_t>(sel[inst]) * g.hm * g.wm;
-  float sum = 0.f;
-  int cnt = 0, minx = g.W, maxx = -1, miny = g.H, maxy = -1;
-  const int y_base = blockIdx.x * QP_ROWS;
-  for (int i = threadIdx.x; i < QP_ROWS * g.W; i += blockDim.x) {
-    const int y = y_base + i / g.W, x = i % g.W;
-    if (y >= g.H) break;
-    const float v = resize2_at(src, g, y, x);
-    if (v > 0.f) {
-      atomicOr(&s_bits[(y - y_base) * words + (x >> 5)], 1u << (x & 31));
-      sum += __fdividef(1.f, 1.f + __expf(-v));   // fast sigmoid: ~2 ulp, the sum is an average over >= 1e3 pixels
-      ++cnt;
-      minx = min(minx, x); maxx = max(maxx, x); miny = min(miny, y); maxy = max(maxy, y);
-    }
-  }
-  __shared__ float s_sum[256];
-  __shared__ int s_i[256][5];
-  s_sum[threadIdx.x] = sum;
-  s_i[threadIdx.x][0] = cnt; s_i[threadIdx.x][1] = minx; s_i[threadIdx.x][2] = maxx;
-  s_i[threadIdx.x][3] = miny; s_i[threadIdx.x][4] = maxy;
-  __syncthreads();
-  for (int i = threadIdx.x; i < QP_ROWS * (Wr / 16); i += blockDim.x) {
-    const int r = i / (Wr / 16), k = i % (Wr / 16);
-    const int y = y_base + r;
-    if (y >= Hr) break;
-    const uint32_t w = s_bits[r * words + (k >> 1)];
-    *reinterpret_cast<uint16_t*>(bits + (static_cast<size_t>(inst) * Hr + y) * (Wr / 8) + 2 * k) =
-        static_cast<uint16_t>(k & 1 ? w >> 16 : w);
-  }
-  for (int s = blockDim.x / 2; s > 0; s >>= 1) {
-    if (threadIdx.x < s) {
-      s_sum[threadIdx.x] += s_sum[threadIdx.x + s];
-      s_i[threadIdx.x][0] += s_i[threadIdx.x + s][0];
-      s_i[threadIdx.x][1] = min(s_i[threadIdx.x][1], s_i[threadIdx.x + s][1]);
-      s_i[threadIdx.x][2] = max(s_i[threadIdx.x][2], s_i[threadIdx.x + s][2]);
-      s_i[threadIdx.x][3] = min(s_i[threadIdx.x][3], s_i[threadIdx.x + s][3]);
-      s_i[threadIdx.x][4] = max(s_i[threadIdx.x][4], s_i[threadIdx.x + s][4]);
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    float* o = part + (static_cast<size_t>(inst) * gridDim.x + blockIdx.x) * 6;
-    o[0] = s_sum[0]; o[1] = static_cast<float>(s_i[0][0]); o[2] = static_cast<float>(s_i[0][1]);
-    o[3] = static_cast<float>(s_i[0][2]); o[4] = static_cast<float>(s_i[0][3]); o[5] = static_cast<float>(s_i[0][4]);
-  }
+  qp_block_partial(sum, cnt, minx, maxx, miny, maxy, part);
 }
 
 __global__ void query_finalize_kernel(const float* __restrict__ part, int nblk, const float* __restrict__ cls_scores,
@@ -1083,20 +987,36 @@ __global__ void query_finalize_kernel(const float* __restrict__ part, int nblk, 
   boxes[i * 4 + 2] = any ? maxx + 1.f : 0.f; boxes[i * 4 + 3] = any ? maxy + 1.f : 0.f;
 }
 
-int query_postprocess(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm, int H,
-                      int W, unsigned char* masks, float* part_ws, float* scores, float* boxes, cudaStream_t stream) {
-  RSP_CHECK_ARG(logits && sel && cls_scores && masks && part_ws && scores && boxes && n_inst > 0 && W % 4 == 0,
-                "query_postprocess: bad args");
-  const int nblk = (H + QP_ROWS - 1) / QP_ROWS;
-  dim3 grid(nblk, n_inst);
-  if (H == 4 * hm && W == 4 * wm && wm % 4 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0)
-    query_mask_x4_kernel<false><<<grid, 256, 0, stream>>>(logits, sel, hm, wm, masks, part_ws);
-  else
-    query_mask_kernel<<<grid, 256, 0, stream>>>(logits, sel, hm, wm, H, W, masks, part_ws);
+// checks the mask kernel's launch, then reduces its partials of grid (nblk, n_inst) into scores and boxes
+static int query_finalize(const float* part_ws, int nblk, const float* cls_scores, int n_inst, int H, int W,
+                          float* scores, float* boxes, cudaStream_t stream) {
   RSP_CHECK_LAUNCH();
   query_finalize_kernel<<<(n_inst + 127) / 128, 128, 0, stream>>>(part_ws, nblk, cls_scores, n_inst, W, H, scores, boxes);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
+}
+
+template <int PX, bool BITS, class Sampler>
+static int query_px(const Sampler& s, const int* sel, const float* cls_scores, int n_inst, int H, int W, int Hr, int Wr,
+                    unsigned char* out, float* part_ws, float* scores, float* boxes, cudaStream_t stream) {
+  // BITS: blocks past row H contribute empty partials (+0 to the sums), so scores equal the byte path's
+  const int nblk = (Hr + QP_ROWS - 1) / QP_ROWS;
+  const size_t smem = BITS ? QP_ROWS * ((Wr + 31) / 32) * sizeof(uint32_t) : 0;
+  query_mask_px_kernel<Sampler, PX, BITS><<<dim3(nblk, n_inst), 256, smem, stream>>>(s, sel, H, W, Hr, Wr, out, part_ws);
+  return query_finalize(part_ws, nblk, cls_scores, n_inst, H, W, scores, boxes, stream);
+}
+
+int query_postprocess(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm, int H,
+                      int W, unsigned char* masks, float* part_ws, float* scores, float* boxes, cudaStream_t stream) {
+  RSP_CHECK_ARG(logits && sel && cls_scores && masks && part_ws && scores && boxes && n_inst > 0 && W % 4 == 0,
+                "query_postprocess: bad args");
+  if (H == 4 * hm && W == 4 * wm && wm % 4 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0) {
+    const int nblk = (H + QP_ROWS - 1) / QP_ROWS;
+    query_mask_x4_kernel<false><<<dim3(nblk, n_inst), 256, 0, stream>>>(logits, sel, hm, wm, masks, part_ws);
+    return query_finalize(part_ws, nblk, cls_scores, n_inst, H, W, scores, boxes, stream);
+  }
+  return query_px<4, false>(OneResize<false, true>{logits, hm, wm, H, W}, sel, cls_scores, n_inst, H, W, H, W, masks, part_ws,
+                            scores, boxes, stream);
 }
 
 int query_postprocess_bits(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm,
@@ -1106,12 +1026,8 @@ int query_postprocess_bits(const float* logits, const int* sel, const float* cls
                 "query_postprocess_bits: needs wm % 4 == 0 and 16-byte aligned logits (x4 path only)");
   const int H = 4 * hm, W = 4 * wm;
   const int nblk = (H + QP_ROWS - 1) / QP_ROWS;
-  dim3 grid(nblk, n_inst);
-  query_mask_x4_kernel<true><<<grid, 256, 0, stream>>>(logits, sel, hm, wm, bits, part_ws);
-  RSP_CHECK_LAUNCH();
-  query_finalize_kernel<<<(n_inst + 127) / 128, 128, 0, stream>>>(part_ws, nblk, cls_scores, n_inst, W, H, scores, boxes);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
+  query_mask_x4_kernel<true><<<dim3(nblk, n_inst), 256, 0, stream>>>(logits, sel, hm, wm, bits, part_ws);
+  return query_finalize(part_ws, nblk, cls_scores, n_inst, H, W, scores, boxes, stream);
 }
 
 int query_postprocess_rescale(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm,
@@ -1119,14 +1035,8 @@ int query_postprocess_rescale(const float* logits, const int* sel, const float* 
                               float* scores, float* boxes, cudaStream_t stream) {
   RSP_CHECK_ARG(logits && sel && cls_scores && masks && part_ws && scores && boxes && n_inst > 0 && crop_h > 0 &&
                 crop_w > 0 && crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0, "query_postprocess_rescale: bad args");
-  Resize2 g{hm, wm, Hb, Wb, crop_h, crop_w, H, W};
-  const int nblk = (H + QP_ROWS - 1) / QP_ROWS;
-  dim3 grid(nblk, n_inst);
-  query_mask_rescale_kernel<<<grid, 256, 0, stream>>>(logits, sel, g, masks, part_ws);
-  RSP_CHECK_LAUNCH();
-  query_finalize_kernel<<<(n_inst + 127) / 128, 128, 0, stream>>>(part_ws, nblk, cls_scores, n_inst, W, H, scores, boxes);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
+  const TwoResizes s{logits, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
+  return query_px<1, false>(s, sel, cls_scores, n_inst, H, W, H, W, masks, part_ws, scores, boxes, stream);
 }
 
 int query_postprocess_rescale_bits(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm,
@@ -1138,16 +1048,8 @@ int query_postprocess_rescale_bits(const float* logits, const int* sel, const fl
                 Wr % 16 == 0 && Wr <= 16384 && (reinterpret_cast<uintptr_t>(bits) & 1) == 0,
                 "query_postprocess_rescale_bits: bad args (H <= Hr, W <= Wr, Wr % 16 == 0, Wr <= 16384, 2-byte "
                 "aligned bits)");
-  Resize2 g{hm, wm, Hb, Wb, crop_h, crop_w, H, W};
-  // blocks past row H contribute empty partials (+0 to the sums): scores equal query_postprocess_rescale's
-  const int nblk = (Hr + QP_ROWS - 1) / QP_ROWS;
-  dim3 grid(nblk, n_inst);
-  const size_t smem = QP_ROWS * ((Wr + 31) / 32) * sizeof(uint32_t);
-  query_mask_rescale_bits_kernel<<<grid, 256, smem, stream>>>(logits, sel, g, Hr, Wr, bits, part_ws);
-  RSP_CHECK_LAUNCH();
-  query_finalize_kernel<<<(n_inst + 127) / 128, 128, 0, stream>>>(part_ws, nblk, cls_scores, n_inst, W, H, scores, boxes);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
+  const TwoResizes s{logits, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
+  return query_px<1, true>(s, sel, cls_scores, n_inst, H, W, Hr, Wr, bits, part_ws, scores, boxes, stream);
 }
 
 }  // namespace rsp

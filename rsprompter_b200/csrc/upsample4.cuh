@@ -77,6 +77,43 @@ __device__ __forceinline__ float bilinear_at(const float* __restrict__ src, int 
          ly * ((1.f - lx) * __ldg(src + y1 * w + x0) + lx * __ldg(src + y1 * w + x1));
 }
 
+// bilinear_at's resize (h, w) -> (H, W) of map m of maps [*, h, w] as a paste sampler: row() sets up an output row,
+// at() returns the value at a column of it.  SIG applies the sigmoid to the 4 taps first.  The fused multiply-adds
+// are explicit because where the blend rounds decides the pixels at the threshold: this is the rounding
+// rsp_mask_paste and rsp_query_postprocess have always had, which differ in the top-row blend (FUSE_RIGHT: the right
+// tap's product is the fused one).
+template <bool SIG, bool FUSE_RIGHT>
+struct OneResize {
+  const float* maps;
+  int h, w, H, W;
+  const float* r0;
+  const float* r1;
+  float ly;
+
+  __device__ __forceinline__ bool row(int m, int y) {
+    const float sy = fmaxf(fmaf(y + 0.5f, static_cast<float>(h) / H, -0.5f), 0.f);
+    const int y0 = min(static_cast<int>(sy), h - 1), y1 = min(y0 + 1, h - 1);
+    ly = sy - y0;
+    r0 = maps + (static_cast<size_t>(m) * h + y0) * w;
+    r1 = maps + (static_cast<size_t>(m) * h + y1) * w;
+    return true;
+  }
+
+  __device__ __forceinline__ float at(int x) const {
+    const float sx = fmaxf(fmaf(x + 0.5f, static_cast<float>(w) / W, -0.5f), 0.f);
+    const int x0 = min(static_cast<int>(sx), w - 1), x1 = min(x0 + 1, w - 1);
+    const float lx = sx - x0;
+    float v00 = __ldg(r0 + x0), v01 = __ldg(r0 + x1), v10 = __ldg(r1 + x0), v11 = __ldg(r1 + x1);
+    if (SIG) {
+      v00 = 1.f / (1.f + expf(-v00)); v01 = 1.f / (1.f + expf(-v01));
+      v10 = 1.f / (1.f + expf(-v10)); v11 = 1.f / (1.f + expf(-v11));
+    }
+    const float top = FUSE_RIGHT ? fmaf(lx, v01, __fmul_rn(1.f - lx, v00)) : fmaf(1.f - lx, v00, __fmul_rn(lx, v01));
+    const float bot = fmaf(1.f - lx, v10, __fmul_rn(lx, v11));
+    return fmaf(1.f - ly, top, __fmul_rn(ly, bot));
+  }
+};
+
 __device__ __forceinline__ float resize2_at(const float* __restrict__ src, const Resize2& g, int y, int x) {
   // second resize: (ch, cw) -> (H, W)
   const float sy = fmaxf((y + 0.5f) * (static_cast<float>(g.ch) / g.H) - 0.5f, 0.f);
@@ -89,5 +126,21 @@ __device__ __forceinline__ float resize2_at(const float* __restrict__ src, const
   const float v10 = bilinear_at(src, g.hm, g.wm, g.Hb, g.Wb, y1, x0), v11 = bilinear_at(src, g.hm, g.wm, g.Hb, g.Wb, y1, x1);
   return (1.f - ly) * ((1.f - lx) * v00 + lx * v01) + ly * ((1.f - lx) * v10 + lx * v11);
 }
+
+// resize2_at of map m of maps [*, hm, wm], row by row as OneResize
+struct TwoResizes {
+  const float* maps;
+  Resize2 g;
+  const float* src;
+  int y;
+
+  __device__ __forceinline__ bool row(int m, int yy) {
+    src = maps + static_cast<size_t>(m) * g.hm * g.wm;
+    y = yy;
+    return true;
+  }
+
+  __device__ __forceinline__ float at(int x) const { return resize2_at(src, g, y, x); }
+};
 
 }  // namespace rsp

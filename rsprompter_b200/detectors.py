@@ -251,21 +251,21 @@ class RSPrompterAnchor(_SamDetectorBase):
         B, M = r["scores"].shape
         logits = r["mask_logits"][:, 0].contiguous()
         fast = all(m is None for m in metas)
-        masks = _lib.mask_paste(logits, hw, thr, 0).view(B, M, hw[0], hw[1]) if fast else None
+        masks = _lib.mask_paste(logits, thr, raw=False, size=hw).view(B, M, hw[0], hw[1]) if fast else None
         counts = r["counts"].cpu().tolist()          # the only device->host read
         for b, ds in enumerate(batch_data_samples):
             n, m = counts[b], metas[b]
             boxes = r["bboxes"][b, :n]
-            if m is None:
-                mk = masks[b, :n] if fast else _lib.mask_paste(logits[b * M:b * M + max(n, 1)], hw, thr, 0)[:n]
-            else:   # resized / padded image: boxes back to the original image, masks through the two resizes
+            geom = dict(size=hw)
+            if m is not None:   # resized / padded image: boxes back to the original image, masks through the two resizes
                 sf, crop = m["scale_factor"], m["crop_hw"]
                 if rescale:
                     boxes = boxes / boxes.new_tensor(sf).repeat(2)
                 else:   # M:1756-1760 scales img_h / img_w once more before the crop; the output stays ori_shape
                     ih, iw = int(round(m["ori_hw"][0] * sf[1])), int(round(m["ori_hw"][1] * sf[0]))
                     crop = (min(int(ih * sf[1]), hw[0]), min(int(iw * sf[0]), hw[1]))
-                mk = _lib.mask_paste_rescale(logits[b * M:b * M + max(n, 1)], hw, crop, m["ori_hw"], thr)[:n]
+                geom = dict(rescale=(hw, crop, m["ori_hw"]))
+            mk = masks[b, :n] if fast else _lib.mask_paste(logits[b * M:b * M + max(n, 1)], thr, raw=False, **geom)[:n]
             ds.pred_instances = InstanceData(bboxes=boxes, scores=r["scores"][b, :n], labels=r["labels"][b, :n], masks=mk)
         return self._rle_masks(self.test_cfg, batch_data_samples)
 
@@ -284,12 +284,12 @@ class RSPrompterAnchor(_SamDetectorBase):
         thr = float(self.test_cfg.rcnn.get("mask_thr_binary", 0.5))
         boxes = r["bboxes"]
         if metas is None:
-            _lib.mask_paste_bits(r["mask_logits"][:, 0].contiguous(), thr, 0, bits=rec.mask_bits)
+            _lib.mask_paste(r["mask_logits"][:, 0].contiguous(), thr, raw=False, bits=rec.mask_bits)
         else:
             logits = r["mask_logits"][:, 0].contiguous()
             for b, m in enumerate(metas):
-                _lib.mask_paste_rescale_bits(logits[b * M:(b + 1) * M], hw, m["crop_hw"], m["ori_hw"], thr,
-                                             bits=rec.mask_bits.view(B * M, *rec.mask_bits.shape[2:])[b * M:(b + 1) * M])
+                _lib.mask_paste(logits[b * M:(b + 1) * M], thr, raw=False, rescale=(hw, m["crop_hw"], m["ori_hw"]),
+                                bits=rec.mask_bits.view(B * M, *rec.mask_bits.shape[2:])[b * M:(b + 1) * M])
             boxes = self._rescaled_boxes(boxes, metas)
         torch.cat([boxes, r["scores"][..., None], r["labels"].to(torch.float32)[..., None]], dim=2, out=rec.rows)
         rec.counts.copy_(r["counts"])

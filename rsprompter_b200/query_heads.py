@@ -435,12 +435,9 @@ class RSMaskFormerFusionHead(BaseModule):
                         query=query, is_thing=keep_thing)
         ms, ds, bs = [], [], []
         for b, m in enumerate(metas):      # image sizes differ: one launch pair per image, no host sync
-            if m is None:
-                mk, det, bx = _lib.query_postprocess(mask_pred, sel[b].contiguous(), sc[b].contiguous(), size)
-            else:
-                out_hw = m["ori_hw"] if rescale else m["crop_hw"]
-                mk, det, bx = _lib.query_postprocess_rescale(mask_pred, sel[b].contiguous(), sc[b].contiguous(), size,
-                                                             m["crop_hw"], out_hw)
+            geom = dict(size=size) if m is None else \
+                dict(rescale=(size, m["crop_hw"], m["ori_hw"] if rescale else m["crop_hw"]))
+            mk, det, bx = _lib.query_postprocess(mask_pred, sel[b].contiguous(), sc[b].contiguous(), **geom)
             ms.append(mk); ds.append(det); bs.append(bx)
         return dict(masks=ms, scores=ds, bboxes=bs, labels=labels, query=query, is_thing=keep_thing)
 
@@ -464,13 +461,14 @@ class RSMaskFormerFusionHead(BaseModule):
             det = torch.empty(B, K, device=cls.device, dtype=torch.float32)
             boxes = torch.empty(B, K, 4, device=cls.device, dtype=torch.float32)
             for b, m in enumerate(metas):
-                _lib.query_postprocess_rescale_bits(mask_pred, sel[b].contiguous(), sc[b].contiguous(), size,
-                                                    m["crop_hw"], m["ori_hw"], bits[b * K:(b + 1) * K], det[b], boxes[b])
+                _lib.query_postprocess(mask_pred, sel[b].contiguous(), sc[b].contiguous(),
+                                       rescale=(size, m["crop_hw"], m["ori_hw"]), bits=bits[b * K:(b + 1) * K],
+                                       scores=det[b], boxes=boxes[b])
             torch.cat([boxes, det[..., None], labels.to(torch.float32)[..., None]], dim=2, out=rec.rows)
             rec.counts.fill_(K)
             return
-        _, det, boxes = _lib.query_postprocess_bits(mask_pred, sel.reshape(-1), sc.reshape(-1).contiguous(),
-                                                    bits=rec.mask_bits.view(B * K, rec.hw[0], rec.hw[1] // 8))
+        _, det, boxes = _lib.query_postprocess(mask_pred, sel.reshape(-1), sc.reshape(-1).contiguous(),
+                                               bits=rec.mask_bits.view(B * K, rec.hw[0], rec.hw[1] // 8))
         torch.cat([boxes.view(B, K, 4), det.view(B, K, 1), labels.to(torch.float32)[..., None]], dim=2, out=rec.rows)
         rec.counts.fill_(K)
 

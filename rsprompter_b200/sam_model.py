@@ -233,7 +233,7 @@ def post_process_masks(masks, original_sizes, reshaped_input_sizes, mask_thresho
         if logits.shape[0] == 0:
             out.append(torch.zeros(*lead, *ori, dtype=torch.bool, device=m.device))
             continue
-        bits = _lib.mask_paste_rescale(logits, tuple(int(v) for v in pad_size), rs, ori, float(mask_threshold), raw=True)
+        bits = _lib.mask_paste(logits, float(mask_threshold), raw=True, rescale=(tuple(int(v) for v in pad_size), rs, ori))
         out.append(bits.view(*lead, *ori))
     return out
 
@@ -291,7 +291,7 @@ class SAMDet(BaseModule):
         logits = out.pred_masks[0][:, 0].contiguous()                     # [nb, 4g, 4g]
         img_hw = tuple(int(v) for v in meta["img_shape"][:2])
         crop = (min(int(ori_h * sf[1]), img_hw[0]), min(int(ori_w * sf[0]), img_hw[1]))
-        return _lib.mask_paste_rescale(logits, img_hw, crop, (ori_h, ori_w), 0.0, raw=True)
+        return _lib.mask_paste(logits, 0.0, raw=True, rescale=(img_hw, crop, (ori_h, ori_w)))
 
     @torch.no_grad()
     def predict(self, batch_inputs, batch_data_samples, rescale: bool = True):

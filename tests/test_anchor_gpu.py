@@ -154,14 +154,14 @@ def test_roi_head_stages(model_and_sd):
 
 
 @pytest.mark.parametrize("hm,size", [(256, (1024, 1024)), (64, (256, 256)), (256, (768, 768)), (48, (176, 208))])
-def test_mask_paste_matches_oracle(hm, size):
+def test_mask_paste_to_size_matches_oracle(hm, size):
     """x4 tiles (the shipped case: logits are image / 4) and the generic-scale kernel, borders included."""
     from oracle import restate_anchor as ra
     from rsprompter_b200 import _lib
     g = torch.Generator().manual_seed(8)
     logits = torch.randn(5, 1, hm, hm, generator=g) * 3
     ref = ra.mask_postprocess(logits, size, 0.5)
-    got = _lib.mask_paste(logits[:, 0].contiguous().cuda(), size, 0.5, 0)
+    got = _lib.mask_paste(logits[:, 0].contiguous().cuda(), 0.5, raw=False, size=size)
     torch.cuda.synchronize()
     assert got.dtype == torch.bool and got.shape == ref.shape
     assert (got.cpu() != ref).float().mean().item() < 1e-5
@@ -188,7 +188,7 @@ def test_end_to_end_predict_contract(model_and_sd):
 
 
 @pytest.mark.parametrize("ori,batch", [((120, 200), (256, 256)), ((512, 512), (1024, 1024)), ((300, 180), (256, 256))])
-def test_mask_paste_rescale_matches_oracle(ori, batch):
+def test_mask_paste_with_rescale_matches_oracle(ori, batch):
     """Resized + padded images (M:1763-1777): sigmoid -> batch shape -> crop -> ori_shape -> threshold, no intermediate."""
     from oracle import restate_anchor as ra
     from rsprompter_b200 import _lib
@@ -202,7 +202,7 @@ def test_mask_paste_rescale_matches_oracle(ori, batch):
     ref, ref_boxes = ra.mask_postprocess_rescale(logits, boxes.clone(), meta, 0.5)
     sf = meta["scale_factor"]
     crop = (min(int(ori[0] * sf[1]), batch[0]), min(int(ori[1] * sf[0]), batch[1]))
-    got = _lib.mask_paste_rescale(logits[:, 0].contiguous().cuda(), batch, crop, ori, 0.5)
+    got = _lib.mask_paste(logits[:, 0].contiguous().cuda(), 0.5, raw=False, rescale=(batch, crop, ori))
     torch.cuda.synchronize()
     assert got.shape == ref.shape and got.dtype == torch.bool
     assert (got.cpu() != ref).float().mean().item() < 2e-5

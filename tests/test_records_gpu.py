@@ -20,26 +20,26 @@ def test_pack_unpack_bits_roundtrip(shape):
     assert torch.equal(_lib.unpack_mask_bits(bits, shape[-1]).cpu(), m)
 
 
-def test_mask_paste_bits_equals_packed_mask_paste():
+def test_mask_paste_into_bits_equals_packed_bytes():
     from rsprompter_b200 import _lib
     g = torch.Generator().manual_seed(1)
     logits = (torch.randn(6, 64, 64, generator=g) * 3).cuda()
     for mode in (0, 1):
         thr = 0.5 if mode == 0 else 0.0
-        ref = _lib.mask_paste(logits, (256, 256), thr, mode)
-        bits = _lib.mask_paste_bits(logits, thr, mode)
+        ref = _lib.mask_paste(logits, thr, raw=mode == 1, size=(256, 256))
+        bits = _lib.mask_paste(logits, thr, raw=mode == 1, bits=torch.empty(6, 256, 32, dtype=torch.uint8).cuda())
         assert bits.shape == (6, 256, 32)
         assert np.array_equal(bits.cpu().numpy(), np.packbits(ref.cpu().numpy(), axis=-1, bitorder="little"))
 
 
-def test_query_postprocess_bits_equals_unpacked():
+def test_query_postprocess_into_bits_equals_unpacked():
     from rsprompter_b200 import _lib
     g = torch.Generator().manual_seed(2)
     logits = (torch.randn(12, 64, 64, generator=g) * 2).cuda()
     sel = torch.tensor([3, 0, 11, 7, 7], dtype=torch.int32).cuda()
     sc = torch.rand(5, generator=g).cuda()
     masks, s0, b0 = _lib.query_postprocess(logits, sel, sc, (256, 256))
-    bits, s1, b1 = _lib.query_postprocess_bits(logits, sel, sc)
+    bits, s1, b1 = _lib.query_postprocess(logits, sel, sc, bits=torch.empty(5, 256, 32, dtype=torch.uint8).cuda())
     assert torch.equal(s0, s1) and torch.equal(b0, b1)
     assert torch.equal(_lib.unpack_mask_bits(bits, 256), masks)
 
