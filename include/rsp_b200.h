@@ -57,8 +57,8 @@ int rsp_conv3x3_nhwc_bf16(const void* x, int B, int H, int W, int C, const void*
                           int out_fp32, void* stream);
 int rsp_conv3x3_geometry_ok(int B, int H, int W, int C);
 
-/* Same contract on CUDA cores (one thread per output); for contractions far below one
- * 128-row tile and as the independent check of the tensor-core kernel in tests. */
+/* Same contract on CUDA cores (one thread per output, GELU with erff): the independent check of the tensor-core
+ * kernel in tests. */
 int rsp_gemm_bf16_simt(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M,
                        int N, int K, const float* bias, const void* residual, int ldr, int res_fp32,
                        int res_mod, const int32_t* row_map, int act, int out_fp32, void* stream);
@@ -126,9 +126,8 @@ int rsp_nhwc_to_nchw(const void* in, int in_fp32, float* out, int B, int HW, int
  * embedding without the repeat_interleave copies of M:367-368 / M:1682-1683.
  * Alignment (a call that breaks it returns RSP_ERR_INVALID, nothing launched):
  *   epi_mode 1  out, residual, bias, ln_gamma, ln_beta 16-byte aligned; ldo, ldr % 8 == 0
- *   epi_mode 2  N % 128 == 0 with out 8-byte aligned and ldo % 4 == 0: bias, ln_gamma, ln_beta 16-byte aligned;
- *               otherwise out 16-byte aligned and ldo % 8 == 0
- *   epi_mode 3  hyper 16-byte aligned, mask_out 8-byte aligned; bias 16-byte aligned when grid_w is even */
+ *   epi_mode 2  N % 128 == 0, out 8-byte aligned, ldo % 4 == 0; bias, ln_gamma, ln_beta 16-byte aligned
+ *   epi_mode 3  hyper and bias 16-byte aligned, mask_out 8-byte aligned */
 int rsp_gemm_bf16_ex(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M, int N,
                      int K, const float* bias, const void* residual, int ldr, int res_fp32, int res_mod,
                      const int32_t* row_map, int act, int out_fp32, int epi_mode, const float* ln_gamma,
@@ -140,7 +139,7 @@ int rsp_gemm_bf16_ex(const void* A, int lda, const void* W, int ldw, void* out, 
  * tap1), W bf16 [128, K], hyper fp32 [prompts, n_out, 32] -> mask_out fp32 [prompts, n_out, 4*grid_h, 4*grid_w].
  * The multimask_output upscale of SamMaskDecoder (HF:521-531, mask_slice 1:): each accumulator tile of
  * upscale_conv2 feeds all n_out products, so the up1 rows are read once.  Output o has the bytes of
- * rsp_gemm_bf16_ex(epi_mode 3) with hyper[:, o].  grid_w even; hyper, bias 16-byte and mask_out 8-byte aligned. */
+ * rsp_gemm_bf16_ex(epi_mode 3) with hyper[:, o].  hyper, bias 16-byte and mask_out 8-byte aligned. */
 int rsp_gemm_upscale_masks(const void* A, int lda, const void* W, int ldw, int M, int K, const float* bias,
                            const float* hyper, int n_out, float* mask_out, int grid_h, int grid_w, void* stream);
 

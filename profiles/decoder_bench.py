@@ -83,8 +83,8 @@ def _gemm_cost(a, w, *args, **kw):
 
 def _upscale_cost(a, w, bias, hyper, gh, gw, *args, **kw):
     M, K = a.shape
-    P = M // (4 * gh * gw)
-    return 2.0 * M * 128 * K, M * K * 2 + P * 16 * gh * gw * 4
+    P, n_out = hyper.shape[0], hyper.shape[1]
+    return 2.0 * M * 128 * K, M * K * 2 + P * n_out * 16 * gh * gw * 4
 
 
 def _t2i_cost(q, K, V, hw, kv_block=None):
@@ -121,14 +121,14 @@ def _family(name: str, args, kw, n_img_rows: int) -> str:
         if w.shape[0] == 256:
             return "t2i k|v gemm"
         return "i2t q gemm"
-    return {"gemm_upscale_mask": "up2 gemm (GELU + hyper)", "t2i_attention": "t2i attention",
+    return {"gemm_upscale_masks": "up2 gemm (GELU + hyper)", "t2i_attention": "t2i attention",
             "i2t_attention": "i2t attention", "t2i_fused": "t2i fused (k|v gemm + attention)",
             "i2t_fused": "i2t fused (q gemm + attention + out_proj + LN4)"}.get(name, "token-side " + name)
 
 
-COSTS = {"gemm": _gemm_cost, "gemm_upscale_mask": _upscale_cost, "t2i_attention": _t2i_cost,
+COSTS = {"gemm": _gemm_cost, "gemm_upscale_masks": _upscale_cost, "t2i_attention": _t2i_cost,
          "i2t_attention": _i2t_cost, "t2i_fused": _t2i_fused_cost, "i2t_fused": _i2t_fused_cost}
-WRAPPED = ("gemm", "gemm_upscale_mask", "t2i_attention", "i2t_attention", "t2i_fused", "i2t_fused", "add_cast_bf16",
+WRAPPED = ("gemm", "gemm_upscale_masks", "t2i_attention", "i2t_attention", "t2i_fused", "i2t_fused", "add_cast_bf16",
            "cast_bf16", "token_self_attention")
 
 

@@ -309,7 +309,7 @@ def gemm_upscale_masks(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, hyp
     """gemm_upscale_mask for n_out <= 3 hypernetwork vectors per prompt in one GEMM (rsp_gemm_upscale_masks).
 
     a: bf16 [P*4*h*w, 64]; hyper fp32 [P, n_out, 32] -> fp32 masks [P, n_out, 4h, 4w]; mask o equals
-    gemm_upscale_mask(a, w, bias, hyper[:, o]) byte for byte.  grid_w must be even."""
+    gemm_upscale_mask(a, w, bias, hyper[:, o]) byte for byte."""
     global launch_count
     _require_cuda(a, w, bias, hyper, out)
     M, K = a.shape

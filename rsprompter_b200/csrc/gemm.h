@@ -6,7 +6,7 @@ namespace rsp {
 // out[row_map[m], n] = act(sum_k A[m,k] * W[n,k] + bias[n]) + residual[row_map[m] % res_mod, n]
 struct GemmArgs {
   const void* A = nullptr;   // bf16 [M, K], row stride lda
-  const void* W = nullptr;   // bf16 [N, K] (nn.Linear layout), row stride ldw; or [K, N] if w_is_kn
+  const void* W = nullptr;   // bf16 [N, K] (nn.Linear layout), row stride ldw
   void* out = nullptr;       // bf16 or fp32 [*, ldo]
   const float* bias = nullptr;     // fp32 [N] or null
   const void* residual = nullptr;  // fp32 or bf16 [*, ldr] or null (may alias out)
@@ -14,13 +14,10 @@ struct GemmArgs {
   int M = 0, N = 0, K = 0;
   int lda = 0, ldw = 0, ldo = 0, ldr = 0;
   int res_mod = 0;    // if > 0 the residual row is (destination row % res_mod)
-  int act = 0;        // 0 none, 1 GELU(erf), 2 ReLU   (applied before the residual add)
+  int act = 0;        // 0 none, 1 GELU (erf; gelu_fast on the wgmma kernel), 2 ReLU   (applied before the residual add)
   int out_fp32 = 0;
   int res_fp32 = 1;
-  int w_is_kn = 0;    // W stored [K, N] (N contiguous): exercises the MN-major UMMA descriptor
-  int force_bn = 0;   // 0 = heuristic; else 32/64/128/256
-  int max_ctas = 0;   // 0 = one CTA per SM
-  // epilogue variants used by the mask decoder (see gemm.cu)
+  // epilogue variants used by the mask decoder (see rsp_gemm_bf16_ex in rsp_b200.h)
   int epi_mode = 0;                   // 0 standard, 1 row LayerNorm, 2 LN over 64-column groups + GELU,
                                       // 3 GELU + hypernetwork dot + 2x2 mask scatter
   const float* ln_gamma = nullptr;
@@ -39,20 +36,18 @@ struct GemmArgs {
   int m_group_rows = 0, w_group_rows = 0;
 };
 
+// checked entry points (gemm.cu): every argument the kernels rely on is checked here, before any launch
 int gemm_bf16(const GemmArgs& a, cudaStream_t stream);
-int gemm_bf16_simt(const GemmArgs& a, cudaStream_t stream);
+int gemm_bf16_simt(const GemmArgs& a, cudaStream_t stream);   // CUDA cores, standard epilogue: the tests' reference
 bool conv3x3_geometry_ok(int B, int H, int W, int C);
 int conv3x3_bf16(const GemmArgs& a, cudaStream_t stream);   // conv_* set; standard epilogue only
-// coalesced-epilogue kernel (gemm_v2.cu); gemm_bf16 dispatches to it when eligible
-bool gemm_v2_eligible(const GemmArgs& a);
-int gemm_bf16_v2(const GemmArgs& a, int bn, cudaStream_t stream);
-bool gemm_v2_ln_row_eligible(const GemmArgs& a);
-int gemm_bf16_v2_ln_row(const GemmArgs& a, cudaStream_t stream);             // N == 256, bf16 residual / out
-int gemm_bf16_v2_ln64_gelu(const GemmArgs& a, cudaStream_t stream);     // N % 128 == 0
-int gemm_bf16_v2_gelu_hyper(const GemmArgs& a, cudaStream_t stream);    // N == 128
+// the multi-output upscale: epi_mode 3 arguments + n_out
+int gemm_upscale_masks(const GemmArgs& a, int n_out, cudaStream_t stream);
+
+// the wgmma kernel (gemm_v2.cu), called by the entry points above with checked arguments
+bool gemm_vector_rows(const GemmArgs& a);   // out / residual / bias rows the standard epilogue moves 8 bytes at a time
+int gemm_bf16_v2(const GemmArgs& a, cudaStream_t stream);   // any epi_mode
 // N == 128, hyper [prompts, n_out, 32], mask_out [prompts, n_out, 4*grid_h, 4*grid_w], 1 <= n_out <= 3
 int gemm_bf16_v2_gelu_hyper_multi(const GemmArgs& a, int n_out, cudaStream_t stream);
-// checked entry of the multi-output upscale (epi_mode 3 arguments + n_out; grid_w even)
-int gemm_upscale_masks(const GemmArgs& a, int n_out, cudaStream_t stream);
 
 }  // namespace rsp

@@ -1,25 +1,28 @@
-// Second-generation epilogue for the persistent wgmma GEMM (bias, GELU / ReLU, residual, row scatter,
-// bf16 / fp32 out, and the fused LayerNorm / upscaler epilogues).  Same mainloop as gemm.cu; what changes
-// is how the accumulator leaves the SM:
+// Persistent, warp-specialised bf16 GEMM for sm_90a:  out = epilogue(A[M,K] * W[N,K]^T), every dense contraction
+// of the inference path (gemm_bf16, conv3x3_bf16 and gemm_upscale_masks in gemm.cu check the arguments and call in
+// here).  Warp 0 is the TMA producer (A and W tiles -> 128B-swizzled smem ring), two warpgroups run the wgmma
+// mainloop (sm90.cuh wg_mainloop) and write the fp32 accumulators into a padded tile in shared memory, from which the
+// epilogue (bias, GELU / ReLU, residual, row scatter, bf16 / fp32 out, and the fused LayerNorm / upscaler epilogues)
+// takes them:
 //   * the epilogue runs on warps of its own (below), each owning 32 rows of the accumulator tile, or on the 8 MMA
 //     warps (2 per 32-row quarter, each owning half of the tile's columns);
 //   * every warp transposes its 32-row x 128-byte slab through a private, bank-conflict-free smem
 //     staging buffer, so global traffic is fully coalesced: each half-warp reads (residual) and
 //     writes one whole 128-byte line per instruction instead of 32 lanes touching 32 different
-//     lines (the thread-per-row pattern of the first version, which left K = 768 GEMMs
-//     epilogue-bound at ~35-55 % of the large-K rate).
+//     lines (a thread-per-row epilogue leaves K = 768 GEMMs epilogue-bound at ~35-55 % of the large-K rate).
+//     Rows that are not 8-byte aligned (odd N or ldo, fp32 rows at 4-byte alignment) go through the same staging
+//     buffer one element per store.  Only the row LayerNorm of the rows EPI_LN_ROW does not take reads its row per
+//     thread (EPI_LN_ROW_T).
 // Two schedules share the kernel template:
 //   * EPI_STD (plain, implicit-conv3x3 and grouped-weight GEMMs), 512 threads: warp 0 is the TMA producer, warpgroups
 //     1-2 only run the wgmma mainloop and write the accumulator tile, warpgroup 3 runs the epilogue from that tile.
 //     The tile changes hands through a "tile full" / "tile empty" mbarrier pair, so the MMA warpgroups start the next
 //     tile's k-loop while the epilogue of the last one is still running; at BN <= 64 the tile is double-buffered.
 //     setmaxnreg moves the producer warpgroup's registers to the MMA and epilogue warpgroups.
-//   * the mask decoder's fused epilogues (row LayerNorm, LN64 + GELU, GELU + hypernetwork), 384 threads: the two MMA
-//     warpgroups run the epilogue themselves after each tile.
+//   * the fused epilogues (row LayerNorm, LN64 + GELU, GELU + hypernetwork), 384 threads: the two MMA warpgroups run
+//     the epilogue themselves after each tile.
 // All shared memory is dynamic (1024-byte aligned by declaration), barriers live at its end:
 //   [ STAGES x (A 16 KB + B BN*128 B) | epilogue warps x 32 x 136 B staging | ACC_BUFS x 128 x (BN + 4) fp32 | barriers ]
-#include <cstdlib>
-
 #include "gemm.h"
 #include "sm90.cuh"
 
@@ -36,8 +39,10 @@ constexpr int BAR_BYTES = 256;
 constexpr int SMEM_MAX = 227 * 1024;
 
 // EPI_GELU_HYPER2 / 3: EPI_GELU_HYPER with 2 / 3 hypernetwork vectors per prompt (multimask_output); the output count
-// is part of the instantiation, so the single-output kernel is compiled exactly as before
-enum { EPI_STD = 0, EPI_LN_ROW = 1, EPI_LN64_GELU = 2, EPI_GELU_HYPER = 3, EPI_GELU_HYPER2 = 4, EPI_GELU_HYPER3 = 5 };
+// is part of the instantiation, so the single-output kernel is compiled exactly as before.
+// EPI_LN_ROW and EPI_LN_ROW_T are the two row-LayerNorm epilogues of epi_mode 1 (see gemm_bf16_v2).
+enum { EPI_STD = 0, EPI_LN_ROW = 1, EPI_LN64_GELU = 2, EPI_GELU_HYPER = 3, EPI_GELU_HYPER2 = 4, EPI_GELU_HYPER3 = 5,
+       EPI_LN_ROW_T = 6 };
 
 __host__ __device__ constexpr int hyper_outputs(int epi) { return epi == EPI_GELU_HYPER3 ? 3 : epi == EPI_GELU_HYPER2 ? 2 : 1; }
 
@@ -58,8 +63,9 @@ struct Cfg {
   static_assert(SMEM_BYTES <= SMEM_MAX, "shared memory");
   static_assert(2 * STAGES + 8 + 2 * ACC_BUFS <= BAR_BYTES / 8, "barrier area");
   // warps per 32-row quarter of the tile, each owning BN / NHALF columns: two halves when the MMA warpgroups run the
-  // epilogue of a wide tile, whole rows for the epilogue warpgroup of the split schedule
-  static constexpr int NHALF = (!SPLIT && BN >= 128) ? 2 : 1;
+  // epilogue of a wide tile, whole rows for the epilogue warpgroup of the split schedule and for EPI_LN_ROW_T
+  // (warps 4-7, thread = row)
+  static constexpr int NHALF = (!SPLIT && BN >= 128 && EPI != EPI_LN_ROW_T) ? 2 : 1;
   static constexpr int COLS_PER_WARP = BN / NHALF;
   // setmaxnreg budgets of the split schedule (launched at 128 per thread: producer + 2 x MMA + epilogue <= 4 x 128)
   static constexpr int REG_PRODUCER = 40;
@@ -83,7 +89,7 @@ struct Dev {
   int res_fp32;
   int num_n_blocks;
   int num_tiles;
-  // EPI 2 / 3 (mask-decoder upscaler, see gemm.cu for the maths)
+  // EPI 1 - 3 (the mask decoder's fused epilogues, see rsp_gemm_bf16_ex in rsp_b200.h for the maths)
   const float* ln_gamma;
   const float* ln_beta;
   float ln_eps;
@@ -94,6 +100,7 @@ struct Dev {
   int mblk_per_group, w_group_rows;   // grouped weights (0 = one W for every row)
   int tma_store;                 // output leaves through tma_c (no scatter, BN >= 64)
   int tma_res;                   // residual slabs arrive through tma_r into the staging buffer (added in place)
+  int scalar_rows;               // standard epilogue: out / residual / bias rows read and written one element at a time
 };
 
 __device__ __forceinline__ int num_kblocks(const Dev& p) { return p.conv_kb > 0 ? 9 * p.conv_kb : (p.K + BK - 1) / BK; }
@@ -104,6 +111,70 @@ __device__ __forceinline__ int residual_row(const Dev& p, int orow) {
     return p.res_block_map[blk] * p.res_block_rows + (orow - blk * p.res_block_rows);
   }
   return p.res_mod > 0 ? (orow % p.res_mod) : orow;
+}
+
+// EPI_LN_ROW_T: v[0..31] += bias[col0..] ; v += residual[rrow, col0..]   (col0 + 32 <= N, 16-byte aligned)
+__device__ __forceinline__ void add_bias_residual32(const Dev& p, float (&v)[32], int rrow, int col0) {
+  if (p.bias) {
+    const float4* b4 = reinterpret_cast<const float4*>(p.bias + col0);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float4 b = __ldg(b4 + i);
+      v[4 * i + 0] += b.x; v[4 * i + 1] += b.y; v[4 * i + 2] += b.z; v[4 * i + 3] += b.w;
+    }
+  }
+  if (p.residual) {
+    if (p.res_fp32) {
+      const float4* r4 = reinterpret_cast<const float4*>(
+          static_cast<const float*>(p.residual) + static_cast<size_t>(rrow) * p.ldr + col0);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float4 x = r4[i];
+        v[4 * i + 0] += x.x; v[4 * i + 1] += x.y; v[4 * i + 2] += x.z; v[4 * i + 3] += x.w;
+      }
+    } else {
+      const uint4* r4 = reinterpret_cast<const uint4*>(
+          static_cast<const __nv_bfloat16*>(p.residual) + static_cast<size_t>(rrow) * p.ldr + col0);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint4 x = r4[i];
+        const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const __nv_bfloat162 h = *reinterpret_cast<const __nv_bfloat162*>(&w[j]);
+          v[8 * i + 2 * j + 0] += __bfloat162float(h.x);
+          v[8 * i + 2 * j + 1] += __bfloat162float(h.y);
+        }
+      }
+    }
+  }
+}
+
+// EPI_LN_ROW_T: out[orow, col0 .. col0 + 31] = v   (16-byte aligned)
+__device__ __forceinline__ void store32(const Dev& p, const float (&v)[32], int orow, int col0) {
+  if (p.out_fp32) {
+    float4* o4 = reinterpret_cast<float4*>(static_cast<float*>(p.out) + static_cast<size_t>(orow) * p.ldo + col0);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) o4[i] = make_float4(v[4 * i + 0], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+  } else {
+    uint4* o4 = reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(p.out) + static_cast<size_t>(orow) * p.ldo + col0);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      o4[i] = make_uint4(pack_bf16x2(v[8 * i + 0], v[8 * i + 1]), pack_bf16x2(v[8 * i + 2], v[8 * i + 3]),
+                         pack_bf16x2(v[8 * i + 4], v[8 * i + 5]), pack_bf16x2(v[8 * i + 6], v[8 * i + 7]));
+  }
+}
+
+// scalar rows of the standard epilogue: one element of the residual / output
+__device__ __forceinline__ float residual_at(const Dev& p, int rrow, int col) {
+  const size_t i = static_cast<size_t>(rrow) * p.ldr + col;
+  return p.res_fp32 ? static_cast<const float*>(p.residual)[i]
+                    : __bfloat162float(static_cast<const __nv_bfloat16*>(p.residual)[i]);
+}
+__device__ __forceinline__ void store_at(const Dev& p, int orow, int col, float x) {
+  const size_t i = static_cast<size_t>(orow) * p.ldo + col;
+  if (p.out_fp32) static_cast<float*>(p.out)[i] = x;
+  else static_cast<__nv_bfloat16*>(p.out)[i] = __float2bfloat16_rn(x);
 }
 
 // Output path of the standard epilogue: chosen per tile, or fixed for a whole loop of tiles
@@ -120,7 +191,7 @@ __device__ __forceinline__ void epilogue_tile(const Dev& p, const CUtensorMap& t
   const int q = e & 3;
   uint8_t* stg = stg_all + e * STG_WARP;
   const uint32_t stg_s = smem_u32(stg);
-  const bool stage_f32 = p.out_fp32 || (p.residual != nullptr);
+  const bool stage_f32 = p.out_fp32 || (p.residual != nullptr) || p.scalar_rows;
   const int W = stage_f32 ? 32 : (C::COLS_PER_WARP < 64 ? C::COLS_PER_WARP : 64);   // columns per pass
   const int n_pass = C::COLS_PER_WARP / W;
   const int lpr = stage_f32 ? 16 : (W * 2) / 8;     // lanes per row at 8 bytes each
@@ -226,6 +297,58 @@ __device__ __forceinline__ void epilogue_tile(const Dev& p, const CUtensorMap& t
       for (int o = 0; o < NO; ++o)
         *reinterpret_cast<float2*>(p.mask_out + ((static_cast<size_t>(n) * NO + o) * 4 * p.grid_h + Y) * W4 + X) =
             make_float2(m2[o][0], m2[o][1]);
+    }
+  } else if constexpr (EPI == EPI_LN_ROW_T) {
+    // out = LayerNorm_N(acc + bias + residual) for N % 32 == 0, N <= BN (one n-block; BN 128 for N <= 128, 256
+    // above): the lane owns the whole row in
+    // the accumulator tile, two passes over it, statistics in fp32 taken sequentially over the N / 32 chunks in
+    // column order.  Shifted sums (pivot = the row's first value): no E[x^2] - E[x]^2 cancellation for rows with a
+    // large mean.  fp32 or bf16 residual and output, res_mod / res_block_map, or no residual: the mask decoder's token
+    // norms (SamTwoWayAttentionBlock layer_norm1-3, layer_norm_final_attn, HF:316-338, 398-404) and layer_norm4 where
+    // the block map's rows are not whole 32-row slabs.
+    const int row = m_blk * BM + q * 32 + lane;
+    const int orow = row < p.M ? row : -1;
+    const int rrow = (orow >= 0 && p.residual) ? residual_row(p, orow) : orow;
+    const uint32_t t_row = acc_row(acc_base, C::ACC_LD, q * 32 + lane);
+    float sum = 0.f, sq = 0.f, piv = 0.f;
+    const int nch = p.N / 32;
+    for (int c = 0; c < nch; ++c) {
+      uint32_t r[32];
+      acc_ld32(t_row + (c * 32) * 4, r);
+      if (orow < 0) continue;
+      float v[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+      add_bias_residual32(p, v, rrow, c * 32);
+      if (c == 0) piv = v[0];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) { const float d = v[i] - piv; sum += d; sq += d * d; }
+    }
+    const float dmean = sum / p.N;
+    const float mean = piv + dmean;
+    // sq / N - dmean^2: one rounding at BN 256, two at BN 128, the rounding each tile width has always had.  Written
+    // out, because whether ptxas fuses a multiply and a subtract depends on its schedule.
+    const float var = BN == 256 ? fmaf(-dmean, dmean, sq / p.N) : __fsub_rn(sq / p.N, __fmul_rn(dmean, dmean));
+    const float rstd = rsqrtf(fmaxf(var, 0.f) + p.ln_eps);
+    for (int c = 0; c < nch; ++c) {
+      uint32_t r[32];
+      acc_ld32(t_row + (c * 32) * 4, r);
+      if (orow < 0) continue;
+      float v[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+      add_bias_residual32(p, v, rrow, c * 32);
+      const float4* g4 = reinterpret_cast<const float4*>(p.ln_gamma + c * 32);
+      const float4* b4 = reinterpret_cast<const float4*>(p.ln_beta + c * 32);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float4 g = __ldg(g4 + i), b = __ldg(b4 + i);
+        v[4 * i + 0] = (v[4 * i + 0] - mean) * rstd * g.x + b.x;
+        v[4 * i + 1] = (v[4 * i + 1] - mean) * rstd * g.y + b.y;
+        v[4 * i + 2] = (v[4 * i + 2] - mean) * rstd * g.z + b.z;
+        v[4 * i + 3] = (v[4 * i + 3] - mean) * rstd * g.w + b.w;
+      }
+      store32(p, v, orow, c * 32);
     }
   } else if constexpr (EPI == EPI_LN_ROW) {
     // out = LayerNorm_256(acc + bias + residual), bf16 (N == BN == 256: the tile holds whole rows).  Two warps
@@ -604,7 +727,10 @@ __device__ __forceinline__ void epilogue_tile(const Dev& p, const CUtensorMap& t
         const int rrow = get_rrow(rr);
         resv[k] = make_float2(0.f, 0.f);
         if (orow >= 0 && col < p.N) {
-          if (p.res_fp32) {
+          if (p.scalar_rows) {
+            resv[k].x = residual_at(p, rrow, col);
+            if (col + 1 < p.N) resv[k].y = residual_at(p, rrow, col + 1);
+          } else if (p.res_fp32) {
             resv[k] = *reinterpret_cast<const float2*>(static_cast<const float*>(p.residual) +
                                                        static_cast<size_t>(rrow) * p.ldr + col);
           } else {
@@ -632,7 +758,7 @@ __device__ __forceinline__ void epilogue_tile(const Dev& p, const CUtensorMap& t
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
           if (p.bias) {
-            if (col0 + 32 <= p.N) {
+            if (col0 + 32 <= p.N && !p.scalar_rows) {
               const float4* b4 = reinterpret_cast<const float4*>(p.bias + col0);
 #pragma unroll
               for (int i = 0; i < 8; ++i) {
@@ -678,14 +804,17 @@ __device__ __forceinline__ void epilogue_tile(const Dev& p, const CUtensorMap& t
             float x0, x1;
             asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x0), "=f"(x1) : "r"(stg_s + rr * STG_ROW + cl * 8));
             if (p.residual) {
-              if (p.res_fp32) {
+              if (p.res_fp32 || p.scalar_rows) {
                 x0 += resv[k].x; x1 += resv[k].y;
               } else {
                 const uint32_t raw = __float_as_uint(resv[k].x);
                 x0 += __uint_as_float(raw << 16); x1 += __uint_as_float(raw & 0xffff0000u);
               }
             }
-            if (p.out_fp32)
+            if (p.scalar_rows) {
+              store_at(p, orow, col, x0);
+              if (col + 1 < p.N) store_at(p, orow, col + 1, x1);
+            } else if (p.out_fp32)
               *reinterpret_cast<float2*>(static_cast<float*>(p.out) + static_cast<size_t>(orow) * p.ldo + col) =
                   make_float2(x0, x1);
             else
@@ -822,8 +951,8 @@ gemm_bf16_wgmma_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __gri
       int it = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
         float acc[BN / 2];
-        wg_mainloop<BN, false, STAGES>(acc, smem_base, C::STAGE_BYTES, A_BYTES, num_kb, wg, kstage, kphase, bar_full,
-                                       bar_empty);
+        wg_mainloop<BN, STAGES>(acc, smem_base, C::STAGE_BYTES, A_BYTES, num_kb, wg, kstage, kphase, bar_full,
+                                bar_empty);
         const int buf = C::ACC_BUFS == 2 ? (it & 1) : 0;
         const uint32_t use = C::ACC_BUFS == 2 ? (it >> 1) : it;   // earlier tiles through this buffer
         mbar_wait(smem_u32(&bar_tempty[buf]), (use & 1) ^ 1);   // the epilogue is done with its previous tile
@@ -839,8 +968,8 @@ gemm_bf16_wgmma_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __gri
         const int n_blk = tile % p.num_n_blocks;
         {
           float acc[BN / 2];
-          wg_mainloop<BN, false, STAGES>(acc, smem_base, C::STAGE_BYTES, A_BYTES, num_kb, wg, kstage, kphase,
-                                         bar_full, bar_empty);
+          wg_mainloop<BN, STAGES>(acc, smem_base, C::STAGE_BYTES, A_BYTES, num_kb, wg, kstage, kphase, bar_full,
+                                  bar_empty);
           named_bar_sync(5, 256);   // the previous tile's epilogue has read the accumulator tile
           acc_store<BN>(acc, acc_base, C::ACC_LD, wg, threadIdx.x & 127);
           named_bar_sync(5, 256);
@@ -889,18 +1018,17 @@ static int launch(const GemmArgs& a, cudaStream_t stream) {
   CUtensorMap tc = tb, tr = tb;
   p.tma_store = 0;
   p.tma_res = 0;
+  p.scalar_rows = EPI == EPI_STD && !gemm_vector_rows(a);
   {
     const uint64_t esz = a.out_fp32 ? 4 : 2;
-    static const bool no_tma_store = getenv("RSP_GEMM_NO_TMA_STORE") != nullptr;
     bool res_ok = true;
     if (a.residual) {
-      static const bool no_tma_res = getenv("RSP_GEMM_NO_TMA_RES") != nullptr;
-      res_ok = !no_tma_res && (a.res_fp32 != 0) == (a.out_fp32 != 0) &&
+      res_ok = (a.res_fp32 != 0) == (a.out_fp32 != 0) &&
                (reinterpret_cast<uintptr_t>(a.residual) & 15) == 0 && (static_cast<uint64_t>(a.ldr) * esz) % 16 == 0 &&
                (a.res_block_map ? (a.res_block_rows % 32 == 0 && a.M % 32 == 0) : (a.res_mod == 0 || a.res_mod % 32 == 0));
     }
-    if (!no_tma_store && (EPI == EPI_STD || EPI == EPI_LN_ROW || EPI == EPI_LN64_GELU) && BN >= 64 && res_ok && !a.row_map &&
-        a.out &&
+    if ((EPI == EPI_STD || EPI == EPI_LN_ROW || EPI == EPI_LN64_GELU) && BN >= 64 && res_ok && !a.row_map &&
+        !p.scalar_rows && a.out &&
         (reinterpret_cast<uintptr_t>(a.out) & 15) == 0 && (static_cast<uint64_t>(a.ldo) * esz) % 16 == 0) {
       uint64_t dims[2] = {static_cast<uint64_t>(a.N), static_cast<uint64_t>(a.M)};
       uint64_t strides[1] = {static_cast<uint64_t>(a.ldo) * esz};
@@ -940,8 +1068,7 @@ static int launch(const GemmArgs& a, cudaStream_t stream) {
     RSP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr_set = true;
   }
-  int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
-  if (a.max_ctas > 0 && grid > a.max_ctas) grid = a.max_ctas;
+  const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
   kern<<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(ta, tb, tc, tr, p);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
@@ -949,9 +1076,9 @@ static int launch(const GemmArgs& a, cudaStream_t stream) {
 
 }  // namespace v2
 
-// Eligibility: standard epilogue, [N,K] weights, 8-byte alignable rows.
-bool gemm_v2_eligible(const GemmArgs& a) {
-  if (a.epi_mode != 0 || a.w_is_kn || !a.out) return false;
+// Rows the standard epilogue moves 8 bytes (and bias 16 bytes) at a time: N, ldo, ldr and the out / residual / bias
+// pointers aligned for it.  Other rows take its scalar path.
+bool gemm_vector_rows(const GemmArgs& a) {
   const bool stage_f32 = a.out_fp32 || a.residual;
   const uintptr_t po = reinterpret_cast<uintptr_t>(a.out), pr = reinterpret_cast<uintptr_t>(a.residual);
   if (stage_f32) {
@@ -964,33 +1091,26 @@ bool gemm_v2_eligible(const GemmArgs& a) {
   return true;
 }
 
-int gemm_bf16_v2(const GemmArgs& a, int bn, cudaStream_t stream) {
-  switch (bn) {
-    case 128: return v2::launch<128, v2::EPI_STD>(a, stream);
-    case 64: return v2::launch<64, v2::EPI_STD>(a, stream);
-    case 32: return v2::launch<32, v2::EPI_STD>(a, stream);
-    default: set_last_error("gemm_v2: unsupported BN %d", bn); return RSP_ERR_INVALID;
-  }
-}
-
-// out = LayerNorm_256(acc + bias + residual), bf16 in / bf16 residual / bf16 out (mask decoder: LN4(keys + attn))
-bool gemm_v2_ln_row_eligible(const GemmArgs& a) {
-  static const bool off = getenv("RSP_GEMM_NO_LN_FUSED") != nullptr;
-  return !off && a.N == 256 && !a.out_fp32 && a.residual && !a.res_fp32 && a.bias && a.ln_gamma && a.ln_beta && !a.row_map &&
-         !a.w_is_kn && a.res_mod == 0 && a.act == 0 && (reinterpret_cast<uintptr_t>(a.out) & 15) == 0 && a.ldo % 8 == 0 &&
-         (reinterpret_cast<uintptr_t>(a.residual) & 15) == 0 && a.ldr % 8 == 0 &&
-         (reinterpret_cast<uintptr_t>(a.bias) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.ln_gamma) & 15) == 0 &&
-         (reinterpret_cast<uintptr_t>(a.ln_beta) & 15) == 0 &&
+// Row LayerNorms that EPI_LN_ROW takes (two warps per row, residual slabs and output by TMA): N == 256, bf16 residual
+// and output, residual rows in whole 32-row slabs (mask decoder: LN4(keys + attn)).  gemm_bf16 has checked the
+// 16-byte alignment of every row.  The others run EPI_LN_ROW_T.
+static bool ln_row_tma(const GemmArgs& a) {
+  return a.N == 256 && !a.out_fp32 && a.residual && !a.res_fp32 && a.bias && a.res_mod == 0 && a.act == 0 &&
          (a.res_block_map ? (a.res_block_rows % 32 == 0 && a.M % 32 == 0) : true);
 }
-int gemm_bf16_v2_ln_row(const GemmArgs& a, cudaStream_t stream) { return v2::launch<256, v2::EPI_LN_ROW>(a, stream); }
 
-// mask-decoder upscaler epilogues on the 8-warp kernel (called from gemm_bf16 for epi_mode 2 / 3)
-int gemm_bf16_v2_ln64_gelu(const GemmArgs& a, cudaStream_t stream) {
-  return v2::launch<128, v2::EPI_LN64_GELU>(a, stream);
-}
-
-int gemm_bf16_v2_gelu_hyper(const GemmArgs& a, cudaStream_t stream) {
+int gemm_bf16_v2(const GemmArgs& a, cudaStream_t stream) {
+  if (a.epi_mode == v2::EPI_STD) {
+    // tiles up to 128 wide: the fp32 accumulator tile of a 256-wide one leaves shared memory for a single stage
+    if (a.N > 64) return v2::launch<128, v2::EPI_STD>(a, stream);
+    if (a.N > 32) return v2::launch<64, v2::EPI_STD>(a, stream);
+    return v2::launch<32, v2::EPI_STD>(a, stream);
+  }
+  if (a.epi_mode == v2::EPI_LN_ROW) {
+    if (ln_row_tma(a)) return v2::launch<256, v2::EPI_LN_ROW>(a, stream);
+    return a.N > 128 ? v2::launch<256, v2::EPI_LN_ROW_T>(a, stream) : v2::launch<128, v2::EPI_LN_ROW_T>(a, stream);
+  }
+  if (a.epi_mode == v2::EPI_LN64_GELU) return v2::launch<128, v2::EPI_LN64_GELU>(a, stream);
   return v2::launch<128, v2::EPI_GELU_HYPER>(a, stream);
 }
 

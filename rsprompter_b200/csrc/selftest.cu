@@ -38,7 +38,7 @@ static uint16_t f2bf(float f) {
 struct Case {
   const char* name;
   int M, N, K;
-  int bias, act, residual, res_fp32, out_fp32, row_map, res_mod, w_is_kn, force_bn;
+  int bias, act, residual, res_fp32, out_fp32, row_map, res_mod;
 };
 
 static int run_case(const Case& c) {
@@ -86,11 +86,11 @@ static int run_case(const Case& c) {
   }
   GemmArgs a;
   a.A = dA; a.W = dW; a.M = M; a.N = N; a.K = K;
-  a.lda = K; a.ldw = c.w_is_kn ? N : K; a.ldo = N; a.ldr = N;
+  a.lda = K; a.ldw = K; a.ldo = N; a.ldr = N;
   a.bias = c.bias ? db : nullptr;
   a.residual = c.residual ? dres : nullptr;
   a.res_fp32 = c.res_fp32; a.out_fp32 = c.out_fp32; a.act = c.act;
-  a.row_map = dmap; a.res_mod = c.res_mod; a.w_is_kn = c.w_is_kn; a.force_bn = c.force_bn;
+  a.row_map = dmap; a.res_mod = c.res_mod;
   a.out = dO1;
   int s = gemm_bf16(a, 0);
   if (s) { printf("[%s] gemm_bf16 failed: %s\n", c.name, last_error()); return 1; }
@@ -142,7 +142,7 @@ static int run_case(const Case& c) {
   return nbad ? 1 : 0;
 }
 
-static void bench_gemm(int M, int N, int K, int bn, int act, int out_fp32, int residual, int res_bf16 = 0, int iters = 20, int res_mod = 0) {
+static void bench_gemm(int M, int N, int K, int act, int out_fp32, int residual, int res_bf16 = 0, int iters = 20, int res_mod = 0) {
   void *dA, *dW, *dO, *dR = nullptr;
   float* db;
   CK(cudaMalloc(&dA, (size_t)M * K * 2));
@@ -156,7 +156,7 @@ static void bench_gemm(int M, int N, int K, int bn, int act, int out_fp32, int r
   (void)res_bf16;
   GemmArgs a;
   a.A = dA; a.W = dW; a.out = dO; a.bias = db; a.M = M; a.N = N; a.K = K;
-  a.lda = K; a.ldw = K; a.ldo = N; a.ldr = N; a.act = act; a.out_fp32 = out_fp32; a.force_bn = bn;
+  a.lda = K; a.ldw = K; a.ldo = N; a.ldr = N; a.act = act; a.out_fp32 = out_fp32;
   a.residual = dR; a.res_fp32 = res_bf16 ? 0 : 1; a.res_mod = res_mod;
   for (int i = 0; i < 3; ++i) gemm_bf16(a, 0);
   CK(cudaDeviceSynchronize());
@@ -171,8 +171,8 @@ static void bench_gemm(int M, int N, int K, int bn, int act, int out_fp32, int r
   ms /= iters;
   const double bytes = (double)M * K * 2 + (double)N * K * 2 + (double)M * N * (out_fp32 ? 4 : 2) +
                        (residual ? (double)M * N * (res_bf16 ? 2 : 4) : 0.0);
-  printf("bench gemm M=%d N=%d K=%d bn=%d act=%d outf32=%d res=%d%s: %.3f ms  %.1f TFLOP/s  %.0f GB/s\n", M, N, K,
-         bn, act, out_fp32, residual, res_bf16 ? "(bf16)" : "", ms, 2.0 * M * N * K / ms * 1e-9, bytes / ms * 1e-6);
+  printf("bench gemm M=%d N=%d K=%d act=%d outf32=%d res=%d%s: %.3f ms  %.1f TFLOP/s  %.0f GB/s\n", M, N, K,
+         act, out_fp32, residual, res_bf16 ? "(bf16)" : "", ms, 2.0 * M * N * K / ms * 1e-9, bytes / ms * 1e-6);
   cudaFree(dA); cudaFree(dW); cudaFree(dO); cudaFree(db);
   if (dR) cudaFree(dR);
 }
@@ -189,46 +189,38 @@ int main(int argc, char** argv) {
   printf("device: %s sm_%d%d, %d SMs\n", prop.name, prop.major, prop.minor, prop.multiProcessorCount);
   if (!strcmp(what, "gemm") || !strcmp(what, "all")) {
     const Case cases[] = {
-        //            name        M     N     K   bias act res rf32 of32 map mod kn  bn
-        {"tiny-f32",            128,  128,   64,  0, 0, 0, 1, 1, 0, 0, 0, 128},
-        {"k128-f32",            256,  256,  128,  0, 0, 0, 1, 1, 0, 0, 0, 0},
-        {"bn256",               384,  512,  256,  1, 0, 0, 1, 1, 0, 0, 0, 256},
-        {"bn64",                200,   64,  192,  1, 2, 0, 1, 0, 0, 0, 0, 64},
-        {"bn32",                200,   32,  192,  1, 2, 0, 1, 0, 0, 0, 0, 32},
-        {"ragged-n",            300,   40,  128,  1, 0, 0, 1, 1, 0, 0, 0, 0},
-        {"bias-gelu-bf16",     1000,  768,  768,  1, 1, 0, 1, 0, 0, 0, 0, 0},
-        {"resid-f32",          1000,  768, 3072,  1, 0, 1, 1, 1, 0, 0, 0, 0},
-        {"resid-bf16",          777,  256,  320,  1, 2, 1, 0, 0, 0, 0, 0, 0},
-        {"rowmap-resid",       4000, 2304,  768,  1, 0, 1, 1, 1, 1, 0, 0, 256},
-        {"posembed-mod",       2048,  768,  768,  1, 0, 1, 1, 1, 0, 512, 0, 0},
-        {"multi-tile-per-cta", 40000, 256,  128,  1, 0, 0, 1, 0, 0, 0, 0, 0},
-        {"w-kn-128",            512,  128,  256,  0, 0, 0, 1, 1, 0, 0, 1, 0},
-        {"w-kn-64",             300,   64,  192,  1, 0, 0, 1, 1, 0, 0, 1, 0},
-        {"w-kn-256n",           512,  256,  128,  0, 0, 0, 1, 1, 0, 0, 1, 0},
+        //            name        M     N     K   bias act res rf32 of32 map mod
+        {"tiny-f32",            128,  128,   64,  0, 0, 0, 1, 1, 0, 0},
+        {"k128-f32",            256,  256,  128,  0, 0, 0, 1, 1, 0, 0},
+        {"n512-f32",            384,  512,  256,  1, 0, 0, 1, 1, 0, 0},
+        {"bn64",                200,   64,  192,  1, 2, 0, 1, 0, 0, 0},
+        {"bn32",                200,   32,  192,  1, 2, 0, 1, 0, 0, 0},
+        {"ragged-n",            300,   40,  128,  1, 0, 0, 1, 1, 0, 0},
+        {"bias-gelu-bf16",     1000,  768,  768,  1, 1, 0, 1, 0, 0, 0},
+        {"resid-f32",          1000,  768, 3072,  1, 0, 1, 1, 1, 0, 0},
+        {"resid-bf16",          777,  256,  320,  1, 2, 1, 0, 0, 0, 0},
+        {"rowmap-resid",       4000, 2304,  768,  1, 0, 1, 1, 1, 1, 0},
+        {"posembed-mod",       2048,  768,  768,  1, 0, 1, 1, 1, 0, 512},
+        {"multi-tile-per-cta", 40000, 256,  128,  1, 0, 0, 1, 0, 0, 0},
     };
     for (const Case& c : cases) fails += run_case(c);
     if (bench) {
       // ViT-H encoder linears at 1024^2, batch 8 (default tile width): qkv over 25 padded 14 x 14 windows per image,
       // proj / lin1 / lin2 over 64 x 64 tokens per image
-      bench_gemm(39200, 3840, 1280, 0, 0, 0, 0);   // qkv: bias -> bf16
-      bench_gemm(32768, 1280, 1280, 0, 0, 1, 1);   // proj: bias + fp32 residual -> fp32
-      bench_gemm(32768, 5120, 1280, 0, 1, 0, 0);   // lin1: bias + GELU -> bf16
-      bench_gemm(32768, 1280, 5120, 0, 0, 1, 1);   // lin2: bias + fp32 residual -> fp32
-      bench_gemm(32768, 2304, 768, 256, 0, 0, 0);
-      bench_gemm(32768, 768, 768, 256, 0, 1, 1);
-      bench_gemm(32768, 3072, 768, 256, 1, 0, 0);
-      bench_gemm(32768, 768, 3072, 256, 0, 1, 1);
-      bench_gemm(32768, 768, 3072, 128, 0, 1, 1);
-      bench_gemm(8192, 8192, 8192, 256, 0, 0, 0);
-      bench_gemm(8192, 8192, 8192, 128, 0, 0, 0);
+      bench_gemm(39200, 3840, 1280, 0, 0, 0);   // qkv: bias -> bf16
+      bench_gemm(32768, 1280, 1280, 0, 1, 1);   // proj: bias + fp32 residual -> fp32
+      bench_gemm(32768, 5120, 1280, 1, 0, 0);   // lin1: bias + GELU -> bf16
+      bench_gemm(32768, 1280, 5120, 0, 1, 1);   // lin2: bias + fp32 residual -> fp32
+      bench_gemm(32768, 768, 3072, 0, 1, 1);
+      bench_gemm(8192, 8192, 8192, 0, 0, 0);
     }
   }
   if (!strcmp(what, "gemmprof")) {
     // mask-decoder shapes (N prompts * 4096 image tokens rows)
-    bench_gemm(1 << 20, 256, 128, 0, 0, 1, 1, 1, 3);   // i2t out_proj + bf16 residual -> fp32
-    bench_gemm(1 << 20, 128, 256, 0, 0, 0, 0, 0, 3);   // k / v / q projections
-    bench_gemm(1 << 20, 256, 128, 0, 0, 0, 0, 0, 3);
-    bench_gemm(1 << 20, 128, 256, 0, 0, 0, 1, 0, 3, 4096);   // k-proj + broadcast fp32 residual (k_proj(pe))
+    bench_gemm(1 << 20, 256, 128, 0, 1, 1, 1, 3);   // i2t out_proj + bf16 residual -> fp32
+    bench_gemm(1 << 20, 128, 256, 0, 0, 0, 0, 3);   // k / v / q projections
+    bench_gemm(1 << 20, 256, 128, 0, 0, 0, 0, 3);
+    bench_gemm(1 << 20, 128, 256, 0, 0, 1, 0, 3, 4096);   // k-proj + broadcast fp32 residual (k_proj(pe))
   }
   if (!strcmp(what, "attn") || !strcmp(what, "all")) fails += selftest_attention(bench);
   printf("selftest: %d failing case(s)\n", fails);

@@ -376,14 +376,14 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // Consumer side of the GEMM ring: warpgroup wg accumulates rows [64 wg, 64 wg + 64) of a 128 x BN tile over num_kb
-// 64-deep k-blocks.  Stage s holds A (128 rows x 128 B, K-major) at base + s * stage_bytes and B at + a_bytes
-// (K-major BN rows, or MN-major: BN / 64 atoms of 64 K-rows x 128 B).  Each of the warpgroup's warps arrives once on
+// 64-deep k-blocks.  Stage s holds A (128 rows x 128 B, K-major) at base + s * stage_bytes and B (BN rows, K-major)
+// at + a_bytes.  Each of the warpgroup's warps arrives once on
 // the stage's "empty" barrier (count 8 for two warpgroups) when its reads are done.
 // One wgmma group stays in flight: k-block kb is committed, then the group of kb - 1 is retired and its stage
 // released, so the tensor cores never wait for the issuing warps between k-blocks.  The whole tile is retired
 // (wait_group 0) before the accumulators are returned.  With a single-stage ring the stage of kb must be released
 // before kb + 1 can be loaded, so there every group is retired at once.
-template <int BN, bool B_MN, int STAGES>
+template <int BN, int STAGES>
 __device__ __forceinline__ void wg_mainloop(float (&d)[BN / 2], uint32_t base, int stage_bytes, int a_bytes,
                                             int num_kb, int wg, int& stage, uint32_t& phase, uint64_t* bar_full,
                                             uint64_t* bar_empty) {
@@ -400,8 +400,8 @@ __device__ __forceinline__ void wg_mainloop(float (&d)[BN / 2], uint32_t base, i
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const uint64_t adesc = make_gdesc(sa + k * 32, 16, 1024);
-      const uint64_t bdesc = B_MN ? make_gdesc(sb + k * 2048, 64 * 128, 1024) : make_gdesc(sb + k * 32, 16, 1024);
-      Wgmma<BN>::template ss<B_MN ? 1 : 0>(d, adesc, bdesc, (kb | k) != 0);
+      const uint64_t bdesc = make_gdesc(sb + k * 32, 16, 1024);
+      Wgmma<BN>::template ss<0>(d, adesc, bdesc, (kb | k) != 0);
     }
     wgmma_commit();
     if constexpr (IN_FLIGHT) {

@@ -305,18 +305,10 @@ class SamMaskDecoderB200(nn.Module):
         up1 = _lib.gemm(keys_b, p["up1_w"], p["up1_b"], ln64_gelu=(*p["up_ln"], 1e-6))   # [N*HW, 4*64]
         up1 = up1.view(N * HW * 4, -1)
         sel = range(1, self.num_mask_tokens) if multimask_output else range(0, 1)
-        if len(sel) > 1 and w % 2 == 0:
-            # every output mask from one pass over up1: [N, n_out, 32] hypernetwork vectors, one GEMM, the masks
-            # written in place ([N, n_out, 4h, 4w]); each equals its single-output launch byte for byte
-            hyper = torch.stack([self._ff(_lib.cast_bf16(qv[:, 1 + i].contiguous()), p["hyper"][i]) for i in sel], dim=1)
-            masks = _lib.gemm_upscale_masks(up1, p["up2_w"], p["up2_b"], hyper, h, w)
-            return masks, iou[:, 1:]
-        masks = []
-        for i in sel:
-            mt = _lib.cast_bf16(qv[:, 1 + i].contiguous())
-            hyper = self._ff(mt, p["hyper"][i])                             # [N, 32]
-            masks.append(_lib.gemm_upscale_mask(up1, p["up2_w"], p["up2_b"], hyper, h, w))
-        masks = torch.stack(masks, dim=1) if len(masks) > 1 else masks[0].unsqueeze(1)
+        # every output mask from one pass over up1: [N, n_out, 32] hypernetwork vectors, one GEMM, the masks written
+        # in place ([N, n_out, 4h, 4w]); each equals its single-output launch byte for byte
+        hyper = torch.stack([self._ff(_lib.cast_bf16(qv[:, 1 + i].contiguous()), p["hyper"][i]) for i in sel], dim=1)
+        masks = _lib.gemm_upscale_masks(up1, p["up2_w"], p["up2_b"], hyper, h, w)
         iou = iou[:, 1:] if multimask_output else iou[:, 0:1]
         return masks, iou
 

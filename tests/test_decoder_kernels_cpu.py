@@ -150,9 +150,10 @@ def test_upscale2_bugs_are_far(h, w, one_hot):
 
 
 # ---------------------------------------------------------------------------------------------------- alignment
-def test_epilogue_alignment_rejected_before_launch():
-    """Every alignment the fused epilogues' vector accesses need is checked on the host: a call that breaks one
-    returns RSP_ERR_INVALID before any device work (so these addresses are never dereferenced)."""
+def test_epilogue_shape_and_alignment_rejected_before_launch():
+    """Every alignment the fused epilogues' vector accesses need, and the column count of epi_mode 2, is checked on
+    the host: a call that breaks one returns RSP_ERR_INVALID before any device work (so these addresses are never
+    dereferenced), with a message that names what was broken."""
     from rsprompter_b200 import _lib
     base = 1 << 24
     A, W, O, R, B, G, E, H, MO = (base * (i + 1) for i in range(9))
@@ -167,17 +168,20 @@ def test_epilogue_alignment_rejected_before_launch():
         return st, (_lib._lib.rsp_last_error() or b"").decode()
 
     cases = [
-        # epi 1: out, residual, bias, gamma, beta all move 16 bytes at a time (v2 and v1 alike)
-        ex(1, out=O + 8, res=R), ex(1, res=R + 8), ex(1, res=R, bias=B + 4), ex(1, res=R, g=G + 8),
-        ex(1, res=R, e=E + 4), ex(1, out=O + 8, res=R, res_fp32=1, out_fp32=1),
-        # epi 2, v2 (N % 128 == 0, out 8-byte aligned): float4 bias / gamma / beta
-        ex(2, bias=B + 4), ex(2, g=G + 8), ex(2, e=E + 4),
-        # epi 2, v1 (out not 8-byte aligned, or N % 128 != 0): 16-byte stores
-        ex(2, out=O + 2), ex(2, out=O + 8, N=64), ex(2, N=64, ldo=260),
-        # epi 3: float4 hyper, float2 mask stores; v2 (even grid_w) also float4 bias
-        ex(3, out=None, N=128, hyper=H + 4, mask=MO, grid=(4, 6)), ex(3, out=None, N=128, hyper=H, mask=MO + 4, grid=(4, 5)),
-        ex(3, out=None, N=128, hyper=H + 8, mask=MO, grid=(4, 5)), ex(3, out=None, N=128, bias=B + 4, hyper=H, mask=MO,
-                                                                      grid=(4, 6)),
+        # epi 1: out, residual, bias, gamma, beta all move 16 bytes at a time (both row-LN epilogues)
+        (ex(1, out=O + 8, res=R), "alignment"), (ex(1, res=R + 8), "alignment"), (ex(1, res=R, bias=B + 4), "alignment"),
+        (ex(1, res=R, g=G + 8), "alignment"), (ex(1, res=R, e=E + 4), "alignment"),
+        (ex(1, out=O + 8, res=R, res_fp32=1, out_fp32=1), "alignment"),
+        # epi 2: float4 bias / gamma / beta, out 8-byte aligned ...
+        (ex(2, bias=B + 4), "alignment"), (ex(2, g=G + 8), "alignment"), (ex(2, e=E + 4), "alignment"),
+        (ex(2, out=O + 2), "alignment"),
+        # ... and N % 128 == 0
+        (ex(2, out=O + 8, N=64), "N %"), (ex(2, N=64, ldo=260), "N %"),
+        # epi 3: float4 hyper and bias, float2 mask stores
+        (ex(3, out=None, N=128, hyper=H + 4, mask=MO, grid=(4, 6)), "alignment"),
+        (ex(3, out=None, N=128, hyper=H, mask=MO + 4, grid=(4, 5)), "alignment"),
+        (ex(3, out=None, N=128, hyper=H + 8, mask=MO, grid=(4, 5)), "alignment"),
+        (ex(3, out=None, N=128, bias=B + 4, hyper=H, mask=MO, grid=(4, 6)), "alignment"),
     ]
-    for i, (st, msg) in enumerate(cases):
-        assert st != 0 and "alignment" in msg, (i, st, msg)
+    for i, ((st, msg), want) in enumerate(cases):
+        assert st != 0 and want in msg, (i, st, msg)

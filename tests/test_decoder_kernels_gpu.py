@@ -171,8 +171,8 @@ def test_upscale1_ln_gelu(h, w, ldo):
 @pytest.mark.parametrize("h,w", [(64, 64), (30, 30), (40, 25)])
 @pytest.mark.parametrize("P", [1, 7, 133])
 def test_upscale2_hyper(h, w, P):
-    """epi_mode 3 (upscale_conv2 + GELU + hypernetwork product): v2 on 64 x 64 and 30 x 30, the v1 fallback on
-    40 x 25 (odd grid_w).  The one-hot hyper case pins the pixel placement Y = 4y + 2ty1 + ty2, X = 4x + 2tx1 + tx2."""
+    """epi_mode 3 (upscale_conv2 + GELU + hypernetwork product) on 64 x 64, 30 x 30 and 40 x 25 (odd grid_w).  The
+    one-hot hyper case pins the pixel placement Y = 4y + 2ty1 + ty2, X = 4x + 2tx1 + tx2."""
     from rsprompter_b200 import _lib
     for one_hot in (False, True):
         up1, W2, b2, hyper = _cuda(*dk.upscale2_inputs(P, h, w, seed=P + h + w, one_hot=one_hot))

@@ -21,6 +21,9 @@ def _rel_err(got, ref):
     (1000, 768, 3072, None, True, torch.float32),
     (777, 40, 256, "relu", False, torch.float32),
     (64, 256, 2048, None, True, torch.float32),
+    # odd N: rows of 4-byte (fp32) and 2-byte (bf16) alignment take the epilogue's scalar path
+    (800, 11, 256, None, False, torch.float32),
+    (300, 11, 256, "relu", True, torch.bfloat16),
 ])
 def test_gemm_matches_fp32_reference(M, N, K, act, res, out_dtype):
     from rsprompter_b200 import _lib
@@ -186,6 +189,8 @@ def test_conv3x3_geometry_gate():
     # fp32 residual and output: the decoder's token path
     pytest.param(8000, 0.0, torch.float32, None, id="fp32res-8000"),
     pytest.param(70, 300.0, torch.float32, None, id="fp32res-70"),
+    # no residual, fp32 output: the decoder's first ln1
+    pytest.param(5600, 0.0, None, None, id="nores-5600"),
 ])
 def test_gemm_fused_row_layernorm_large_mean(M, offset, res_dtype, block):
     """LN(acc + bias + residual) fused into the GEMM epilogue (mask decoder layer_norm4 / token norms, HF:346-347) on
@@ -200,16 +205,18 @@ def test_gemm_fused_row_layernorm_large_mean(M, offset, res_dtype, block):
     w = (torch.randn(N, K, generator=g) * 0.05).to(torch.bfloat16)
     bias = torch.randn(N, generator=g) * 0.1
     rows, bmap = block if block else (M, None)
-    res = (torch.randn((max(bmap) + 1) * rows if bmap else M, N, generator=g) + offset).to(res_dtype)
+    res = None if res_dtype is None else (torch.randn((max(bmap) + 1) * rows if bmap else M, N, generator=g) +
+                                          offset).to(res_dtype)
     gamma, beta = 1 + 0.1 * torch.randn(N, generator=g), 0.1 * torch.randn(N, generator=g)
     rm = {} if bmap is None else dict(res_block_map=torch.tensor(bmap, dtype=torch.int32), res_block_rows=rows)
     ref = dk.ln_row(a, w, bias, res, gamma, beta, 1e-6, **rm)
-    if res_dtype == torch.float32:
+    if res_dtype in (torch.float32, None):
         out_dtypes = (torch.float32,)
     else:
         out_dtypes = (torch.bfloat16, torch.float32) if M < 128 else (torch.bfloat16,)
     for out_dtype in out_dtypes:
-        out = _lib.gemm(a.cuda(), w.cuda(), bias.cuda(), residual=res.cuda(), ln=(gamma.cuda(), beta.cuda(), 1e-6),
+        out = _lib.gemm(a.cuda(), w.cuda(), bias.cuda(), residual=None if res is None else res.cuda(),
+                        ln=(gamma.cuda(), beta.cuda(), 1e-6),
                         out_dtype=out_dtype, **{k: (v.cuda() if torch.is_tensor(v) else v) for k, v in rm.items()})
         torch.cuda.synchronize()
         err = (out.double().cpu() - ref).abs()
