@@ -15,8 +15,6 @@
 //   query_postprocess         bilinear 256^2 -> S^2 + (> 0) + mask score + tight box per selected instance
 //                             (M:652-656, maskformer_fusion_head.py:149-182, mask/utils.py:56-77), no S^2 fp32
 //                             intermediate and no per-instance host sync
-#include <cstdlib>
-
 #include "query.h"
 #include "sm90.cuh"
 #include "upsample4.cuh"
@@ -730,8 +728,8 @@ int mask_embed_src(const float* mpp, const float* const* wts, const float* emb, 
                    int hm, int wm, int h, int w, float eps, void* src, void* src_pe, cudaStream_t stream) {
   RSP_CHECK_ARG(mpp && wts && emb && pos && src && N > 0 && hm == 4 * h && wm == 4 * w, "mask_embed_src: bad args");
   MaskEmbedW W{wts[0], wts[1], wts[2], wts[3], wts[4], wts[5], wts[6], wts[7], wts[8], wts[9]};
-  static const bool fp32_path = getenv("RSP_MASK_EMBED_FP32") != nullptr;     // A/B switch (tests compare the two)
-  if (!src_pe && (h * w) % 128 == 0 && w % 4 == 0 && (reinterpret_cast<uintptr_t>(mpp) & 15) == 0 && !fp32_path) {
+  // whole 128-pixel blocks without src_pe take the tensor-core kernel, every other shape the fp32 one
+  if (!src_pe && (h * w) % 128 == 0 && w % 4 == 0 && (reinterpret_cast<uintptr_t>(mpp) & 15) == 0) {
     dim3 grid(h * w / 128, N);
     mask_embed_src_mma_kernel<<<grid, 128, 0, stream>>>(mpp, W, emb, n_per_img, hm, wm, h, w, eps,
                                                         static_cast<__nv_bfloat16*>(src));
