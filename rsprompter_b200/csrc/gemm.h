@@ -47,6 +47,9 @@ int gemm_upscale_masks(const GemmArgs& a, int n_out, cudaStream_t stream);
 // the wgmma kernel (gemm_v2.cu), called by the entry points above with checked arguments
 bool gemm_vector_rows(const GemmArgs& a);   // out / residual / bias rows the standard epilogue moves 8 bytes at a time
 int gemm_bf16_v2(const GemmArgs& a, cudaStream_t stream);   // any epi_mode
+// epi_mode 0 on the schedule given (wide: 128 x 256 tiles, epilogue in registers; else the split schedule), without
+// gemm_bf16_v2's choice between them: the self-test's A/B of the two
+int gemm_bf16_v2_std(const GemmArgs& a, bool wide, cudaStream_t stream);
 // N == 128, hyper [prompts, n_out, 32], mask_out [prompts, n_out, 4*grid_h, 4*grid_w], 1 <= n_out <= 3
 int gemm_bf16_v2_gelu_hyper_multi(const GemmArgs& a, int n_out, cudaStream_t stream);
 

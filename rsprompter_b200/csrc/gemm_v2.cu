@@ -13,7 +13,7 @@
 //     Rows that are not 8-byte aligned (odd N or ldo, fp32 rows at 4-byte alignment) go through the same staging
 //     buffer one element per store.  Only the row LayerNorm of the rows EPI_LN_ROW does not take reads its row per
 //     thread (EPI_LN_ROW_T).
-// Two schedules share the kernel template:
+// Three schedules share the kernel template:
 //   * EPI_STD (plain, implicit-conv3x3 and grouped-weight GEMMs), 512 threads: warp 0 is the TMA producer, warpgroups
 //     1-2 only run the wgmma mainloop and write the accumulator tile, warpgroup 3 runs the epilogue from that tile.
 //     The tile changes hands through a "tile full" / "tile empty" mbarrier pair, so the MMA warpgroups start the next
@@ -21,6 +21,8 @@
 //     setmaxnreg moves the producer warpgroup's registers to the MMA and epilogue warpgroups.
 //   * the fused epilogues (row LayerNorm, LN64 + GELU, GELU + hypernetwork), 384 threads: the two MMA warpgroups run
 //     the epilogue themselves after each tile.
+//   * EPI_STD_WIDE (bf16-output plain GEMMs with long k-loops and many tiles), 384 threads, 128 x 256 tiles: the MMA
+//     warpgroups run the epilogue from their accumulator registers, with no accumulator tile (epilogue_wide).
 // All shared memory is dynamic (1024-byte aligned by declaration), barriers live at its end:
 //   [ STAGES x (A 16 KB + B BN*128 B) | epilogue warps x 32 x 136 B staging | ACC_BUFS x 128 x (BN + 4) fp32 | barriers ]
 #include "gemm.h"
@@ -41,8 +43,10 @@ constexpr int SMEM_MAX = 227 * 1024;
 // EPI_GELU_HYPER2 / 3: EPI_GELU_HYPER with 2 / 3 hypernetwork vectors per prompt (multimask_output); the output count
 // is part of the instantiation, so the single-output kernel is compiled exactly as before.
 // EPI_LN_ROW and EPI_LN_ROW_T are the two row-LayerNorm epilogues of epi_mode 1 (see gemm_bf16_v2).
+// EPI_STD_WIDE is the standard epilogue (bias, GELU / ReLU, bf16 out by TMA; no residual, no scatter) on 128 x 256
+// tiles, run by the MMA warpgroups straight from their accumulator registers (see gemm_bf16_v2 for when it is used).
 enum { EPI_STD = 0, EPI_LN_ROW = 1, EPI_LN64_GELU = 2, EPI_GELU_HYPER = 3, EPI_GELU_HYPER2 = 4, EPI_GELU_HYPER3 = 5,
-       EPI_LN_ROW_T = 6 };
+       EPI_LN_ROW_T = 6, EPI_STD_WIDE = 7 };
 
 __host__ __device__ constexpr int hyper_outputs(int epi) { return epi == EPI_GELU_HYPER3 ? 3 : epi == EPI_GELU_HYPER2 ? 2 : 1; }
 
@@ -50,15 +54,19 @@ template <int BN, int EPI>
 struct Cfg {
   static constexpr bool SPLIT = EPI == EPI_STD;   // epilogue on its own warpgroup (BN <= 128)
   static_assert(!SPLIT || BN <= 128, "a 64 x 256 wgmma needs more registers than a 512-thread block has per thread");
+  // accumulators never leave the registers: no accumulator tile, and 16-row output slabs (one warp's rows)
+  static constexpr bool WIDE = EPI == EPI_STD_WIDE;
+  static_assert(!WIDE || BN == 256, "the register epilogue is written for the 64 x 256 fragment");
   static constexpr int THREADS = SPLIT ? 512 : 384;
   static constexpr int EPI_WARPS = SPLIT ? 4 : 8;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int ACC_LD = BN + 4;
   static constexpr int ACC_BYTES = BM * ACC_LD * 4;
-  static constexpr int ACC_BUFS = (SPLIT && BN <= 64) ? 2 : 1;
+  static constexpr int ACC_BUFS = WIDE ? 0 : (SPLIT && BN <= 64) ? 2 : 1;
   static constexpr int STG_BYTES = EPI_WARPS * STG_WARP;
-  static constexpr int STAGES = SPLIT ? ((BN == 128) ? 4 : (BN == 64) ? 5 : 8) : ((BN == 256) ? 1 : 3);   // 227 KB
+  static constexpr int STAGES =
+      WIDE ? 4 : SPLIT ? ((BN == 128) ? 4 : (BN == 64) ? 5 : 8) : ((BN == 256) ? 1 : 3);   // 227 KB
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + ACC_BUFS * ACC_BYTES + BAR_BYTES;
   static_assert(SMEM_BYTES <= SMEM_MAX, "shared memory");
   static_assert(2 * STAGES + 8 + 2 * ACC_BUFS <= BAR_BYTES / 8, "barrier area");
@@ -68,10 +76,12 @@ struct Cfg {
   static constexpr int NHALF = (!SPLIT && BN >= 128 && EPI != EPI_LN_ROW_T) ? 2 : 1;
   static constexpr int COLS_PER_WARP = BN / NHALF;
   // setmaxnreg budgets of the split schedule (launched at 128 per thread: producer + 2 x MMA + epilogue <= 4 x 128)
+  // and of the wide one (launched at 168: producer + 2 x MMA <= 3 x 168; 128 of the MMA registers are accumulators)
   static constexpr int REG_PRODUCER = 40;
-  static constexpr int REG_MMA = 168;
-  static constexpr int REG_EPI = 512 - REG_PRODUCER - 2 * REG_MMA;
-  static_assert(REG_EPI >= 128 && REG_EPI % 8 == 0, "the epilogue warpgroup takes registers, never gives them up");
+  static constexpr int REG_MMA = WIDE ? 232 : 168;
+  static_assert(!WIDE || REG_PRODUCER + 2 * REG_MMA <= 3 * 168, "wide schedule register budget");
+  static constexpr int REG_EPI = SPLIT ? 512 - REG_PRODUCER - 2 * REG_MMA : 0;
+  static_assert(!SPLIT || (REG_EPI >= 128 && REG_EPI % 8 == 0), "the epilogue warpgroup takes registers, never gives them up");
 };
 
 struct Dev {
@@ -860,6 +870,51 @@ __device__ __forceinline__ void epilogue_loop(const Dev& p, const CUtensorMap& t
   }
 }
 
+// Epilogue of the wide schedule, run by each MMA warp on its own accumulator fragment.  Warp e holds rows
+// [64 wg + 16 (e & 3), + 16) of the 128 x 256 tile; its lane l holds rows l / 4 and l / 4 + 8 of those, and in every
+// 8-column group c the columns 8 c + 2 (l % 4) + {0, 1} (acc[4 c + {0, 1}] and acc[4 c + {2, 3}]).  Bias, activation
+// and bf16 rounding are the split epilogue's, in its order, so both schedules write the same bytes.  The warp's four
+// 16 x 64 slabs leave through the two 2 KB halves of its staging buffer (128-byte swizzled, as the 64 x 16 box of
+// tma_c expects) as TMA stores; a store is waited for only before its half is rewritten, so the stores of one tile
+// drain while the next tile's k-loop runs.
+__device__ __forceinline__ void epilogue_wide(const Dev& p, const CUtensorMap& tma_c, const float (&acc)[128],
+                                              int m_blk, int n_blk, int wg, int e, uint8_t* stg_all) {
+  const int lane = threadIdx.x & 31;
+  const int r = lane >> 2;                           // rows r and r + 8 of the warp's 16; (r + 8) & 7 == r
+  const int row0 = m_blk * BM + wg * 64 + (e & 3) * 16;
+  const uint32_t slab = smem_u32(stg_all) + e * 4096;
+  const float* bias = p.bias;
+  const int act = p.act;
+#pragma unroll
+  for (int s = 0; s < 4; ++s) {
+    const int col0 = n_blk * 256 + s * 64;
+    const uint32_t half = slab + (s & 1) * 2048;
+    if (lane == 0) bulk_wait_read1();                // the store that last read this half is done with it
+    __syncwarp();
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      float v[4] = {acc[32 * s + 4 * c], acc[32 * s + 4 * c + 1], acc[32 * s + 4 * c + 2], acc[32 * s + 4 * c + 3]};
+      if (bias) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col0 + 8 * c + 2 * (lane & 3)));
+        v[0] += b.x; v[1] += b.y; v[2] += b.x; v[3] += b.y;
+      }
+      if (act == 1) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) v[i] = gelu_fast(v[i]);
+      } else if (act == 2) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) v[i] = fmaxf(v[i], 0.f);
+      }
+      const uint32_t a = half + r * 128 + ((c ^ r) << 4) + 4 * (lane & 3);
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(pack_bf16x2(v[0], v[1])) : "memory");
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + 8 * 128), "r"(pack_bf16x2(v[2], v[3])) : "memory");
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) { tma_store_2d(&tma_c, half, col0, row0); bulk_commit(); }
+  }
+}
+
 template <int BN, int EPI>
 __global__ void __launch_bounds__(Cfg<BN, EPI>::THREADS, 1)
 gemm_bf16_wgmma_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
@@ -899,7 +954,7 @@ gemm_bf16_wgmma_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __gri
 
   // each role's setmaxnreg comes first in its branch: ptxas allocates the branch's registers under that budget
   if (warp < 4) {
-    if constexpr (C::SPLIT) setmaxnreg_dec<C::REG_PRODUCER>();
+    if constexpr (C::SPLIT || C::WIDE) setmaxnreg_dec<C::REG_PRODUCER>();
     if (warp == 0 && lane == 0) {
       const int num_kb = num_kblocks(p);
       // ---------------------------------------------------------- TMA producer
@@ -942,12 +997,21 @@ gemm_bf16_wgmma_v2_kernel(const __grid_constant__ CUtensorMap tma_a, const __gri
     }
   } else if (warp < 12) {
     // ------------------------------------------------------------ MMA warpgroups: rows [64 wg, 64 wg + 64) of each tile
-    if constexpr (C::SPLIT) setmaxnreg_inc<C::REG_MMA>();
+    if constexpr (C::SPLIT || C::WIDE) setmaxnreg_inc<C::REG_MMA>();
     const int wg = (warp - 4) >> 2;
     const int num_kb = num_kblocks(p);   // computed per role: a value live across setmaxnreg goes to local memory
     int kstage = 0;
     uint32_t kphase = 0;
-    if constexpr (C::SPLIT) {
+    if constexpr (C::WIDE) {
+      // the producer refills the ring for the next tile while these warps run the epilogue
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        float acc[BN / 2];
+        wg_mainloop<BN, STAGES>(acc, smem_base, C::STAGE_BYTES, A_BYTES, num_kb, wg, kstage, kphase, bar_full,
+                                bar_empty);
+        epilogue_wide(p, tma_c, acc, tile / p.num_n_blocks, tile % p.num_n_blocks, wg, warp - 4, stg_all);
+      }
+      if (lane == 0) bulk_wait0();   // every slab is in global memory before the CTA retires
+    } else if constexpr (C::SPLIT) {
       int it = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
         float acc[BN / 2];
@@ -1027,12 +1091,12 @@ static int launch(const GemmArgs& a, cudaStream_t stream) {
                (reinterpret_cast<uintptr_t>(a.residual) & 15) == 0 && (static_cast<uint64_t>(a.ldr) * esz) % 16 == 0 &&
                (a.res_block_map ? (a.res_block_rows % 32 == 0 && a.M % 32 == 0) : (a.res_mod == 0 || a.res_mod % 32 == 0));
     }
-    if ((EPI == EPI_STD || EPI == EPI_LN_ROW || EPI == EPI_LN64_GELU) && BN >= 64 && res_ok && !a.row_map &&
-        !p.scalar_rows && a.out &&
+    if ((EPI == EPI_STD || EPI == EPI_STD_WIDE || EPI == EPI_LN_ROW || EPI == EPI_LN64_GELU) && BN >= 64 && res_ok &&
+        !a.row_map && !p.scalar_rows && a.out &&
         (reinterpret_cast<uintptr_t>(a.out) & 15) == 0 && (static_cast<uint64_t>(a.ldo) * esz) % 16 == 0) {
       uint64_t dims[2] = {static_cast<uint64_t>(a.N), static_cast<uint64_t>(a.M)};
       uint64_t strides[1] = {static_cast<uint64_t>(a.ldo) * esz};
-      uint32_t box[2] = {a.out_fp32 ? 32u : 64u, 32u};
+      uint32_t box[2] = {a.out_fp32 ? 32u : 64u, C::WIDE ? 16u : 32u};
       RSP_TRY(make_tmap(&tc, a.out, 2, dims, strides, box, a.out_fp32));
       p.tma_store = 1;
       if (a.residual) {
@@ -1048,6 +1112,10 @@ static int launch(const GemmArgs& a, cudaStream_t stream) {
   }
   if (EPI == EPI_LN_ROW && !(p.tma_store && p.tma_res)) {
     set_last_error("gemm_v2: fused row LayerNorm needs TMA-eligible bf16 output and residual");
+    return RSP_ERR_INVALID;
+  }
+  if (C::WIDE && !(p.tma_store && !a.residual && !a.out_fp32 && a.N % BN == 0 && a.conv_c == 0 && a.m_group_rows == 0)) {
+    set_last_error("gemm_v2: the wide schedule needs a plain GEMM with TMA-eligible bf16 output, no residual, N %% 256 == 0");
     return RSP_ERR_INVALID;
   }
   p.M = a.M; p.N = a.N; p.K = a.K;
@@ -1099,12 +1167,33 @@ static bool ln_row_tma(const GemmArgs& a) {
          (a.res_block_map ? (a.res_block_rows % 32 == 0 && a.M % 32 == 0) : true);
 }
 
+// Standard-epilogue GEMMs the wide schedule can take: plain 2-D A, bf16 output through TMA, no residual or row scatter,
+// whole 256-wide n-blocks and 64-deep k-blocks.
+static bool std_wide_shape(const GemmArgs& a) {
+  return a.epi_mode == v2::EPI_STD && !a.residual && !a.row_map && !a.out_fp32 && a.conv_c == 0 &&
+         a.m_group_rows == 0 && a.N % 256 == 0 && a.K % 64 == 0 && gemm_vector_rows(a) && a.out &&
+         (reinterpret_cast<uintptr_t>(a.out) & 15) == 0 && a.ldo % 8 == 0;
+}
+
+int gemm_bf16_v2_std(const GemmArgs& a, bool wide, cudaStream_t stream) {
+  if (wide) return v2::launch<256, v2::EPI_STD_WIDE>(a, stream);
+  if (a.N > 64) return v2::launch<128, v2::EPI_STD>(a, stream);
+  if (a.N > 32) return v2::launch<64, v2::EPI_STD>(a, stream);
+  return v2::launch<32, v2::EPI_STD>(a, stream);
+}
+
 int gemm_bf16_v2(const GemmArgs& a, cudaStream_t stream) {
   if (a.epi_mode == v2::EPI_STD) {
-    // tiles up to 128 wide: the fp32 accumulator tile of a 256-wide one leaves shared memory for a single stage
-    if (a.N > 64) return v2::launch<128, v2::EPI_STD>(a, stream);
-    if (a.N > 32) return v2::launch<64, v2::EPI_STD>(a, stream);
-    return v2::launch<32, v2::EPI_STD>(a, stream);
+    // 128 x 256 tiles with the epilogue in registers where they pay.  The epilogue stalls the tensor cores once per
+    // tile, so the k-loop must be long enough to amortise it, and a wide tile is twice the work of the split
+    // schedule's, so the last partial wave costs twice as much.  `rsp_selftest gemm bench` (H100 SXM, 700 W):
+    // K = 1280 at 29 - 39 waves of wide tiles (ViT-H qkv / lin1, 32 768 - 39 200 rows) runs 1.06 - 1.16x faster;
+    // K = 768 (ViT-B qkv / lin1, same rows) 0.94 - 0.99x, K = 512 0.82x, and K = 1280 at 7 - 10 waves 0.86 - 0.91x.
+    // Every other call takes 128-wide tiles or narrower with the epilogue on its own warpgroup: the fp32 accumulator
+    // tile of a 256-wide one would leave shared memory for a single stage.
+    const long long wide_tiles = static_cast<long long>((a.M + v2::BM - 1) / v2::BM) * (a.N / 256);
+    const bool wide = std_wide_shape(a) && a.K >= 1024 && wide_tiles >= 16ll * num_sms();
+    return gemm_bf16_v2_std(a, wide, stream);
   }
   if (a.epi_mode == v2::EPI_LN_ROW) {
     if (ln_row_tma(a)) return v2::launch<256, v2::EPI_LN_ROW>(a, stream);

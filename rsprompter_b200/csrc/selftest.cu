@@ -177,6 +177,69 @@ static void bench_gemm(int M, int N, int K, int act, int out_fp32, int residual,
   if (dR) cudaFree(dR);
 }
 
+// A/B of the two standard-epilogue schedules on one bf16-output shape: 128 x 128 tiles with the epilogue on its own
+// warpgroup, and 128 x 256 tiles with the epilogue in registers.  Seeded random operands; the two outputs must be
+// byte-identical.  The schedules are timed alternately (rounds x iters launches each, after a warm-up) so that clock
+// and co-tenant drift hits both alike.  Returns 1 if the outputs differ.
+static int bench_gemm_ab(const char* name, int M, int N, int K, int act, int rounds = 5, int iters = 10) {
+  std::vector<uint16_t> hA((size_t)M * K), hW((size_t)N * K);
+  for (auto& x : hA) x = f2bf(frand());
+  for (auto& x : hW) x = f2bf(frand() * 0.25f);
+  std::vector<float> hb(N);
+  for (auto& x : hb) x = frand();
+  void *dA, *dW, *dO[2];
+  float* db;
+  const size_t osz = (size_t)M * N * 2;
+  CK(cudaMalloc(&dA, hA.size() * 2));
+  CK(cudaMalloc(&dW, hW.size() * 2));
+  CK(cudaMalloc(&db, N * 4));
+  CK(cudaMalloc(&dO[0], osz));
+  CK(cudaMalloc(&dO[1], osz));
+  CK(cudaMemcpy(dA, hA.data(), hA.size() * 2, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(dW, hW.data(), hW.size() * 2, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(db, hb.data(), N * 4, cudaMemcpyHostToDevice));
+  CK(cudaMemset(dO[0], 0xff, osz));
+  CK(cudaMemset(dO[1], 0x7f, osz));
+  GemmArgs a;
+  a.A = dA; a.W = dW; a.bias = db; a.M = M; a.N = N; a.K = K;
+  a.lda = K; a.ldw = K; a.ldo = N; a.act = act;
+  for (int w = 0; w < 2; ++w) {
+    a.out = dO[w];
+    for (int i = 0; i < 3; ++i)
+      if (gemm_bf16_v2_std(a, w == 1, 0)) { printf("[%s] launch failed: %s\n", name, last_error()); exit(3); }
+  }
+  CK(cudaDeviceSynchronize());
+  cudaEvent_t e0, e1;
+  cudaEventCreate(&e0); cudaEventCreate(&e1);
+  float ms[2] = {0.f, 0.f};
+  for (int r = 0; r < rounds; ++r) {
+    for (int w = 0; w < 2; ++w) {
+      a.out = dO[w];
+      cudaEventRecord(e0);
+      for (int i = 0; i < iters; ++i) gemm_bf16_v2_std(a, w == 1, 0);
+      cudaEventRecord(e1);
+      CK(cudaEventSynchronize(e1));
+      float t;
+      cudaEventElapsedTime(&t, e0, e1);
+      ms[w] += t;
+    }
+  }
+  std::vector<uint8_t> h0(osz), h1(osz);
+  CK(cudaMemcpy(h0.data(), dO[0], osz, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(h1.data(), dO[1], osz, cudaMemcpyDeviceToHost));
+  size_t ndiff = 0;
+  for (size_t i = 0; i < osz; i += 2) ndiff += memcmp(&h0[i], &h1[i], 2) != 0;
+  const double flop = 2.0 * M * N * K;
+  const double t128 = ms[0] / (rounds * iters), t256 = ms[1] / (rounds * iters);
+  printf("ab gemm %-10s M=%d N=%d K=%d act=%d: 128x128 %.3f ms %.1f TFLOP/s | 128x256 %.3f ms %.1f TFLOP/s | "
+         "speed-up %.3f | outputs %s (%zu of %zu differ)\n",
+         name, M, N, K, act, t128, flop / t128 * 1e-9, t256, flop / t256 * 1e-9, t128 / t256,
+         ndiff ? "DIFFER" : "identical", ndiff, osz / 2);
+  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  cudaFree(dA); cudaFree(dW); cudaFree(db); cudaFree(dO[0]); cudaFree(dO[1]);
+  return ndiff ? 1 : 0;
+}
+
 int selftest_attention(int bench);
 
 
@@ -202,6 +265,7 @@ int main(int argc, char** argv) {
         {"rowmap-resid",       4000, 2304,  768,  1, 0, 1, 1, 1, 1, 0},
         {"posembed-mod",       2048,  768,  768,  1, 0, 1, 1, 1, 0, 512},
         {"multi-tile-per-cta", 40000, 256,  128,  1, 0, 0, 1, 0, 0, 0},
+        {"wide-bias-gelu",    65000, 1280, 1024,  1, 1, 0, 1, 0, 0, 0},   // 128 x 256 schedule
     };
     for (const Case& c : cases) fails += run_case(c);
     if (bench) {
@@ -213,6 +277,20 @@ int main(int argc, char** argv) {
       bench_gemm(32768, 1280, 5120, 0, 1, 1);   // lin2: bias + fp32 residual -> fp32
       bench_gemm(32768, 768, 3072, 0, 1, 1);
       bench_gemm(8192, 8192, 8192, 0, 0, 0);
+      // the bf16-output encoder linears on both schedules (ViT-H: 1280 wide, ViT-B: 768; qkv over 25 windows of
+      // 14 x 14 or over 64 x 64 global tokens per image, batch 8), then qkv / lin1 at fewer tokens around the number
+      // of 128 x 256 tiles and the depth K where gemm_bf16_v2 starts to take the wide schedule
+      fails += bench_gemm_ab("vith-qkv", 39200, 3840, 1280, 0);
+      fails += bench_gemm_ab("vith-qkv", 32768, 3840, 1280, 0);
+      fails += bench_gemm_ab("vith-lin1", 32768, 5120, 1280, 1);
+      fails += bench_gemm_ab("vitb-qkv", 39200, 2304, 768, 0);
+      fails += bench_gemm_ab("vitb-qkv", 32768, 2304, 768, 0);
+      fails += bench_gemm_ab("vitb-lin1", 32768, 3072, 768, 1);
+      for (int m : {1024, 2048, 4096, 8192}) {
+        fails += bench_gemm_ab("vith-qkv", m, 3840, 1280, 0);
+        fails += bench_gemm_ab("vith-lin1", m, 5120, 1280, 1);
+      }
+      for (int k : {256, 512}) fails += bench_gemm_ab("k-sweep", 32768, 1280, k, 0);
     }
   }
   if (!strcmp(what, "gemmprof")) {
