@@ -402,6 +402,22 @@ int rsp_query_postprocess_rescale_bits(const float* logits, const int32_t* sel, 
                                        int Wr, uint8_t* bits, float* part_ws, float* scores, float* boxes,
                                        void* stream);
 
+/* SAM automatic mask generation, per candidate mask, without the original-size fp32 mask ever existing.  Replaces, for
+ * one crop layer, HF SamImageProcessor.post_process_masks(binarize=False) (image_processing_sam.py:423-425) followed by
+ * filter_masks (:350-363): iou_scores > pred_iou_thresh, _compute_stability_score (:449-457), masks > mask_threshold and
+ * _batched_mask_to_box (:460-506).  maps fp32 [n, hm, wm] low-res logits, geometry as rsp_mask_paste_rescale_bits
+ * (bilinear to (Hb, Wb), crop, bilinear to (H, W)); every pixel is that kernel's sample, so the > thr decisions are its
+ * bits exactly.  Outputs per mask: counts int32 [n, 3] = pixels > thr_hi, > thr_lo, > thr (thr_hi / thr_lo = mask_threshold
+ * +/- stability_score_offset, rounded to fp32 as torch compares with a python scalar); boxes int32 [n, 4] inclusive
+ * pixel xyxy of > thr, [0, 0, 0, 0] when empty; stability fp32 [n] = fp32(count_hi) / fp32(count_lo) (NaN for 0 / 0).
+ * With iou fp32 [n] non-null, keep uint8 [n] = (pred_iou_thresh <= 0 or iou > pred_iou_thresh) and
+ * (stability_score_thresh <= 0 or stability > stability_score_thresh).  part_ws int32 [n, ceil(H / 16), 7].
+ * Integer reductions only: two calls give identical outputs.  n > 0, H * W < 2^31, n * ceil(H / 16) < 2^31. */
+int rsp_sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                       float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                       float stability_score_thresh, int32_t* part_ws, int32_t* counts, int32_t* boxes,
+                       float* stability, uint8_t* keep, void* stream);
+
 /* FCNMaskHead mask paste (SAMSegMaskRCNN; fcn_mask_head.py:_do_paste_mask + threshold :388-392): activated RoI masks
  * probs fp32 [n, hm, wm] are sampled with F.grid_sample(bilinear, align_corners=False, zero padding) semantics at the
  * image pixel centres mapped into boxes fp32 [n, 4] (x1, y1, x2, y2) -> out uint8 [n, H, W] = (value >= thr); packed != 0 (W % 16 == 0): the

@@ -119,6 +119,8 @@ _SIGNATURES = {
     "rsp_mask_rle_placed_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
     "rsp_gemm_upscale_masks": ([_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _i, _vp], _i),
     "rsp_sam_mask_embed": ([_vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp], _i),
+    "rsp_sam_mask_stats": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _vp, _vp, _vp, _vp, _vp,
+                            _vp], _i),
 }
 
 
@@ -893,6 +895,37 @@ def mask_paste(logits: torch.Tensor, thr: float, *, raw: bool, size: tuple | Non
                "rsp_mask_paste_rescale_bits")
     launch_count += 1
     return out.view(torch.bool) if bits is None else bits
+
+
+def sam_mask_stats(logits: torch.Tensor, rescale: tuple, mask_threshold: float = 0.0,
+                   stability_score_offset: float = 1.0, iou: torch.Tensor | None = None, pred_iou_thresh: float = 0.0,
+                   stability_score_thresh: float = 0.0):
+    """Per-candidate statistics of SAM mask generation (rsp_sam_mask_stats): logits fp32 [n, hm, wm], rescale =
+    (pad_hw, reshaped_hw, original_hw) as mask_paste's.  -> counts int32 [n, 3] (> thr + offset, > thr - offset,
+    > thr), boxes int32 [n, 4] (HF's inclusive xyxy of > thr), stability fp32 [n], keep bool [n] (None without iou)."""
+    global launch_count
+    _require_cuda(logits, iou)
+    assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.dim() == 3
+    n, hm, wm = logits.shape
+    (Hb, Wb), (ch, cw), (H, W) = rescale
+    dev = logits.device
+    counts = torch.empty(n, 3, device=dev, dtype=torch.int32)
+    boxes = torch.empty(n, 4, device=dev, dtype=torch.int32)
+    stability = torch.empty(n, device=dev, dtype=torch.float32)
+    keep = None
+    if iou is not None:
+        assert iou.dtype == torch.float32 and iou.is_contiguous() and iou.numel() == n
+        keep = torch.empty(n, device=dev, dtype=torch.uint8)
+    if n == 0:
+        return counts, boxes, stability, None if keep is None else keep.view(torch.bool)
+    part = torch.empty(n, (H + 15) // 16, 7, device=dev, dtype=torch.int32)
+    thr = float(mask_threshold)
+    _check(_lib.rsp_sam_mask_stats(_ptr(logits), n, hm, wm, Hb, Wb, ch, cw, H, W, thr,
+                                   thr + float(stability_score_offset), thr - float(stability_score_offset), _ptr(iou),
+                                   float(pred_iou_thresh), float(stability_score_thresh), _ptr(part), _ptr(counts),
+                                   _ptr(boxes), _ptr(stability), _ptr(keep), _stream()), "rsp_sam_mask_stats")
+    launch_count += 2
+    return counts, boxes, stability, None if keep is None else keep.view(torch.bool)
 
 
 def sigmoid_f32(x: torch.Tensor) -> torch.Tensor:

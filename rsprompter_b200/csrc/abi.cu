@@ -384,6 +384,14 @@ int rsp_query_postprocess_rescale_bits(const float* logits, const int32_t* sel, 
                                         bits, part_ws, scores, boxes, S(stream));
 }
 
+int rsp_sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                       float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                       float stability_score_thresh, int32_t* part_ws, int32_t* counts, int32_t* boxes,
+                       float* stability, uint8_t* keep, void* stream) {
+  return sam_mask_stats(maps, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, thr, thr_hi, thr_lo, iou, pred_iou_thresh,
+                        stability_score_thresh, part_ws, counts, boxes, stability, keep, S(stream));
+}
+
 }  // extern "C"
 
 #include "records.h"

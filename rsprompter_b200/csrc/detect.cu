@@ -958,6 +958,124 @@ int mask_paste_boxes(const float* probs, const float* boxes, unsigned char* out,
                 : paste_px<2, false>(s, out, n, H, W, H, W, thr, stream);
 }
 
+// ---------------------------------------------------------------------------------------
+// SAM automatic mask generation, per candidate mask (HF SamImageProcessor.post_process_masks(binarize=False) followed
+// by filter_masks' _compute_stability_score, > mask_threshold and _batched_mask_to_box): every pixel of the original-size
+// mask comes from the TwoResizes sampler of mask_paste_rescale_bits, so its > thr decision is that kernel's bit, and
+// only integers leave a block.  Block m * bands + band covers rows [band * SMS_ROWS, +SMS_ROWS) of mask m (the bands of
+// a mask are consecutive blocks, so its low-res map is read while it is in L2); thread = 16 consecutive pixels of a
+// row, as in mask_paste_px_kernel.  part: int32 [n, bands, 7] = (count > thr_hi,
+// count > thr_lo, count > thr, x_min, y_min, x_max, y_max of > thr).
+constexpr int SMS_ROWS = 16;
+constexpr int SMS_THREADS = 256;
+constexpr int SMS_FIELDS = 7;
+
+__global__ void __launch_bounds__(SMS_THREADS, 4)   // 64 registers: 4 blocks per SM
+sam_mask_stats_kernel(TwoResizes s, int H, int W, float thr, float thr_hi, float thr_lo, int bands,
+                      int* __restrict__ part) {
+  const int band = static_cast<int>(blockIdx.x % bands), m = static_cast<int>(blockIdx.x / bands);
+  const int y0 = band * SMS_ROWS;
+  const int rows = min(SMS_ROWS, H - y0);
+  const int w16 = (W + 15) / 16;
+  int n_hi = 0, n_lo = 0, n_mid = 0;
+  int x_min = INT_MAX, y_min = INT_MAX, x_max = -1, y_max = -1;
+  for (int it = threadIdx.x; it < rows * w16; it += SMS_THREADS) {
+    const int y = y0 + it / w16, x0 = 16 * (it % w16);
+    s.row(m, y);
+    uint32_t bits = 0u;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+      const int x = x0 + k;
+      if (x >= W) break;
+      const float v = s.at(x);
+      n_hi += v > thr_hi;
+      n_lo += v > thr_lo;
+      if (v > thr) bits |= 1u << k;
+    }
+    if (bits) {
+      n_mid += __popc(bits);
+      x_min = min(x_min, x0 + __ffs(bits) - 1);
+      x_max = max(x_max, x0 + 31 - __clz(bits));
+      y_min = min(y_min, y);
+      y_max = max(y_max, y);
+    }
+  }
+  const unsigned all = 0xffffffffu;
+  int v[SMS_FIELDS] = {__reduce_add_sync(all, n_hi), __reduce_add_sync(all, n_lo), __reduce_add_sync(all, n_mid),
+                       __reduce_min_sync(all, x_min), __reduce_min_sync(all, y_min), __reduce_max_sync(all, x_max),
+                       __reduce_max_sync(all, y_max)};
+  __shared__ int red[SMS_THREADS / 32][SMS_FIELDS];
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  if (lane == 0) {
+#pragma unroll
+    for (int f = 0; f < SMS_FIELDS; ++f) red[warp][f] = v[f];
+  }
+  __syncthreads();
+  if (threadIdx.x < SMS_FIELDS) {
+    const int f = threadIdx.x;
+    int r = red[0][f];
+    for (int w = 1; w < SMS_THREADS / 32; ++w) {
+      const int o = red[w][f];
+      r = f < 3 ? r + o : f < 5 ? min(r, o) : max(r, o);
+    }
+    part[(static_cast<size_t>(m) * bands + band) * SMS_FIELDS + f] = r;
+  }
+}
+
+// one warp per mask: the band partials -> counts, the HF box ([0, 0, 0, 0] when nothing is > thr), the stability score
+// (count > thr_hi) / (count > thr_lo) as torch's int32 / int32 true division (NaN for 0 / 0) and, with iou, the keep
+// flag of filter_masks (a threshold > 0 enables its test; NaN fails every test).
+__global__ void sam_mask_stats_finish_kernel(const int* __restrict__ part, int n, int bands,
+                                             const float* __restrict__ iou, float pred_iou_thresh,
+                                             float stability_thresh, int* __restrict__ counts, int* __restrict__ boxes,
+                                             float* __restrict__ stability, unsigned char* __restrict__ keep) {
+  const int m = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
+  if (m >= n) return;
+  int v[SMS_FIELDS] = {0, 0, 0, INT_MAX, INT_MAX, -1, -1};
+  for (int b = lane; b < bands; b += 32) {
+    const int* p = part + (static_cast<size_t>(m) * bands + b) * SMS_FIELDS;
+#pragma unroll
+    for (int f = 0; f < SMS_FIELDS; ++f) v[f] = f < 3 ? v[f] + p[f] : f < 5 ? min(v[f], p[f]) : max(v[f], p[f]);
+  }
+  const unsigned all = 0xffffffffu;
+#pragma unroll
+  for (int f = 0; f < SMS_FIELDS; ++f)
+    v[f] = f < 3 ? __reduce_add_sync(all, v[f]) : f < 5 ? __reduce_min_sync(all, v[f]) : __reduce_max_sync(all, v[f]);
+  if (lane != 0) return;
+#pragma unroll
+  for (int f = 0; f < 3; ++f) counts[m * 3 + f] = v[f];
+  const bool empty = v[2] == 0;
+#pragma unroll
+  for (int f = 0; f < 4; ++f) boxes[m * 4 + f] = empty ? 0 : v[3 + f];
+  const float st = __fdiv_rn(__int2float_rn(v[0]), __int2float_rn(v[1]));
+  stability[m] = st;
+  if (iou != nullptr) {
+    bool k = true;
+    if (pred_iou_thresh > 0.f) k = k && iou[m] > pred_iou_thresh;
+    if (stability_thresh > 0.f) k = k && st > stability_thresh;
+    keep[m] = k ? 1 : 0;
+  }
+}
+
+int sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                   float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                   float stability_thresh, int* part_ws, int* counts, int* boxes, float* stability,
+                   unsigned char* keep, cudaStream_t stream) {
+  const int bands = (H + SMS_ROWS - 1) / SMS_ROWS;
+  RSP_CHECK_ARG(maps && part_ws && counts && boxes && stability && (!iou || keep) && n > 0 && hm > 0 && wm > 0 &&
+                Hb > 0 && Wb > 0 && crop_h > 0 && crop_w > 0 && crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 &&
+                static_cast<long long>(H) * W <= INT_MAX && static_cast<long long>(n) * bands <= INT_MAX,
+                "sam_mask_stats: bad args (n > 0, crop within (Hb, Wb), H * W < 2^31, n * ceil(H / 16) < 2^31)");
+  const TwoResizes s{maps, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
+  sam_mask_stats_kernel<<<static_cast<unsigned>(n) * bands, SMS_THREADS, 0, stream>>>(s, H, W, thr, thr_hi, thr_lo,
+                                                                                     bands, part_ws);
+  RSP_CHECK_LAUNCH();
+  sam_mask_stats_finish_kernel<<<(n + 7) / 8, 256, 0, stream>>>(part_ws, n, bands, iou, pred_iou_thresh,
+                                                                 stability_thresh, counts, boxes, stability, keep);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
 __global__ void sigmoid_f32_kernel(const float4* __restrict__ in, float4* __restrict__ out, long long n4) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n4) return;

@@ -35,6 +35,10 @@ int mask_paste_bits(const float* maps, unsigned char* bits, int n, int hm, int w
                     cudaStream_t stream);
 int mask_paste_boxes(const float* probs, const float* boxes, unsigned char* out, int n, int hm, int wm, int H, int W,
                      float thr, int packed, cudaStream_t stream);
+int sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                   float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                   float stability_thresh, int* part_ws, int* counts, int* boxes, float* stability,
+                   unsigned char* keep, cudaStream_t stream);
 int sigmoid_f32(const float* in, float* out, long long n, cudaStream_t stream);
 int pool2_nhwc(const void* in, void* out, int B, int H, int W, int C, int mode, cudaStream_t stream);
 int zero_border_nhwc(void* x, int N, int H, int W, int C, cudaStream_t stream);

@@ -1,0 +1,334 @@
+"""Segment everything with SAM on the GPU: HF transformers' ``pipeline("mask-generation")`` for one crop layer.
+
+HF's MaskGenerationPipeline (pipelines/mask_generation.py:187-335) prompts the model with a regular point grid, turns
+every candidate mask into an fp32 mask at the original image size (SamImageProcessor.post_process_masks(binarize=False),
+image_processing_sam.py:379-430), filters it by predicted IoU and stability score, boxes it (filter_masks :301-377) and
+de-duplicates with a box NMS (post_process_for_mask_generation :432-446).  Here:
+
+  * every image of the call is encoded in one batch, and the grids of all images run through the mask decoder in
+    calls of ``points_per_batch`` prompts (prompts of several images share a call through the decoder's block maps);
+  * ``rsp_sam_mask_stats`` reduces each call's low-res logits to three pixel counts, a box and the keep flag,
+    sampling every original-size pixel with the two-resizes-and-crop sampler of ``rsp_mask_paste_rescale_bits``:
+    the original-size fp32 mask never exists;
+  * one ``rsp_nms_batched`` + ``rsp_compact_keep`` per call de-duplicates every image's survivors, ties broken by
+    candidate order (point-major, mask-minor, HF's ``flatten(0, 1)``);
+  * only the kept masks are pasted, as bits, by ``rsp_mask_paste_rescale_bits``; ``output_rle_mask=True`` encodes
+    them as COCO RLE on the GPU.
+
+The low-res logits of every candidate of every image of the call stay on the device until the NMS has run: 256 KB
+per candidate, 3 per point, 805 MB per image at the default 32 x 32 grid, so a call on B images holds B times that at
+once (pass fewer images per call to bound it).  Host synchronisations per call: the read of the kept counts and
+candidates, and two more with ``output_rle_mask``, whatever the grid size and the number of masks.
+
+``crops_n_layers > 0`` is not built: HF's own crop path cannot run (``_generate_crop_boxes`` stacks crops of different
+sizes), so there are no reference semantics for it.  Hole and sprinkle removal are not built either.
+
+``python -m rsprompter_b200.mask_generation IMAGE --arch base --checkpoint sam.safetensors --out masks.json`` writes
+one dict per mask (COCO RLE ``segmentation``, xywh ``bbox``, ``predicted_iou``, ``stability_score``,
+``point_coords``)."""
+from __future__ import annotations
+
+import argparse
+import json
+
+import torch
+
+from . import _lib
+
+# SamImageProcessor defaults (image_processing_sam.py:61-75): ImageNet mean / std on [0, 1] pixels
+IMAGE_MEAN = (0.485, 0.456, 0.406)
+IMAGE_STD = (0.229, 0.224, 0.225)
+
+CROP_ERROR = ("crops_n_layers > 0 is not supported: HF's own crop path cannot run (_generate_crop_boxes torch.stack()s "
+              "crops of different sizes and fails with 'stack expects each tensor to be equal size'), so there are no "
+              "reference semantics to follow")
+
+
+def preprocess_shape(hw: tuple, longest_edge: int) -> tuple:
+    """SamImageProcessor._get_preprocess_shape (image_processing_sam.py:113-122): the resized, unpadded (h, w)."""
+    oldh, oldw = int(hw[0]), int(hw[1])
+    scale = longest_edge * 1.0 / max(oldh, oldw)
+    return int(oldh * scale + 0.5), int(oldw * scale + 0.5)
+
+
+def point_grid(points_per_side: int, hw: tuple, target_size: int) -> tuple:
+    """The prompts of one image: _build_point_grid (image_processing_sam.py:624-631) scaled by (W, H) as
+    _generate_crop_images does for the whole-image crop (:649-653), then _normalize_coordinates (:659-684) into the
+    model frame.  -> (points in original pixels, points in the model frame), fp32 [n * n, 2] on the host."""
+    offset = 1 / (2 * points_per_side)
+    side = torch.linspace(offset, 1 - offset, points_per_side)
+    grid = torch.stack([torch.tile(side[None, :], (points_per_side, 1)), torch.tile(side[:, None], (1, points_per_side))],
+                       dim=-1).reshape(-1, 2)
+    H, W = int(hw[0]), int(hw[1])
+    pts = grid * torch.tensor([H, W]).flip(dims=(0,)).unsqueeze(0)
+    new_h, new_w = preprocess_shape((H, W), target_size)
+    model = pts.clone().float()
+    model[..., 0] = model[..., 0] * (new_w / W)
+    model[..., 1] = model[..., 1] * (new_h / H)
+    return pts, model
+
+
+def _check_params(points_per_side, points_per_batch, crops_n_layers, max_hole_area, max_sprinkle_area) -> None:
+    if crops_n_layers:
+        raise ValueError(CROP_ERROR)
+    if max_hole_area is not None or max_sprinkle_area is not None:
+        raise ValueError("max_hole_area / max_sprinkle_area are not supported: SamImageProcessor.post_process_masks "
+                         "takes no hole or sprinkle arguments")
+    if points_per_batch is None or points_per_batch <= 0:
+        raise ValueError("Cannot have points_per_batch<=0. Must be >=1 to returned batched outputs.")
+    if points_per_side is None or points_per_side < 1:
+        raise ValueError(f"points_per_side must be >= 1, got {points_per_side}")
+
+
+def _sam(model):
+    from .sam_model import RSSamModel, SamModelB200
+    if isinstance(model, RSSamModel):
+        return model.sam_model
+    if isinstance(model, SamModelB200):
+        return model
+    raise TypeError(f"generate_masks takes an RSSamModel or SamModelB200, not {type(model).__name__}")
+
+
+def _sizes(v, B: int, name: str) -> list:
+    if v is None:
+        raise ValueError(f"pixel_values needs {name}: one (h, w) per image, as SamProcessor returns them")
+    v = v.tolist() if isinstance(v, torch.Tensor) else list(v)
+    if len(v) != B:
+        raise ValueError(f"{name} has {len(v)} entries for {B} images")
+    return [(int(h), int(w)) for h, w in v]
+
+
+def _inputs(sam, images, pixel_values, original_sizes, reshaped_input_sizes, dev):
+    """-> (pixel_values fp32 [B, 3, S, S] on dev, original (h, w) per image, reshaped (h, w) per image)."""
+    S = sam.varch.image_size
+    if (images is None) == (pixel_values is None):
+        raise ValueError("pass exactly one of images and pixel_values")
+    if pixel_values is not None:
+        if pixel_values.dim() != 4 or tuple(pixel_values.shape[1:]) != (3, S, S):
+            raise ValueError(f"pixel_values must be [B, 3, {S}, {S}], got {tuple(pixel_values.shape)}")
+        B = pixel_values.shape[0]
+        sizes = _sizes(original_sizes, B, "original_sizes")
+        reshaped = _sizes(reshaped_input_sizes, B, "reshaped_input_sizes")
+        for rs in reshaped:
+            if not (0 < rs[0] <= S and 0 < rs[1] <= S):
+                raise ValueError(f"reshaped input size {rs} is outside the {S} x {S} input")
+        return pixel_values.to(dev, torch.float32).contiguous(), sizes, reshaped
+    imgs = [images] if isinstance(images, torch.Tensor) and images.dim() == 3 else list(images)
+    if not imgs:
+        raise ValueError("no images")
+    for t in imgs:
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[0] != 3:
+            raise ValueError("images must be uint8 RGB tensors [3, H, W]")
+    sizes = [(int(t.shape[1]), int(t.shape[2])) for t in imgs]
+    reshaped = [preprocess_shape(hw, S) for hw in sizes]
+    views = [t if t.device == dev else t.contiguous().pin_memory().to(dev, non_blocking=True) for t in imgs]
+    mean = tuple(255.0 * m for m in IMAGE_MEAN)
+    std = tuple(255.0 * s for s in IMAGE_STD)
+    pix = torch.empty(len(imgs), 3, S, S, device=dev, dtype=torch.float32)
+    _lib.resize_pad_u8(views, reshaped, pix, mean, std, False, mean)      # padded with the mean: 0 once normalised
+    return pix, sizes, reshaped
+
+
+def _candidates(sam, emb_nhwc, sizes, reshaped, p) -> dict:
+    """The grids of every image through the decoder in calls of points_per_batch prompts, each call's logits through
+    rsp_sam_mask_stats.  -> per-candidate device tensors, candidate c of image b at [b, c] (point c // 3, mask c % 3)."""
+    B, g, C = emb_nhwc.shape[0], emb_nhwc.shape[1], emb_nhwc.shape[3]
+    S = sam.varch.image_size
+    dev = emb_nhwc.device
+    n_pts = p["points_per_side"] ** 2
+    grids = [point_grid(p["points_per_side"], hw, S) for hw in sizes]
+    pts_orig = torch.stack([a for a, _ in grids]).pin_memory().to(dev, non_blocking=True)       # [B, n_pts, 2]
+    pts_model = torch.stack([b for _, b in grids]).view(1, B * n_pts, 1, 2).pin_memory().to(dev, non_blocking=True)
+    labels = torch.ones(1, B * n_pts, 1, dtype=torch.int32, device=dev)
+    sparse = sam.embed_points(pts_model, labels, pad=True).reshape(B * n_pts, 2, C).contiguous()
+    prompt_img = torch.arange(B, device=dev, dtype=torch.int32).repeat_interleave(n_pts)
+    pos_rows = sam.shared_image_embedding.image_wide_rows(g)
+    dense = sam.prompt_encoder.no_mask_embed.weight[0].to(torch.float32).contiguous()
+    emb_rows = emb_nhwc.reshape(B, g * g, C)
+    hm = wm = 4 * g
+    n_out = sam.mask_decoder.num_mask_tokens - 1
+    Nc = n_pts * n_out
+    logits = torch.empty(B * Nc, hm, wm, device=dev, dtype=torch.float32)
+    iou = torch.empty(B * Nc, device=dev, dtype=torch.float32)
+    stab = torch.empty(B * Nc, device=dev, dtype=torch.float32)
+    boxes = torch.empty(B * Nc, 4, device=dev, dtype=torch.int32)
+    keep = torch.empty(B * Nc, device=dev, dtype=torch.bool)
+    ppb = p["points_per_batch"]
+    for q0 in range(0, B * n_pts, ppb):
+        q1 = min(q0 + ppb, B * n_pts)
+        b0, b1 = q0 // n_pts, (q1 - 1) // n_pts + 1             # the images this call's prompts belong to
+        m, s = sam.mask_decoder.decode(emb_rows[b0:b1].reshape(-1, C), pos_rows, sparse[q0:q1], (g, g),
+                                       prompt_img=(prompt_img[q0:q1] - b0).contiguous(), dense_vec=dense,
+                                       multimask_output=True)
+        logits[q0 * n_out:q1 * n_out].copy_(m.view(-1, hm, wm))
+        iou[q0 * n_out:q1 * n_out].copy_(s.reshape(-1))
+        for b in range(b0, b1):
+            r0, r1 = max(q0, b * n_pts) * n_out, min(q1, (b + 1) * n_pts) * n_out
+            _, bx, st, kp = _lib.sam_mask_stats(
+                logits[r0:r1], ((S, S), reshaped[b], sizes[b]), p["mask_threshold"], p["stability_score_offset"],
+                iou[r0:r1], p["pred_iou_thresh"], p["stability_score_thresh"])
+            boxes[r0:r1].copy_(bx)
+            stab[r0:r1].copy_(st)
+            keep[r0:r1].copy_(kp)
+    return dict(logits=logits, iou=iou.view(B, Nc), stability=stab.view(B, Nc), boxes=boxes.view(B, Nc, 4),
+                keep=keep.view(B, Nc), points=pts_orig, n_out=n_out, sizes=sizes, reshaped=reshaped)
+
+
+def _nms(cand: dict, iou_thr: float) -> tuple:
+    """batched_nms(boxes.float(), scores, zeros, iou_thr) over every image's survivors (post_process_for_mask_generation,
+    image_processing_sam.py:715-720), in keep order.  -> (kept candidate index int64 [B, Nc] on the device, kept count
+    per image on the host, the same indices on the host); the one host synchronisation."""
+    iou, keep = cand["iou"], cand["keep"]
+    B, Nc = iou.shape
+    key = torch.where(keep, iou, torch.full_like(iou, -float("inf")))
+    _, order = torch.sort(key, dim=1, descending=True, stable=True)     # survivors first; ties by candidate order
+    nvalid = keep.sum(1).to(torch.int32)
+    boxes_s = torch.gather(cand["boxes"].float(), 1, order[..., None].expand(-1, -1, 4)).contiguous()
+    scores_s = torch.gather(iou, 1, order).contiguous()
+    ids = torch.zeros(B, Nc, device=iou.device, dtype=torch.int64)
+    kept = _lib.nms_batched(boxes_s, ids, nvalid, iou_thr)
+    _, _, _, oi, cnt = _lib.compact_keep(kept, boxes_s, scores_s, None, Nc)
+    idx = torch.gather(order, 1, oi.clamp(min=0).long())
+    host = torch.cat([cnt.long(), idx.view(-1)]).cpu()
+    return idx, host[:B].tolist(), host[B:].view(B, Nc)
+
+
+def _outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch.Tensor, mask_threshold: float,
+             output_rle_mask: bool, target_size: int) -> list:
+    """Per image: the kept masks pasted as bits, and the kept rows of every per-candidate output."""
+    B, Nc = cand["iou"].shape
+    out, rle_groups = [], []
+    for b in range(B):
+        k = counts[b]
+        H, W = cand["sizes"][b]
+        ci = idx[b, :k]
+        ld = (W + 15) // 16 * 2
+        bits = torch.empty(k, H, ld, device=idx.device, dtype=torch.uint8)
+        if k:
+            lg = cand["logits"].index_select(0, ci + b * Nc)
+            _lib.mask_paste(lg, mask_threshold, raw=True, rescale=((target_size, target_size), cand["reshaped"][b], (H, W)),
+                            bits=bits)
+            rle_groups.append((bits, [(j * H * ld, ld, H, H, W, H, W, 0, 0) for j in range(k)]))
+        out.append(dict(masks=bits, scores=cand["iou"][b].index_select(0, ci),
+                        stability_scores=cand["stability"][b].index_select(0, ci),
+                        boxes=cand["boxes"][b].index_select(0, ci).long(),
+                        points=cand["points"][b].index_select(0, ci // cand["n_out"]),
+                        candidates=idx_host[b, :k].clone(), size=(H, W)))
+    if output_rle_mask:
+        strings = iter(_lib.mask_rle_placed(rle_groups, packed=True))
+        for r in out:
+            r["rle"] = [dict(size=list(r["size"]), counts=next(strings)) for _ in range(r["masks"].shape[0])]
+    return out
+
+
+@torch.no_grad()
+def generate_masks(model, images=None, *, pixel_values=None, original_sizes=None, reshaped_input_sizes=None,
+                   points_per_side: int = 32, points_per_batch: int = 64, pred_iou_thresh: float = 0.88,
+                   stability_score_thresh: float = 0.95, stability_score_offset: float = 1.0,
+                   mask_threshold: float = 0.0, crops_nms_thresh: float = 0.7, crops_n_layers: int = 0,
+                   max_hole_area=None, max_sprinkle_area=None, output_rle_mask: bool = False) -> list:
+    """Every mask of each image, as HF's mask-generation pipeline finds them with crops_n_layers=0.
+
+    ``model``: an RSSamModel or SamModelB200.  Images go in one of two forms:
+
+      * ``images``: uint8 RGB [3, H, W] tensors (one, or a list of any sizes, on the host or the device), resized by
+        ``rsp_resize_pad_u8`` to SamImageProcessor's size (longest edge = the model's image size), normalised with its
+        ImageNet mean and std (x 255) and padded with 0 to the square input.  The resize is cv2 ``INTER_LINEAR``
+        arithmetic (this project's and mmdet's), not the antialiased bilinear resize of torchvision that
+        SamImageProcessor runs, so the pixel values are close to HF's but not the same bytes;
+      * ``pixel_values`` fp32 [B, 3, S, S] with ``original_sizes`` and ``reshaped_input_sizes`` (one (h, w) per
+        image): exactly what SamProcessor returns, for results comparable to HF's.
+
+    Parameters carry HF's names and defaults (``points_per_side`` is HF's ``points_per_crop``); a threshold of 0
+    disables its test, as in filter_masks.  ``crops_n_layers > 0``, ``max_hole_area`` and ``max_sprinkle_area`` raise
+    ValueError.
+
+    Returns one dict per image, rows in NMS keep order (descending predicted IoU):
+      masks             uint8 [k, H, ceil(W / 16) * 2] bit-packed rows, pixel x = bit x % 8 of byte x // 8
+                        (``masks_to_bool`` unpacks them)
+      scores            fp32 [k] predicted IoU
+      stability_scores  fp32 [k]
+      boxes             int64 [k, 4] inclusive pixel xyxy (HF's _batched_mask_to_box)
+      points            fp32 [k, 2] the prompt of each mask, in original pixels
+      candidates        int64 [k] (host) candidate index: point * 3 + output mask
+      size              (H, W)
+      rle               with output_rle_mask: COCO compressed RLE dicts {'size': [H, W], 'counts': bytes}
+    All tensors but ``candidates`` are on the model's device.
+
+    Memory: the low-res logits of every candidate of every image stay resident until the NMS, 3 x points_per_side^2 x
+    256 KB per image (805 MB at the default grid), so B images in one call need B times that at once."""
+    _check_params(points_per_side, points_per_batch, crops_n_layers, max_hole_area, max_sprinkle_area)
+    sam = _sam(model)
+    dev = sam.prompt_encoder.no_mask_embed.weight.device
+    pix, sizes, reshaped = _inputs(sam, images, pixel_values, original_sizes, reshaped_input_sizes, dev)
+    p = dict(points_per_side=int(points_per_side), points_per_batch=int(points_per_batch),
+             pred_iou_thresh=float(pred_iou_thresh), stability_score_thresh=float(stability_score_thresh),
+             stability_score_offset=float(stability_score_offset), mask_threshold=float(mask_threshold))
+    emb = sam._encode(pix)
+    cand = _candidates(sam, emb, sizes, reshaped, p)
+    idx, counts, idx_host = _nms(cand, float(crops_nms_thresh))
+    return _outputs(cand, idx, counts, idx_host, float(mask_threshold), output_rle_mask, sam.varch.image_size)
+
+
+def masks_to_bool(result: dict) -> torch.Tensor:
+    """The bit-packed ``masks`` of one generate_masks result -> bool [k, H, W] on the same device."""
+    bits = result["masks"]
+    H, W = result["size"]
+    if bits.shape[0] == 0:
+        return torch.zeros(0, H, W, dtype=torch.bool, device=bits.device)
+    return _lib.unpack_mask_bits(bits, bits.shape[2] * 8)[..., :W]
+
+
+def mask_dicts(result: dict) -> list:
+    """The result of one image as JSON-ready dicts: COCO RLE ``segmentation`` (needs output_rle_mask=True), xywh
+    ``bbox`` from the inclusive box, ``predicted_iou``, ``stability_score``, ``point_coords`` [[x, y]]."""
+    out = []
+    for rle, (x1, y1, x2, y2), s, st, pt in zip(result["rle"], result["boxes"].tolist(), result["scores"].tolist(),
+                                               result["stability_scores"].tolist(), result["points"].tolist()):
+        out.append(dict(segmentation=dict(size=rle["size"], counts=rle["counts"].decode()),
+                        bbox=[x1, y1, x2 - x1, y2 - y1], predicted_iou=s, stability_score=st, point_coords=[pt]))
+    return out
+
+
+def main(argv=None) -> list:
+    ap = argparse.ArgumentParser(description="Segment everything in one image with SAM (HF mask-generation, one crop "
+                                             "layer) and write the masks as COCO RLE")
+    ap.add_argument("image")
+    ap.add_argument("--arch", required=True, choices=["base", "large", "huge"])
+    ap.add_argument("--checkpoint", required=True, help="HF SamModel weights (.pth / .bin or .safetensors)")
+    ap.add_argument("--points-per-side", type=int, default=32)
+    ap.add_argument("--points-per-batch", type=int, default=64)
+    ap.add_argument("--pred-iou-thresh", type=float, default=0.88)
+    ap.add_argument("--stability-score-thresh", type=float, default=0.95)
+    ap.add_argument("--stability-score-offset", type=float, default=1.0)
+    ap.add_argument("--mask-threshold", type=float, default=0.0)
+    ap.add_argument("--crops-nms-thresh", type=float, default=0.7)
+    ap.add_argument("--out", default=None, help="JSON file for the mask dicts (default: stdout)")
+    args = ap.parse_args(argv)
+
+    import cv2
+
+    from .sam_model import RSSamModel
+    model = RSSamModel(f"facebook/sam-vit-{args.arch}", init_cfg=dict(type="Pretrained", checkpoint=args.checkpoint))
+    model = model.cuda().eval()
+    img = cv2.imread(args.image, cv2.IMREAD_COLOR)
+    if img is None:
+        raise FileNotFoundError(args.image)
+    rgb = torch.from_numpy(img).permute(2, 0, 1).flip(0)                 # BGR HWC -> RGB [3, H, W] view
+    res = generate_masks(model, rgb.contiguous(), points_per_side=args.points_per_side,
+                         points_per_batch=args.points_per_batch, pred_iou_thresh=args.pred_iou_thresh,
+                         stability_score_thresh=args.stability_score_thresh,
+                         stability_score_offset=args.stability_score_offset, mask_threshold=args.mask_threshold,
+                         crops_nms_thresh=args.crops_nms_thresh, output_rle_mask=True)[0]
+    rows = mask_dicts(res)
+    text = json.dumps(rows)
+    if args.out:
+        with open(args.out, "w") as f:
+            f.write(text)
+    else:
+        print(text)
+    return rows
+
+
+if __name__ == "__main__":
+    main()

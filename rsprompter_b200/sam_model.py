@@ -261,6 +261,11 @@ class RSSamModel(BaseModule):
     def get_prompt_embeddings(self, input_points=None, input_labels=None, input_boxes=None, input_masks=None):
         return self.sam_model.get_prompt_embeddings(input_points, input_labels, input_boxes, input_masks)
 
+    def generate_masks(self, images=None, **kwargs) -> list:
+        """Segment everything: HF's mask-generation pipeline with one crop layer (see mask_generation.generate_masks)."""
+        from .mask_generation import generate_masks
+        return generate_masks(self, images, **kwargs)
+
 
 @MODELS.register_module(force=True)
 class SAMDet(BaseModule):
