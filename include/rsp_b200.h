@@ -418,6 +418,23 @@ int rsp_sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb,
                        float stability_score_thresh, int32_t* part_ws, int32_t* counts, int32_t* boxes,
                        float* stability, uint8_t* keep, void* stream);
 
+/* SAM automatic mask generation's small-region removal (min_mask_region_area) on bit-packed masks.  Replaces, per
+ * kept mask, segment_anything/utils/amg.py remove_small_regions(mask, area_thresh, mode) as
+ * SamAutomaticMaskGenerator.postprocess_small_regions calls it (cv2.connectedComponentsWithStats(., 8) + np.isin), and
+ * batched_mask_to_box of its result.  in / out uint8 [n, H, ld] bit rows (pixel x = bit x % 8 of byte x / 8, ld even,
+ * 8 * ld >= W, ld <= 4 * ceil(W / 32); rsp_mask_paste_rescale_bits' ld = ceil(W / 16) * 2); bits at x >= W are
+ * ignored on input and written as 0; out must not overlap in.  The working mask is ~mask (mode 0, holes) or mask
+ * (mode 1, islands); its 8-connected components of area < min_area are "small":
+ *   holes    out = mask | (every small component)
+ *   islands  out = the components of area >= min_area; when there are none, only the largest (ties: the component
+ *            whose first 2 x 2 pixel block (y / 2, x / 2) comes first in raster order, cv2's label order)
+ *   changed  uint8 [n] = some component is small (even when out equals the mask, as in SAM)
+ *   boxes    int32 [n, 4] inclusive pixel xyxy of out, [0, 0, 0, 0] when empty.
+ * ws: n * (32 + 4 * ceil(H / 2) * ceil(W / 2)) bytes, 8-byte aligned.  Atomics touch intermediate labels only: two
+ * calls give identical outputs.  n > 0, H * W < 2^31. */
+int rsp_mask_small_regions_bits(const uint8_t* in, uint8_t* out, int n, int H, int W, int ld, long long min_area,
+                                int mode, void* ws, uint8_t* changed, int32_t* boxes, void* stream);
+
 /* FCNMaskHead mask paste (SAMSegMaskRCNN; fcn_mask_head.py:_do_paste_mask + threshold :388-392): activated RoI masks
  * probs fp32 [n, hm, wm] are sampled with F.grid_sample(bilinear, align_corners=False, zero padding) semantics at the
  * image pixel centres mapped into boxes fp32 [n, 4] (x1, y1, x2, y2) -> out uint8 [n, H, W] = (value >= thr); packed != 0 (W % 16 == 0): the

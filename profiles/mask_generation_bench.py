@@ -119,11 +119,23 @@ def _hf_post(proc, cand, p, nms_thr=0.7):
     return len(out[0])
 
 
-def _ours_post(cand, p):
+def _nms(cand):
     from rsprompter_b200 import mask_generation as mg
+    return mg._nms(cand["iou"], cand["keep"], cand["boxes"], 0.7)
+
+
+def _paste_rle(cand, idx, counts, idx_host):
+    """The kept masks pasted as bits, then their COCO RLE, as generate_masks(output_rle_mask=True) does."""
+    from rsprompter_b200 import mask_generation as mg
+    out = mg._outputs(cand, idx, counts, idx_host, 0.0, 1024)
+    mg._add_rle(out)
+    return out
+
+
+def _ours_post(cand, p):
     _stats_pass(cand, p)
-    idx, counts, idx_host = mg._nms(cand, 0.7)
-    mg._outputs(cand, idx, counts, idx_host, 0.0, True, 1024)
+    idx, counts, idx_host = _nms(cand)
+    _paste_rle(cand, idx, counts, idx_host)
     return counts[0]
 
 
@@ -141,8 +153,8 @@ def _case(model, arch_name, hw, tname, repeats, proc) -> dict:
         (pix, sizes, reshaped), _ = _sync_ms(lambda: mg._inputs(sm, img, None, None, None, img.device))
         emb, t_enc = _sync_ms(lambda: sm._encode(pix))
         cand, t_dec = _sync_ms(lambda: mg._candidates(sm, emb, sizes, reshaped, p))
-        (idx, counts, idx_host), t_nms = _sync_ms(lambda: mg._nms(cand, 0.7))
-        out, t_out = _sync_ms(lambda: mg._outputs(cand, idx, counts, idx_host, 0.0, True, 1024))
+        (idx, counts, idx_host), t_nms = _sync_ms(lambda: _nms(cand))
+        out, t_out = _sync_ms(lambda: _paste_rle(cand, idx, counts, idx_host))
         for k, v in zip(split, (t_enc, t_dec, t_nms, t_out)):
             split[k].append(v)
     n_cand = cand["logits"].shape[0]

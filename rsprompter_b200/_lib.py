@@ -121,6 +121,7 @@ _SIGNATURES = {
     "rsp_sam_mask_embed": ([_vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp], _i),
     "rsp_sam_mask_stats": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _vp, _vp, _vp, _vp, _vp,
                             _vp], _i),
+    "rsp_mask_small_regions_bits": ([_vp, _vp, _i, _i, _i, _i, ctypes.c_longlong, _i, _vp, _vp, _vp, _vp], _i),
 }
 
 
@@ -926,6 +927,46 @@ def sam_mask_stats(logits: torch.Tensor, rescale: tuple, mask_threshold: float =
                                    _ptr(boxes), _ptr(stability), _ptr(keep), _stream()), "rsp_sam_mask_stats")
     launch_count += 2
     return counts, boxes, stability, None if keep is None else keep.view(torch.bool)
+
+
+SMALL_REGION_MODES = {"holes": 0, "islands": 1}     # segment_anything remove_small_regions' modes
+
+
+def small_regions_ws_bytes(n: int, H: int, W: int) -> int:
+    """Device workspace of mask_small_regions_bits for n masks of H x W: 32 bytes per mask and an int32 label per
+    2 x 2 pixel block."""
+    return n * (32 + 4 * ((H + 1) // 2) * ((W + 1) // 2))
+
+
+def mask_small_regions_bits(bits: torch.Tensor, W: int, min_area: int, mode: str, out: torch.Tensor | None = None,
+                            ws: torch.Tensor | None = None):
+    """SAM's remove_small_regions (rsp_mask_small_regions_bits) on bit-packed masks uint8 [n, H, ld] of width W:
+    components of the working mask (~mask for mode "holes", mask for "islands") with area < min_area (an int) are
+    filled / removed.  -> out uint8 [n, H, ld] (bits at x >= W zero), changed bool [n], boxes int32 [n, 4] (inclusive
+    xyxy of out, zeros when empty).  ws: uint8 of at least small_regions_ws_bytes(n, H, W) bytes, or None."""
+    global launch_count
+    _require_cuda(bits, out, ws)
+    assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.dim() == 3
+    n, H, ld = bits.shape
+    dev = bits.device
+    if out is None:
+        out = torch.empty_like(bits)
+    assert out.dtype == torch.uint8 and out.is_contiguous() and out.shape == bits.shape
+    changed = torch.empty(n, device=dev, dtype=torch.uint8)
+    boxes = torch.empty(n, 4, device=dev, dtype=torch.int32)
+    if n == 0:
+        return out, changed.view(torch.bool), boxes
+    if not -2 ** 63 <= int(min_area) < 2 ** 63:
+        raise ValueError(f"min_area {min_area} does not fit the kernel's 64-bit threshold")
+    need = small_regions_ws_bytes(n, H, W)
+    if ws is None:
+        ws = torch.empty(need, device=dev, dtype=torch.uint8)
+    assert ws.dtype == torch.uint8 and ws.is_contiguous() and ws.numel() >= need
+    _check(_lib.rsp_mask_small_regions_bits(_ptr(bits), _ptr(out), n, H, int(W), ld, int(min_area),
+                                            SMALL_REGION_MODES[mode], _ptr(ws), _ptr(changed), _ptr(boxes),
+                                            _stream()), "rsp_mask_small_regions_bits")
+    launch_count += 7
+    return out, changed.view(torch.bool), boxes
 
 
 def sigmoid_f32(x: torch.Tensor) -> torch.Tensor:

@@ -456,3 +456,14 @@ int rsp_mask_rle_placed_write(const uint8_t* src, int packed, const int64_t* des
 }
 
 }  // extern "C"
+
+#include "regions.h"
+
+extern "C" {
+
+int rsp_mask_small_regions_bits(const uint8_t* in, uint8_t* out, int n, int H, int W, int ld, long long min_area,
+                                int mode, void* ws, uint8_t* changed, int32_t* boxes, void* stream) {
+  return mask_small_regions_bits(in, out, n, H, W, ld, min_area, mode, ws, changed, boxes, S(stream));
+}
+
+}  // extern "C"

@@ -18,10 +18,15 @@ de-duplicates with a box NMS (post_process_for_mask_generation :432-446).  Here:
 The low-res logits of every candidate of every image of the call stay on the device until the NMS has run: 256 KB
 per candidate, 3 per point, 805 MB per image at the default 32 x 32 grid, so a call on B images holds B times that at
 once (pass fewer images per call to bound it).  Host synchronisations per call: the read of the kept counts and
-candidates, and two more with ``output_rle_mask``, whatever the grid size and the number of masks.
+candidates, two more with ``output_rle_mask`` and one more with ``min_mask_region_area`` > 0 (none when no mask is
+kept), whatever the grid size and the number of masks.
 
 ``crops_n_layers > 0`` is not built: HF's own crop path cannot run (``_generate_crop_boxes`` stacks crops of different
-sizes), so there are no reference semantics for it.  Hole and sprinkle removal are not built either.
+sizes), so there are no reference semantics for it.  HF's ``max_hole_area`` / ``max_sprinkle_area`` are not built
+either (HF's SAM processor has no such arguments and its SAM2 processor ignores them).  SAM's ``min_mask_region_area``
+is: ``rsp_mask_small_regions_bits`` fills small holes and removes small islands of the kept masks on the GPU (connected
+components of the bit-packed masks by a block-based union-find), and a second ``rsp_nms_batched`` ranks the masks it
+changed after those it left alone: one more host synchronisation per call.
 
 ``python -m rsprompter_b200.mask_generation IMAGE --arch base --checkpoint sam.safetensors --out masks.json`` writes
 one dict per mask (COCO RLE ``segmentation``, xywh ``bbox``, ``predicted_iou``, ``stability_score``,
@@ -30,6 +35,7 @@ from __future__ import annotations
 
 import argparse
 import json
+import math
 
 import torch
 
@@ -174,16 +180,16 @@ def _candidates(sam, emb_nhwc, sizes, reshaped, p) -> dict:
                 keep=keep.view(B, Nc), points=pts_orig, n_out=n_out, sizes=sizes, reshaped=reshaped)
 
 
-def _nms(cand: dict, iou_thr: float) -> tuple:
+def _nms(iou: torch.Tensor, keep: torch.Tensor, boxes: torch.Tensor, iou_thr: float) -> tuple:
     """batched_nms(boxes.float(), scores, zeros, iou_thr) over every image's survivors (post_process_for_mask_generation,
-    image_processing_sam.py:715-720), in keep order.  -> (kept candidate index int64 [B, Nc] on the device, kept count
-    per image on the host, the same indices on the host); the one host synchronisation."""
-    iou, keep = cand["iou"], cand["keep"]
+    image_processing_sam.py:715-720), in keep order: scores iou fp32 [B, Nc], survivors keep bool [B, Nc], boxes
+    [B, Nc, 4].  -> (kept index int64 [B, Nc] on the device, kept count per image on the host, the same indices on the
+    host); one host synchronisation."""
     B, Nc = iou.shape
     key = torch.where(keep, iou, torch.full_like(iou, -float("inf")))
     _, order = torch.sort(key, dim=1, descending=True, stable=True)     # survivors first; ties by candidate order
     nvalid = keep.sum(1).to(torch.int32)
-    boxes_s = torch.gather(cand["boxes"].float(), 1, order[..., None].expand(-1, -1, 4)).contiguous()
+    boxes_s = torch.gather(boxes.float(), 1, order[..., None].expand(-1, -1, 4)).contiguous()
     scores_s = torch.gather(iou, 1, order).contiguous()
     ids = torch.zeros(B, Nc, device=iou.device, dtype=torch.int64)
     kept = _lib.nms_batched(boxes_s, ids, nvalid, iou_thr)
@@ -194,10 +200,10 @@ def _nms(cand: dict, iou_thr: float) -> tuple:
 
 
 def _outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch.Tensor, mask_threshold: float,
-             output_rle_mask: bool, target_size: int) -> list:
+             target_size: int) -> list:
     """Per image: the kept masks pasted as bits, and the kept rows of every per-candidate output."""
     B, Nc = cand["iou"].shape
-    out, rle_groups = [], []
+    out = []
     for b in range(B):
         k = counts[b]
         H, W = cand["sizes"][b]
@@ -208,17 +214,82 @@ def _outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch.Tensor
             lg = cand["logits"].index_select(0, ci + b * Nc)
             _lib.mask_paste(lg, mask_threshold, raw=True, rescale=((target_size, target_size), cand["reshaped"][b], (H, W)),
                             bits=bits)
-            rle_groups.append((bits, [(j * H * ld, ld, H, H, W, H, W, 0, 0) for j in range(k)]))
         out.append(dict(masks=bits, scores=cand["iou"][b].index_select(0, ci),
                         stability_scores=cand["stability"][b].index_select(0, ci),
                         boxes=cand["boxes"][b].index_select(0, ci).long(),
                         points=cand["points"][b].index_select(0, ci // cand["n_out"]),
                         candidates=idx_host[b, :k].clone(), size=(H, W)))
-    if output_rle_mask:
-        strings = iter(_lib.mask_rle_placed(rle_groups, packed=True))
-        for r in out:
-            r["rle"] = [dict(size=list(r["size"]), counts=next(strings)) for _ in range(r["masks"].shape[0])]
     return out
+
+
+# Device bytes of the label workspace of one rsp_mask_small_regions_bits launch (4 bytes per 2 x 2 pixel block, 1 MB
+# per 1024 x 1024 mask): masks are cleaned in chunks that fit, with results independent of the chunk size.
+SMALL_REGIONS_WORKSPACE_BYTES = 256 << 20
+
+
+def _check_region_area(min_mask_region_area) -> float:
+    a = float(min_mask_region_area)
+    if not math.isfinite(a):
+        raise ValueError(f"min_mask_region_area must be finite, got {min_mask_region_area}")
+    return a
+
+
+def _remove_small_regions(out: list, min_area: float, iou_thr: float) -> list:
+    """SAM's postprocess_small_regions (min_mask_region_area) on every image's kept masks: holes then islands by
+    rsp_mask_small_regions_bits, the boxes of the cleaned masks, and a box NMS with score float(unchanged) at iou_thr
+    through _nms.  Ties keep the first NMS's order (a stable sort; SAM's torchvision sort is not stable).  -> the
+    results in the new keep order, ``masks`` and ``boxes`` those of the cleaned masks; one host synchronisation."""
+    K = max(r["masks"].shape[0] for r in out)
+    if K == 0:
+        return out
+    dev = out[0]["masks"].device
+    B = len(out)
+    unchanged = torch.zeros(B, K, device=dev, dtype=torch.float32)
+    valid = torch.zeros(B, K, device=dev, dtype=torch.bool)
+    boxes = torch.zeros(B, K, 4, device=dev, dtype=torch.int32)
+    for b, r in enumerate(out):
+        bits = r["masks"]
+        k, H = bits.shape[0], bits.shape[1]
+        W = r["size"][1]
+        if k == 0:
+            continue
+        # areas are integers, so "< A" is "< ceil(A)"; every A above H * W (one more than the largest area) gives the
+        # same result, and the clamp keeps a huge finite A within the kernel's 64-bit threshold
+        thr = min(math.ceil(min_area), H * W + 1)
+        chunk = max(1, SMALL_REGIONS_WORKSPACE_BYTES // _lib.small_regions_ws_bytes(1, H, W))
+        ws = torch.empty(_lib.small_regions_ws_bytes(min(chunk, k), H, W), device=dev, dtype=torch.uint8)
+        tmp = torch.empty_like(bits[:chunk])
+        for j0 in range(0, k, chunk):
+            j1 = min(j0 + chunk, k)
+            part = bits[j0:j1]
+            _, ch_h, _ = _lib.mask_small_regions_bits(part, W, thr, "holes", out=tmp[:j1 - j0], ws=ws)
+            _, ch_i, bx = _lib.mask_small_regions_bits(tmp[:j1 - j0], W, thr, "islands", out=part, ws=ws)
+            unchanged[b, j0:j1] = (~(ch_h | ch_i)).float()
+            boxes[b, j0:j1] = bx
+        valid[b, :k] = True
+    idx, counts, idx_host = _nms(unchanged, valid, boxes, iou_thr)
+    res = []
+    for b, r in enumerate(out):
+        rows = idx[b, :counts[b]]
+        res.append(dict(masks=r["masks"].index_select(0, rows), scores=r["scores"].index_select(0, rows),
+                        stability_scores=r["stability_scores"].index_select(0, rows),
+                        boxes=boxes[b].index_select(0, rows).long(), points=r["points"].index_select(0, rows),
+                        candidates=r["candidates"][idx_host[b, :counts[b]]], size=r["size"]))
+    return res
+
+
+def _add_rle(out: list) -> None:
+    """COCO RLE strings of every image's masks, in one batch on the GPU."""
+    rle_groups = []
+    for r in out:
+        bits = r["masks"]
+        k, (H, W) = bits.shape[0], r["size"]
+        if k:
+            ld = bits.shape[2]
+            rle_groups.append((bits, [(j * H * ld, ld, H, H, W, H, W, 0, 0) for j in range(k)]))
+    strings = iter(_lib.mask_rle_placed(rle_groups, packed=True))
+    for r in out:
+        r["rle"] = [dict(size=list(r["size"]), counts=next(strings)) for _ in range(r["masks"].shape[0])]
 
 
 @torch.no_grad()
@@ -226,7 +297,8 @@ def generate_masks(model, images=None, *, pixel_values=None, original_sizes=None
                    points_per_side: int = 32, points_per_batch: int = 64, pred_iou_thresh: float = 0.88,
                    stability_score_thresh: float = 0.95, stability_score_offset: float = 1.0,
                    mask_threshold: float = 0.0, crops_nms_thresh: float = 0.7, crops_n_layers: int = 0,
-                   max_hole_area=None, max_sprinkle_area=None, output_rle_mask: bool = False) -> list:
+                   max_hole_area=None, max_sprinkle_area=None, min_mask_region_area: float = 0,
+                   output_rle_mask: bool = False) -> list:
     """Every mask of each image, as HF's mask-generation pipeline finds them with crops_n_layers=0.
 
     ``model``: an RSSamModel or SamModelB200.  Images go in one of two forms:
@@ -243,7 +315,16 @@ def generate_masks(model, images=None, *, pixel_values=None, original_sizes=None
     disables its test, as in filter_masks.  ``crops_n_layers > 0``, ``max_hole_area`` and ``max_sprinkle_area`` raise
     ValueError.
 
-    Returns one dict per image, rows in NMS keep order (descending predicted IoU):
+    ``min_mask_region_area`` = A > 0 is SAM's (SamAutomaticMaskGenerator.postprocess_small_regions) on the kept masks
+    at their original size: 8-connected background components of area < A are filled (border ones included), then of
+    the foreground components only those of area >= A are kept, or the largest alone when none is (ties: cv2's label
+    order).  Masks are then boxed again and go through a second box NMS at ``crops_nms_thresh`` with score 1 for a
+    mask that neither step changed and 0 otherwise, so unchanged masks come first.  A step counts as a change when it
+    finds a small component, as in SAM, even if the mask stays the same.  Ties keep the first NMS's order: this sort is
+    stable, SAM's torchvision sort is not.  A <= 0 (SAM's default) skips the step; a non-finite A raises ValueError.
+
+    Returns one dict per image, rows in NMS keep order (descending predicted IoU; with min_mask_region_area, the
+    order of the second NMS):
       masks             uint8 [k, H, ceil(W / 16) * 2] bit-packed rows, pixel x = bit x % 8 of byte x // 8
                         (``masks_to_bool`` unpacks them)
       scores            fp32 [k] predicted IoU
@@ -258,6 +339,7 @@ def generate_masks(model, images=None, *, pixel_values=None, original_sizes=None
     Memory: the low-res logits of every candidate of every image stay resident until the NMS, 3 x points_per_side^2 x
     256 KB per image (805 MB at the default grid), so B images in one call need B times that at once."""
     _check_params(points_per_side, points_per_batch, crops_n_layers, max_hole_area, max_sprinkle_area)
+    min_area = _check_region_area(min_mask_region_area)
     sam = _sam(model)
     dev = sam.prompt_encoder.no_mask_embed.weight.device
     pix, sizes, reshaped = _inputs(sam, images, pixel_values, original_sizes, reshaped_input_sizes, dev)
@@ -266,8 +348,13 @@ def generate_masks(model, images=None, *, pixel_values=None, original_sizes=None
              stability_score_offset=float(stability_score_offset), mask_threshold=float(mask_threshold))
     emb = sam._encode(pix)
     cand = _candidates(sam, emb, sizes, reshaped, p)
-    idx, counts, idx_host = _nms(cand, float(crops_nms_thresh))
-    return _outputs(cand, idx, counts, idx_host, float(mask_threshold), output_rle_mask, sam.varch.image_size)
+    idx, counts, idx_host = _nms(cand["iou"], cand["keep"], cand["boxes"], float(crops_nms_thresh))
+    out = _outputs(cand, idx, counts, idx_host, float(mask_threshold), sam.varch.image_size)
+    if min_area > 0:
+        out = _remove_small_regions(out, min_area, float(crops_nms_thresh))
+    if output_rle_mask:
+        _add_rle(out)
+    return out
 
 
 def masks_to_bool(result: dict) -> torch.Tensor:
@@ -303,6 +390,8 @@ def main(argv=None) -> list:
     ap.add_argument("--stability-score-offset", type=float, default=1.0)
     ap.add_argument("--mask-threshold", type=float, default=0.0)
     ap.add_argument("--crops-nms-thresh", type=float, default=0.7)
+    ap.add_argument("--min-mask-region-area", type=float, default=0.0,
+                    help="fill holes and remove islands smaller than this many pixels (SAM's min_mask_region_area)")
     ap.add_argument("--out", default=None, help="JSON file for the mask dicts (default: stdout)")
     args = ap.parse_args(argv)
 
@@ -319,7 +408,8 @@ def main(argv=None) -> list:
                          points_per_batch=args.points_per_batch, pred_iou_thresh=args.pred_iou_thresh,
                          stability_score_thresh=args.stability_score_thresh,
                          stability_score_offset=args.stability_score_offset, mask_threshold=args.mask_threshold,
-                         crops_nms_thresh=args.crops_nms_thresh, output_rle_mask=True)[0]
+                         crops_nms_thresh=args.crops_nms_thresh, min_mask_region_area=args.min_mask_region_area,
+                         output_rle_mask=True)[0]
     rows = mask_dicts(res)
     text = json.dumps(rows)
     if args.out:
