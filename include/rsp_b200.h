@@ -418,6 +418,18 @@ int rsp_sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb,
                        float stability_score_thresh, int32_t* part_ws, int32_t* counts, int32_t* boxes,
                        float* stability, uint8_t* keep, void* stream);
 
+/* rsp_sam_mask_stats for the masks of one crop of a larger scene, with HF filter_masks' crop-edge rule in the keep flag
+ * (image_processing_sam.py _is_box_near_crop_edge(box, crop_box, [0, 0, scene_w, scene_h], atol=20)): the H x W masks
+ * are the crop box (crop_x0, crop_y0, crop_x1, crop_y1) of a scene_h x scene_w scene, and a mask is also dropped when a
+ * side of its box (its empty-mask [0, 0, 0, 0] included), shifted by (crop_x0, crop_y0) and rounded to fp32, lies within
+ * 20 of the crop box's side and not within 20 of the scene's.  Applied in the same launch as the other tests; iou is
+ * required.  Every other output and argument as rsp_sam_mask_stats. */
+int rsp_sam_mask_stats_crop(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H,
+                            int W, float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                            float stability_score_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1,
+                            int scene_h, int scene_w, int32_t* part_ws, int32_t* counts, int32_t* boxes,
+                            float* stability, uint8_t* keep, void* stream);
+
 /* SAM automatic mask generation's small-region removal (min_mask_region_area) on bit-packed masks.  Replaces, per
  * kept mask, segment_anything/utils/amg.py remove_small_regions(mask, area_thresh, mode) as
  * SamAutomaticMaskGenerator.postprocess_small_regions calls it (cv2.connectedComponentsWithStats(., 8) + np.isin), and

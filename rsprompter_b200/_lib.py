@@ -121,6 +121,8 @@ _SIGNATURES = {
     "rsp_sam_mask_embed": ([_vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp], _i),
     "rsp_sam_mask_stats": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _vp, _vp, _vp, _vp, _vp,
                             _vp], _i),
+    "rsp_sam_mask_stats_crop": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _i, _i, _i, _i, _i,
+                                 _i, _vp, _vp, _vp, _vp, _vp, _vp], _i),
     "rsp_mask_small_regions_bits": ([_vp, _vp, _i, _i, _i, _i, ctypes.c_longlong, _i, _vp, _vp, _vp, _vp], _i),
 }
 
@@ -900,12 +902,15 @@ def mask_paste(logits: torch.Tensor, thr: float, *, raw: bool, size: tuple | Non
 
 def sam_mask_stats(logits: torch.Tensor, rescale: tuple, mask_threshold: float = 0.0,
                    stability_score_offset: float = 1.0, iou: torch.Tensor | None = None, pred_iou_thresh: float = 0.0,
-                   stability_score_thresh: float = 0.0):
+                   stability_score_thresh: float = 0.0, crop: tuple | None = None):
     """Per-candidate statistics of SAM mask generation (rsp_sam_mask_stats): logits fp32 [n, hm, wm], rescale =
     (pad_hw, reshaped_hw, original_hw) as mask_paste's.  -> counts int32 [n, 3] (> thr + offset, > thr - offset,
-    > thr), boxes int32 [n, 4] (HF's inclusive xyxy of > thr), stability fp32 [n], keep bool [n] (None without iou)."""
+    > thr), boxes int32 [n, 4] (HF's inclusive xyxy of > thr), stability fp32 [n], keep bool [n] (None without iou).
+    ``crop`` = ((x0, y0, x1, y1), (scene_h, scene_w)): the masks are that crop box of a larger scene, and the keep flag
+    also applies HF's crop-edge rule (rsp_sam_mask_stats_crop; needs iou)."""
     global launch_count
     _require_cuda(logits, iou)
+    assert crop is None or iou is not None, "the crop-edge rule is part of the keep flag: pass iou"
     assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.dim() == 3
     n, hm, wm = logits.shape
     (Hb, Wb), (ch, cw), (H, W) = rescale
@@ -921,10 +926,18 @@ def sam_mask_stats(logits: torch.Tensor, rescale: tuple, mask_threshold: float =
         return counts, boxes, stability, None if keep is None else keep.view(torch.bool)
     part = torch.empty(n, (H + 15) // 16, 7, device=dev, dtype=torch.int32)
     thr = float(mask_threshold)
-    _check(_lib.rsp_sam_mask_stats(_ptr(logits), n, hm, wm, Hb, Wb, ch, cw, H, W, thr,
-                                   thr + float(stability_score_offset), thr - float(stability_score_offset), _ptr(iou),
-                                   float(pred_iou_thresh), float(stability_score_thresh), _ptr(part), _ptr(counts),
-                                   _ptr(boxes), _ptr(stability), _ptr(keep), _stream()), "rsp_sam_mask_stats")
+    thr_hi, thr_lo = thr + float(stability_score_offset), thr - float(stability_score_offset)
+    if crop is None:
+        _check(_lib.rsp_sam_mask_stats(_ptr(logits), n, hm, wm, Hb, Wb, ch, cw, H, W, thr, thr_hi, thr_lo, _ptr(iou),
+                                       float(pred_iou_thresh), float(stability_score_thresh), _ptr(part), _ptr(counts),
+                                       _ptr(boxes), _ptr(stability), _ptr(keep), _stream()), "rsp_sam_mask_stats")
+    else:
+        (x0, y0, x1, y1), (sh, sw) = crop
+        _check(_lib.rsp_sam_mask_stats_crop(_ptr(logits), n, hm, wm, Hb, Wb, ch, cw, H, W, thr, thr_hi, thr_lo,
+                                            _ptr(iou), float(pred_iou_thresh), float(stability_score_thresh), int(x0),
+                                            int(y0), int(x1), int(y1), int(sh), int(sw), _ptr(part), _ptr(counts),
+                                            _ptr(boxes), _ptr(stability), _ptr(keep), _stream()),
+               "rsp_sam_mask_stats_crop")
     launch_count += 2
     return counts, boxes, stability, None if keep is None else keep.view(torch.bool)
 

@@ -392,6 +392,16 @@ int rsp_sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb,
                         stability_score_thresh, part_ws, counts, boxes, stability, keep, S(stream));
 }
 
+int rsp_sam_mask_stats_crop(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H,
+                            int W, float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                            float stability_score_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1,
+                            int scene_h, int scene_w, int32_t* part_ws, int32_t* counts, int32_t* boxes,
+                            float* stability, uint8_t* keep, void* stream) {
+  return sam_mask_stats_crop(maps, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, thr, thr_hi, thr_lo, iou, pred_iou_thresh,
+                             stability_score_thresh, crop_x0, crop_y0, crop_x1, crop_y1, scene_h, scene_w, part_ws,
+                             counts, boxes, stability, keep, S(stream));
+}
+
 }  // extern "C"
 
 #include "records.h"

@@ -1022,13 +1022,38 @@ sam_mask_stats_kernel(TwoResizes s, int H, int W, float thr, float thr_hi, float
   }
 }
 
+// The crop-edge rule of HF's filter_masks (image_processing_sam.py _is_box_near_crop_edge with atol 20, rtol 0): a
+// mask's box, shifted by the crop's origin into the scene, is dropped when a side lies within 20 of the crop box's side
+// and not within 20 of the scene's, in the fp32 arithmetic torch.isclose runs on (box + offset).float().
+struct CropEdge {
+  int x0, y0, x1, y1;   // the crop box in scene pixels, xyxy
+  int H, W;             // the scene
+};
+
+__device__ __forceinline__ bool near_crop_edge(const int* box, const CropEdge& c) {
+  const int off[4] = {c.x0, c.y0, c.x0, c.y0};
+  const int crop[4] = {c.x0, c.y0, c.x1, c.y1};
+  const int scene[4] = {0, 0, c.W, c.H};
+  bool near = false;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float b = __int2float_rn(box[k] + off[k]);
+    near = near || (fabsf(__fsub_rn(b, __int2float_rn(crop[k]))) <= 20.f &&
+                    !(fabsf(__fsub_rn(b, __int2float_rn(scene[k]))) <= 20.f));
+  }
+  return near;
+}
+
 // one warp per mask: the band partials -> counts, the HF box ([0, 0, 0, 0] when nothing is > thr), the stability score
 // (count > thr_hi) / (count > thr_lo) as torch's int32 / int32 true division (NaN for 0 / 0) and, with iou, the keep
-// flag of filter_masks (a threshold > 0 enables its test; NaN fails every test).
-__global__ void sam_mask_stats_finish_kernel(const int* __restrict__ part, int n, int bands,
-                                             const float* __restrict__ iou, float pred_iou_thresh,
-                                             float stability_thresh, int* __restrict__ counts, int* __restrict__ boxes,
-                                             float* __restrict__ stability, unsigned char* __restrict__ keep) {
+// flag of filter_masks (a threshold > 0 enables its test; NaN fails every test).  kCrop adds the crop-edge rule to the
+// keep flag.
+template <bool kCrop>
+__device__ __forceinline__ void sam_mask_stats_finish(const int* __restrict__ part, int n, int bands,
+                                                      const float* __restrict__ iou, float pred_iou_thresh,
+                                                      float stability_thresh, int* __restrict__ counts,
+                                                      int* __restrict__ boxes, float* __restrict__ stability,
+                                                      unsigned char* __restrict__ keep, const CropEdge& crop) {
   const int m = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
   if (m >= n) return;
   int v[SMS_FIELDS] = {0, 0, 0, INT_MAX, INT_MAX, -1, -1};
@@ -1045,22 +1070,44 @@ __global__ void sam_mask_stats_finish_kernel(const int* __restrict__ part, int n
 #pragma unroll
   for (int f = 0; f < 3; ++f) counts[m * 3 + f] = v[f];
   const bool empty = v[2] == 0;
+  int box[4];
 #pragma unroll
-  for (int f = 0; f < 4; ++f) boxes[m * 4 + f] = empty ? 0 : v[3 + f];
+  for (int f = 0; f < 4; ++f) {
+    box[f] = empty ? 0 : v[3 + f];
+    boxes[m * 4 + f] = box[f];
+  }
   const float st = __fdiv_rn(__int2float_rn(v[0]), __int2float_rn(v[1]));
   stability[m] = st;
   if (iou != nullptr) {
     bool k = true;
     if (pred_iou_thresh > 0.f) k = k && iou[m] > pred_iou_thresh;
     if (stability_thresh > 0.f) k = k && st > stability_thresh;
+    if (kCrop) k = k && !near_crop_edge(box, crop);
     keep[m] = k ? 1 : 0;
   }
 }
 
-int sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
-                   float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                   float stability_thresh, int* part_ws, int* counts, int* boxes, float* stability,
-                   unsigned char* keep, cudaStream_t stream) {
+__global__ void sam_mask_stats_finish_kernel(const int* __restrict__ part, int n, int bands,
+                                             const float* __restrict__ iou, float pred_iou_thresh,
+                                             float stability_thresh, int* __restrict__ counts, int* __restrict__ boxes,
+                                             float* __restrict__ stability, unsigned char* __restrict__ keep) {
+  sam_mask_stats_finish<false>(part, n, bands, iou, pred_iou_thresh, stability_thresh, counts, boxes, stability, keep,
+                               CropEdge{});
+}
+
+__global__ void crop_mask_stats_finish_kernel(const int* __restrict__ part, int n, int bands,
+                                              const float* __restrict__ iou, float pred_iou_thresh,
+                                              float stability_thresh, int* __restrict__ counts,
+                                              int* __restrict__ boxes, float* __restrict__ stability,
+                                              unsigned char* __restrict__ keep, CropEdge crop) {
+  sam_mask_stats_finish<true>(part, n, bands, iou, pred_iou_thresh, stability_thresh, counts, boxes, stability, keep,
+                              crop);
+}
+
+static int sam_mask_stats_impl(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H,
+                               int W, float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                               float stability_thresh, int* part_ws, int* counts, int* boxes, float* stability,
+                               unsigned char* keep, const CropEdge* edge, cudaStream_t stream) {
   const int bands = (H + SMS_ROWS - 1) / SMS_ROWS;
   RSP_CHECK_ARG(maps && part_ws && counts && boxes && stability && (!iou || keep) && n > 0 && hm > 0 && wm > 0 &&
                 Hb > 0 && Wb > 0 && crop_h > 0 && crop_w > 0 && crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 &&
@@ -1070,10 +1117,36 @@ int sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int
   sam_mask_stats_kernel<<<static_cast<unsigned>(n) * bands, SMS_THREADS, 0, stream>>>(s, H, W, thr, thr_hi, thr_lo,
                                                                                      bands, part_ws);
   RSP_CHECK_LAUNCH();
-  sam_mask_stats_finish_kernel<<<(n + 7) / 8, 256, 0, stream>>>(part_ws, n, bands, iou, pred_iou_thresh,
-                                                                 stability_thresh, counts, boxes, stability, keep);
+  if (edge)
+    crop_mask_stats_finish_kernel<<<(n + 7) / 8, 256, 0, stream>>>(part_ws, n, bands, iou, pred_iou_thresh,
+                                                                    stability_thresh, counts, boxes, stability, keep,
+                                                                    *edge);
+  else
+    sam_mask_stats_finish_kernel<<<(n + 7) / 8, 256, 0, stream>>>(part_ws, n, bands, iou, pred_iou_thresh,
+                                                                   stability_thresh, counts, boxes, stability, keep);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
+}
+
+int sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                   float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                   float stability_thresh, int* part_ws, int* counts, int* boxes, float* stability,
+                   unsigned char* keep, cudaStream_t stream) {
+  return sam_mask_stats_impl(maps, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, thr, thr_hi, thr_lo, iou, pred_iou_thresh,
+                             stability_thresh, part_ws, counts, boxes, stability, keep, nullptr, stream);
+}
+
+int sam_mask_stats_crop(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                        float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                        float stability_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1, int scene_h,
+                        int scene_w, int* part_ws, int* counts, int* boxes, float* stability, unsigned char* keep,
+                        cudaStream_t stream) {
+  RSP_CHECK_ARG(iou && crop_x0 >= 0 && crop_y0 >= 0 && crop_x1 > crop_x0 && crop_y1 > crop_y0 &&
+                crop_x1 <= scene_w && crop_y1 <= scene_h && crop_x1 - crop_x0 == W && crop_y1 - crop_y0 == H,
+                "sam_mask_stats_crop: bad args (iou needed; the crop box is the H x W mask's place in the scene)");
+  const CropEdge edge{crop_x0, crop_y0, crop_x1, crop_y1, scene_h, scene_w};
+  return sam_mask_stats_impl(maps, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, thr, thr_hi, thr_lo, iou, pred_iou_thresh,
+                             stability_thresh, part_ws, counts, boxes, stability, keep, &edge, stream);
 }
 
 __global__ void sigmoid_f32_kernel(const float4* __restrict__ in, float4* __restrict__ out, long long n4) {

@@ -39,6 +39,11 @@ int sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int
                    float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
                    float stability_thresh, int* part_ws, int* counts, int* boxes, float* stability,
                    unsigned char* keep, cudaStream_t stream);
+int sam_mask_stats_crop(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                        float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                        float stability_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1, int scene_h,
+                        int scene_w, int* part_ws, int* counts, int* boxes, float* stability, unsigned char* keep,
+                        cudaStream_t stream);
 int sigmoid_f32(const float* in, float* out, long long n, cudaStream_t stream);
 int pool2_nhwc(const void* in, void* out, int B, int H, int W, int C, int mode, cudaStream_t stream);
 int zero_border_nhwc(void* x, int N, int H, int W, int C, cudaStream_t stream);

@@ -28,9 +28,14 @@ is: ``rsp_mask_small_regions_bits`` fills small holes and removes small islands 
 components of the bit-packed masks by a block-based union-find), and a second ``rsp_nms_batched`` ranks the masks it
 changed after those it left alone: one more host synchronisation per call.
 
+``generate_scene_masks`` runs the same stages over the overlapping windows of a whole scene (large_image's slicing),
+with HF's crop-edge rule applied in ``rsp_sam_mask_stats_crop``, RLE of the whole scene from each window's bits, and
+one cross-window box NMS.
+
 ``python -m rsprompter_b200.mask_generation IMAGE --arch base --checkpoint sam.safetensors --out masks.json`` writes
 one dict per mask (COCO RLE ``segmentation``, xywh ``bbox``, ``predicted_iou``, ``stability_score``,
-``point_coords``)."""
+``point_coords``); with ``--patch-size P`` the image is a scene cut into P x P windows, and each dict also has the
+window's ``crop_box``."""
 from __future__ import annotations
 
 import argparse
@@ -135,9 +140,11 @@ def _inputs(sam, images, pixel_values, original_sizes, reshaped_input_sizes, dev
     return pix, sizes, reshaped
 
 
-def _candidates(sam, emb_nhwc, sizes, reshaped, p) -> dict:
+def _candidates(sam, emb_nhwc, sizes, reshaped, p, crops=None) -> dict:
     """The grids of every image through the decoder in calls of points_per_batch prompts, each call's logits through
-    rsp_sam_mask_stats.  -> per-candidate device tensors, candidate c of image b at [b, c] (point c // 3, mask c % 3)."""
+    rsp_sam_mask_stats.  -> per-candidate device tensors, candidate c of image b at [b, c] (point c // 3, mask c % 3).
+    ``crops``: per image, ((x0, y0, x1, y1), (H, W)) when it is that crop box of an H x W scene; the keep flags then
+    include the crop-edge rule (rsp_sam_mask_stats_crop)."""
     B, g, C = emb_nhwc.shape[0], emb_nhwc.shape[1], emb_nhwc.shape[3]
     S = sam.varch.image_size
     dev = emb_nhwc.device
@@ -172,7 +179,7 @@ def _candidates(sam, emb_nhwc, sizes, reshaped, p) -> dict:
             r0, r1 = max(q0, b * n_pts) * n_out, min(q1, (b + 1) * n_pts) * n_out
             _, bx, st, kp = _lib.sam_mask_stats(
                 logits[r0:r1], ((S, S), reshaped[b], sizes[b]), p["mask_threshold"], p["stability_score_offset"],
-                iou[r0:r1], p["pred_iou_thresh"], p["stability_score_thresh"])
+                iou[r0:r1], p["pred_iou_thresh"], p["stability_score_thresh"], crop=None if crops is None else crops[b])
             boxes[r0:r1].copy_(bx)
             stab[r0:r1].copy_(st)
             keep[r0:r1].copy_(kp)
@@ -278,18 +285,21 @@ def _remove_small_regions(out: list, min_area: float, iou_thr: float) -> list:
     return res
 
 
-def _add_rle(out: list) -> None:
-    """COCO RLE strings of every image's masks, in one batch on the GPU."""
-    rle_groups = []
-    for r in out:
+def _add_rle(out: list, places: list | None = None) -> None:
+    """COCO RLE strings of every image's masks, in one batch on the GPU.  ``places``: per image, (SH, SW, y0, x0) to
+    encode its masks as masks of an SH x SW canvas that is zero but for the image at (y0, x0)."""
+    rle_groups, sizes = [], []
+    for b, r in enumerate(out):
         bits = r["masks"]
         k, (H, W) = bits.shape[0], r["size"]
+        SH, SW, y0, x0 = (H, W, 0, 0) if places is None else places[b]
+        sizes.append([SH, SW])
         if k:
             ld = bits.shape[2]
-            rle_groups.append((bits, [(j * H * ld, ld, H, H, W, H, W, 0, 0) for j in range(k)]))
+            rle_groups.append((bits, [(j * H * ld, ld, H, H, W, SH, SW, y0, x0) for j in range(k)]))
     strings = iter(_lib.mask_rle_placed(rle_groups, packed=True))
-    for r in out:
-        r["rle"] = [dict(size=list(r["size"]), counts=next(strings)) for _ in range(r["masks"].shape[0])]
+    for r, size in zip(out, sizes):
+        r["rle"] = [dict(size=list(size), counts=next(strings)) for _ in range(r["masks"].shape[0])]
 
 
 @torch.no_grad()
@@ -357,6 +367,177 @@ def generate_masks(model, images=None, *, pixel_values=None, original_sizes=None
     return out
 
 
+def scene_crop_boxes(hw: tuple, patch_size: int, overlap_ratio: float) -> list:
+    """The windows of generate_scene_masks over an H x W scene: large_image.slice_origins' P x P windows, each cut to
+    its in-scene part, as crop boxes (x0, y0, min(x0 + P, W), min(y0 + P, H)) in slice order."""
+    from .large_image import slice_origins
+    H, W = int(hw[0]), int(hw[1])
+    P = int(patch_size)
+    return [(x0, y0, min(x0 + P, W), min(y0 + P, H)) for x0, y0 in slice_origins((H, W), P, overlap_ratio)]
+
+
+def _device_scene(scene: torch.Tensor, dev) -> torch.Tensor:
+    """The scene [3, H, W] on dev, copied once in its own memory order (a permuted HWC array stays HWC)."""
+    if scene.device == dev:
+        return scene
+    hwc = scene.permute(1, 2, 0)
+    if hwc.is_contiguous():
+        return hwc.pin_memory().to(dev, non_blocking=True).permute(2, 0, 1)
+    return scene.contiguous().pin_memory().to(dev, non_blocking=True)
+
+
+def _free_bytes(dev) -> int:
+    free, _ = torch.cuda.mem_get_info(dev)
+    return free + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+
+
+@torch.no_grad()
+def generate_scene_masks(model, scene, *, patch_size: int | None = None, overlap_ratio: float = 0.25,
+                         batch_size: int = 4, points_per_side: int = 32, points_per_batch: int = 64,
+                         pred_iou_thresh: float = 0.88, stability_score_thresh: float = 0.95,
+                         stability_score_offset: float = 1.0, mask_threshold: float = 0.0,
+                         crops_nms_thresh: float = 0.7, crops_n_layers: int = 0, max_hole_area=None,
+                         max_sprinkle_area=None, min_mask_region_area: float = 0) -> dict:
+    """Every mask of a whole scene: generate_masks on overlapping windows, merged across windows.
+
+    ``scene``: uint8 RGB [3, H, W] with any strides (a permuted HWC array is fine), on the host or the device; it is
+    copied to the device once.  The windows are large_image.slice_origins' P x P windows (P = ``patch_size``, default
+    the model's image size; consecutive windows overlap by int(overlap_ratio * P), the last of a row or column is
+    shifted inward to end at the scene's edge), each cut to its in-scene part: the crop box (x0, y0, x1, y1) with
+    x1 = min(x0 + P, W), y1 = min(y0 + P, H) (``scene_crop_boxes``).
+
+    Each window is exactly ``generate_masks(scene[:, y0:y1, x0:x1], ...)`` with the same parameters, plus the crop-edge
+    rule of HF's filter_masks (SAM's _process_batch) after the predicted-IoU and stability filters and before the
+    window's NMS: a candidate is dropped when a side of its box, shifted into the scene, lies within 20 px of the crop
+    box's side but not within 20 px of the scene's (HF's _is_box_near_crop_edge, fp32).  The survivors of every
+    window are shifted into scene coordinates and merged by one box NMS at the same ``crops_nms_thresh``, scored by
+    predicted IoU (post_process_for_mask_generation's NMS over every window): a stable descending sort, ties by
+    (window in slice order, rank in the window's keep order).  A scene that fits in one window (H <= P and W <= P) is
+    generate_masks(scene, output_rle_mask=True): the crop box is the scene, so the rule drops nothing.
+
+    Objects larger than the overlap: as with SAM's crop layers without the whole-image layer, a mask is kept only
+    from a window in which its box is more than 20 px from every interior edge.  An object is certain to be found
+    only when its extent is below about int(overlap_ratio * P) - 42 px (214 px at the defaults); larger objects
+    crossing windows (fields, water bodies) may be found in none.
+
+    Windows run ``batch_size`` at a time through generate_masks' stages: the low-res logits of a batch (805 MB per
+    window at the default grid) are freed before the next batch, and the kept masks of each window are encoded as
+    COCO RLE of the whole H x W scene straight from the window's bits, which are then freed.  Masks the merge later
+    suppresses were encoded for nothing: the price of memory that does not grow with the scene.  Host
+    synchronisations: those of generate_masks(output_rle_mask=True) per batch, and one for the merge when some mask
+    was kept.  More than large_image.MAX_MERGE_CANDIDATES survivors raise ValueError before the merge; a merge
+    workspace (N^2 / 8 bytes) or a batch (scene copy, logits, pixel values and the worst case of bits) larger than
+    free device memory raises RuntimeError, the batch before any window runs.
+
+    Returns one dict, rows in the merge's keep order, all in scene coordinates:
+      rle               COCO compressed RLE dicts {'size': [H, W], 'counts': bytes}
+      scores            fp32 [k] predicted IoU
+      stability_scores  fp32 [k]
+      boxes             int64 [k, 4] inclusive pixel xyxy
+      points            fp32 [k, 2] the prompt of each mask
+      tiles             int64 [k] window index (slice order)
+      crop_boxes        int64 [k, 4] xyxy crop box of each mask's window
+      candidates        int64 [k] (host) candidate index in its window: point * 3 + output mask
+      size              (H, W)
+    All tensors but ``candidates`` are on the model's device."""
+    _check_params(points_per_side, points_per_batch, crops_n_layers, max_hole_area, max_sprinkle_area)
+    min_area = _check_region_area(min_mask_region_area)
+    if not isinstance(scene, torch.Tensor) or scene.dtype != torch.uint8 or scene.dim() != 3 or scene.shape[0] != 3:
+        raise ValueError("the scene must be a uint8 RGB tensor [3, H, W], got "
+                         + (f"{scene.dtype} {tuple(scene.shape)}" if isinstance(scene, torch.Tensor)
+                            else type(scene).__name__))
+    H, W = int(scene.shape[1]), int(scene.shape[2])
+    if H < 1 or W < 1:
+        raise ValueError(f"the scene is empty: {H} x {W}")
+    if patch_size is not None and int(patch_size) < 1:
+        raise ValueError(f"patch_size must be >= 1, got {patch_size}")
+    if not 0 <= overlap_ratio < 1:
+        raise ValueError(f"overlap_ratio must be in [0, 1), got {overlap_ratio}")
+    if batch_size < 1:
+        raise ValueError(f"batch_size must be >= 1, got {batch_size}")
+    sam = _sam(model)
+    dev = sam.prompt_encoder.no_mask_embed.weight.device
+    S = sam.varch.image_size
+    P = S if patch_size is None else int(patch_size)
+    crops = scene_crop_boxes((H, W), P, overlap_ratio)
+    T = len(crops)
+    B = min(int(batch_size), T)
+    p = dict(points_per_side=int(points_per_side), points_per_batch=int(points_per_batch),
+             pred_iou_thresh=float(pred_iou_thresh), stability_score_thresh=float(stability_score_thresh),
+             stability_score_offset=float(stability_score_offset), mask_threshold=float(mask_threshold))
+    nms_thr = float(crops_nms_thresh)
+
+    # what one batch holds at once, checked before any window runs
+    n_cand = 3 * p["points_per_side"] ** 2
+    hm = 4 * (S // sam.varch.patch_size)
+    ph, pw = min(P, H), min(P, W)
+    need = ((0 if scene.device == dev else 3 * H * W) + B * n_cand * hm * hm * 4 + B * 3 * S * S * 4
+            + B * n_cand * ph * ((pw + 15) // 16 * 2))
+    free = _free_bytes(dev)
+    if need > free:
+        raise RuntimeError(f"a {H} x {W} scene in batches of {B} windows of {P}^2 needs {need / 2**30:.2f} GiB on {dev} "
+                           f"(the scene, {n_cand} candidates' low-res logits per window, the pixel values and the bits "
+                           f"if every candidate were kept); {free / 2**30:.2f} GiB are free")
+
+    img = _device_scene(scene, dev)
+    tiles = []
+    for b0 in range(0, T, B):
+        boxes_b = crops[b0:b0 + B]
+        views = [img[:, y0:y1, x0:x1] for x0, y0, x1, y1 in boxes_b]
+        pix, sizes, reshaped = _inputs(sam, views, None, None, None, dev)
+        cand = _candidates(sam, sam._encode(pix), sizes, reshaped, p, crops=[(cb, (H, W)) for cb in boxes_b])
+        del pix
+        idx, counts, idx_host = _nms(cand["iou"], cand["keep"], cand["boxes"], nms_thr)
+        out = _outputs(cand, idx, counts, idx_host, p["mask_threshold"], S)
+        del cand, idx                                           # the batch's low-res logits
+        if min_area > 0:
+            out = _remove_small_regions(out, min_area, nms_thr)
+        _add_rle(out, places=[(H, W, y0, x0) for x0, y0, _, _ in boxes_b])
+        for r in out:
+            del r["masks"]                                      # only the rows and strings stay
+        tiles.extend(out)
+    return _merge_tiles(tiles, crops, (H, W), nms_thr, dev)
+
+
+def _merge_tiles(tiles: list, crops: list, hw: tuple, nms_thr: float, dev) -> dict:
+    """The cross-window NMS of generate_scene_masks over every window's rows (in slice order, each in keep order)."""
+    from .large_image import MAX_MERGE_CANDIDATES
+    counts = [r["scores"].shape[0] for r in tiles]
+    N = sum(counts)
+    if N > MAX_MERGE_CANDIDATES:
+        raise ValueError(f"{len(tiles)} windows kept {N} masks; the cross-window merge's dense NMS takes at most "
+                         f"{MAX_MERGE_CANDIDATES} candidates")
+    ws = N * ((N + 63) // 64) * 8
+    free = _free_bytes(dev)
+    if ws > free:
+        raise RuntimeError(f"the merge of {N} masks from {len(tiles)} windows needs a {ws / 2**30:.2f} GiB NMS workspace "
+                           f"on {dev}; {free / 2**30:.2f} GiB are free")
+    tile_h = torch.repeat_interleave(torch.arange(len(tiles)), torch.tensor(counts, dtype=torch.int64))
+    crop_h = torch.tensor(crops, dtype=torch.int64).view(-1, 4)[tile_h]
+    res = dict(rle=[], scores=torch.zeros(0, device=dev), stability_scores=torch.zeros(0, device=dev),
+               boxes=torch.zeros(0, 4, device=dev, dtype=torch.int64), points=torch.zeros(0, 2, device=dev),
+               tiles=torch.zeros(0, device=dev, dtype=torch.int64),
+               crop_boxes=torch.zeros(0, 4, device=dev, dtype=torch.int64),
+               candidates=torch.zeros(0, dtype=torch.int64), size=(int(hw[0]), int(hw[1])))
+    if N == 0:
+        return res
+    crop_d = crop_h.pin_memory().to(dev, non_blocking=True)
+    off = crop_h[:, [0, 1, 0, 1]].pin_memory().to(dev, non_blocking=True)     # indexed on the host: no sync
+    scores = torch.cat([r["scores"] for r in tiles])
+    boxes = torch.cat([r["boxes"] for r in tiles]) + off
+    points = torch.cat([r["points"] for r in tiles]) + off[:, :2].float()
+    idx, cnt, idx_host = _nms(scores[None], torch.ones(1, N, device=dev, dtype=torch.bool), boxes[None], nms_thr)
+    k = cnt[0]
+    rows, rows_h = idx[0, :k], idx_host[0, :k]
+    rle = [s for r in tiles for s in r["rle"]]
+    res.update(rle=[rle[i] for i in rows_h.tolist()], scores=scores.index_select(0, rows),
+               stability_scores=torch.cat([r["stability_scores"] for r in tiles]).index_select(0, rows),
+               boxes=boxes.index_select(0, rows), points=points.index_select(0, rows),
+               tiles=tile_h[rows_h].pin_memory().to(dev, non_blocking=True), crop_boxes=crop_d.index_select(0, rows),
+               candidates=torch.cat([r["candidates"] for r in tiles])[rows_h])
+    return res
+
+
 def masks_to_bool(result: dict) -> torch.Tensor:
     """The bit-packed ``masks`` of one generate_masks result -> bool [k, H, W] on the same device."""
     bits = result["masks"]
@@ -368,18 +549,26 @@ def masks_to_bool(result: dict) -> torch.Tensor:
 
 def mask_dicts(result: dict) -> list:
     """The result of one image as JSON-ready dicts: COCO RLE ``segmentation`` (needs output_rle_mask=True), xywh
-    ``bbox`` from the inclusive box, ``predicted_iou``, ``stability_score``, ``point_coords`` [[x, y]]."""
+    ``bbox`` from the inclusive box, ``predicted_iou``, ``stability_score``, ``point_coords`` [[x, y]], and for a
+    generate_scene_masks result the window's ``crop_box`` (xywh, as SAM's automatic mask generator writes it)."""
     out = []
-    for rle, (x1, y1, x2, y2), s, st, pt in zip(result["rle"], result["boxes"].tolist(), result["scores"].tolist(),
-                                               result["stability_scores"].tolist(), result["points"].tolist()):
-        out.append(dict(segmentation=dict(size=rle["size"], counts=rle["counts"].decode()),
-                        bbox=[x1, y1, x2 - x1, y2 - y1], predicted_iou=s, stability_score=st, point_coords=[pt]))
+    crops = result["crop_boxes"].tolist() if "crop_boxes" in result else None
+    for i, (rle, (x1, y1, x2, y2), s, st, pt) in enumerate(zip(
+            result["rle"], result["boxes"].tolist(), result["scores"].tolist(), result["stability_scores"].tolist(),
+            result["points"].tolist())):
+        row = dict(segmentation=dict(size=rle["size"], counts=rle["counts"].decode()),
+                   bbox=[x1, y1, x2 - x1, y2 - y1], predicted_iou=s, stability_score=st, point_coords=[pt])
+        if crops is not None:
+            cx0, cy0, cx1, cy1 = crops[i]
+            row["crop_box"] = [cx0, cy0, cx1 - cx0, cy1 - cy0]
+        out.append(row)
     return out
 
 
 def main(argv=None) -> list:
     ap = argparse.ArgumentParser(description="Segment everything in one image with SAM (HF mask-generation, one crop "
-                                             "layer) and write the masks as COCO RLE")
+                                             "layer) and write the masks as COCO RLE; with --patch-size, in a whole "
+                                             "scene cut into overlapping windows")
     ap.add_argument("image")
     ap.add_argument("--arch", required=True, choices=["base", "large", "huge"])
     ap.add_argument("--checkpoint", required=True, help="HF SamModel weights (.pth / .bin or .safetensors)")
@@ -392,6 +581,13 @@ def main(argv=None) -> list:
     ap.add_argument("--crops-nms-thresh", type=float, default=0.7)
     ap.add_argument("--min-mask-region-area", type=float, default=0.0,
                     help="fill holes and remove islands smaller than this many pixels (SAM's min_mask_region_area)")
+    ap.add_argument("--patch-size", type=int, default=None,
+                    help="scene mode: segment P x P windows of the image and merge them across windows, masks of the "
+                         "whole image (each window is resized to the model size).  A mask is kept only from a window "
+                         "where its box is more than 20 px from every interior window edge, so objects wider than "
+                         "about int(overlap * P) - 42 px may be missed")
+    ap.add_argument("--patch-overlap-ratio", type=float, default=0.25, help="scene mode: window overlap ratio")
+    ap.add_argument("--batch-size", type=int, default=4, help="scene mode: windows run at once")
     ap.add_argument("--out", default=None, help="JSON file for the mask dicts (default: stdout)")
     args = ap.parse_args(argv)
 
@@ -403,13 +599,17 @@ def main(argv=None) -> list:
     img = cv2.imread(args.image, cv2.IMREAD_COLOR)
     if img is None:
         raise FileNotFoundError(args.image)
-    rgb = torch.from_numpy(img).permute(2, 0, 1).flip(0)                 # BGR HWC -> RGB [3, H, W] view
-    res = generate_masks(model, rgb.contiguous(), points_per_side=args.points_per_side,
-                         points_per_batch=args.points_per_batch, pred_iou_thresh=args.pred_iou_thresh,
-                         stability_score_thresh=args.stability_score_thresh,
-                         stability_score_offset=args.stability_score_offset, mask_threshold=args.mask_threshold,
-                         crops_nms_thresh=args.crops_nms_thresh, min_mask_region_area=args.min_mask_region_area,
-                         output_rle_mask=True)[0]
+    kw = dict(points_per_side=args.points_per_side, points_per_batch=args.points_per_batch,
+              pred_iou_thresh=args.pred_iou_thresh, stability_score_thresh=args.stability_score_thresh,
+              stability_score_offset=args.stability_score_offset, mask_threshold=args.mask_threshold,
+              crops_nms_thresh=args.crops_nms_thresh, min_mask_region_area=args.min_mask_region_area)
+    if args.patch_size is not None:
+        rgb = torch.from_numpy(cv2.cvtColor(img, cv2.COLOR_BGR2RGB)).permute(2, 0, 1)      # [3, H, W] view of HWC
+        res = generate_scene_masks(model, rgb, patch_size=args.patch_size, overlap_ratio=args.patch_overlap_ratio,
+                                   batch_size=args.batch_size, **kw)
+    else:
+        rgb = torch.from_numpy(img).permute(2, 0, 1).flip(0)                 # BGR HWC -> RGB [3, H, W] view
+        res = generate_masks(model, rgb.contiguous(), output_rle_mask=True, **kw)[0]
     rows = mask_dicts(res)
     text = json.dumps(rows)
     if args.out:

@@ -266,6 +266,11 @@ class RSSamModel(BaseModule):
         from .mask_generation import generate_masks
         return generate_masks(self, images, **kwargs)
 
+    def generate_scene_masks(self, scene, **kwargs) -> dict:
+        """Segment everything in a whole scene, window by window (see mask_generation.generate_scene_masks)."""
+        from .mask_generation import generate_scene_masks
+        return generate_scene_masks(self, scene, **kwargs)
+
 
 @MODELS.register_module(force=True)
 class SAMDet(BaseModule):
