@@ -402,6 +402,34 @@ int rsp_query_postprocess_rescale_bits(const float* logits, const int32_t* sel, 
                                        int Wr, uint8_t* bits, float* part_ws, float* scores, float* boxes,
                                        void* stream);
 
+/* Panoptic post-processing of the query variants: MaskFormerFusionHead.panoptic_postprocess
+ * (mmdet/models/seg_heads/panoptic_fusion_heads/maskformer_fusion_head.py:41-106) after the resize of
+ * RSMaskFormerFusionHead.predict (M:663-715; M:652-656 up-sampling), for n_img images of nq queries each, with no host
+ * read.  Per image i, over the queries q with keep[i*nq+q] (softmax max score > object_mask_thr, label != num_classes,
+ * computed by the caller), in ascending q:
+ *   sig = 1 / (1 + expf(-v)) of the resized logit v, prob = scores[i*nq+q] * sig; per pixel the argmax of prob (the
+ *   lowest q on ties); mask_area = #(argmax == q), original_area = #(sig >= 0.5); q is skipped unless both are > 0 and
+ *   (double) mask_area / original_area >= *iou_thr; a stuff label (>= num_things) writes the label, a thing writes
+ *   label + 1000 * instance_id (instance_id from 1, advancing on written things); with filter_low_score only pixels
+ *   with sig >= 0.5 of their argmax query are written.  Every other pixel is num_classes.
+ * logits fp32 [n_img*nq, hm, wm]; keep uint8 / scores fp32 / labels int32 [n_img*nq]; iou_thr: a HOST pointer to one
+ * double (Python's float).  Workspaces: idx_ws uint16 [n_img, H*W], bits_ws uint32 [n_img, ceil(H*W/32)].  Outputs:
+ * areas int32 [2, n_img*nq] (mask_area, then original_area; 0 for queries not kept), seg int32 [n_img*nq] (the segment
+ * id of q, -1 when skipped or not kept), pan int32 [n_img, H, W].  nq < 65535, num_classes < 1000.
+ * This entry point: one bilinear resize (hm, wm) -> (H, W) (the batch shape). */
+int rsp_panoptic_postprocess(const float* logits, const uint8_t* keep, const float* scores, const int32_t* labels,
+                             int n_img, int nq, int hm, int wm, int H, int W, int num_things, int num_classes,
+                             const double* iou_thr, int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws,
+                             int32_t* areas, int32_t* seg, int32_t* pan, void* stream);
+
+/* rsp_panoptic_postprocess through the two resizes of a resized / padded image (M:652-656 + 679-691): logits ->
+ * (Hb, Wb) -> crop [:crop_h, :crop_w] -> (H, W) (ori_shape with rescale, the crop itself without). */
+int rsp_panoptic_postprocess_rescale(const float* logits, const uint8_t* keep, const float* scores,
+                                     const int32_t* labels, int n_img, int nq, int hm, int wm, int Hb, int Wb,
+                                     int crop_h, int crop_w, int H, int W, int num_things, int num_classes,
+                                     const double* iou_thr, int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws,
+                                     int32_t* areas, int32_t* seg, int32_t* pan, void* stream);
+
 /* SAM automatic mask generation, per candidate mask, without the original-size fp32 mask ever existing.  Replaces, for
  * one crop layer, HF SamImageProcessor.post_process_masks(binarize=False) (image_processing_sam.py:423-425) followed by
  * filter_masks (:350-363): iou_scores > pred_iou_thresh, _compute_stability_score (:449-457), masks > mask_threshold and

@@ -6,7 +6,7 @@ reference's ``custom_imports=['mmdet.rsprompter']`` (configs/rsprompter/_base_/r
 The CUDA extension (``librsp_b200.so``) is mandatory: there is no CPU or eager fallback.
 """
 from . import _lib  # noqa: F401  (fails loudly when the extension is missing)
-from .registry import MODELS, BaseModule, Config, ConfigDict, DetDataSample, InstanceData  # noqa: F401
+from .registry import MODELS, BaseModule, Config, ConfigDict, DetDataSample, InstanceData, PixelData  # noqa: F401
 from . import sam_encoder  # noqa: F401
 
 __version__ = "0.1.0"

@@ -124,6 +124,10 @@ _SIGNATURES = {
     "rsp_sam_mask_stats_crop": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _i, _i, _i, _i, _i,
                                  _i, _vp, _vp, _vp, _vp, _vp, _vp], _i),
     "rsp_mask_small_regions_bits": ([_vp, _vp, _i, _i, _i, _i, ctypes.c_longlong, _i, _vp, _vp, _vp, _vp], _i),
+    "rsp_panoptic_postprocess": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp,
+                                  _vp], _i),
+    "rsp_panoptic_postprocess_rescale": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i,
+                                          _vp, _vp, _vp, _vp, _vp, _vp], _i),
 }
 
 
@@ -1229,6 +1233,60 @@ def query_postprocess(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch
                "rsp_query_postprocess_rescale_bits")
     launch_count += 2
     return (masks.view(torch.bool) if bits is None else bits), scores, boxes
+
+
+PANOPTIC_INSTANCE_OFFSET = 1000      # mmdet.evaluation.functional.INSTANCE_OFFSET
+
+
+def check_panoptic_bounds(nq: int, num_classes: int) -> None:
+    """ValueError unless the panoptic kernels can represent the result: query indices in uint16 (one value left for
+    "no kept query"), labels below INSTANCE_OFFSET, and every segment id (label + instance_id * 1000) in int32."""
+    if not 0 < nq <= 65535:
+        raise ValueError(f"panoptic post-processing takes 1 to 65535 queries per image, got {nq}")
+    if not 0 < num_classes < PANOPTIC_INSTANCE_OFFSET:
+        raise ValueError(f"panoptic segment ids hold labels below {PANOPTIC_INSTANCE_OFFSET}, got num_classes "
+                         f"{num_classes}")
+    if nq * PANOPTIC_INSTANCE_OFFSET + num_classes > 2 ** 31 - 1:
+        raise ValueError(f"panoptic segment ids of {nq} queries do not fit in int32")
+
+
+def panoptic_postprocess(logits: torch.Tensor, keep: torch.Tensor, scores: torch.Tensor, labels: torch.Tensor,
+                         num_things: int, num_classes: int, iou_thr: float, filter_low_score: bool,
+                         size: tuple | None = None, *, rescale: tuple | None = None):
+    """MaskFormerFusionHead.panoptic_postprocess (maskformer_fusion_head.py:41-106) of B images on the device, with no
+    host read.  logits fp32 [B*nq, hm, wm] low-res mask logits; keep bool [B, nq]; scores fp32 / labels int [B, nq]
+    (softmax max and argmax of the class logits); size = (H, W): one bilinear resize; rescale = (batch_hw, crop_hw,
+    out_hw): to batch_hw -> crop -> to out_hw (M:652-656 + 679-691).  -> (pan int32 [B, 1, H, W], dict(mask_area,
+    original_area, segment_id) int32 [B, nq]: the per-query counts and written ids, 0 / 0 / -1 for queries not kept)."""
+    global launch_count
+    B, nq = keep.shape
+    check_panoptic_bounds(nq, num_classes)
+    assert (size is None) != (rescale is None)
+    _require_cuda(logits, keep, scores, labels)
+    assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.shape[0] == B * nq
+    _, hm, wm = logits.shape
+    H, W = size if rescale is None else rescale[2]
+    dev = logits.device
+    keep = keep.to(torch.uint8).contiguous()
+    scores = scores.to(torch.float32).contiguous()
+    labels = labels.to(torch.int32).contiguous()
+    idx = torch.empty(B, H * W, device=dev, dtype=torch.int16)
+    bits = torch.empty(B, (H * W + 31) // 32, device=dev, dtype=torch.int32)
+    areas = torch.empty(2, B, nq, device=dev, dtype=torch.int32)
+    seg = torch.empty(B, nq, device=dev, dtype=torch.int32)
+    pan = torch.empty(B, 1, H, W, device=dev, dtype=torch.int32)
+    thr = ctypes.c_double(float(iou_thr))
+    head = (_ptr(logits), _ptr(keep), _ptr(scores), _ptr(labels), B, nq, hm, wm)
+    tail = (int(num_things), int(num_classes), ctypes.addressof(thr), int(bool(filter_low_score)), _ptr(idx), _ptr(bits),
+            _ptr(areas), _ptr(seg), _ptr(pan), _stream())
+    if rescale is None:
+        _check(_lib.rsp_panoptic_postprocess(*head, H, W, *tail), "rsp_panoptic_postprocess")
+    else:
+        (Hb, Wb), (ch, cw), _ = rescale
+        _check(_lib.rsp_panoptic_postprocess_rescale(*head, Hb, Wb, ch, cw, H, W, *tail),
+               "rsp_panoptic_postprocess_rescale")
+    launch_count += 3
+    return pan, dict(mask_area=areas[0], original_area=areas[1], segment_id=seg)
 
 
 # ------------------------------------------------------------------------------ result-record payload

@@ -384,6 +384,24 @@ int rsp_query_postprocess_rescale_bits(const float* logits, const int32_t* sel, 
                                         bits, part_ws, scores, boxes, S(stream));
 }
 
+int rsp_panoptic_postprocess(const float* logits, const uint8_t* keep, const float* scores, const int32_t* labels,
+                             int n_img, int nq, int hm, int wm, int H, int W, int num_things, int num_classes,
+                             const double* iou_thr, int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws,
+                             int32_t* areas, int32_t* seg, int32_t* pan, void* stream) {
+  return panoptic_postprocess(logits, keep, scores, labels, n_img, nq, hm, wm, H, W, num_things, num_classes, iou_thr,
+                              filter_low_score, idx_ws, bits_ws, areas, seg, pan, S(stream));
+}
+
+int rsp_panoptic_postprocess_rescale(const float* logits, const uint8_t* keep, const float* scores,
+                                     const int32_t* labels, int n_img, int nq, int hm, int wm, int Hb, int Wb,
+                                     int crop_h, int crop_w, int H, int W, int num_things, int num_classes,
+                                     const double* iou_thr, int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws,
+                                     int32_t* areas, int32_t* seg, int32_t* pan, void* stream) {
+  return panoptic_postprocess_rescale(logits, keep, scores, labels, n_img, nq, hm, wm, Hb, Wb, crop_h, crop_w, H, W,
+                                      num_things, num_classes, iou_thr, filter_low_score, idx_ws, bits_ws, areas, seg,
+                                      pan, S(stream));
+}
+
 int rsp_sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
                        float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
                        float stability_score_thresh, int32_t* part_ws, int32_t* counts, int32_t* boxes,

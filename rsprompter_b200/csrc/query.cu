@@ -1050,4 +1050,188 @@ int query_postprocess_rescale_bits(const float* logits, const int* sel, const fl
   return query_px<1, true>(s, sel, cls_scores, n_inst, H, W, Hr, Wr, bits, part_ws, scores, boxes, stream);
 }
 
+// ------------------------------------------------------------------------------------ panoptic post-process
+// MaskFormerFusionHead.panoptic_postprocess (maskformer_fusion_head.py:41-106) for every image of a batch, in three
+// passes with no host read between them (the reference reads two counts per kept query back to the host):
+//   argmax  per pixel, argmax over the kept queries of score * sigmoid(logit) (first query on ties, as torch.argmax),
+//           the query index as uint16 (PAN_NONE: nothing kept), one bit for sigmoid(best) >= 0.5, and per query the
+//           integer counts original_area (sigmoid >= 0.5) and mask_area (argmax == q)
+//   decide  per image, the kept queries in order: skip, or the segment id (instance ids advance on written things)
+//   write   the int32 map from the index map, the bit and the segment ids
+// Queries are addressed by their index: the kept queries in kept order are the kept indices in ascending order.
+constexpr int PAN_THREADS = 256, PAN_PPT = 8;
+constexpr int PAN_TILE = PAN_THREADS * PAN_PPT;   // a block's pixels: PAN_TILE consecutive pixels in raster order
+constexpr int PAN_CHUNK = 2048;                   // queries per round of block-local counts
+constexpr int PAN_NONE = 0xffff;
+constexpr int PAN_INSTANCE_OFFSET = 1000;         // mmdet.evaluation.functional.INSTANCE_OFFSET
+
+// adds `one` of the calling lane to counter s_cnt[key - c0] for keys in [c0, c1), one shared atomic per distinct key
+__device__ __forceinline__ void pan_count(int* s_cnt, int key, int c0, int c1) {
+  const bool in = key >= c0 && key < c1;
+  const unsigned act = __ballot_sync(0xffffffffu, in);
+  if (!in) return;
+  const unsigned peers = __match_any_sync(act, key);
+  if ((threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&s_cnt[key - c0], __popc(peers));
+}
+
+// grid (ceil(H*W / PAN_TILE), images); sampler map index = image * nq + query.  areas: mask_area [images, nq] then
+// original_area [images, nq], zeroed by the caller; the integer sums do not depend on the order of the atomics.
+template <class Sampler>
+__global__ void __launch_bounds__(PAN_THREADS)
+panoptic_argmax_kernel(Sampler s, const uint8_t* __restrict__ keep, const float* __restrict__ scores, int nq, int H,
+                       int W, uint16_t* __restrict__ idx, uint32_t* __restrict__ bits, int* __restrict__ mask_area,
+                       int* __restrict__ orig_area) {
+  __shared__ int s_cnt[PAN_CHUNK];
+  const int img = blockIdx.y, lane = threadIdx.x & 31;
+  const int HW = H * W;
+  const int p0 = blockIdx.x * PAN_TILE;
+  int py[PAN_PPT], px[PAN_PPT], bi[PAN_PPT];
+  float best[PAN_PPT];
+#pragma unroll
+  for (int j = 0; j < PAN_PPT; ++j) {
+    const int p = p0 + j * PAN_THREADS + threadIdx.x;
+    py[j] = p < HW ? p / W : -1;
+    px[j] = p - (p / W) * W;
+    best[j] = -1.f;                 // every prob is >= 0: the first kept query takes the pixel
+    bi[j] = PAN_NONE;               // bit 16: sigmoid(best) >= 0.5
+  }
+  const uint8_t* kp = keep + static_cast<size_t>(img) * nq;
+  const float* sp = scores + static_cast<size_t>(img) * nq;
+  for (int c0 = 0; c0 < nq; c0 += PAN_CHUNK) {
+    const int c1 = min(nq, c0 + PAN_CHUNK);
+    for (int i = threadIdx.x; i < c1 - c0; i += PAN_THREADS) s_cnt[i] = 0;
+    __syncthreads();
+    for (int q = c0; q < c1; ++q) {
+      if (!kp[q]) continue;
+      const float sc = sp[q];
+      const int m = img * nq + q;
+      int cnt = 0;
+#pragma unroll
+      for (int j = 0; j < PAN_PPT; ++j) {
+        if (py[j] < 0) continue;
+        s.row(m, py[j]);
+        const float sig = 1.f / (1.f + expf(-s.at(px[j])));      // torch's CUDA sigmoid
+        const float prob = __fmul_rn(sc, sig);
+        const bool on = sig >= 0.5f;
+        cnt += on;
+        if (prob > best[j]) { best[j] = prob; bi[j] = q | (on ? 0x10000 : 0); }
+      }
+      cnt = __reduce_add_sync(0xffffffffu, cnt);
+      if (lane == 0 && cnt) atomicAdd(&s_cnt[q - c0], cnt);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < c1 - c0; i += PAN_THREADS)
+      if (s_cnt[i]) atomicAdd(&orig_area[static_cast<size_t>(img) * nq + c0 + i], s_cnt[i]);
+    __syncthreads();
+  }
+  for (int c0 = 0; c0 < nq; c0 += PAN_CHUNK) {
+    const int c1 = min(nq, c0 + PAN_CHUNK);
+    for (int i = threadIdx.x; i < c1 - c0; i += PAN_THREADS) s_cnt[i] = 0;
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < PAN_PPT; ++j) pan_count(s_cnt, py[j] < 0 ? -1 : bi[j] & 0xffff, c0, c1);
+    __syncthreads();
+    for (int i = threadIdx.x; i < c1 - c0; i += PAN_THREADS)
+      if (s_cnt[i]) atomicAdd(&mask_area[static_cast<size_t>(img) * nq + c0 + i], s_cnt[i]);
+    __syncthreads();
+  }
+  const size_t base = static_cast<size_t>(img) * HW;
+  const size_t wbase = static_cast<size_t>(img) * ((HW + 31) / 32);
+#pragma unroll
+  for (int j = 0; j < PAN_PPT; ++j) {
+    const int p = p0 + j * PAN_THREADS + threadIdx.x;
+    if (p < HW) idx[base + p] = static_cast<uint16_t>(bi[j] & 0xffff);
+    const unsigned word = __ballot_sync(0xffffffffu, p < HW && (bi[j] >> 16));
+    if (lane == 0 && p < HW) bits[wbase + p / 32] = word;     // p % 32 == 0: the warp's 32 pixels are one word
+  }
+}
+
+// one thread per image: maskformer_fusion_head.py:83-104 over the kept queries in order.  seg[q]: the segment id
+// written where the argmax is q, or -1 (skipped or not kept: those pixels keep num_classes).
+__global__ void panoptic_decide_kernel(const uint8_t* __restrict__ keep, const int* __restrict__ labels,
+                                       const int* __restrict__ mask_area, const int* __restrict__ orig_area, int n_img,
+                                       int nq, int num_things, double iou_thr, int* __restrict__ seg) {
+  const int img = blockIdx.x * blockDim.x + threadIdx.x;
+  if (img >= n_img) return;
+  int instance_id = 1;
+  for (int q = 0; q < nq; ++q) {
+    const size_t i = static_cast<size_t>(img) * nq + q;
+    int v = -1;
+    const int ma = mask_area[i], oa = orig_area[i];
+    // Python's true division of the two counts (correctly rounded double) against the float threshold
+    if (keep[i] && ma > 0 && oa > 0 && !(static_cast<double>(ma) / static_cast<double>(oa) < iou_thr)) {
+      const int label = labels[i];
+      v = label < num_things ? label + instance_id++ * PAN_INSTANCE_OFFSET : label;
+    }
+    seg[i] = v;
+  }
+}
+
+// grid (ceil(H*W / 256), images): pan = seg[argmax] where it is not -1 (and, with filter_low_score, where
+// sigmoid(best) >= 0.5), num_classes everywhere else
+__global__ void panoptic_write_kernel(const uint16_t* __restrict__ idx, const uint32_t* __restrict__ bits,
+                                      const int* __restrict__ seg, int nq, int HW, int num_classes, int filter_low_score,
+                                      int* __restrict__ pan) {
+  const int img = blockIdx.y;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= HW) return;
+  const size_t o = static_cast<size_t>(img) * HW + p;
+  const int k = idx[o];
+  int v = num_classes;
+  if (k != PAN_NONE) {
+    const int sv = seg[static_cast<size_t>(img) * nq + k];
+    const bool on = (bits[static_cast<size_t>(img) * ((HW + 31) / 32) + p / 32] >> (p & 31)) & 1u;
+    if (sv >= 0 && (!filter_low_score || on)) v = sv;
+  }
+  pan[o] = v;
+}
+
+template <class Sampler>
+static int panoptic_run(const Sampler& s, const uint8_t* keep, const float* scores, const int* labels, int n_img,
+                        int nq, int H, int W, int num_things, int num_classes, double iou_thr, int filter_low_score,
+                        uint16_t* idx_ws, uint32_t* bits_ws, int* areas, int* seg, int* pan, cudaStream_t stream) {
+  const int HW = H * W;
+  const size_t n = static_cast<size_t>(n_img) * nq;
+  RSP_CHECK_CUDA(cudaMemsetAsync(areas, 0, 2 * n * sizeof(int), stream));
+  panoptic_argmax_kernel<Sampler><<<dim3((HW + PAN_TILE - 1) / PAN_TILE, n_img), PAN_THREADS, 0, stream>>>(
+      s, keep, scores, nq, H, W, idx_ws, bits_ws, areas, areas + n);
+  RSP_CHECK_LAUNCH();
+  panoptic_decide_kernel<<<(n_img + 31) / 32, 32, 0, stream>>>(keep, labels, areas, areas + n, n_img, nq, num_things,
+                                                              iou_thr, seg);
+  RSP_CHECK_LAUNCH();
+  panoptic_write_kernel<<<dim3((HW + 255) / 256, n_img), 256, 0, stream>>>(idx_ws, bits_ws, seg, nq, HW, num_classes,
+                                                                          filter_low_score, pan);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
+#define RSP_PANOPTIC_ARGS_OK                                                                                          \
+  (logits && keep && scores && labels && idx_ws && bits_ws && areas && seg && pan && n_img > 0 && n_img <= 65535 &&     \
+   nq > 0 && nq < PAN_NONE && hm > 0 && wm > 0 && H > 0 && W > 0 &&                                                     \
+   static_cast<long long>(H) * W <= 0x7fffffffLL - PAN_TILE && num_things >= 0 && num_things <= num_classes &&      \
+   num_classes < PAN_INSTANCE_OFFSET &&                                                                              \
+   static_cast<long long>(nq) * PAN_INSTANCE_OFFSET + num_classes <= 0x7fffffffLL && iou_thr)
+
+int panoptic_postprocess(const float* logits, const uint8_t* keep, const float* scores, const int* labels, int n_img,
+                         int nq, int hm, int wm, int H, int W, int num_things, int num_classes, const double* iou_thr,
+                         int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws, int* areas, int* seg, int* pan,
+                         cudaStream_t stream) {
+  RSP_CHECK_ARG(RSP_PANOPTIC_ARGS_OK, "panoptic_postprocess: bad args (nq < 65535, num_classes < 1000)");
+  return panoptic_run(OneResize<false, true>{logits, hm, wm, H, W}, keep, scores, labels, n_img, nq, H, W, num_things,
+                      num_classes, *iou_thr, filter_low_score, idx_ws, bits_ws, areas, seg, pan, stream);
+}
+
+int panoptic_postprocess_rescale(const float* logits, const uint8_t* keep, const float* scores, const int* labels,
+                                 int n_img, int nq, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                                 int num_things, int num_classes, const double* iou_thr, int filter_low_score,
+                                 uint16_t* idx_ws, uint32_t* bits_ws, int* areas, int* seg, int* pan,
+                                 cudaStream_t stream) {
+  RSP_CHECK_ARG(RSP_PANOPTIC_ARGS_OK && crop_h > 0 && crop_w > 0 && crop_h <= Hb && crop_w <= Wb,
+                "panoptic_postprocess_rescale: bad args (nq < 65535, num_classes < 1000, crop within the batch shape)");
+  const TwoResizes s{logits, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
+  return panoptic_run(s, keep, scores, labels, n_img, nq, H, W, num_things, num_classes, *iou_thr, filter_low_score,
+                      idx_ws, bits_ws, areas, seg, pan, stream);
+}
+#undef RSP_PANOPTIC_ARGS_OK
+
 }  // namespace rsp

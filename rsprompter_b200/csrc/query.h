@@ -27,5 +27,14 @@ int query_postprocess_rescale_bits(const float* logits, const int* sel, const fl
                                    int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr, int Wr,
                                    unsigned char* bits, float* part_ws, float* scores, float* boxes,
                                    cudaStream_t stream);
+int panoptic_postprocess(const float* logits, const uint8_t* keep, const float* scores, const int* labels, int n_img,
+                         int nq, int hm, int wm, int H, int W, int num_things, int num_classes, const double* iou_thr,
+                         int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws, int* areas, int* seg, int* pan,
+                         cudaStream_t stream);
+int panoptic_postprocess_rescale(const float* logits, const uint8_t* keep, const float* scores, const int* labels,
+                                 int n_img, int nq, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                                 int num_things, int num_classes, const double* iou_thr, int filter_low_score,
+                                 uint16_t* idx_ws, uint32_t* bits_ws, int* areas, int* seg, int* pan,
+                                 cudaStream_t stream);
 
 }  // namespace rsp

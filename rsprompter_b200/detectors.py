@@ -3,7 +3,9 @@
 ``predict(batch_inputs, batch_data_samples, rescale=True)`` keeps the reference contract
 (mmdet BaseDetector.forward mode='predict', detectors/base.py:58-99): it returns the data samples
 with ``pred_instances`` holding ``bboxes``, ``scores``, ``labels`` and boolean ``masks`` (COCO RLE dicts with
-``test_cfg.rle_masks``).
+``test_cfg.rle_masks``).  The query detectors follow ``test_cfg``'s ``instance_on`` / ``panoptic_on`` flags as the
+reference does: ``panoptic_on`` (default True) adds ``pred_panoptic_seg`` (a ``PixelData`` with an int32 ``sem_seg``
+[1, H, W]); ``pred_instances`` is set only with ``instance_on``.
 Everything between the input tensor and the final per-image split runs on the device without
 host synchronisation; the one device->host read is the per-image detection count.
 """
@@ -13,7 +15,7 @@ import torch
 
 from . import _lib
 from .necks import PseudoFeatureAggregator
-from .registry import MODELS, BaseModule, ConfigDict, DetDataSample, InstanceData, make_data_samples
+from .registry import MODELS, BaseModule, ConfigDict, DetDataSample, InstanceData, PixelData, make_data_samples
 from .results import ResultRecord, encode_mask_results
 from .sam_encoder import MMPretrainSamVisionEncoder, SamVisionEncoderOutput
 
@@ -195,7 +197,9 @@ class _SamDetectorBase(BaseModule):
         non-tensor masks through (coco_metric.py:364-367), so evaluation copies no mask pixel to the host."""
         if test_cfg is None or not test_cfg.get("rle_masks", False):
             return batch_data_samples
-        insts = [ds.pred_instances for ds in batch_data_samples]
+        insts = [ds.pred_instances for ds in batch_data_samples if "pred_instances" in ds]
+        if not insts:           # panoptic-only results
+            return batch_data_samples
         for inst, rles in zip(insts, encode_mask_results([inst.masks for inst in insts])):
             inst.masks = rles
         return batch_data_samples
@@ -346,18 +350,28 @@ class RSPrompterQuery(_SamDetectorBase):
         if batch_data_samples is None:
             batch_data_samples = make_data_samples(batch_inputs.shape[0], tuple(batch_inputs.shape[-2:]))
         hw, metas = self._metas(batch_data_samples, batch_inputs)
-        if self.test_cfg.get("panoptic_on", True) or self.test_cfg.get("semantic_on", False):
-            raise NotImplementedError("rsprompter_b200 implements instance_on post-processing (every RSPrompter config)")
+        # M:672-676 / maskformer_fusion_head.py:226-230 defaults; MaskFormer.add_pred_to_datasample (maskformer.py:142-148)
+        if self.test_cfg.get("semantic_on", False):
+            raise NotImplementedError("semantic segmentation results are not supported (as in the reference)")
+        panoptic_on, instance_on = self.test_cfg.get("panoptic_on", True), self.test_cfg.get("instance_on", False)
+        if panoptic_on:
+            _lib.check_panoptic_bounds(self.panoptic_head.num_queries, self.panoptic_fusion_head.num_classes)
         r = self._raw(batch_inputs)
-        out = self.panoptic_fusion_head.instance_postprocess_batched(r["cls"], r["mask_logits"], hw, metas=metas,
-                                                                     rescale=rescale)
-        stuff = self.panoptic_fusion_head.num_stuff_classes > 0
-        for b, ds in enumerate(batch_data_samples):
-            inst = dict(bboxes=out["bboxes"][b], scores=out["scores"][b], labels=out["labels"][b], masks=out["masks"][b])
-            if stuff:                                   # maskformer_fusion_head.py:160-164 (data-dependent size)
-                k = out["is_thing"][b]
-                inst = {n: v[k] for n, v in inst.items()}
-            ds.pred_instances = InstanceData(**inst)
+        head = self.panoptic_fusion_head
+        if instance_on:
+            out = head.instance_postprocess_batched(r["cls"], r["mask_logits"], hw, metas=metas, rescale=rescale)
+            stuff = head.num_stuff_classes > 0
+            for b, ds in enumerate(batch_data_samples):
+                inst = dict(bboxes=out["bboxes"][b], scores=out["scores"][b], labels=out["labels"][b],
+                            masks=out["masks"][b])
+                if stuff:                                   # maskformer_fusion_head.py:160-164 (data-dependent size)
+                    k = out["is_thing"][b]
+                    inst = {n: v[k] for n, v in inst.items()}
+                ds.pred_instances = InstanceData(**inst)
+        if panoptic_on:
+            pans, _ = head.panoptic_postprocess_batched(r["cls"], r["mask_logits"], hw, metas=metas, rescale=rescale)
+            for ds, pan in zip(batch_data_samples, pans):
+                ds.pred_panoptic_seg = PixelData(sem_seg=pan)
         return self._rle_masks(self.test_cfg, batch_data_samples)
 
     @torch.no_grad()

@@ -405,7 +405,8 @@ class RSMask2FormerHead(_PrepMixin, BaseModule):
 
 @MODELS.register_module(force=True)
 class RSMaskFormerFusionHead(BaseModule):
-    """M:661-715 + MaskFormerFusionHead.instance_postprocess (maskformer_fusion_head.py:126-182)."""
+    """M:661-715 + MaskFormerFusionHead.instance_postprocess / panoptic_postprocess (maskformer_fusion_head.py:126-182,
+    41-106)."""
 
     def __init__(self, num_things_classes=80, num_stuff_classes=0, test_cfg=None, loss_panoptic=None, init_cfg=None,
                  **kwargs):
@@ -440,6 +441,34 @@ class RSMaskFormerFusionHead(BaseModule):
             mk, det, bx = _lib.query_postprocess(mask_pred, sel[b].contiguous(), sc[b].contiguous(), **geom)
             ms.append(mk); ds.append(det); bs.append(bx)
         return dict(masks=ms, scores=ds, bboxes=bs, labels=labels, query=query, is_thing=keep_thing)
+
+    @torch.no_grad()
+    def panoptic_postprocess_batched(self, cls: torch.Tensor, mask_pred: torch.Tensor, size: tuple,
+                                     metas: list | None = None, rescale: bool = True):
+        """MaskFormerFusionHead.panoptic_postprocess (maskformer_fusion_head.py:41-106) of every image, on the masks
+        instance_postprocess_batched resamples (M:652-656 up-sampling, M:679-691 crop / rescale), with no host read.
+        cls fp32 [B, nq, C+1]; mask_pred fp32 [B*nq, hm, wm] low-res logits -> (per-image int32 [1, H, W] maps,
+        per-image dicts of the per-query mask_area / original_area / segment_id, int32 [nq])."""
+        B, nq, _ = cls.shape
+        _lib.check_panoptic_bounds(nq, self.num_classes)
+        cfg = self.test_cfg
+        thr = float(cfg.get("object_mask_thr", 0.8))
+        args = (self.num_things_classes, self.num_classes, float(cfg.get("iou_thr", 0.8)),
+                bool(cfg.get("filter_low_score", False)))
+        scores, labels = torch.softmax(cls, dim=-1).max(-1)
+        keep = labels.ne(self.num_classes) & (scores > thr)
+        if metas is None or all(m is None for m in metas):
+            pan, st = _lib.panoptic_postprocess(mask_pred, keep, scores, labels, *args, size=size)
+            return list(pan), [{k: v[b] for k, v in st.items()} for b in range(B)]
+        pans, stats = [], []
+        for b, m in enumerate(metas):      # image sizes differ: one launch triple per image, no host sync
+            geom = dict(size=size) if m is None else \
+                dict(rescale=(size, m["crop_hw"], m["ori_hw"] if rescale else m["crop_hw"]))
+            pan, st = _lib.panoptic_postprocess(mask_pred[b * nq:(b + 1) * nq], keep[b:b + 1], scores[b:b + 1],
+                                                labels[b:b + 1], *args, **geom)
+            pans.append(pan[0])
+            stats.append({k: v[0] for k, v in st.items()})
+        return pans, stats
 
     @torch.no_grad()
     def instance_postprocess_record(self, cls: torch.Tensor, mask_pred: torch.Tensor, rec, metas: list | None = None,
@@ -606,7 +635,8 @@ class Mask2FormerHead(_PrepMixin, BaseModule):
 @MODELS.register_module(force=True)
 class MaskFormerFusionHead(RSMaskFormerFusionHead):
     """seg_heads/panoptic_fusion_heads/maskformer_fusion_head.py (this repository's copy crops with the scaled original
-    size exactly as M:679-691 does, :239-252): instance_on post-processing shared with RSMaskFormerFusionHead."""
+    size exactly as M:679-691 does, :239-252): instance and panoptic post-processing shared with
+    RSMaskFormerFusionHead."""
 
 
 __all__ = ["MSDeformAttnPixelDecoder", "RSMask2FormerHead", "RSMaskFormerFusionHead", "Mask2FormerHead",

@@ -22,7 +22,7 @@ from torch import nn
 try:  # pragma: no cover - not available in this image
     from mmengine.config import Config, ConfigDict  # type: ignore
     from mmengine.model import BaseModule  # type: ignore
-    from mmengine.structures import InstanceData  # type: ignore
+    from mmengine.structures import InstanceData, PixelData  # type: ignore
     from mmdet.registry import MODELS as _MMDET_MODELS  # type: ignore
     from mmdet.structures import DetDataSample  # type: ignore
     HAVE_MMENGINE = True
@@ -292,6 +292,46 @@ if not HAVE_MMENGINE:
         def cpu(self) -> "InstanceData":
             return self.to("cpu")
 
+    class PixelData:
+        """Per-image pixel-map container (mmengine.structures.PixelData work-alike): attribute fields holding
+        [C, H, W] tensors (``pred_panoptic_seg.sem_seg``), ``.to`` / ``.cpu``."""
+
+        def __init__(self, metainfo: dict | None = None, **fields: Any):
+            object.__setattr__(self, "_fields", {})
+            object.__setattr__(self, "_metainfo", dict(metainfo or {}))
+            for k, v in fields.items():
+                setattr(self, k, v)
+
+        def __setattr__(self, name: str, value: Any) -> None:
+            self._fields[name] = value
+
+        def __getattr__(self, name: str) -> Any:
+            fields = object.__getattribute__(self, "_fields")
+            if name in fields:
+                return fields[name]
+            meta = object.__getattribute__(self, "_metainfo")
+            if name in meta:
+                return meta[name]
+            raise AttributeError(name)
+
+        def __contains__(self, name: str) -> bool:
+            return name in self._fields
+
+        def get(self, name: str, default: Any = None) -> Any:
+            return self._fields.get(name, default)
+
+        def keys(self):
+            return self._fields.keys()
+
+        def to(self, *args: Any, **kwargs: Any) -> "PixelData":
+            out = PixelData(metainfo=self._metainfo)
+            for k, v in self._fields.items():
+                out._fields[k] = v.to(*args, **kwargs) if hasattr(v, "to") else v
+            return out
+
+        def cpu(self) -> "PixelData":
+            return self.to("cpu")
+
     class DetDataSample:
         """mmdet.structures.DetDataSample work-alike: metainfo + prediction slots."""
 
@@ -340,5 +380,5 @@ def make_data_samples(batch: int, size: int | tuple[int, int]) -> list:
             for _ in range(batch)]
 
 
-__all__ = ["MODELS", "Config", "ConfigDict", "BaseModule", "InstanceData", "DetDataSample",
+__all__ = ["MODELS", "Config", "ConfigDict", "BaseModule", "InstanceData", "PixelData", "DetDataSample",
            "HAVE_MMENGINE", "make_data_samples"]
