@@ -224,6 +224,18 @@ int rsp_nms_batched(const float* boxes, const int64_t* ids, const int32_t* nvali
 int rsp_nms_batched_topk(const float* boxes, const int64_t* ids, const int32_t* nvalid, int B, int n, float thr,
                          void* mask_ws, float* max_coord_ws, uint8_t* keep, int max_keep, void* stream);
 
+/* Greedy non-maximum merging (sahi's GREEDYNMM postprocess; no reference counterpart: the reference's large-image
+ * merge is mmcv batched_nms).  Score-sorted candidates as rsp_nms_batched takes them: boxes fp32 [B, n, 4], labels
+ * int64 [B, n], nvalid int32 [B].  Candidates i < j match when their labels are equal and the metric of their boxes as
+ * given (no label offset) is >= thr: metric 0 IoU = inter / ((area_i + area_j) - inter), metric 1 IoS = inter /
+ * min(area_i, area_j), area = (x2 - x1) * (y2 - y1), inter = max(0, min(x2) - max(x1)) * max(0, min(y2) - max(y1)),
+ * fp32 without contraction; a NaN (0 / 0) does not match.  Greedy in order: a candidate no keeper absorbed is kept
+ * (keep uint8 [B, n], as rsp_nms_batched with this match) and absorbs every later unabsorbed candidate it matches;
+ * owner int32 [B, n] = the index of the keeper that absorbed candidate i, -1 for keepers and invalid slots.
+ * Workspace: mask_ws uint64 [B, n, ceil(n/64)]; at most 393 216 candidates per image. */
+int rsp_nmm_batched(const float* boxes, const int64_t* labels, const int32_t* nvalid, int B, int n, float thr,
+                    int metric, void* mask_ws, uint8_t* keep, int32_t* owner, void* stream);
+
 /* First K kept candidates per image, in order, zero padded; counts int32 [B].  labels / out_labels /
  * out_index may be NULL.  Replaces results[keep][:max_per_img] (rpn_head.py:289, bbox_nms.py:97-99). */
 int rsp_compact_keep(const uint8_t* keep, const float* boxes, const float* scores, const int64_t* labels,
@@ -515,6 +527,20 @@ int rsp_mask_rle_placed_lengths(const uint8_t* src, int packed, const int64_t* d
                                 int64_t* offsets, void* stream);
 int rsp_mask_rle_placed_write(const uint8_t* src, int packed, const int64_t* desc, int n, const int64_t* offsets,
                               char* pool, int32_t* lengths, void* stream);
+/* ... of canvases that are each the OR of K >= 1 placed parts (the union mask of a group of tiles' masks that greedy
+ * non-maximum merging joined: sahi's GREEDYNMM postprocess ORs the members' shifted masks; no reference counterpart).
+ * desc int64 [n, 4] = (canvas H, W, first part, K), parts int64 [num_parts, 7] = (byte offset of the source mask from
+ * src, source row bytes, source rows, visible h, w, origin y0, x0), each in DEVICE and HOST memory (the write pass
+ * takes the device copies only).  Canvas i is zero except where one of its parts, placed as in
+ * rsp_mask_rle_placed_*, is set; neither the canvas nor the OR is formed (the work is proportional to the parts'
+ * bounding rectangle times K).  With K = 1 the string is rsp_mask_rle_placed_*'s.  RSP_ERR_INVALID, nothing launched,
+ * unless every canvas has 1 .. 2^31 - 1 pixels and parts within [0, num_parts), and every part passes the placed
+ * checks.  Pool, offsets and lengths as above. */
+int rsp_mask_rle_union_lengths(const uint8_t* src, int packed, const int64_t* desc, const int64_t* desc_host, int n,
+                               const int64_t* parts, const int64_t* parts_host, int num_parts, int64_t* offsets,
+                               void* stream);
+int rsp_mask_rle_union_write(const uint8_t* src, int packed, const int64_t* desc, int n, const int64_t* parts,
+                             const int64_t* offsets, char* pool, int32_t* lengths, void* stream);
 
 /* ---- DetDataPreprocessor on the device (SURVEY 8(f2); data_preprocessor.py:110-148, ImgDataPreprocessor.forward,
  * BatchFixedSizePad :300).  mean3 / std3: HOST arrays of 3 floats in OUTPUT channel order. ---- */

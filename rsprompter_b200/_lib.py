@@ -74,6 +74,7 @@ _SIGNATURES = {
     "rsp_nms_batched_topk": ([_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _i, _vp], _i),
     "rsp_bbox_cls_decode_shapes": ([_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp], _i),
     "rsp_nms_batched": ([_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp], _i),
+    "rsp_nmm_batched": ([_vp, _vp, _vp, _i, _i, _f, _i, _vp, _vp, _vp, _vp], _i),
     "rsp_compact_keep": ([_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp], _i),
     "rsp_soft_nms_workspace_bytes": ([_i, _i, _i, _vp], _i),
     "rsp_soft_nms_batched": ([_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _f, _i, _i, _i, _vp, ctypes.c_size_t, _vp, _vp,
@@ -117,6 +118,8 @@ _SIGNATURES = {
     "rsp_mask_rle_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
     "rsp_mask_rle_placed_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp], _i),
     "rsp_mask_rle_placed_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
+    "rsp_mask_rle_union_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp], _i),
+    "rsp_mask_rle_union_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp], _i),
     "rsp_gemm_upscale_masks": ([_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _i, _vp], _i),
     "rsp_sam_mask_embed": ([_vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp], _i),
     "rsp_sam_mask_stats": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _vp, _vp, _vp, _vp, _vp,
@@ -764,6 +767,31 @@ def nms_batched(boxes: torch.Tensor, ids: torch.Tensor, nvalid: torch.Tensor, io
                                      _ptr(mx), _ptr(keep), int(max_keep), _stream()), "rsp_nms_batched_topk")
     launch_count += 3
     return keep
+
+
+NMM_METRICS = {"iou": 0, "ios": 1}
+
+
+def nmm_batched(boxes: torch.Tensor, labels: torch.Tensor, nvalid: torch.Tensor, thr: float, metric: str = "ios"):
+    """Greedy non-maximum merging (see rsp_nmm_batched): boxes fp32 [B, n, 4] sorted by descending score, labels int64
+    [B, n], nvalid int32 [B] -> keep uint8 [B, n], owner int32 [B, n] (the absorbing keeper's index, -1 for keepers and
+    invalid slots).  A match is label equality and IoU or IoS (``metric``) >= thr."""
+    global launch_count
+    if metric not in NMM_METRICS:
+        raise ValueError(f"match metric must be one of {sorted(NMM_METRICS)}, got {metric!r}")
+    _require_cuda(boxes, labels, nvalid)
+    B, n, _ = boxes.shape
+    assert boxes.dtype == torch.float32 and boxes.is_contiguous()
+    assert labels.dtype == torch.int64 and labels.is_contiguous() and labels.shape == (B, n)
+    assert nvalid.dtype == torch.int32 and nvalid.is_contiguous() and nvalid.numel() == B
+    words = (n + 63) // 64
+    mask_ws = torch.empty(B * n * words, device=boxes.device, dtype=torch.int64)
+    keep = torch.empty(B, n, device=boxes.device, dtype=torch.uint8)
+    owner = torch.empty(B, n, device=boxes.device, dtype=torch.int32)
+    _check(_lib.rsp_nmm_batched(_ptr(boxes), _ptr(labels), _ptr(nvalid), B, n, float(thr), NMM_METRICS[metric],
+                                _ptr(mask_ws), _ptr(keep), _ptr(owner), _stream()), "rsp_nmm_batched")
+    launch_count += 2
+    return keep, owner
 
 
 def compact_keep(keep: torch.Tensor, boxes: torch.Tensor, scores: torch.Tensor, labels: torch.Tensor | None,
@@ -1430,22 +1458,61 @@ def mask_rle_placed(groups: list, packed: bool) -> list:
     return _rle_strings(base, packed, rows, groups[0][0].device, placed=True)
 
 
-def _rle_strings(base: int, packed: bool, rows: list, dev, placed: bool) -> list:
-    """The length pass + offset scan, one device->host read of the total, the write pass, one copy of the chars."""
+def mask_rle_union(sources: list, canvases: list, packed: bool) -> list:
+    """pycocotools compressed RLE strings (bytes, in order) of canvases that are each the OR of one or more placed
+    masks, neither the canvas nor the OR ever formed.  ``sources`` are contiguous CUDA tensors (bool / uint8 pixels, or
+    bit-packed rows with packed=True); ``canvases`` = [(H, W, parts)], parts = [(source index, byte offset in that
+    source, row bytes, rows, h, w, y0, x0)], each placed as in mask_rle_placed.  One part gives mask_rle_placed's
+    string.  The work is proportional to the parts' bounding rectangle; host syncs and copies as mask_rle."""
+    canvases = [(int(H), int(W), list(pl)) for H, W, pl in canvases]
+    if not canvases:
+        return []
+    if any(not pl for _, _, pl in canvases):
+        raise ValueError("every union canvas needs at least one part")
+    _require_cuda(*sources)
+    base = min(t.data_ptr() for t in sources)
+    for t in sources:
+        assert t.is_contiguous() and t.dtype in (torch.bool, torch.uint8)
+    rows, parts = [], []
+    for H, W, pl in canvases:
+        rows.append((H, W, len(parts), len(pl)))
+        for p in pl:
+            si, off, ld, nrows, h, w, y0, x0 = (int(v) for v in p)
+            t = sources[si]
+            assert 0 <= off and off + (h - 1) * ld + ((w + 7) // 8 if packed else w) <= t.numel(), "mask outside src"
+            parts.append((off + t.data_ptr() - base, ld, nrows, h, w, y0, x0))
+    return _rle_strings(base, packed, rows, sources[0].device, placed=True, parts=parts)
+
+
+def _rle_strings(base: int, packed: bool, rows: list, dev, placed: bool, parts: list | None = None) -> list:
+    """The length pass + offset scan, one device->host read of the total, the write pass, one copy of the chars.
+    ``parts``: the union mode, rows are its canvases."""
     global launch_count
     n = len(rows)
-    lengths_fn, write_fn = ((_lib.rsp_mask_rle_placed_lengths, _lib.rsp_mask_rle_placed_write) if placed else
-                            (_lib.rsp_mask_rle_lengths, _lib.rsp_mask_rle_write))
-    what = "rsp_mask_rle_placed" if placed else "rsp_mask_rle"
     desc_host = torch.tensor(rows, dtype=torch.int64).pin_memory()
     desc = desc_host.to(dev, non_blocking=True)
     offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
-    _check(lengths_fn(base, int(packed), _ptr(desc), _ptr(desc_host), n, _ptr(offsets), _stream()), what + "_lengths")
+    if parts is not None:
+        what = "rsp_mask_rle_union"
+        parts_host = torch.tensor(parts, dtype=torch.int64).pin_memory()
+        parts_d = parts_host.to(dev, non_blocking=True)
+        _check(_lib.rsp_mask_rle_union_lengths(base, int(packed), _ptr(desc), _ptr(desc_host), n, _ptr(parts_d),
+                                               _ptr(parts_host), len(parts), _ptr(offsets), _stream()), what + "_lengths")
+    else:
+        lengths_fn = _lib.rsp_mask_rle_placed_lengths if placed else _lib.rsp_mask_rle_lengths
+        what = "rsp_mask_rle_placed" if placed else "rsp_mask_rle"
+        _check(lengths_fn(base, int(packed), _ptr(desc), _ptr(desc_host), n, _ptr(offsets), _stream()),
+               what + "_lengths")
     total = int(offsets[n].item())                       # host sync 1: the exact pool size
     pool = torch.empty(total, dtype=torch.uint8, device=dev)
     lengths = torch.empty(n, dtype=torch.int32, device=dev)
-    _check(write_fn(base, int(packed), _ptr(desc), n, _ptr(offsets), _ptr(pool), _ptr(lengths), _stream()),
-           what + "_write")
+    if parts is not None:
+        _check(_lib.rsp_mask_rle_union_write(base, int(packed), _ptr(desc), n, _ptr(parts_d), _ptr(offsets), _ptr(pool),
+                                             _ptr(lengths), _stream()), what + "_write")
+    else:
+        write_fn = _lib.rsp_mask_rle_placed_write if placed else _lib.rsp_mask_rle_write
+        _check(write_fn(base, int(packed), _ptr(desc), n, _ptr(offsets), _ptr(pool), _ptr(lengths), _stream()),
+               what + "_write")
     launch_count += 3
     host_pool = torch.empty(total, dtype=torch.uint8, pin_memory=True)
     host_len = torch.empty(n, dtype=torch.int32, pin_memory=True)

@@ -240,6 +240,12 @@ int rsp_nms_batched_topk(const float* boxes, const int64_t* ids, const int32_t* 
                      static_cast<unsigned long long*>(mask_ws), max_coord_ws, keep, max_keep, S(stream));
 }
 
+int rsp_nmm_batched(const float* boxes, const int64_t* labels, const int32_t* nvalid, int B, int n, float thr,
+                    int metric, void* mask_ws, uint8_t* keep, int32_t* owner, void* stream) {
+  return nmm_batched(boxes, reinterpret_cast<const long long*>(labels), nvalid, B, n, thr, metric,
+                     static_cast<unsigned long long*>(mask_ws), keep, owner, S(stream));
+}
+
 int rsp_compact_keep(const uint8_t* keep, const float* boxes, const float* scores, const int64_t* labels,
                      int B, int n, int K, float* out_boxes, float* out_scores, int64_t* out_labels,
                      int32_t* out_index, int32_t* counts, void* stream) {
@@ -481,6 +487,23 @@ int rsp_mask_rle_placed_write(const uint8_t* src, int packed, const int64_t* des
                               char* pool, int32_t* lengths, void* stream) {
   return mask_rle_placed_write(src, packed, reinterpret_cast<const long long*>(desc), n,
                                reinterpret_cast<const long long*>(offsets), pool, lengths, S(stream));
+}
+
+int rsp_mask_rle_union_lengths(const uint8_t* src, int packed, const int64_t* desc, const int64_t* desc_host, int n,
+                               const int64_t* parts, const int64_t* parts_host, int num_parts, int64_t* offsets,
+                               void* stream) {
+  return mask_rle_union_lengths(src, packed, reinterpret_cast<const long long*>(desc),
+                                reinterpret_cast<const long long*>(desc_host), n,
+                                reinterpret_cast<const long long*>(parts),
+                                reinterpret_cast<const long long*>(parts_host), num_parts,
+                                reinterpret_cast<long long*>(offsets), S(stream));
+}
+
+int rsp_mask_rle_union_write(const uint8_t* src, int packed, const int64_t* desc, int n, const int64_t* parts,
+                             const int64_t* offsets, char* pool, int32_t* lengths, void* stream) {
+  return mask_rle_union_write(src, packed, reinterpret_cast<const long long*>(desc), n,
+                              reinterpret_cast<const long long*>(parts), reinterpret_cast<const long long*>(offsets),
+                              pool, lengths, S(stream));
 }
 
 }  // extern "C"

@@ -6,6 +6,9 @@
 //   bbox_cls_decode   softmax class scores + per-class delta2bbox (bbox_head.py:520-545)
 //   nms_batched       mmcv.ops.batched_nms semantics: boxes offset by id * (max + 1), greedy NMS,
 //                     suppress when IoU > thr (bbox_nms.py:95, rpn_head.py:285)
+//   nmm_batched       greedy non-maximum merging (sahi GREEDYNMM, no reference counterpart): the NMS bitmask of
+//                     an IoU or IoS >= thr match within a label, and the greedy scan also records which keeper
+//                     absorbed each candidate
 //   compact_keep      first K kept candidates per image -> dense [B, K] outputs + counts
 //   roi_align_nhwc    mmcv RoIAlign(aligned=True, sampling_ratio=0, avg) over 4 FPN levels with the
 //                     level mapping of SingleRoIExtractor (single_level_roi_extractor.py:55-119); the
@@ -206,13 +209,67 @@ __global__ void nms_mask_kernel(const float* __restrict__ boxes, const long long
   mask[(static_cast<size_t>(b) * n + i) * words + blockIdx.x] = bits;
 }
 
+// Greedy non-maximum merging's match bitmask, in nms_mask_kernel's layout: bit j of row i (j > i) is set when
+// candidates i and j have the same label and IoU (kMetric 0) or IoS (kMetric 1) >= thr, on the boxes as given (no
+// label offset, which would change the fp32 rounding).  area = (x2 - x1) * (y2 - y1), inter = max(0, min(x2) -
+// max(x1)) * max(0, min(y2) - max(y1)), iou = inter / ((area_i + area_j) - inter), ios = inter / min(area_i, area_j),
+// each step rounded once; a NaN (0 / 0) does not match.
+template <int kMetric>
+__device__ __forceinline__ bool match_ge(const float a[4], const float b[4], float thr) {
+  const float left = fmaxf(a[0], b[0]), right = fminf(a[2], b[2]);
+  const float top = fmaxf(a[1], b[1]), bottom = fminf(a[3], b[3]);
+  const float w = fmaxf(fsub(right, left), 0.f), h = fmaxf(fsub(bottom, top), 0.f);
+  const float inter = fmul(w, h);
+  const float sa = fmul(fsub(a[2], a[0]), fsub(a[3], a[1]));
+  const float sb = fmul(fsub(b[2], b[0]), fsub(b[3], b[1]));
+  const float v = kMetric == 0 ? __fdiv_rn(inter, fsub(fadd(sa, sb), inter)) : __fdiv_rn(inter, fminf(sa, sb));
+  return v >= thr;
+}
+
+template <int kMetric>
+__global__ void nmm_mask_kernel(const float* __restrict__ boxes, const long long* __restrict__ labels,
+                                const int* __restrict__ nvalid, int n, float thr, unsigned long long* __restrict__ mask) {
+  const int b = blockIdx.z;
+  const int nv = nvalid[b];
+  const int row0 = blockIdx.y * 64, col0 = blockIdx.x * 64;
+  if (row0 >= nv || col0 >= nv || blockIdx.x < blockIdx.y) return;
+  __shared__ float cb[64][4];
+  __shared__ long long cl[64];
+  const int cn = min(64, nv - col0);
+  if (threadIdx.x < cn) {
+    const size_t j = static_cast<size_t>(b) * n + col0 + threadIdx.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) cb[threadIdx.x][k] = boxes[j * 4 + k];
+    cl[threadIdx.x] = labels[j];
+  }
+  __syncthreads();
+  const int i = row0 + threadIdx.x;
+  if (i >= nv) return;
+  const size_t gi = static_cast<size_t>(b) * n + i;
+  float a[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) a[k] = boxes[gi * 4 + k];
+  const long long la = labels[gi];
+  unsigned long long bits = 0;
+  const int start = (row0 == col0) ? threadIdx.x + 1 : 0;
+  for (int j = start; j < cn; ++j)
+    if (cl[j] == la && match_ge<kMetric>(a, cb[j], thr)) bits |= 1ull << j;
+  const int words = (n + 63) / 64;
+  mask[(static_cast<size_t>(b) * n + i) * words + blockIdx.x] = bits;
+}
+
 // one CTA (4 warps) per image: greedy scan in score order, 64 candidates at a time.  Warp 0 resolves a
 // block serially in registers (the 64 diagonal mask words are held two per lane and broadcast by
 // shuffle); then all 128 threads OR the kept rows' remaining words into the suppression bitmap,
 // eight independent loads in flight per thread (the mask is L2-resident).
+// kOwner (greedy merging): owner[i] = the kept row that suppressed candidate i, -1 for kept and invalid ones.  A bit
+// belongs to the first kept row, in order, whose word sets it: in the diagonal block the bits dw & ~cur of a kept
+// row, off the diagonal the bits a kept row's word adds to the ones of earlier kept rows (they are ORed in ascending
+// row order, and remv already holds those of earlier blocks).
+template <bool kOwner>
 __global__ void __launch_bounds__(128)
 nms_scan_kernel(const unsigned long long* __restrict__ mask, const int* __restrict__ nvalid, int n, int max_keep,
-                unsigned char* __restrict__ keep) {
+                unsigned char* __restrict__ keep, int* __restrict__ owner) {
   extern __shared__ unsigned long long remv[];
   __shared__ unsigned long long kept_s;
   const int b = blockIdx.x;
@@ -221,6 +278,8 @@ nms_scan_kernel(const unsigned long long* __restrict__ mask, const int* __restri
   const int nvw = (nv + 63) / 64;
   const int tid = threadIdx.x, lane = tid & 31;
   for (int w = tid; w < words; w += blockDim.x) remv[w] = 0ull;
+  if (kOwner)
+    for (int i = tid; i < n; i += blockDim.x) owner[static_cast<size_t>(b) * n + i] = -1;
   __syncthreads();
   const unsigned long long* mbase = mask + static_cast<size_t>(b) * n * words;
   int kept_total = 0;     // the caller reads only the first max_keep kept candidates (compact_keep): stop once they exist
@@ -232,14 +291,24 @@ nms_scan_kernel(const unsigned long long* __restrict__ mask, const int* __restri
         const unsigned long long d0 = (r0 < nv) ? mbase[static_cast<size_t>(r0) * words + blk] : 0ull;
         const unsigned long long d1 = (r1 < nv) ? mbase[static_cast<size_t>(r1) * words + blk] : 0ull;
         unsigned long long cur = remv[blk], keptbits = 0ull;
+        int o0 = -1, o1 = -1;   // kOwner: owners of rows r0 and r1
         for (int tbit = 0; tbit < 64; ++tbit) {
           const unsigned long long dw = __shfl_sync(0xffffffffu, tbit < 32 ? d0 : d1, tbit & 31);
           if (i0 + tbit < nv && !((cur >> tbit) & 1ull)) {
             keptbits |= 1ull << tbit;
+            if (kOwner) {
+              const unsigned long long fresh = dw & ~cur;
+              if ((fresh >> lane) & 1ull) o0 = i0 + tbit;
+              if ((fresh >> (lane + 32)) & 1ull) o1 = i0 + tbit;
+            }
             cur |= dw;
           }
         }
         if (lane == 0) kept_s = keptbits;
+        if (kOwner) {
+          if (o0 >= 0) owner[static_cast<size_t>(b) * n + r0] = o0;
+          if (o1 >= 0) owner[static_cast<size_t>(b) * n + r1] = o1;
+        }
       }
       __syncthreads();
       const unsigned long long keptbits = kept_s;
@@ -249,6 +318,7 @@ nms_scan_kernel(const unsigned long long* __restrict__ mask, const int* __restri
         unsigned long long kb = keptbits;
         while (kb) {
           unsigned long long v[8];
+          int row[8];
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
             v[u] = 0ull;
@@ -256,10 +326,21 @@ nms_scan_kernel(const unsigned long long* __restrict__ mask, const int* __restri
               const int tbit = __ffsll(static_cast<long long>(kb)) - 1;
               kb &= kb - 1;
               v[u] = mbase[static_cast<size_t>(i0 + tbit) * words + w];
+              if (kOwner) row[u] = i0 + tbit;
             }
           }
 #pragma unroll
-          for (int u = 0; u < 8; ++u) acc |= v[u];
+          for (int u = 0; u < 8; ++u) {
+            if (kOwner) {
+              unsigned long long fresh = v[u] & ~acc;
+              while (fresh) {
+                const int j = __ffsll(static_cast<long long>(fresh)) - 1;
+                fresh &= fresh - 1;
+                owner[static_cast<size_t>(b) * n + w * 64 + j] = row[u];
+              }
+            }
+            acc |= v[u];
+          }
         }
         remv[w] = acc;
       }
@@ -284,7 +365,22 @@ int nms_batched(const float* boxes, const long long* ids, const int* nvalid, int
   dim3 grid(words, words, B);
   nms_mask_kernel<<<grid, 64, 0, stream>>>(boxes, ids, nvalid, max_coord_ws, n, thr, mask_ws);
   RSP_CHECK_LAUNCH();
-  nms_scan_kernel<<<B, 128, words * 8, stream>>>(mask_ws, nvalid, n, max_keep, keep);
+  nms_scan_kernel<false><<<B, 128, words * 8, stream>>>(mask_ws, nvalid, n, max_keep, keep, nullptr);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
+int nmm_batched(const float* boxes, const long long* labels, const int* nvalid, int B, int n, float thr, int metric,
+                unsigned long long* mask_ws, unsigned char* keep, int* owner, cudaStream_t stream) {
+  RSP_CHECK_ARG(boxes && labels && nvalid && mask_ws && keep && owner && B > 0 && n > 0, "nmm: bad args");
+  RSP_CHECK_ARG(metric == 0 || metric == 1, "nmm: metric 0 (IoU) or 1 (IoS), got %d", metric);
+  const int words = (n + 63) / 64;
+  RSP_CHECK_ARG(words * 8 <= 48 * 1024, "nmm: at most %d candidates per image", 48 * 1024 / 8 * 64);
+  dim3 grid(words, words, B);
+  if (metric == 0) nmm_mask_kernel<0><<<grid, 64, 0, stream>>>(boxes, labels, nvalid, n, thr, mask_ws);
+  else nmm_mask_kernel<1><<<grid, 64, 0, stream>>>(boxes, labels, nvalid, n, thr, mask_ws);
+  RSP_CHECK_LAUNCH();
+  nms_scan_kernel<true><<<B, 128, words * 8, stream>>>(mask_ws, nvalid, n, 0, keep, owner);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
 }

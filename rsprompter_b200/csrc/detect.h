@@ -14,6 +14,8 @@ int bbox_cls_decode(const float* cls, int ld_cls, const float* reg, int ld_reg, 
 int nms_batched(const float* boxes, const long long* ids, const int* nvalid, int B, int n, float thr,
                 unsigned long long* mask_ws, float* max_coord_ws, unsigned char* keep, int max_keep,
                 cudaStream_t stream);   // max_keep > 0: flags past the first max_keep kept candidates may be 0
+int nmm_batched(const float* boxes, const long long* labels, const int* nvalid, int B, int n, float thr, int metric,
+                unsigned long long* mask_ws, unsigned char* keep, int* owner, cudaStream_t stream);
 int compact_keep(const unsigned char* keep, const float* boxes, const float* scores, const long long* labels,
                  int B, int n, int K, float* out_boxes, float* out_scores, long long* out_labels,
                  int* out_index, int* counts, cudaStream_t stream);

@@ -99,11 +99,52 @@ struct MaskView {
     if (kPacked) return (__ldg(row + (x >> 3)) >> (x & 7)) & 1u;
     return __ldg(row + x) != 0 ? 1u : 0u;
   }
+  // rows y .. y + rows - 1 (rows <= 16) of column x, row y + k in bit k
+  __device__ __forceinline__ unsigned chunk(int y, int x, int rows) const {
+    unsigned w = 0u;
+    if (rows == 16) {
+#pragma unroll
+      for (int k = 0; k < 16; ++k) w |= at(y + k, x) << k;
+    } else {
+      for (int k = 0; k < rows; ++k) w |= at(y + k, x) << k;
+    }
+    return w;
+  }
+};
+
+// The OR of K placed parts, seen through the rectangle that bounds them (canvas rows ry0.., columns rx0..).  Part p is
+// parts[7p .. 7p + 6] = (byte offset from src, row bytes, rows, visible h, w, canvas y0, x0).  A chunk ORs the bits of
+// every part that covers its column and some of its rows; the canvas is never formed.
+template <bool kPacked>
+struct UnionView {
+  const unsigned char* src;
+  const long long* parts;
+  int k;
+  int ry0, rx0;
+  __device__ __forceinline__ unsigned chunk(int y, int x, int rows) const {
+    const int cy = ry0 + y, cx = rx0 + x;
+    unsigned w = 0u;
+#pragma unroll 1
+    for (int p = 0; p < k; ++p) {
+      const long long* d = parts + 7 * p;
+      const int px0 = static_cast<int>(__ldg(d + 6)), pw = static_cast<int>(__ldg(d + 4));
+      if (cx < px0 || cx >= px0 + pw) continue;
+      const int py0 = static_cast<int>(__ldg(d + 5)), ph = static_cast<int>(__ldg(d + 3));
+      const int a = max(cy, py0), e = min(cy + rows, py0 + ph);
+      if (a >= e) continue;
+      const MaskView<kPacked> mv{src + __ldg(d), static_cast<int>(__ldg(d + 1))};
+#pragma unroll 4
+      for (int r = a; r < e; ++r) w |= mv.at(r - py0, cx - px0) << (r - cy);
+    }
+    return w;
+  }
+  __device__ __forceinline__ unsigned at(int y, int x) const { return chunk(y, x, 1); }
 };
 
 // Where the h x w source mask lies in the H x W canvas whose runs are encoded: canvas[y0 + y, x0 + x] = mask[y, x],
-// zero elsewhere.  The plain mode is h = H, w = W at the origin.  Only the w source columns are walked; the zero
-// rows and columns around them enter through the boundary positions alone.
+// zero elsewhere.  The plain mode is h = H, w = W at the origin; the union mode's "mask" is the rectangle bounding
+// its parts.  Only the w source columns are walked; the zero rows and columns around them enter through the boundary
+// positions alone.
 struct Placement {
   int h, w;     // visible extent
   int H, W;     // canvas
@@ -116,20 +157,14 @@ struct Placement {
 // Otherwise the pixels above and below the mask are zero: a run that reaches the mask's last row ends one past it
 // (unless that is the end of the canvas, where the final count closes it).  A plain mask spans its canvas, so that
 // last boundary exists only for placed ones.
-template <bool kPlaced, bool kPacked, typename F>
-__device__ __forceinline__ void for_each_boundary(const MaskView<kPacked>& mv, const Placement& pl, int x, F&& f) {
+template <bool kPlaced, typename V, typename F>
+__device__ __forceinline__ void for_each_boundary(const V& mv, const Placement& pl, int x, F&& f) {
   const bool full_height = pl.y0 == 0 && pl.h == pl.H;
   unsigned prev = full_height && x > 0 ? mv.at(pl.h - 1, x - 1) : 0u;
   const int base = (pl.x0 + x) * pl.H + pl.y0;
   for (int y0 = 0; y0 < pl.h; y0 += 16) {
     const int rows = min(16, pl.h - y0);
-    unsigned w = 0u;
-    if (rows == 16) {
-#pragma unroll
-      for (int k = 0; k < 16; ++k) w |= mv.at(y0 + k, x) << k;
-    } else {
-      for (int k = 0; k < rows; ++k) w |= mv.at(y0 + k, x) << k;
-    }
+    const unsigned w = mv.chunk(y0, x, rows);
     unsigned change = (w ^ ((w << 1) | prev)) & ((1u << rows) - 1u);
     prev = (w >> (rows - 1)) & 1u;
     while (change) {
@@ -160,21 +195,18 @@ __device__ __forceinline__ void load_desc(const long long* desc, int i, MaskView
   }
 }
 
-// kWrite = false: offsets[i + 1] = chars of mask i.  kWrite = true: the chars into pool[offsets[i], offsets[i+1]).
-template <bool kPacked, bool kWrite, bool kPlaced>
-__global__ void __launch_bounds__(kThreads) mask_rle_kernel(const unsigned char* __restrict__ src,
-                                                            const long long* __restrict__ desc, long long* offsets,
-                                                            char* __restrict__ pool, int* __restrict__ lengths) {
-  using CtxScan = cub::BlockScan<RleCtx, kThreads, cub::BLOCK_SCAN_WARP_SCANS>;
-  using SumScan = cub::BlockScan<long long, kThreads, cub::BLOCK_SCAN_WARP_SCANS>;
-  __shared__ union {
-    typename CtxScan::TempStorage ctx;
-    typename SumScan::TempStorage sum;
-  } tmp;
-  const int i = blockIdx.x;
-  MaskView<kPacked> mv;
-  Placement pl;
-  load_desc<kPacked, kPlaced>(desc, i, mv, pl, src);
+using CtxScan = cub::BlockScan<RleCtx, kThreads, cub::BLOCK_SCAN_WARP_SCANS>;
+using SumScan = cub::BlockScan<long long, kThreads, cub::BLOCK_SCAN_WARP_SCANS>;
+union RleTemp {
+  typename CtxScan::TempStorage ctx;
+  typename SumScan::TempStorage sum;
+};
+
+// The encode of canvas i, shared by every mode.  kWrite = false: offsets[i + 1] = its chars.  kWrite = true: the chars
+// into pool[offsets[i], offsets[i+1]).
+template <bool kWrite, bool kPlaced, typename V>
+__device__ __forceinline__ void rle_encode(const V& mv, const Placement& pl, int i, long long* offsets, char* pool,
+                                           int* lengths, RleTemp& tmp) {
   char* out = nullptr;
   const char* end = nullptr;
   if (kWrite) {
@@ -235,6 +267,44 @@ __global__ void __launch_bounds__(kThreads) mask_rle_kernel(const unsigned char*
   }
 }
 
+template <bool kPacked, bool kWrite, bool kPlaced>
+__global__ void __launch_bounds__(kThreads) mask_rle_kernel(const unsigned char* __restrict__ src,
+                                                            const long long* __restrict__ desc, long long* offsets,
+                                                            char* __restrict__ pool, int* __restrict__ lengths) {
+  __shared__ RleTemp tmp;
+  const int i = blockIdx.x;
+  MaskView<kPacked> mv;
+  Placement pl;
+  load_desc<kPacked, kPlaced>(desc, i, mv, pl, src);
+  rle_encode<kWrite, kPlaced>(mv, pl, i, offsets, pool, lengths, tmp);
+}
+
+// Union mode: canvas i is desc[4i .. 4i + 3] = (H, W, first part, parts), its parts' rows of `parts` as UnionView
+// reads them.  The rectangle bounding the parts is walked as one placed mask.
+template <bool kPacked, bool kWrite>
+__global__ void __launch_bounds__(kThreads) mask_rle_union_kernel(const unsigned char* __restrict__ src,
+                                                                  const long long* __restrict__ desc,
+                                                                  const long long* __restrict__ parts,
+                                                                  long long* offsets, char* __restrict__ pool,
+                                                                  int* __restrict__ lengths) {
+  __shared__ RleTemp tmp;
+  const int i = blockIdx.x;
+  const long long* d = desc + 4 * i;
+  const int H = static_cast<int>(d[0]), W = static_cast<int>(d[1]), k = static_cast<int>(d[3]);
+  const long long* pp = parts + 7 * d[2];
+  int y0 = INT_MAX, x0 = INT_MAX, y1 = 0, x1 = 0;
+  for (int p = 0; p < k; ++p) {
+    const long long* q = pp + 7 * p;
+    y0 = min(y0, static_cast<int>(q[5]));
+    x0 = min(x0, static_cast<int>(q[6]));
+    y1 = max(y1, static_cast<int>(q[5] + q[3]));
+    x1 = max(x1, static_cast<int>(q[6] + q[4]));
+  }
+  const UnionView<kPacked> uv{src, pp, k, y0, x0};
+  const Placement pl{y1 - y0, x1 - x0, H, W, y0, x0};
+  rle_encode<kWrite, true>(uv, pl, i, offsets, pool, lengths, tmp);
+}
+
 // offsets[1..n] = inclusive sum of the per-mask char counts stored there, offsets[0] = 0
 __global__ void __launch_bounds__(kScanThreads) rle_offsets_kernel(long long* offsets, int n) {
   using Scan = cub::BlockScan<long long, kScanThreads, cub::BLOCK_SCAN_WARP_SCANS>;
@@ -274,6 +344,13 @@ int rle_write(const unsigned char* src, int packed, const long long* desc, int n
   else mask_rle_kernel<false, true, kPlaced><<<n, kThreads, 0, stream>>>(src, desc, offs, pool, lengths);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
+}
+
+template <bool kWrite>
+void rle_union_launch(const unsigned char* src, int packed, const long long* desc, int n, const long long* parts,
+                      long long* offsets, char* pool, int* lengths, cudaStream_t stream) {
+  if (packed) mask_rle_union_kernel<true, kWrite><<<n, kThreads, 0, stream>>>(src, desc, parts, offsets, pool, lengths);
+  else mask_rle_union_kernel<false, kWrite><<<n, kThreads, 0, stream>>>(src, desc, parts, offsets, pool, lengths);
 }
 
 }  // namespace
@@ -322,6 +399,49 @@ int mask_rle_placed_write(const unsigned char* src, int packed, const long long*
   RSP_CHECK_ARG(src && desc && offsets && pool && lengths && n > 0 && (packed == 0 || packed == 1),
                 "mask_rle_placed_write: bad args");
   return rle_write<true>(src, packed, desc, n, offsets, pool, lengths, stream);
+}
+
+int mask_rle_union_lengths(const unsigned char* src, int packed, const long long* desc, const long long* desc_host,
+                           int n, const long long* parts, const long long* parts_host, int num_parts, long long* offsets,
+                           cudaStream_t stream) {
+  RSP_CHECK_ARG(src && desc && desc_host && parts && parts_host && offsets && n > 0 && num_parts > 0 &&
+                (packed == 0 || packed == 1), "mask_rle_union_lengths: bad args");
+  for (int i = 0; i < n; ++i) {
+    const long long H = desc_host[4 * i], W = desc_host[4 * i + 1], first = desc_host[4 * i + 2],
+                    k = desc_host[4 * i + 3];
+    RSP_CHECK_ARG(H >= 1 && W >= 1 && H <= INT_MAX && W <= INT_MAX && H * W <= INT_MAX,
+                  "mask_rle_union_lengths: mask %d: canvas %lld x %lld (1 .. 2^31 - 1 pixels)", i, H, W);
+    RSP_CHECK_ARG(first >= 0 && k >= 1 && k <= num_parts - first,
+                  "mask_rle_union_lengths: mask %d: parts [%lld, %lld + %lld) outside the %d parts", i, first, first, k,
+                  num_parts);
+    for (long long p = first; p < first + k; ++p) {
+      const long long* d = parts_host + 7 * p;
+      const long long off = d[0], ld = d[1], rows = d[2], h = d[3], w = d[4], y0 = d[5], x0 = d[6];
+      RSP_CHECK_ARG(y0 >= 0 && x0 >= 0 && y0 < H && x0 < W,
+                    "mask_rle_union_lengths: mask %d, part %lld: origin (%lld, %lld) outside the %lld x %lld canvas", i,
+                    p, y0, x0, H, W);
+      RSP_CHECK_ARG(h >= 1 && w >= 1 && h <= H - y0 && w <= W - x0,
+                    "mask_rle_union_lengths: mask %d, part %lld: %lld x %lld at (%lld, %lld) leaves the %lld x %lld "
+                    "canvas", i, p, h, w, y0, x0, H, W);
+      RSP_CHECK_ARG(off >= 0 && ld <= INT_MAX && h <= rows && w <= (packed ? 8 * ld : ld),
+                    "mask_rle_union_lengths: mask %d, part %lld: visible %lld x %lld exceeds the source (%lld rows of "
+                    "%lld bytes, offset %lld)", i, p, h, w, rows, ld, off);
+    }
+  }
+  rle_union_launch<false>(src, packed, desc, n, parts, offsets, nullptr, nullptr, stream);
+  RSP_CHECK_LAUNCH();
+  rle_offsets_kernel<<<1, kScanThreads, 0, stream>>>(offsets, n);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
+int mask_rle_union_write(const unsigned char* src, int packed, const long long* desc, int n, const long long* parts,
+                         const long long* offsets, char* pool, int* lengths, cudaStream_t stream) {
+  RSP_CHECK_ARG(src && desc && parts && offsets && pool && lengths && n > 0 && (packed == 0 || packed == 1),
+                "mask_rle_union_write: bad args");
+  rle_union_launch<true>(src, packed, desc, n, parts, const_cast<long long*>(offsets), pool, lengths, stream);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
 }
 
 }  // namespace rsp

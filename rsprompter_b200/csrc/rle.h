@@ -17,5 +17,10 @@ int mask_rle_placed_lengths(const unsigned char* src, int packed, const long lon
                             int n, long long* offsets, cudaStream_t stream);
 int mask_rle_placed_write(const unsigned char* src, int packed, const long long* desc, int n, const long long* offsets,
                           char* pool, int* lengths, cudaStream_t stream);
+int mask_rle_union_lengths(const unsigned char* src, int packed, const long long* desc, const long long* desc_host,
+                           int n, const long long* parts, const long long* parts_host, int num_parts, long long* offsets,
+                           cudaStream_t stream);
+int mask_rle_union_write(const unsigned char* src, int packed, const long long* desc, int n, const long long* parts,
+                         const long long* offsets, char* pool, int* lengths, cudaStream_t stream);
 
 }  // namespace rsp

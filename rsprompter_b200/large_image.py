@@ -13,12 +13,15 @@ merged with one class-aware NMS (``merge_results_by_nms``).  Here all of it stay
   * every batch leaves ``predict_records`` as one ResultRecord, resident until the merge;
   * the merge is ``rsp_nms_batched`` + ``rsp_compact_keep`` over every valid slot of every tile (mmcv
     ``batched_nms`` semantics, label offset included), or ``rsp_soft_nms_batched`` with ``merge_nms_type='soft_nms'``
-    (the demo's ``--merge-nms-type``);
-  * the kept masks are encoded as COCO RLE of the whole scene by ``rsp_mask_rle_placed_*`` straight from the
-    records' bits: the full-scene bool mask sahi's ``shift_masks`` builds for every instance never exists.
+    (the demo's ``--merge-nms-type``), or greedy non-maximum merging with ``merge_nms_type='greedy_nmm'`` (sahi's
+    GREEDYNMM postprocess, ``rsp_nmm_batched``): an object cut by a tile seam comes out as one instance with the
+    union of its fragments' boxes and masks;
+  * the kept masks are encoded as COCO RLE of the whole scene by ``rsp_mask_rle_placed_*`` (``rsp_mask_rle_union_*``
+    for merged groups) straight from the records' bits: the full-scene bool mask sahi's ``shift_masks`` builds for
+    every instance never exists.
 
-The merge's hard NMS is dense: at most 393 216 candidates (tiles x slots), with an n^2 / 8-byte workspace.  The soft
-merge takes the same number of candidates with an O(n) workspace.
+The merge's hard NMS and greedy merging are dense: at most 393 216 candidates (tiles x slots), with an n^2 / 8-byte
+workspace.  The soft merge takes the same number of candidates with an O(n) workspace.
 
 ``python -m rsprompter_b200.large_image CONFIG IMAGE`` writes the COCO result dicts of one scene."""
 from __future__ import annotations
@@ -62,11 +65,20 @@ def slice_origins(hw: tuple, patch: int, overlap_ratio: float) -> list:
     return out
 
 
-MERGE_NMS_TYPES = ("nms", "soft_nms")
+MERGE_NMS_TYPES = ("nms", "soft_nms", "greedy_nmm")
+MATCH_METRICS = ("ios", "iou")
+
+
+def _check_merge_args(nms_type: str, match_metric: str) -> None:
+    if nms_type not in MERGE_NMS_TYPES:
+        raise ValueError(f"merge nms type {nms_type!r} is not supported (supported: {', '.join(MERGE_NMS_TYPES)})")
+    if nms_type == "greedy_nmm" and match_metric not in MATCH_METRICS:
+        raise ValueError(f"match metric {match_metric!r} is not supported (supported: {', '.join(MATCH_METRICS)})")
 
 
 def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_thr: float = 0.25,
-                       score_thr: float = 0.0, window: tuple | None = None, nms_type: str = "nms") -> dict:
+                       score_thr: float = 0.0, window: tuple | None = None, nms_type: str = "nms",
+                       match_metric: str = "ios") -> dict:
     """Class-aware NMS of every valid slot of every tile, in scene coordinates.
 
     ``records`` are ResultRecords of tiles (one image per tile; records of one call share slots and device) and
@@ -86,11 +98,21 @@ def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_
     10 000 candidates, by decayed score at or above it.  ``score_thr`` then drops kept rows scored below it.  Filtering
     before a soft merge would not be the same: a low-scored box can be selected early and decay others.
 
+    ``nms_type='greedy_nmm'`` merges instead of suppressing, as sahi's GREEDYNMM postprocess does: candidates (filtered
+    and sorted as for nms) match when their labels are equal and their ``match_metric`` ('ios': intersection over the
+    smaller area, or 'iou') is >= merge_iou_thr, in fp32 on the scene boxes.  Walking the sorted candidates, one that no
+    earlier keeper absorbed becomes a keeper and absorbs every later unabsorbed candidate it matches, so the keepers
+    are exactly nms's kept rows and each other candidate joins the first keeper in order that matches it (no
+    transitivity: what a member matches is not absorbed through it).  A keeper's row has the element-wise union of its
+    members' boxes, its own score and label; its mask is the OR of its members' masks.  Unlike sahi's loop, a member
+    is not tested again against the growing merged box: every matched member joins its group.  The result also has
+    members int64 [m, 3] (record, image, slot) and member_offsets int64 [k + 1] on the host: group i is
+    members[member_offsets[i]:member_offsets[i + 1]], its keeper first, then its absorbed members in sort order.
+
     Returns dict(bboxes fp32 [k, 4], scores [k], labels int64 [k] on the device, in descending score order (soft: keep
     order), and source int64 [k, 3] on the host: (record, image, slot) of each kept row).  One host synchronisation
     (two for soft_nms: the number of label groups is read first)."""
-    if nms_type not in MERGE_NMS_TYPES:
-        raise ValueError(f"merge nms type {nms_type!r} is not supported (supported: {', '.join(MERGE_NMS_TYPES)})")
+    _check_merge_args(nms_type, match_metric)
     H, W = int(scene_hw[0]), int(scene_hw[1])
     assert len(records) == len(origins) and records, "one origin list per record"
     M = records[0].slots
@@ -129,6 +151,8 @@ def merge_tile_records(records: list, origins: list, scene_hw: tuple, merge_iou_
     boxes_s = boxes.reshape(N, 4)[order].contiguous()
     scores_s = scores.reshape(N)[order].contiguous()
     labels_s = rows[..., 5].reshape(N)[order].long().contiguous()
+    if nms_type == "greedy_nmm":
+        return _nmm_merge(boxes_s, scores_s, labels_s, nvalid, order, merge_iou_thr, match_metric, src, M)
     keep = _lib.nms_batched(boxes_s[None], labels_s[None], nvalid, merge_iou_thr)
     ob, os_, ol, oi, cnt = _lib.compact_keep(keep, boxes_s[None], scores_s[None], labels_s[None], N)
     flat = order[oi[0].clamp(min=0).long()]
@@ -165,6 +189,33 @@ def _soft_merge(boxes, scores, labels, valid, iou_thr, score_thr, src, M) -> dic
                 source=torch.cat([src[tile], slot[:, None]], dim=1))
 
 
+def _nmm_merge(boxes_s, scores_s, labels_s, nvalid, order, thr, metric, src, M) -> dict:
+    """The greedy_nmm branch of merge_tile_records over the N sorted candidates (valid prefix of nvalid)."""
+    N = int(boxes_s.shape[0])
+    dev = boxes_s.device
+    keep, owner = _lib.nmm_batched(boxes_s[None], labels_s[None], nvalid, thr, metric)
+    pos = torch.arange(N, device=dev)
+    grp = torch.where(keep[0].bool(), pos, owner[0].long())          # each valid candidate's keeper, -1 invalid
+    member = grp >= 0
+    idx = grp.clamp(min=0)[:, None].expand(N, 2)
+    lo = boxes_s[:, :2].scatter_reduce(0, idx, torch.where(member[:, None], boxes_s[:, :2], math.inf), "amin")
+    hi = boxes_s[:, 2:].scatter_reduce(0, idx, torch.where(member[:, None], boxes_s[:, 2:], -math.inf), "amax")
+    merged = torch.cat([lo, hi], dim=1).contiguous()
+    ob, os_, ol, oi, cnt = _lib.compact_keep(keep, merged[None], scores_s[None], labels_s[None], N)
+    # members grouped by keeper in keeper order; a keeper precedes what it absorbed, so the stable sort puts it first
+    gkey, morder = torch.sort(torch.where(member, grp, N), stable=True)
+    kpos = oi[0].long().clamp(min=0)
+    starts = torch.searchsorted(gkey, kpos)
+    host = torch.cat([cnt.long(), nvalid.long(), order[kpos], starts, order[morder]]).cpu()   # the one host sync
+    k, m = int(host[0]), int(host[1])
+    flat = host[2:2 + k]
+    offsets = torch.cat([host[2 + N:2 + N + k], torch.tensor([m])])
+    mflat = host[2 + 2 * N:2 + 2 * N + m]
+    return dict(bboxes=ob[0, :k], scores=os_[0, :k], labels=ol[0, :k],
+                source=torch.cat([src[flat // M], (flat % M)[:, None]], dim=1),
+                members=torch.cat([src[mflat // M], (mflat % M)[:, None]], dim=1), member_offsets=offsets)
+
+
 def _slots(model) -> int:
     if isinstance(model, RSPrompterQuery):
         return int(model.test_cfg.get("max_per_image", 100))
@@ -178,7 +229,7 @@ def _record_nbytes(B: int, M: int, hw: tuple) -> int:
 @torch.no_grad()
 def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr: float = 0.25,
                         score_thr: float = 0.0, batch_size: int = 8, patch_size: int | None = None,
-                        merge_nms_type: str = "nms") -> DetDataSample:
+                        merge_nms_type: str = "nms", merge_match_metric: str = "ios") -> DetDataSample:
     """Detect a whole scene: slice, run the tiles in batches, merge across tiles, encode the kept masks.
 
     ``image`` is the scene as mmcv.imread decodes it, uint8 [H, W, 3] BGR: a numpy array or a tensor on the host
@@ -191,21 +242,26 @@ def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr
     host synchronisation happens per tile or per batch; the merge reads the kept rows once and the RLE encode
     synchronises twice.
 
-    ``merge_nms_type`` ('nms' or 'soft_nms', the demo's ``--merge-nms-type``) selects the cross-tile merge; see
-    merge_tile_records for what soft_nms returns and how ``score_thr`` applies to it.
+    ``merge_nms_type`` ('nms' or 'soft_nms', the demo's ``--merge-nms-type``, or 'greedy_nmm') selects the cross-tile
+    merge; see merge_tile_records for what soft_nms returns and how ``score_thr`` applies to it.  'greedy_nmm' joins
+    matching rows (``merge_match_metric`` 'ios' or 'iou' >= merge_iou_thr) into one instance with the union box and
+    the union mask of its members.
 
     Returns a DetDataSample with ori_shape = img_shape = (H, W), scale_factor (1, 1) and pred_instances: bboxes,
     scores, labels on the device in descending score order, masks a list of {'size': [H, W], 'counts': bytes} (the
     test_cfg.rle_masks convention, passed through by CocoMetric.process)."""
-    if merge_nms_type not in MERGE_NMS_TYPES:
-        raise ValueError(f"merge nms type {merge_nms_type!r} is not supported (supported: {', '.join(MERGE_NMS_TYPES)})")
+    _check_merge_args(merge_nms_type, merge_match_metric)
     records, batches = run_tiles(model, image, overlap_ratio, batch_size, patch_size=patch_size,
                                  merge_nms_type=merge_nms_type)
     H, W = int(image.shape[0]), int(image.shape[1])
     window = None if patch_size is None else (int(patch_size), int(patch_size))
     merged = merge_tile_records(records, batches, (H, W), merge_iou_thr=merge_iou_thr, score_thr=score_thr,
-                                window=window, nms_type=merge_nms_type)
-    masks = encode_kept_masks(records, batches, merged["source"], (H, W), window=window)
+                                window=window, nms_type=merge_nms_type, match_metric=merge_match_metric)
+    if merge_nms_type == "greedy_nmm":
+        masks = encode_merged_masks(records, batches, merged["members"], merged["member_offsets"], (H, W),
+                                    window=window)
+    else:
+        masks = encode_kept_masks(records, batches, merged["source"], (H, W), window=window)
     ds = DetDataSample(metainfo=dict(ori_shape=(H, W), img_shape=(H, W), scale_factor=(1.0, 1.0)))
     ds.pred_instances = InstanceData(bboxes=merged["bboxes"], scores=merged["scores"], labels=merged["labels"],
                                      masks=masks)
@@ -246,7 +302,7 @@ def run_tiles(model, image, overlap_ratio: float = 0.25, batch_size: int = 8, pa
         raise ValueError(f"{len(origins)} tiles x {M} slots = {N} merge candidates; the dense NMS takes at most "
                          f"{MAX_MERGE_CANDIDATES}")
     merge_ws = (_lib.soft_nms_workspace_bytes(1, N, 1024) + N * 64 if merge_nms_type == "soft_nms"   # O(N) + gathers
-                else N * ((N + 63) // 64) * 8)
+                else N * ((N + 63) // 64) * 8 + (N * 4 if merge_nms_type == "greedy_nmm" else 0))   # + owner
     need = (len(batches) * _record_nbytes(B, M, rec_hw) + (0 if img.is_cuda else H * W * 3)
             + merge_ws + (B * 3 * S * S * 4 if resize else 0))
     free, _ = torch.cuda.mem_get_info(dev)
@@ -326,6 +382,30 @@ def encode_kept_masks(records: list, origins: list, source: torch.Tensor, scene_
     return [dict(size=[H, W], counts=c) for c in _lib.mask_rle_placed(groups, packed=True)]
 
 
+def encode_merged_masks(records: list, origins: list, members: torch.Tensor, member_offsets: torch.Tensor,
+                        scene_hw: tuple, window: tuple | None = None) -> list:
+    """COCO RLE dicts of greedy_nmm's merged rows: row i is the OR of the masks of members[member_offsets[i]:
+    member_offsets[i + 1]] (rows (record, image, slot) from merge_tile_records), each placed in the H x W scene at its
+    tile origin and cut to its tile window, encoded by rsp_mask_rle_union_* from the records' bits (a group of one is
+    the placed encode's string); two host synchronisations.  ``window`` as in merge_tile_records."""
+    H, W = int(scene_hw[0]), int(scene_hw[1])
+    mem = members.tolist()
+    offs = member_offsets.tolist()
+    canvases = []
+    for i in range(len(offs) - 1):
+        parts = []
+        for r, b, s in mem[offs[i]:offs[i + 1]]:
+            rec = records[r]
+            P, M = rec.hw[0], rec.slots
+            ph, pw = window or rec.hw
+            ld = rec.hw[1] // 8
+            x0, y0 = origins[r][b]
+            parts.append((r, (b * M + s) * P * ld, ld, P, min(ph, H - y0), min(pw, W - x0), y0, x0))
+        canvases.append((H, W, parts))
+    return [dict(size=[H, W], counts=c)
+            for c in _lib.mask_rle_union([rec.buf for rec in records], canvases, packed=True)]
+
+
 def coco_results(ds: DetDataSample, image_id=0, label_to_cat=None) -> list:
     """COCO result dicts of one scene, as CocoMetric.results2json writes them: xywh bbox, score, category_id and the
     RLE segmentation with ``counts`` as str."""
@@ -338,7 +418,7 @@ def coco_results(ds: DetDataSample, image_id=0, label_to_cat=None) -> list:
     return out
 
 
-def main(argv=None) -> list:
+def build_parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(description="Detect one large scene: sliced inference, merge, COCO RLE masks")
     ap.add_argument("config")
     ap.add_argument("image")
@@ -347,13 +427,21 @@ def main(argv=None) -> list:
     ap.add_argument("--merge-iou-thr", type=float, default=0.25)
     ap.add_argument("--score-thr", type=float, default=0.0)
     ap.add_argument("--merge-nms-type", default="nms", choices=MERGE_NMS_TYPES,
-                    help="NMS type of the cross-tile merge (soft_nms: linear, sigma 0.5, min_score 1e-3)")
+                    help="NMS type of the cross-tile merge (soft_nms: linear, sigma 0.5, min_score 1e-3; greedy_nmm: "
+                         "matching rows are merged into one instance with the union box and mask)")
+    ap.add_argument("--merge-match-metric", default="ios", choices=MATCH_METRICS,
+                    help="match metric of greedy_nmm, compared with --merge-iou-thr (ios: intersection over the "
+                         "smaller area)")
     ap.add_argument("--batch-size", type=int, default=8)
     ap.add_argument("--patch-size", type=int, default=None,
                     help="window size; each window is resized to the model size (default: model-size windows, "
                          "not resized)")
     ap.add_argument("--out", default=None, help="JSON file for the result dicts (default: stdout)")
-    args = ap.parse_args(argv)
+    return ap
+
+
+def main(argv=None) -> list:
+    args = build_parser().parse_args(argv)
 
     import cv2
 
@@ -369,7 +457,7 @@ def main(argv=None) -> list:
         raise FileNotFoundError(args.image)
     ds = predict_large_image(model, img, overlap_ratio=args.patch_overlap_ratio, merge_iou_thr=args.merge_iou_thr,
                              score_thr=args.score_thr, batch_size=args.batch_size, patch_size=args.patch_size,
-                             merge_nms_type=args.merge_nms_type)
+                             merge_nms_type=args.merge_nms_type, merge_match_metric=args.merge_match_metric)
     res = coco_results(ds)
     text = json.dumps(res)
     if args.out:
