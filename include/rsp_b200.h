@@ -65,8 +65,12 @@ int rsp_gemm_bf16_simt(const void* A, int lda, const void* W, int ldw, void* out
 
 /* ViT-SAM attention core: out = softmax(hd^-0.5 * q k^T + rel_h + rel_w) v per (sequence, head).
  * qkv bf16 [n_seq*T, 3*H*hd] (columns [q|k|v], heads contiguous inside each); rel_h / rel_w
- * bf16 [2S-1, hd]; out bf16 [n_seq*T, H*hd].  T = S*S; S = 14 (windows) or 64 (global),
- * hd = 64 or 80.  The T x T bias of get_decomposed_rel_pos is never materialised.
+ * bf16 [2S-1, hd]; out bf16 [n_seq*T, H*hd].  T = S*S; S = 14 (windows) or 32 / 64 (global) on the
+ * tensor cores, other S on rsp_vit_attention_simt; hd = 64 or 80.  The T x T bias of get_decomposed_rel_pos is
+ * never materialised.  The tensor-core kernel multiplies P by V in fp16 (V converted from bf16): the output is
+ * finite and within the float64 bound of oracle/encoder_attention.py for |v| <= 65280 (the largest bf16 that is a
+ * finite fp16; larger |v| become inf), and each |v| below 2^-14 (fp16 subnormal) carries an absolute error of up
+ * to 2^-25.
  * Replaces: SamVisionAttention.forward after the qkv Linear and before proj (HF:803-831,
  * HF:729-801) / Attention.forward + add_decomposed_rel_pos (VS:202-221, VS:117-157). */
 int rsp_vit_attention(const void* qkv, const void* rel_h, const void* rel_w, void* out, int n_seq,
