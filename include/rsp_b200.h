@@ -571,6 +571,26 @@ int rsp_preprocess_u8(const uint8_t* img, int h, int w, long long stride_c, long
 int rsp_resize_pad_u8(const int64_t* desc, const int64_t* desc_host, int B, float* out, int Hp, int Wp,
                       const float* mean3, const float* std3, int swap_rb, const float* pad3, void* stream);
 
+/* SamImageProcessor's resize for a batch of images of different sizes, one call (two launches): the keep-ratio
+ * resize of transformers 5.5's TorchvisionBackend, tvF.resize(uint8, BILINEAR, antialias=True)
+ * (image_processing_backends.py:251), whose filter support widens with the downscale, where rsp_resize_pad_u8 is cv2
+ * INTER_LINEAR (2 x 2 taps at any scale, which aliases at 4-20x).  Grey levels byte-identical to torchvision's CPU
+ * uint8 path: per axis whose size changes, a triangle filter of support max(in / out, 1) with weights computed in
+ * double and fixed to int(w * 2^prec + 0.5), each output clamp((2^(prec-1) + sum(p * w)) >> prec, 0, 255); horizontal
+ * pass first, to uint8, then vertical.  The host builds the weight tables (rsprompter_b200._lib.resize_aa_table); an
+ * axis whose size does not change gets the identity table (one tap, weight 2^prec), which is exact.
+ * desc / desc_host int64 [B, 16], DEVICE and HOST copies: rsp_resize_pad_u8's 8 fields, then (workspace byte offset,
+ * x table offset, x row length, x prec, y table offset, y row length, y prec, 0); workspace offsets are the prefix
+ * sums of 3 * h * new_w in image order.  tab / tab_host int32 [n_tab], DEVICE and HOST copies: per axis, one row per
+ * output index of (first tap, tap count, weights), every tap inside the source axis.  ws: DEVICE uint8 of at least
+ * *bytes of rsp_resize_aa_pad_u8_ws_bytes(desc_host, B, bytes) = sum of 3 * h * new_w, the horizontal pass of each image
+ * (61 MB for a 20 000^2 scene to 1024).  out, normalisation, channel order and pad exactly as rsp_resize_pad_u8,
+ * applied to the resized uint8 pixel. */
+int rsp_resize_aa_pad_u8_ws_bytes(const int64_t* desc_host, int B, long long* bytes);
+int rsp_resize_aa_pad_u8(const int64_t* desc, const int64_t* desc_host, const int32_t* tab, const int32_t* tab_host,
+                         long long n_tab, int B, uint8_t* ws, long long ws_bytes, float* out, int Hp, int Wp,
+                         const float* mean3, const float* std3, int swap_rb, const float* pad3, void* stream);
+
 /* The same arithmetic fused into the patch-embed operand loader: uint8 batch [B, 3, H, W] (hwc = 0) or [B, H, W, 3]
  * (hwc = 1), contiguous, 16-byte aligned, H, W % 16 == 0 -> bf16 patch rows [B*(H/16)*(W/16), 768] in (c, ky, kx)
  * order = rsp_patchify16(rsp_preprocess_u8(img)) bit for bit; the fp32 image never exists. */

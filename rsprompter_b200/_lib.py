@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
+import functools
 import subprocess
 from pathlib import Path
 
@@ -111,6 +112,9 @@ _SIGNATURES = {
                            _i, _f, _vp], _i),
     "rsp_patchify16_u8": ([_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp], _i),
     "rsp_resize_pad_u8": ([_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _vp], _i),
+    "rsp_resize_aa_pad_u8_ws_bytes": ([_vp, _i, _vp], _i),
+    "rsp_resize_aa_pad_u8": ([_vp, _vp, _vp, _vp, ctypes.c_longlong, _i, _vp, ctypes.c_longlong, _vp, _i, _i, _vp, _vp,
+                              _i, _vp, _vp], _i),
     "rsp_mask_paste_rescale_bits": ([_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp], _i),
     "rsp_query_postprocess_rescale_bits": ([_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp,
                                             _vp, _vp], _i),
@@ -1388,6 +1392,71 @@ def resize_pad_u8(imgs: list, sizes: list, out: torch.Tensor, mean, std, swap_rb
                                   _host_f3(mean), _host_f3(std), int(swap_rb), _host_f3(pad), _stream()),
            "rsp_resize_pad_u8")
     launch_count += 1
+    return out
+
+
+@functools.lru_cache(maxsize=64)
+def resize_aa_table(n_in: int, n_out: int) -> tuple:
+    """One axis of torchvision's antialiased bilinear uint8 resize (aten UpSampleKernel.cpp,
+    _compute_index_ranges_weights and _compute_index_ranges_int16_weights): triangle weights of support
+    max(n_in / n_out, 1) in double, normalised by their sequential sum, fixed to int(w * 2^prec + 0.5) with prec the
+    first value whose next doubling would reach 2^15 (at most 22).  n_in == n_out gives the identity (one tap of
+    2^14).  -> (int32 [n_out, 2 + k] rows of (first tap, tap count, weights), prec)."""
+    n_in, n_out = int(n_in), int(n_out)
+    if n_in == n_out:
+        return torch.stack([torch.arange(n_out), torch.ones(n_out, dtype=torch.int64),
+                            torch.full((n_out,), 1 << 14)], 1).to(torch.int32), 14
+    scale = n_in / n_out
+    support = scale if scale >= 1.0 else 1.0
+    inv = 1.0 / scale if scale >= 1.0 else 1.0
+    center = scale * (torch.arange(n_out, dtype=torch.float64) + 0.5)
+    xmin = (center - support + 0.5).to(torch.int64).clamp(min=0)
+    xsize = (center + support + 0.5).to(torch.int64).clamp(max=n_in) - xmin
+    k = int(xsize.max())
+    j = torch.arange(k)
+    w = (1.0 - (((j[None] + xmin[:, None]).double() - center[:, None] + 0.5) * inv).abs()).clamp(min=0.0)
+    w = torch.where(j[None] < xsize[:, None], w, 0.0)
+    w = w / torch.cumsum(w, 1)[:, -1:]                 # the sum in tap order, as the C loop adds them
+    w_max = float(w.max())
+    prec = 0
+    while prec < 22 and int(0.5 + w_max * (1 << (prec + 1))) < (1 << 15):
+        prec += 1
+    wi = (w * (1 << prec) + 0.5).to(torch.int64)
+    return torch.cat([xmin[:, None], xsize[:, None], wi], 1).to(torch.int32), prec
+
+
+def resize_aa_pad_u8(imgs: list, sizes: list, out: torch.Tensor, mean, std, swap_rb: bool, pad) -> torch.Tensor:
+    """resize_pad_u8 with SamImageProcessor's resize, torchvision's antialiased bilinear (rsp_resize_aa_pad_u8): the
+    same arguments and output, grey levels byte-identical to tvF.resize(uint8, antialias=True).  The horizontal pass
+    goes through a device workspace of sum(3 * h * new_w) bytes, allocated here."""
+    global launch_count
+    _require_cuda(out, *imgs)
+    B = len(imgs)
+    assert B == len(sizes) == out.shape[0] and B > 0
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.dim() == 4 and out.shape[1] == 3
+    rows, tabs, n_tab, ws_off = [], [], 0, 0
+    for t, (nh, nw) in zip(imgs, sizes):
+        assert t.dtype == torch.uint8 and t.dim() == 3 and t.shape[0] == 3
+        h, w = int(t.shape[1]), int(t.shape[2])
+        tx, px = resize_aa_table(w, int(nw))
+        ty, py = resize_aa_table(h, int(nh))
+        rows.append([t.data_ptr(), *t.stride(), h, w, int(nh), int(nw), ws_off, n_tab, tx.shape[1], px,
+                     n_tab + tx.numel(), ty.shape[1], py, 0])
+        tabs += [tx.view(-1), ty.view(-1)]
+        n_tab += tx.numel() + ty.numel()
+        ws_off += 3 * h * int(nw)
+    host = torch.tensor(rows, dtype=torch.int64).pin_memory()
+    tab_host = torch.cat(tabs).pin_memory()
+    desc = host.to(out.device, non_blocking=True)
+    tab = tab_host.to(out.device, non_blocking=True)
+    n = ctypes.c_longlong(0)
+    _check(_lib.rsp_resize_aa_pad_u8_ws_bytes(host.data_ptr(), B, ctypes.byref(n)), "rsp_resize_aa_pad_u8_ws_bytes")
+    ws_bytes = n.value
+    ws = torch.empty(ws_bytes, device=out.device, dtype=torch.uint8)
+    _check(_lib.rsp_resize_aa_pad_u8(_ptr(desc), host.data_ptr(), _ptr(tab), tab_host.data_ptr(), n_tab, B, _ptr(ws),
+                                     ws_bytes, _ptr(out), out.shape[2], out.shape[3], _host_f3(mean), _host_f3(std),
+                                     int(swap_rb), _host_f3(pad), _stream()), "rsp_resize_aa_pad_u8")
+    launch_count += 2
     return out
 
 

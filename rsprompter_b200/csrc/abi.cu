@@ -452,6 +452,17 @@ int rsp_resize_pad_u8(const int64_t* desc, const int64_t* desc_host, int B, floa
                        Hp, Wp, mean3, std3, swap_rb, pad3, S(stream));
 }
 
+int rsp_resize_aa_pad_u8_ws_bytes(const int64_t* desc_host, int B, long long* bytes) {
+  return resize_aa_pad_u8_ws_bytes(reinterpret_cast<const long long*>(desc_host), B, bytes);
+}
+
+int rsp_resize_aa_pad_u8(const int64_t* desc, const int64_t* desc_host, const int32_t* tab, const int32_t* tab_host,
+                         long long n_tab, int B, uint8_t* ws, long long ws_bytes, float* out, int Hp, int Wp,
+                         const float* mean3, const float* std3, int swap_rb, const float* pad3, void* stream) {
+  return resize_aa_pad_u8(reinterpret_cast<const long long*>(desc), reinterpret_cast<const long long*>(desc_host), tab,
+                          tab_host, n_tab, B, ws, ws_bytes, out, Hp, Wp, mean3, std3, swap_rb, pad3, S(stream));
+}
+
 int rsp_patchify16_u8(const uint8_t* img, int hwc, void* out, int B, int H, int W, const float* mean3, const float* std3,
                       int swap_rb, void* stream) {
   return patchify16_u8(img, hwc, out, B, H, W, mean3, std3, swap_rb, S(stream));

@@ -190,6 +190,129 @@ int resize_pad_u8(const long long* desc, const long long* desc_host, int B, floa
   return RSP_OK;
 }
 
+// torchvision's antialiased uint8 bilinear resize (aten UpSampleKernel's separable int16-weight path), in two passes
+// over host-built integer weight tables.  desc int64 [B, 16] per image = resize_pad_u8's 8 fields, then (workspace
+// byte offset, x table offset, x row length, x precision, y table offset, y row length, y precision, 0); a table row
+// (int32) = (first tap, tap count, weights...).  Integer MACs only: the result does not depend on device float.
+__device__ __forceinline__ unsigned char aa_round(int acc, int prec) {
+  return static_cast<unsigned char>(min(max((acc + (1 << (prec - 1))) >> prec, 0), 255));
+}
+
+// thread = one (source row, output column): 3 channels of the horizontal pass -> ws uint8 [3, h, new_w]
+__global__ void resize_aa_h_kernel(const long long* __restrict__ desc, const int* __restrict__ tab,
+                                   unsigned char* __restrict__ ws) {
+  const long long* d = desc + static_cast<size_t>(blockIdx.y) * 16;
+  const int h = static_cast<int>(d[4]), nw = static_cast<int>(d[7]);
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= static_cast<long long>(h) * nw) return;
+  const int x = static_cast<int>(idx % nw), y = static_cast<int>(idx / nw);
+  const int* row = tab + d[9] + static_cast<long long>(x) * d[10];
+  const int x0 = row[0], n = row[1], prec = static_cast<int>(d[11]);
+  const long long sc = d[1], sx = d[3];
+  const unsigned char* src = reinterpret_cast<const unsigned char*>(d[0]) + y * d[2] + x0 * sx;
+  int acc0 = 0, acc1 = 0, acc2 = 0;
+  for (int j = 0; j < n; ++j) {
+    const int wj = __ldg(row + 2 + j);
+    const unsigned char* p = src + j * sx;
+    acc0 += wj * p[0];
+    acc1 += wj * p[sc];
+    acc2 += wj * p[2 * sc];
+  }
+  const long long plane = static_cast<long long>(h) * nw;
+  unsigned char* o = ws + d[8] + idx;
+  o[0] = aa_round(acc0, prec);
+  o[plane] = aa_round(acc1, prec);
+  o[2 * plane] = aa_round(acc2, prec);
+}
+
+// thread = one output pixel of the padded plane: the vertical pass over ws, then resize_pad_u8's normalisation
+__global__ void resize_aa_v_pad_kernel(const long long* __restrict__ desc, const int* __restrict__ tab,
+                                       const unsigned char* __restrict__ ws, float* __restrict__ out, int Hp, int Wp,
+                                       Norm3 nm, int swap_rb, Norm3 pad) {
+  const long long plane = static_cast<long long>(Hp) * Wp;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= plane) return;
+  const long long* d = desc + static_cast<size_t>(blockIdx.y) * 16;
+  const int x = static_cast<int>(idx % Wp), y = static_cast<int>(idx / Wp);
+  const int h = static_cast<int>(d[4]), nh = static_cast<int>(d[6]), nw = static_cast<int>(d[7]);
+  float v[3];
+  if (y < nh && x < nw) {
+    const int* row = tab + d[12] + static_cast<long long>(y) * d[13];
+    const int y0 = row[0], n = row[1], prec = static_cast<int>(d[14]);
+    const long long ip = static_cast<long long>(h) * nw;
+    const unsigned char* src = ws + d[8] + static_cast<long long>(y0) * nw + x;
+    int acc[3] = {0, 0, 0};
+    for (int j = 0; j < n; ++j) {
+      const int wj = __ldg(row + 2 + j);
+      const unsigned char* p = src + static_cast<long long>(j) * nw;
+      acc[0] += wj * p[0];
+      acc[1] += wj * p[ip];
+      acc[2] += wj * p[2 * ip];
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float u = static_cast<float>(aa_round(acc[swap_rb ? 2 - c : c], prec));
+      v[c] = __fdiv_rn(__fsub_rn(u, nm.mean[c]), nm.stdv[c]);
+    }
+  } else {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = __fdiv_rn(__fsub_rn(pad.mean[swap_rb ? 2 - c : c], nm.mean[c]), nm.stdv[c]);
+  }
+  float* o = out + static_cast<size_t>(blockIdx.y) * 3 * plane + idx;
+  o[0] = v[0]; o[plane] = v[1]; o[2 * plane] = v[2];
+}
+
+int resize_aa_pad_u8_ws_bytes(const long long* desc_host, int B, long long* bytes) {
+  RSP_CHECK_ARG(desc_host && bytes && B > 0, "resize_aa_pad_u8_ws_bytes: bad args");
+  long long n = 0;
+  for (int b = 0; b < B; ++b) n += 3 * desc_host[static_cast<size_t>(b) * 16 + 4] * desc_host[static_cast<size_t>(b) * 16 + 7];
+  *bytes = n;
+  return RSP_OK;
+}
+
+// one table of n_out rows of length len: every row's taps inside [0, n_in), at most len - 2 of them
+static bool aa_table_ok(const int* tab_host, long long n_tab, long long off, long long len, long long n_out,
+                        long long n_in) {
+  if (off < 0 || len < 3 || n_out <= 0 || off + n_out * len > n_tab) return false;
+  for (long long i = 0; i < n_out; ++i) {
+    const int* r = tab_host + off + i * len;
+    if (r[0] < 0 || r[1] < 1 || r[1] > len - 2 || static_cast<long long>(r[0]) + r[1] > n_in) return false;
+  }
+  return true;
+}
+
+int resize_aa_pad_u8(const long long* desc, const long long* desc_host, const int* tab, const int* tab_host,
+                     long long n_tab, int B, unsigned char* ws, long long ws_bytes, float* out, int Hp, int Wp,
+                     const float* mean3, const float* std3, int swap_rb, const float* pad3, cudaStream_t stream) {
+  RSP_CHECK_ARG(desc && desc_host && tab && tab_host && ws && out && mean3 && std3 && pad3 && B > 0 && B <= 65535 &&
+                Hp > 0 && Wp > 0 && n_tab > 0, "resize_aa_pad_u8: bad args");
+  long long ws_off = 0, max_h = 0;
+  for (int b = 0; b < B; ++b) {
+    const long long* d = desc_host + static_cast<size_t>(b) * 16;
+    RSP_CHECK_ARG(d[0] != 0 && d[1] > 0 && d[2] > 0 && d[3] > 0 && d[4] > 0 && d[5] > 0 && d[6] > 0 && d[7] > 0 &&
+                  d[6] <= Hp && d[7] <= Wp && d[4] < (1LL << 31) && d[5] < (1LL << 31) && d[8] == ws_off &&
+                  d[11] >= 1 && d[11] <= 22 && d[14] >= 1 && d[14] <= 22,
+                  "resize_aa_pad_u8: bad descriptor (positive strides and sizes, the resized image inside the pad "
+                  "size, workspace offsets in image order, precisions in [1, 22])");
+    RSP_CHECK_ARG(aa_table_ok(tab_host, n_tab, d[9], d[10], d[7], d[5]) &&
+                  aa_table_ok(tab_host, n_tab, d[12], d[13], d[6], d[4]),
+                  "resize_aa_pad_u8: a weight table row reads outside its source axis or the table");
+    ws_off += 3 * d[4] * d[7];
+    max_h = max(max_h, d[4] * d[7]);
+  }
+  RSP_CHECK_ARG(ws_off <= ws_bytes, "resize_aa_pad_u8: workspace too small (resize_aa_pad_u8_ws_bytes)");
+  resize_aa_h_kernel<<<dim3(static_cast<unsigned>((max_h + 255) / 256), static_cast<unsigned>(B)), 256, 0, stream>>>(
+      desc, tab, ws);
+  RSP_CHECK_LAUNCH();
+  Norm3 nm{{mean3[0], mean3[1], mean3[2]}, {std3[0], std3[1], std3[2]}};
+  Norm3 pad{{pad3[0], pad3[1], pad3[2]}, {0.f, 0.f, 0.f}};
+  const long long plane = static_cast<long long>(Hp) * Wp;
+  resize_aa_v_pad_kernel<<<dim3(static_cast<unsigned>((plane + 255) / 256), static_cast<unsigned>(B)), 256, 0, stream>>>(
+      desc, tab, ws, out, Hp, Wp, nm, swap_rb, pad);
+  RSP_CHECK_LAUNCH();
+  return RSP_OK;
+}
+
 __device__ __forceinline__ void store_patch_seg(__nv_bfloat16* dst, const float f[16]) {
   reinterpret_cast<uint4*>(dst)[0] = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]),
                                                 pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));

@@ -10,6 +10,10 @@ int preprocess_u8(const unsigned char* img, int h, int w, long long stride_c, lo
                   cudaStream_t stream);
 int resize_pad_u8(const long long* desc, const long long* desc_host, int B, float* out, int Hp, int Wp,
                   const float* mean3, const float* std3, int swap_rb, const float* pad3, cudaStream_t stream);
+int resize_aa_pad_u8_ws_bytes(const long long* desc_host, int B, long long* bytes);
+int resize_aa_pad_u8(const long long* desc, const long long* desc_host, const int* tab, const int* tab_host,
+                     long long n_tab, int B, unsigned char* ws, long long ws_bytes, float* out, int Hp, int Wp,
+                     const float* mean3, const float* std3, int swap_rb, const float* pad3, cudaStream_t stream);
 int patchify16_u8(const unsigned char* img, int hwc, void* out, int B, int H, int W, const float* mean3,
                   const float* std3, int swap_rb, cudaStream_t stream);
 

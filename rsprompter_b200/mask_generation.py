@@ -30,17 +30,21 @@ changed after those it left alone: one more host synchronisation per call.
 
 ``generate_scene_masks`` runs the same stages over the overlapping windows of a whole scene (large_image's slicing),
 with HF's crop-edge rule applied in ``rsp_sam_mask_stats_crop``, RLE of the whole scene from each window's bits, and
-one cross-window box NMS.
+one cross-window box NMS; ``coarse_patch_sizes`` adds layers of larger windows up to the whole scene, resized by
+``rsp_resize_aa_pad_u8`` (SamImageProcessor's antialiased resize) and merged under the finer layers as SAM merges
+its crop layers.
 
 ``python -m rsprompter_b200.mask_generation IMAGE --arch base --checkpoint sam.safetensors --out masks.json`` writes
 one dict per mask (COCO RLE ``segmentation``, xywh ``bbox``, ``predicted_iou``, ``stability_score``,
 ``point_coords``); with ``--patch-size P`` the image is a scene cut into P x P windows, and each dict also has the
-window's ``crop_box``."""
+window's ``crop_box``; ``--coarse-patch-sizes P1 [P2 ...]`` adds layers of coarser windows up to the whole scene,
+and each dict then has its ``layer``."""
 from __future__ import annotations
 
 import argparse
 import json
 import math
+import numbers
 
 import torch
 
@@ -109,8 +113,9 @@ def _sizes(v, B: int, name: str) -> list:
     return [(int(h), int(w)) for h, w in v]
 
 
-def _inputs(sam, images, pixel_values, original_sizes, reshaped_input_sizes, dev):
-    """-> (pixel_values fp32 [B, 3, S, S] on dev, original (h, w) per image, reshaped (h, w) per image)."""
+def _inputs(sam, images, pixel_values, original_sizes, reshaped_input_sizes, dev, antialias: bool = False):
+    """-> (pixel_values fp32 [B, 3, S, S] on dev, original (h, w) per image, reshaped (h, w) per image).  Images are
+    resized by rsp_resize_pad_u8, or with ``antialias`` by rsp_resize_aa_pad_u8 (SamImageProcessor's resize)."""
     S = sam.varch.image_size
     if (images is None) == (pixel_values is None):
         raise ValueError("pass exactly one of images and pixel_values")
@@ -136,7 +141,8 @@ def _inputs(sam, images, pixel_values, original_sizes, reshaped_input_sizes, dev
     mean = tuple(255.0 * m for m in IMAGE_MEAN)
     std = tuple(255.0 * s for s in IMAGE_STD)
     pix = torch.empty(len(imgs), 3, S, S, device=dev, dtype=torch.float32)
-    _lib.resize_pad_u8(views, reshaped, pix, mean, std, False, mean)      # padded with the mean: 0 once normalised
+    resize = _lib.resize_aa_pad_u8 if antialias else _lib.resize_pad_u8
+    resize(views, reshaped, pix, mean, std, False, mean)                  # padded with the mean: 0 once normalised
     return pix, sizes, reshaped
 
 
@@ -206,6 +212,18 @@ def _nms(iou: torch.Tensor, keep: torch.Tensor, boxes: torch.Tensor, iou_thr: fl
     return idx, host[:B].tolist(), host[B:].view(B, Nc)
 
 
+def _paste(cand: dict, b: int, ci: torch.Tensor, mask_threshold: float, target_size: int) -> torch.Tensor:
+    """The candidates ci (device indices) of image b pasted as bits at the image's original size."""
+    Nc = cand["iou"].shape[1]
+    H, W = cand["sizes"][b]
+    bits = torch.empty(ci.shape[0], H, (W + 15) // 16 * 2, device=ci.device, dtype=torch.uint8)
+    if ci.shape[0]:
+        lg = cand["logits"].index_select(0, ci + b * Nc)
+        _lib.mask_paste(lg, mask_threshold, raw=True, rescale=((target_size, target_size), cand["reshaped"][b], (H, W)),
+                        bits=bits)
+    return bits
+
+
 def _outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch.Tensor, mask_threshold: float,
              target_size: int) -> list:
     """Per image: the kept masks pasted as bits, and the kept rows of every per-candidate output."""
@@ -215,12 +233,7 @@ def _outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch.Tensor
         k = counts[b]
         H, W = cand["sizes"][b]
         ci = idx[b, :k]
-        ld = (W + 15) // 16 * 2
-        bits = torch.empty(k, H, ld, device=idx.device, dtype=torch.uint8)
-        if k:
-            lg = cand["logits"].index_select(0, ci + b * Nc)
-            _lib.mask_paste(lg, mask_threshold, raw=True, rescale=((target_size, target_size), cand["reshaped"][b], (H, W)),
-                            bits=bits)
+        bits = _paste(cand, b, ci, mask_threshold, target_size)
         out.append(dict(masks=bits, scores=cand["iou"][b].index_select(0, ci),
                         stability_scores=cand["stability"][b].index_select(0, ci),
                         boxes=cand["boxes"][b].index_select(0, ci).long(),
@@ -241,6 +254,29 @@ def _check_region_area(min_mask_region_area) -> float:
     return a
 
 
+def _clean(bits: torch.Tensor, W: int, min_area: float) -> tuple:
+    """rsp_mask_small_regions_bits' holes then islands on the masks bits uint8 [k, H, ld] (k > 0), in place, in chunks
+    whose label workspace fits SMALL_REGIONS_WORKSPACE_BYTES.  -> (unchanged fp32 [k], 1 for a mask neither step
+    changed, boxes int32 [k, 4] of the cleaned masks)."""
+    k, H = bits.shape[0], bits.shape[1]
+    # areas are integers, so "< A" is "< ceil(A)"; every A above H * W (one more than the largest area) gives the
+    # same result, and the clamp keeps a huge finite A within the kernel's 64-bit threshold
+    thr = min(math.ceil(min_area), H * W + 1)
+    chunk = max(1, SMALL_REGIONS_WORKSPACE_BYTES // _lib.small_regions_ws_bytes(1, H, W))
+    ws = torch.empty(_lib.small_regions_ws_bytes(min(chunk, k), H, W), device=bits.device, dtype=torch.uint8)
+    tmp = torch.empty_like(bits[:chunk])
+    unchanged = torch.empty(k, device=bits.device, dtype=torch.float32)
+    boxes = torch.empty(k, 4, device=bits.device, dtype=torch.int32)
+    for j0 in range(0, k, chunk):
+        j1 = min(j0 + chunk, k)
+        part = bits[j0:j1]
+        _, ch_h, _ = _lib.mask_small_regions_bits(part, W, thr, "holes", out=tmp[:j1 - j0], ws=ws)
+        _, ch_i, bx = _lib.mask_small_regions_bits(tmp[:j1 - j0], W, thr, "islands", out=part, ws=ws)
+        unchanged[j0:j1] = (~(ch_h | ch_i)).float()
+        boxes[j0:j1] = bx
+    return unchanged, boxes
+
+
 def _remove_small_regions(out: list, min_area: float, iou_thr: float) -> list:
     """SAM's postprocess_small_regions (min_mask_region_area) on every image's kept masks: holes then islands by
     rsp_mask_small_regions_bits, the boxes of the cleaned masks, and a box NMS with score float(unchanged) at iou_thr
@@ -255,24 +291,10 @@ def _remove_small_regions(out: list, min_area: float, iou_thr: float) -> list:
     valid = torch.zeros(B, K, device=dev, dtype=torch.bool)
     boxes = torch.zeros(B, K, 4, device=dev, dtype=torch.int32)
     for b, r in enumerate(out):
-        bits = r["masks"]
-        k, H = bits.shape[0], bits.shape[1]
-        W = r["size"][1]
+        k = r["masks"].shape[0]
         if k == 0:
             continue
-        # areas are integers, so "< A" is "< ceil(A)"; every A above H * W (one more than the largest area) gives the
-        # same result, and the clamp keeps a huge finite A within the kernel's 64-bit threshold
-        thr = min(math.ceil(min_area), H * W + 1)
-        chunk = max(1, SMALL_REGIONS_WORKSPACE_BYTES // _lib.small_regions_ws_bytes(1, H, W))
-        ws = torch.empty(_lib.small_regions_ws_bytes(min(chunk, k), H, W), device=dev, dtype=torch.uint8)
-        tmp = torch.empty_like(bits[:chunk])
-        for j0 in range(0, k, chunk):
-            j1 = min(j0 + chunk, k)
-            part = bits[j0:j1]
-            _, ch_h, _ = _lib.mask_small_regions_bits(part, W, thr, "holes", out=tmp[:j1 - j0], ws=ws)
-            _, ch_i, bx = _lib.mask_small_regions_bits(tmp[:j1 - j0], W, thr, "islands", out=part, ws=ws)
-            unchanged[b, j0:j1] = (~(ch_h | ch_i)).float()
-            boxes[b, j0:j1] = bx
+        unchanged[b, :k], boxes[b, :k] = _clean(r["masks"], r["size"][1], min_area)
         valid[b, :k] = True
     idx, counts, idx_host = _nms(unchanged, valid, boxes, iou_thr)
     res = []
@@ -376,6 +398,104 @@ def scene_crop_boxes(hw: tuple, patch_size: int, overlap_ratio: float) -> list:
     return [(x0, y0, min(x0 + P, W), min(y0 + P, H)) for x0, y0 in slice_origins((H, W), P, overlap_ratio)]
 
 
+def scene_layer_windows(hw: tuple, patch_size: int, overlap_ratio: float, coarse_patch_sizes=()) -> list:
+    """The windows of every layer of generate_scene_masks: [(layer, crop boxes)], layer 0 the base windows of
+    ``patch_size``, layer l those of coarse_patch_sizes[l - 1] (scene_crop_boxes of each size; a size >= max(H, W)
+    is one window, the scene).  A layer whose windows are those of the previous layer that runs is left out."""
+    out = [(0, scene_crop_boxes(hw, patch_size, overlap_ratio))]
+    for l, p in enumerate(coarse_patch_sizes, 1):
+        boxes = scene_crop_boxes(hw, p, overlap_ratio)
+        if boxes != out[-1][1]:
+            out.append((l, boxes))
+    return out
+
+
+def _coarse_sizes(coarse_patch_sizes, hw: tuple) -> list:
+    sizes = []
+    for v in coarse_patch_sizes:
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+            raise ValueError(f"coarse_patch_sizes must be integers, got {v!r}")
+        sizes.append(int(v))
+    if any(b <= a for a, b in zip(sizes, sizes[1:])):
+        raise ValueError(f"coarse_patch_sizes must be strictly increasing, got {tuple(sizes)}")
+    H, W = hw
+    for c in sizes:
+        if min(c, H) * min(c, W) >= 1 << 31:
+            raise ValueError(f"a {min(c, H)} x {min(c, W)} window of coarse patch size {c} has 2^31 pixels or more, "
+                             f"beyond the mask statistics and RLE kernels")
+    return sizes
+
+
+# Device bytes of the bit-packed masks one batch of coarse-layer windows holds at once.  A coarse window's masks are
+# large (P^2 / 8 bytes each, H * W / 8 for the whole scene: 50 MB at 20 000^2), so they are pasted, cleaned and
+# encoded in chunks of at most this many bytes (at least one mask), with results independent of the chunk size.
+COARSE_MASK_BYTES = 1 << 30
+
+
+def _chunks(counts: list, per_mask: list, budget: int) -> list:
+    """Every window's kept rows as consecutive (window, j0, j1) segments, grouped so that one group's masks take at most
+    ``budget`` bytes (at least one mask per group)."""
+    groups, cur, used = [], [], 0
+    for b, k in enumerate(counts):
+        j = 0
+        while j < k:
+            room = (budget - used) // per_mask[b]
+            if room == 0 and cur:
+                groups.append(cur)
+                cur, used = [], 0
+                continue
+            j1 = min(k, j + max(room, 1))
+            cur.append((b, j, j1))
+            used += (j1 - j) * per_mask[b]
+            j = j1
+    if cur:
+        groups.append(cur)
+    return groups
+
+
+def _coarse_outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch.Tensor, p: dict, target_size: int,
+                    min_area: float, nms_thr: float, places: list) -> list:
+    """_outputs, then _remove_small_regions with min_area > 0, then _add_rle(places), for a batch of coarse-layer
+    windows, with the kept masks pasted, cleaned and encoded in groups of at most COARSE_MASK_BYTES: the same rows and
+    strings, without the masks.  Host synchronisations: the RLE's per group, one more for the second NMS."""
+    B = len(counts)
+    dev = idx.device
+    per_mask = [H * ((W + 15) // 16 * 2) for H, W in cand["sizes"]]
+    K = max(counts)
+    unchanged = torch.zeros(B, K, device=dev, dtype=torch.float32)
+    valid = torch.zeros(B, K, device=dev, dtype=torch.bool)
+    boxes = cand["boxes"].gather(1, idx[:, :K, None].expand(-1, -1, 4)).contiguous()
+    rle = [[] for _ in range(B)]
+    for group in _chunks(counts, per_mask, COARSE_MASK_BYTES):
+        parts = []
+        for b, j0, j1 in group:
+            bits = _paste(cand, b, idx[b, j0:j1], p["mask_threshold"], target_size)
+            if min_area > 0:
+                unchanged[b, j0:j1], boxes[b, j0:j1] = _clean(bits, cand["sizes"][b][1], min_area)
+            parts.append(dict(masks=bits, size=cand["sizes"][b]))
+        _add_rle(parts, places=[places[b] for b, _, _ in group])
+        for (b, _, _), r in zip(group, parts):
+            rle[b].extend(r["rle"])
+    out = []
+    for b in range(B):
+        k = counts[b]
+        ci = idx[b, :k]
+        valid[b, :k] = True
+        out.append(dict(scores=cand["iou"][b].index_select(0, ci),
+                        stability_scores=cand["stability"][b].index_select(0, ci), boxes=boxes[b, :k].long(),
+                        points=cand["points"][b].index_select(0, ci // cand["n_out"]),
+                        candidates=idx_host[b, :k].clone(), rle=rle[b], size=cand["sizes"][b]))
+    if min_area <= 0 or K == 0:
+        return out
+    rows_d, cnt, rows_h = _nms(unchanged, valid, boxes, nms_thr)
+    for b, r in enumerate(out):
+        rows, rh = rows_d[b, :cnt[b]], rows_h[b, :cnt[b]]
+        r.update(scores=r["scores"].index_select(0, rows), stability_scores=r["stability_scores"].index_select(0, rows),
+                 boxes=boxes[b].index_select(0, rows).long(), points=r["points"].index_select(0, rows),
+                 candidates=r["candidates"][rh], rle=[r["rle"][i] for i in rh.tolist()])
+    return out
+
+
 def _device_scene(scene: torch.Tensor, dev) -> torch.Tensor:
     """The scene [3, H, W] on dev, copied once in its own memory order (a permuted HWC array stays HWC)."""
     if scene.device == dev:
@@ -397,7 +517,8 @@ def generate_scene_masks(model, scene, *, patch_size: int | None = None, overlap
                          pred_iou_thresh: float = 0.88, stability_score_thresh: float = 0.95,
                          stability_score_offset: float = 1.0, mask_threshold: float = 0.0,
                          crops_nms_thresh: float = 0.7, crops_n_layers: int = 0, max_hole_area=None,
-                         max_sprinkle_area=None, min_mask_region_area: float = 0) -> dict:
+                         max_sprinkle_area=None, min_mask_region_area: float = 0,
+                         coarse_patch_sizes: tuple = ()) -> dict:
     """Every mask of a whole scene: generate_masks on overlapping windows, merged across windows.
 
     ``scene``: uint8 RGB [3, H, W] with any strides (a permuted HWC array is fine), on the host or the device; it is
@@ -418,14 +539,29 @@ def generate_scene_masks(model, scene, *, patch_size: int | None = None, overlap
     Objects larger than the overlap: as with SAM's crop layers without the whole-image layer, a mask is kept only
     from a window in which its box is more than 20 px from every interior edge.  An object is certain to be found
     only when its extent is below about int(overlap_ratio * P) - 42 px (214 px at the defaults); larger objects
-    crossing windows (fields, water bodies) may be found in none.
+    crossing windows (fields, water bodies) may be found in none, unless a coarse layer finds them.
+
+    ``coarse_patch_sizes`` (P_1 < P_2 < ..., each > P, integers): SAM's crop layers in the other direction, a pyramid
+    of coarser windows above the base ones (``scene_layer_windows``).  Layer l is scene_crop_boxes of P_l with the
+    same overlap; a size >= max(H, W) is one window, the whole scene, whose edge rule drops nothing.  A layer whose
+    windows are those of the previous layer (two sizes that both cover the scene, or a base layer that already is the
+    scene) is run once.  Each coarse window runs the same stages, but is resized to the model input by
+    ``rsp_resize_aa_pad_u8``, SamImageProcessor's antialiased resize (rsp_resize_pad_u8's cv2 resize aliases at these
+    downscales; the base layer keeps it, so its rows do not change).  Each layer's windows are merged as the base
+    layer's; then SAM's crop-layer rule prefers the smaller crop: one box NMS at ``crops_nms_thresh`` over [base rows,
+    layer 1 rows, ...] ranked by position, so every base row is kept, and a coarse row is kept iff it overlaps no
+    earlier kept row above the threshold.  Unlike SAM, whose 1 / crop-area scores tie within a layer, rows of one
+    layer are ranked by predicted IoU.  A coarse window's kept masks are pasted, cleaned and encoded in groups of at
+    most COARSE_MASK_BYTES.  Every coarse window must have fewer than 2^31 pixels (the mask statistics and RLE
+    kernels' limit); invalid sizes raise ValueError before device work.
 
     Windows run ``batch_size`` at a time through generate_masks' stages: the low-res logits of a batch (805 MB per
     window at the default grid) are freed before the next batch, and the kept masks of each window are encoded as
     COCO RLE of the whole H x W scene straight from the window's bits, which are then freed.  Masks the merge later
     suppresses were encoded for nothing: the price of memory that does not grow with the scene.  Host
     synchronisations: those of generate_masks(output_rle_mask=True) per batch, and one for the merge when some mask
-    was kept.  More than large_image.MAX_MERGE_CANDIDATES survivors raise ValueError before the merge; a merge
+    was kept; with coarse layers, the RLE's two per group of COARSE_MASK_BYTES rather than per batch in them, one
+    merge per layer and one for the cross-layer NMS.  More than large_image.MAX_MERGE_CANDIDATES survivors raise ValueError before the merge; a merge
     workspace (N^2 / 8 bytes) or a batch (scene copy, logits, pixel values and the worst case of bits) larger than
     free device memory raises RuntimeError, the batch before any window runs.
 
@@ -435,8 +571,9 @@ def generate_scene_masks(model, scene, *, patch_size: int | None = None, overlap
       stability_scores  fp32 [k]
       boxes             int64 [k, 4] inclusive pixel xyxy
       points            fp32 [k, 2] the prompt of each mask
-      tiles             int64 [k] window index (slice order)
+      tiles             int64 [k] window index in its layer (slice order)
       crop_boxes        int64 [k, 4] xyxy crop box of each mask's window
+      layers            int64 [k] 0 for the base layer, l for coarse_patch_sizes[l - 1]
       candidates        int64 [k] (host) candidate index in its window: point * 3 + output mask
       size              (H, W)
     All tensors but ``candidates`` are on the model's device."""
@@ -455,63 +592,111 @@ def generate_scene_masks(model, scene, *, patch_size: int | None = None, overlap
         raise ValueError(f"overlap_ratio must be in [0, 1), got {overlap_ratio}")
     if batch_size < 1:
         raise ValueError(f"batch_size must be >= 1, got {batch_size}")
+    coarse = _coarse_sizes(coarse_patch_sizes, (H, W))
+    if coarse and patch_size is not None and coarse[0] <= int(patch_size):
+        raise ValueError(f"coarse_patch_sizes must be greater than the patch size {int(patch_size)}, got {tuple(coarse)}")
     sam = _sam(model)
     dev = sam.prompt_encoder.no_mask_embed.weight.device
     S = sam.varch.image_size
     P = S if patch_size is None else int(patch_size)
-    crops = scene_crop_boxes((H, W), P, overlap_ratio)
-    T = len(crops)
-    B = min(int(batch_size), T)
+    if coarse and coarse[0] <= P:
+        raise ValueError(f"coarse_patch_sizes must be greater than the patch size {P}, got {tuple(coarse)}")
+    layers = scene_layer_windows((H, W), P, overlap_ratio, coarse)
     p = dict(points_per_side=int(points_per_side), points_per_batch=int(points_per_batch),
              pred_iou_thresh=float(pred_iou_thresh), stability_score_thresh=float(stability_score_thresh),
              stability_score_offset=float(stability_score_offset), mask_threshold=float(mask_threshold))
     nms_thr = float(crops_nms_thresh)
 
-    # what one batch holds at once, checked before any window runs
+    # what one batch of each layer holds at once, checked before any window runs
     n_cand = 3 * p["points_per_side"] ** 2
     hm = 4 * (S // sam.varch.patch_size)
-    ph, pw = min(P, H), min(P, W)
-    need = ((0 if scene.device == dev else 3 * H * W) + B * n_cand * hm * hm * 4 + B * 3 * S * S * 4
-            + B * n_cand * ph * ((pw + 15) // 16 * 2))
     free = _free_bytes(dev)
-    if need > free:
-        raise RuntimeError(f"a {H} x {W} scene in batches of {B} windows of {P}^2 needs {need / 2**30:.2f} GiB on {dev} "
-                           f"(the scene, {n_cand} candidates' low-res logits per window, the pixel values and the bits "
-                           f"if every candidate were kept); {free / 2**30:.2f} GiB are free")
+    for l, crops in layers:
+        B = min(int(batch_size), len(crops))
+        Pl = P if l == 0 else coarse[l - 1]
+        ph, pw = min(Pl, H), min(Pl, W)
+        bits = B * n_cand * ph * ((pw + 15) // 16 * 2)
+        if l:               # one group of masks, and the antialiased resize's horizontal pass
+            bits = min(bits, max(COARSE_MASK_BYTES, ph * ((pw + 15) // 16 * 2))) + B * 3 * ph * S
+        need = ((0 if scene.device == dev else 3 * H * W) + B * n_cand * hm * hm * 4 + B * 3 * S * S * 4 + bits)
+        if need > free:
+            raise RuntimeError(f"a {H} x {W} scene in batches of {B} windows of {Pl}^2 needs {need / 2**30:.2f} GiB on "
+                               f"{dev} (the scene, {n_cand} candidates' low-res logits per window, the pixel values and "
+                               f"the bits if every candidate were kept); {free / 2**30:.2f} GiB are free")
 
     img = _device_scene(scene, dev)
-    tiles = []
-    for b0 in range(0, T, B):
-        boxes_b = crops[b0:b0 + B]
-        views = [img[:, y0:y1, x0:x1] for x0, y0, x1, y1 in boxes_b]
-        pix, sizes, reshaped = _inputs(sam, views, None, None, None, dev)
-        cand = _candidates(sam, sam._encode(pix), sizes, reshaped, p, crops=[(cb, (H, W)) for cb in boxes_b])
-        del pix
-        idx, counts, idx_host = _nms(cand["iou"], cand["keep"], cand["boxes"], nms_thr)
-        out = _outputs(cand, idx, counts, idx_host, p["mask_threshold"], S)
-        del cand, idx                                           # the batch's low-res logits
-        if min_area > 0:
-            out = _remove_small_regions(out, min_area, nms_thr)
-        _add_rle(out, places=[(H, W, y0, x0) for x0, y0, _, _ in boxes_b])
-        for r in out:
-            del r["masks"]                                      # only the rows and strings stay
-        tiles.extend(out)
-    return _merge_tiles(tiles, crops, (H, W), nms_thr, dev)
+    merged = []
+    for l, crops in layers:
+        B = min(int(batch_size), len(crops))
+        tiles = []
+        for b0 in range(0, len(crops), B):
+            boxes_b = crops[b0:b0 + B]
+            views = [img[:, y0:y1, x0:x1] for x0, y0, x1, y1 in boxes_b]
+            pix, sizes, reshaped = _inputs(sam, views, None, None, None, dev, antialias=l > 0)
+            cand = _candidates(sam, sam._encode(pix), sizes, reshaped, p, crops=[(cb, (H, W)) for cb in boxes_b])
+            del pix
+            idx, counts, idx_host = _nms(cand["iou"], cand["keep"], cand["boxes"], nms_thr)
+            places = [(H, W, y0, x0) for x0, y0, _, _ in boxes_b]
+            if l:
+                out = _coarse_outputs(cand, idx, counts, idx_host, p, S, min_area, nms_thr, places)
+                del cand, idx
+            else:
+                out = _outputs(cand, idx, counts, idx_host, p["mask_threshold"], S)
+                del cand, idx                                   # the batch's low-res logits
+                if min_area > 0:
+                    out = _remove_small_regions(out, min_area, nms_thr)
+                _add_rle(out, places=places)
+                for r in out:
+                    del r["masks"]                              # only the rows and strings stay
+            tiles.extend(out)
+        merged.append((l, _merge_tiles(tiles, crops, (H, W), nms_thr, dev)))
+    if len(merged) == 1:
+        res = merged[0][1]
+        res["layers"] = torch.zeros(len(res["rle"]), device=dev, dtype=torch.int64)
+        return res
+    return _merge_layers(merged, nms_thr, dev)
 
 
-def _merge_tiles(tiles: list, crops: list, hw: tuple, nms_thr: float, dev) -> dict:
-    """The cross-window NMS of generate_scene_masks over every window's rows (in slice order, each in keep order)."""
+def _check_merge(N: int, what: str, dev) -> None:
     from .large_image import MAX_MERGE_CANDIDATES
-    counts = [r["scores"].shape[0] for r in tiles]
-    N = sum(counts)
     if N > MAX_MERGE_CANDIDATES:
-        raise ValueError(f"{len(tiles)} windows kept {N} masks; the cross-window merge's dense NMS takes at most "
+        raise ValueError(f"{what} kept {N} masks; the cross-window merge's dense NMS takes at most "
                          f"{MAX_MERGE_CANDIDATES} candidates")
     ws = N * ((N + 63) // 64) * 8
     free = _free_bytes(dev)
     if ws > free:
-        raise RuntimeError(f"the merge of {N} masks from {len(tiles)} windows needs a {ws / 2**30:.2f} GiB NMS workspace "
+        raise RuntimeError(f"the merge of {N} masks from {what} needs a {ws / 2**30:.2f} GiB NMS workspace "
                            f"on {dev}; {free / 2**30:.2f} GiB are free")
+
+
+def _merge_layers(merged: list, nms_thr: float, dev) -> dict:
+    """SAM's crop-layer rule over every layer's merged rows (``merged`` = [(layer, _merge_tiles result)], base first):
+    one box NMS over their concatenation ranked by position (equal scores and a stable sort), so a row is dropped only
+    by an earlier kept row, of its own layer or a finer one.  One host synchronisation."""
+    n = [len(m["rle"]) for _, m in merged]
+    N = sum(n)
+    _check_merge(N, f"{len(merged)} layers", dev)
+    layer_h = torch.repeat_interleave(torch.tensor([l for l, _ in merged]), torch.tensor(n, dtype=torch.int64))
+    cat = {key: torch.cat([m[key] for _, m in merged])
+           for key in ("scores", "stability_scores", "boxes", "points", "tiles", "crop_boxes", "candidates")}
+    res = dict(size=merged[0][1]["size"])
+    if N == 0:
+        return dict(res, rle=[], layers=layer_h.to(dev), **cat)
+    idx, cnt, idx_host = _nms(torch.zeros(1, N, device=dev), torch.ones(1, N, device=dev, dtype=torch.bool),
+                              cat["boxes"][None], nms_thr)
+    rows, rows_h = idx[0, :cnt[0]], idx_host[0, :cnt[0]]
+    rle = [s for _, m in merged for s in m["rle"]]
+    res.update({key: v.index_select(0, rows) for key, v in cat.items() if key != "candidates"})
+    res.update(rle=[rle[i] for i in rows_h.tolist()], candidates=cat["candidates"][rows_h],
+               layers=layer_h[rows_h].pin_memory().to(dev, non_blocking=True))
+    return res
+
+
+def _merge_tiles(tiles: list, crops: list, hw: tuple, nms_thr: float, dev) -> dict:
+    """The cross-window NMS of generate_scene_masks over every window's rows (in slice order, each in keep order)."""
+    counts = [r["scores"].shape[0] for r in tiles]
+    N = sum(counts)
+    _check_merge(N, f"{len(tiles)} windows", dev)
     tile_h = torch.repeat_interleave(torch.arange(len(tiles)), torch.tensor(counts, dtype=torch.int64))
     crop_h = torch.tensor(crops, dtype=torch.int64).view(-1, 4)[tile_h]
     res = dict(rle=[], scores=torch.zeros(0, device=dev), stability_scores=torch.zeros(0, device=dev),
@@ -588,8 +773,14 @@ def main(argv=None) -> list:
                          "about int(overlap * P) - 42 px may be missed")
     ap.add_argument("--patch-overlap-ratio", type=float, default=0.25, help="scene mode: window overlap ratio")
     ap.add_argument("--batch-size", type=int, default=4, help="scene mode: windows run at once")
+    ap.add_argument("--coarse-patch-sizes", type=int, nargs="+", default=None, metavar="P",
+                    help="scene mode: layers of coarser windows of these sizes (increasing, above --patch-size; one "
+                         ">= the scene's long side is the whole scene) that find objects larger than the overlap; "
+                         "each dict then has the \"layer\" it came from (0 = the --patch-size windows)")
     ap.add_argument("--out", default=None, help="JSON file for the mask dicts (default: stdout)")
     args = ap.parse_args(argv)
+    if args.coarse_patch_sizes is not None and args.patch_size is None:
+        ap.error("--coarse-patch-sizes needs --patch-size (scene mode)")
 
     import cv2
 
@@ -606,11 +797,15 @@ def main(argv=None) -> list:
     if args.patch_size is not None:
         rgb = torch.from_numpy(cv2.cvtColor(img, cv2.COLOR_BGR2RGB)).permute(2, 0, 1)      # [3, H, W] view of HWC
         res = generate_scene_masks(model, rgb, patch_size=args.patch_size, overlap_ratio=args.patch_overlap_ratio,
-                                   batch_size=args.batch_size, **kw)
+                                   batch_size=args.batch_size, coarse_patch_sizes=tuple(args.coarse_patch_sizes or ()),
+                                   **kw)
     else:
         rgb = torch.from_numpy(img).permute(2, 0, 1).flip(0)                 # BGR HWC -> RGB [3, H, W] view
         res = generate_masks(model, rgb.contiguous(), output_rle_mask=True, **kw)[0]
     rows = mask_dicts(res)
+    if args.coarse_patch_sizes is not None:
+        for row, layer in zip(rows, res["layers"].tolist()):
+            row["layer"] = layer
     text = json.dumps(rows)
     if args.out:
         with open(args.out, "w") as f:
