@@ -17,6 +17,7 @@
  *     rsp_last_error() returns a thread-local message for the last non-zero return.
  *   - bf16 = __nv_bfloat16 storage; matrices are row-major with an explicit leading
  *     dimension counted in elements.
+ *   - an optional input is a NULL pointer or a zero size; options never get sibling entry points.
  */
 #ifndef RSP_B200_H_
 #define RSP_B200_H_
@@ -27,7 +28,7 @@
 extern "C" {
 #endif
 
-#define RSP_ABI_VERSION 2
+#define RSP_ABI_VERSION 3
 
 int rsp_abi_version(void);
 const char* rsp_last_error(void);
@@ -42,10 +43,31 @@ const char* rsp_last_error(void);
  * Replaces: nn.Linear in SamVisionAttention.qkv/.proj (HF:717-718), SamMLPBlock (HF:132-143),
  * mmcv FFN (VS:282-288), patch-embed / 1x1 / im2col'ed 3x3 convs (HF:116,975-992; M:1009-1057,
  * 1296-1363; mmdet rpn_head.py:93-97), bbox-head FCs, and the SamAttention projections of the
- * mask decoder (HF:231-270). */
+ * mask decoder (HF:231-270).
+ * The fused epilogues of the SAM mask decoder (HF:461-543):
+ *   epi_mode 0  standard (as above)
+ *   epi_mode 1  out = LayerNorm_N(acc + bias + residual) * ln_gamma + ln_beta, N % 32 == 0, N <= 256:
+ *               layer_norm1-4 / layer_norm_final_attn fused into the preceding out_proj / lin2
+ *               (HF:316-347, 398-404)
+ *   epi_mode 2  columns = (tap, 64 ch): out = GELU(LN_64(acc + bias)): upscale_conv1 as a GEMM over the
+ *               2x2 taps + upscale_layer_norm + GELU (HF:519-520); output rows are then (pixel, tap)
+ *   epi_mode 3  rows = (prompt, y, x, tap1), columns = (tap2, 32 ch): mask_out[prompt, 4y+.., 4x+..] =
+ *               sum_c GELU(acc + bias)[tap2, c] * hyper[prompt, c]: upscale_conv2 + GELU + the
+ *               hypernetwork product (HF:521-531); `out` is unused
+ * ln_gamma / ln_beta / ln_eps serve epi_mode 1 and 2, hyper / mask_out / grid_h / grid_w epi_mode 3.
+ * res_block_map (int32 [M / res_block_rows], NULL = none) redirects the residual of row r to row
+ * map[r / res_block_rows] * res_block_rows + r % res_block_rows: prompts of one image share its
+ * embedding without the repeat_interleave copies of M:367-368 / M:1682-1683.
+ * epi_mode 0 with a NULL res_block_map is the plain GEMM above.
+ * Alignment (a call that breaks it returns RSP_ERR_INVALID, nothing launched):
+ *   epi_mode 1  out, residual, bias, ln_gamma, ln_beta 16-byte aligned; ldo, ldr % 8 == 0
+ *   epi_mode 2  N % 128 == 0, out 8-byte aligned, ldo % 4 == 0; bias, ln_gamma, ln_beta 16-byte aligned
+ *   epi_mode 3  hyper and bias 16-byte aligned, mask_out 8-byte aligned */
 int rsp_gemm_bf16(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M, int N,
                   int K, const float* bias, const void* residual, int ldr, int res_fp32, int res_mod,
-                  const int32_t* row_map, int act, int out_fp32, void* stream);
+                  const int32_t* row_map, int act, int out_fp32, int epi_mode, const float* ln_gamma,
+                  const float* ln_beta, float ln_eps, const int32_t* res_block_map, int res_block_rows,
+                  const float* hyper, float* mask_out, int grid_h, int grid_w, void* stream);
 
 /* 3x3 / stride 1 / pad 1 convolution on a bf16 NHWC map as an implicit GEMM (replaces F.conv2d of the FPN / RPN /
  * pixel-decoder ConvModules, e.g. M:1205-1216, dense_heads/rpn_head.py:60-75): x [B,H,W,C], Wt bf16 [N, 9*C] with
@@ -57,8 +79,8 @@ int rsp_conv3x3_nhwc_bf16(const void* x, int B, int H, int W, int C, const void*
                           int out_fp32, void* stream);
 int rsp_conv3x3_geometry_ok(int B, int H, int W, int C);
 
-/* Same contract on CUDA cores (one thread per output, GELU with erff): the independent check of the tensor-core
- * kernel in tests. */
+/* rsp_gemm_bf16's standard epilogue (epi_mode 0, no res_block_map) on CUDA cores (one thread per output, GELU with
+ * erff): the independent check of the tensor-core kernel in tests. */
 int rsp_gemm_bf16_simt(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M,
                        int N, int K, const float* bias, const void* residual, int ldr, int res_fp32,
                        int res_mod, const int32_t* row_map, int act, int out_fp32, void* stream);
@@ -71,15 +93,14 @@ int rsp_gemm_bf16_simt(const void* A, int lda, const void* W, int ldw, void* out
  * finite and within the float64 bound of oracle/encoder_attention.py for |v| <= 65280 (the largest bf16 that is a
  * finite fp16; larger |v| become inf), and each |v| below 2^-14 (fp16 subnormal) carries an absolute error of up
  * to 2^-25.
+ * out_row_map NULL: output rows in order.  Otherwise window_unpartition + crop (HF:925-952) is fused into the store:
+ * output row r of the (window-ordered) sequences goes to row out_row_map[r] of `out` (int32 [n_seq*T], -1 = padding
+ * token, dropped), so the projection that follows is a plain GEMM over the B*g*g token rows.
  * Replaces: SamVisionAttention.forward after the qkv Linear and before proj (HF:803-831,
- * HF:729-801) / Attention.forward + add_decomposed_rel_pos (VS:202-221, VS:117-157). */
+ * HF:729-801) / Attention.forward + add_decomposed_rel_pos (VS:202-221, VS:117-157).
+ * rsp_vit_attention_simt: the same on CUDA cores, without out_row_map (rows in order). */
 int rsp_vit_attention(const void* qkv, const void* rel_h, const void* rel_w, void* out, int n_seq,
-                      int T, int S, int H, int hd, void* stream);
-/* rsp_vit_attention with window_unpartition + crop (HF:925-952) fused into the store: output row r of the
- * (window-ordered) sequences goes to row out_row_map[r] of `out` (int32 [n_seq*T], -1 = padding token, dropped),
- * so the projection that follows is a plain GEMM over the B*g*g token rows. */
-int rsp_vit_attention_scatter(const void* qkv, const void* rel_h, const void* rel_w, void* out, int n_seq, int T,
-                              int Sg, int H, int hd, const int32_t* out_row_map, void* stream);
+                      int T, int S, int H, int hd, const int32_t* out_row_map, void* stream);
 
 int rsp_vit_attention_simt(const void* qkv, const void* rel_h, const void* rel_w, void* out,
                            int n_seq, int T, int S, int H, int hd, void* stream);
@@ -96,7 +117,7 @@ int rsp_layernorm(const void* in, int in_fp32, int ld_in, void* out, int out_fp3
                   float eps, int act, void* copy_out, int ld_copy, void* stream);
 
 /* out = LayerNorm(x + residual) over bf16 rows of C <= 256 channels (fp32 statistics): x bf16 [rows, C];
- * residual fp32 or bf16 [*, C], optionally block-mapped as in rsp_gemm_bf16_ex.  The
+ * residual fp32 or bf16 [*, C], optionally block-mapped as in rsp_gemm_bf16.  The
  * keys = layer_norm4(keys + attn_out) step of SamTwoWayAttentionBlock (HF:345-347).  If out_pe is not
  * NULL it also receives bf16(out + pos[row % pos_mod]) (pos fp32 [pos_mod, C]): "key = keys +
  * key_point_embedding" (HF:326,339), the operand of the following k / q projections. */
@@ -115,35 +136,11 @@ int rsp_im2col_nhwc(const void* in, void* out, int B, int H, int W, int C, int K
 /* [B, HW, C] (bf16 or fp32) -> fp32 [B, C, HW]: hands NCHW tensors back at module boundaries. */
 int rsp_nhwc_to_nchw(const void* in, int in_fp32, float* out, int B, int HW, int C, void* stream);
 
-/* rsp_gemm_bf16 with the fused epilogues of the SAM mask decoder (HF:461-543):
- *   epi_mode 0  standard (as rsp_gemm_bf16)
- *   epi_mode 1  out = LayerNorm_N(acc + bias + residual) * ln_gamma + ln_beta, N % 32 == 0, N <= 256:
- *               layer_norm1-4 / layer_norm_final_attn fused into the preceding out_proj / lin2
- *               (HF:316-347, 398-404)
- *   epi_mode 2  columns = (tap, 64 ch): out = GELU(LN_64(acc + bias)): upscale_conv1 as a GEMM over the
- *               2x2 taps + upscale_layer_norm + GELU (HF:519-520); output rows are then (pixel, tap)
- *   epi_mode 3  rows = (prompt, y, x, tap1), columns = (tap2, 32 ch): mask_out[prompt, 4y+.., 4x+..] =
- *               sum_c GELU(acc + bias)[tap2, c] * hyper[prompt, c]: upscale_conv2 + GELU + the
- *               hypernetwork product (HF:521-531); `out` is unused
- * res_block_map (int32 [M / res_block_rows]) redirects the residual of row r to row
- * map[r / res_block_rows] * res_block_rows + r % res_block_rows: prompts of one image share its
- * embedding without the repeat_interleave copies of M:367-368 / M:1682-1683.
- * Alignment (a call that breaks it returns RSP_ERR_INVALID, nothing launched):
- *   epi_mode 1  out, residual, bias, ln_gamma, ln_beta 16-byte aligned; ldo, ldr % 8 == 0
- *   epi_mode 2  N % 128 == 0, out 8-byte aligned, ldo % 4 == 0; bias, ln_gamma, ln_beta 16-byte aligned
- *   epi_mode 3  hyper and bias 16-byte aligned, mask_out 8-byte aligned */
-int rsp_gemm_bf16_ex(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M, int N,
-                     int K, const float* bias, const void* residual, int ldr, int res_fp32, int res_mod,
-                     const int32_t* row_map, int act, int out_fp32, int epi_mode, const float* ln_gamma,
-                     const float* ln_beta, float ln_eps, const int32_t* res_block_map,
-                     int res_block_rows, const float* hyper, float* mask_out, int grid_h, int grid_w,
-                     void* stream);
-
 /* epi_mode 3 for n_out (1..3) hypernetwork vectors per prompt in one GEMM: A bf16 [M, K] up1 rows (prompt, y, x,
  * tap1), W bf16 [128, K], hyper fp32 [prompts, n_out, 32] -> mask_out fp32 [prompts, n_out, 4*grid_h, 4*grid_w].
  * The multimask_output upscale of SamMaskDecoder (HF:521-531, mask_slice 1:): each accumulator tile of
  * upscale_conv2 feeds all n_out products, so the up1 rows are read once.  Output o has the bytes of
- * rsp_gemm_bf16_ex(epi_mode 3) with hyper[:, o].  hyper, bias 16-byte and mask_out 8-byte aligned. */
+ * rsp_gemm_bf16(epi_mode 3) with hyper[:, o].  hyper, bias 16-byte and mask_out 8-byte aligned. */
 int rsp_gemm_upscale_masks(const void* A, int lda, const void* W, int ldw, int M, int K, const float* bias,
                            const float* hyper, int n_out, float* mask_out, int grid_h, int grid_w, void* stream);
 
@@ -177,7 +174,7 @@ int rsp_t2i_fused(const void* keys, int ldk, const void* kvw, const float* kvb, 
  * keys bf16 [N*HW, 256] (row stride ldk; also the residual), Wq bf16 [128, 256], qb fp32 [128], pe_q bf16 [HW, 128],
  * ktok / vtok bf16 [N, Tq, 128], Wo bf16 [256, 128], ob / ln_g / ln_b fp32 [256], out bf16 [N*HW, 256]; HW % 64 == 0.
  * Q and the attention output never reach global memory; the bytes equal rsp_gemm_bf16 (Qimg) ->
- * rsp_i2t_attention -> rsp_gemm_bf16_ex (epi_mode 1, residual = keys). */
+ * rsp_i2t_attention -> rsp_gemm_bf16 (epi_mode 1, residual = keys). */
 int rsp_i2t_fused(const void* keys, int ldk, const void* wq, const float* qb, const void* pe_q, const void* ktok,
                   const void* vtok, const void* wo, const float* ob, const float* ln_g, const float* ln_b, float eps,
                   void* out, int N, int Tq, int HW, void* stream);
@@ -191,42 +188,39 @@ int rsp_i2t_fused(const void* keys, int ldk, const void* wq, const float* qb, co
  * scores[B, out_ld] at column out_off.  head_out fp32 [B*H*W, ld]: columns [0,A) objectness logits,
  * [A, 5A) deltas.  Anchors are generated analytically (AnchorGenerator, anchor_generator.py:161-301,
  * base_anchors fp32 [A, 4]); boxes failing min_bbox_size get score -1 (rpn_head.py:267-271).
- * stds4: HOST array of the coder's 4 target_stds (bbox_coder.stds; means must be 0).
+ * stds4: HOST array of the coder's 4 target_stds (bbox_coder.stds; means must be 0).  Boxes are clipped to
+ * (img_h, img_w) when img_shapes is NULL, otherwise every image to its own img_meta['img_shape']
+ * (rpn_head.py:208-215): img_shapes = DEVICE fp32 [B, 2] (h, w) per image - batches whose images were padded to a
+ * common shape by DetDataPreprocessor; img_h / img_w are then unused.
  * Replaces RPNHead._predict_by_feat_single's per-level body + DeltaXYWHBBoxCoder.decode
  * (rpn_head.py:188-226; delta_xywh_bbox_coder.py:325-359). */
 int rsp_rpn_decode(const float* head_out, int ld, const int64_t* topk_idx, int K, int B, int H, int W,
                    int A, int stride, const float* base_anchors, const float* stds4, float img_h, float img_w,
-                   float min_size, int out_off, int out_ld, float* boxes, float* scores, void* stream);
-/* ... clipping every image to its own img_meta['img_shape'] (rpn_head.py:208-215): img_shapes = DEVICE fp32 [B, 2]
- * (h, w) per image - batches whose images were padded to a common shape by DetDataPreprocessor. */
-int rsp_rpn_decode_shapes(const float* head_out, int ld, const int64_t* topk_idx, int K, int B, int H, int W, int A,
-                          int stride, const float* base_anchors, const float* stds4, const float* img_shapes,
-                          float min_size, int out_off, int out_ld, float* boxes, float* scores, void* stream);
+                   const float* img_shapes, float min_size, int out_off, int out_ld, float* boxes, float* scores,
+                   void* stream);
 
 /* RoI bbox head post-processing before NMS: softmax over C+1 logits, per-class delta2bbox with the
  * coder's target_stds (stds4: HOST array of 4 floats), score_thr filter; rois fp32 [n, 5], roi_valid uint8 [n] or NULL.  Outputs
- * scores [n*C] (-1 = filtered), boxes [n*C, 4], labels int64 [n*C].
+ * scores [n*C] (-1 = filtered), boxes [n*C, 4], labels int64 [n*C].  Boxes are clipped to (img_h, img_w) when
+ * img_shapes is NULL, otherwise to the per-image img_shape (bbox_head.py:545-548): img_shapes DEVICE fp32 [B, 2],
+ * indexed by rois[:, 0]; img_h / img_w are then unused.
  * Replaces BBoxHead._predict_by_feat_single up to multiclass_nms (bbox_head.py:520-555,
  * bbox_nms.py:45-75). */
 int rsp_bbox_cls_decode(const float* cls, int ld_cls, const float* reg, int ld_reg, const float* rois,
                         const uint8_t* roi_valid, int n, int C, const float* stds4, float img_h, float img_w,
-                        float score_thr, float* scores, float* boxes, int64_t* labels, void* stream);
-/* ... clipping to the per-image img_shape (bbox_head.py:545-548): img_shapes DEVICE fp32 [B, 2], indexed by rois[:, 0]. */
-int rsp_bbox_cls_decode_shapes(const float* cls, int ld_cls, const float* reg, int ld_reg, const float* rois,
-                               const uint8_t* roi_valid, int n, int C, const float* stds4, const float* img_shapes,
-                               float score_thr, float* scores, float* boxes, int64_t* labels, void* stream);
+                        const float* img_shapes, float score_thr, float* scores, float* boxes, int64_t* labels,
+                        void* stream);
 
 /* mmcv.ops.batched_nms semantics on score-sorted candidates: boxes fp32 [B, n, 4], ids int64 [B, n]
  * (level or class; boxes are offset by id * (max_coord + 1) exactly as mmcv does), nvalid int32 [B]
  * = length of the valid sorted prefix; keep uint8 [B, n].  Suppression when IoU > thr.
- * Workspaces: mask_ws uint64 [B, n, ceil(n/64)], max_coord_ws fp32 [B].
+ * Workspaces: mask_ws uint64 [B, n, ceil(n/64)], max_coord_ws fp32 [B].  max_keep 0 scans every candidate; max_keep > 0
+ * is for callers that only read the first max_keep kept candidates (batched_nms(...)[:max_per_img],
+ * rpn_head.py:285-291, bbox_nms.py:95-103): the greedy scan stops once max_keep candidates are kept, later keep flags
+ * are 0.
  * Replaces mmcv.ops.batched_nms / nms (rpn_head.py:285, bbox_nms.py:95). */
 int rsp_nms_batched(const float* boxes, const int64_t* ids, const int32_t* nvalid, int B, int n, float thr,
-                    void* mask_ws, float* max_coord_ws, uint8_t* keep, void* stream);
-/* ... for callers that only read the first max_keep kept candidates (batched_nms(...)[:max_per_img], rpn_head.py:285-291,
- * bbox_nms.py:95-103): the greedy scan stops once max_keep candidates are kept, later keep flags are 0. */
-int rsp_nms_batched_topk(const float* boxes, const int64_t* ids, const int32_t* nvalid, int B, int n, float thr,
-                         void* mask_ws, float* max_coord_ws, uint8_t* keep, int max_keep, void* stream);
+                    void* mask_ws, float* max_coord_ws, uint8_t* keep, int max_keep, void* stream);
 
 /* Greedy non-maximum merging (sahi's GREEDYNMM postprocess; no reference counterpart: the reference's large-image
  * merge is mmcv batched_nms).  Score-sorted candidates as rsp_nms_batched takes them: boxes fp32 [B, n, 4], labels
@@ -273,12 +267,23 @@ int rsp_roi_align_nhwc(const void* const* feats, const float* const* pes, const 
                        const int32_t* Ws, const float* scales, int num_levels, const float* rois, int n,
                        int C, int P, float finest_scale, void* out, void* stream);
 
-/* Mask post-processing: logits fp32 [n, hm, wm] -> uint8 [n, H, W] (W % 16 == 0), bilinear with
- * align_corners=False.  mode 0: bilinear(sigmoid(x)) >= thr (M:1758-1780); mode 1: bilinear(x) > thr
- * (M:652-656 + maskformer_fusion_head.py:169); mode 2: as mode 0 on input that rsp_sigmoid_f32 has
- * already activated (one exp per low-resolution pixel instead of four per output pixel). */
-int rsp_mask_paste(const float* logits, uint8_t* out, int n, int hm, int wm, int H, int W, float thr,
-                   int mode, void* stream);
+/* Mask post-processing: maps fp32 [n, hm, wm] -> thresholded masks, bilinear with align_corners=False.
+ * mode 0: bilinear(sigmoid(x)) >= thr (M:1758-1780); mode 1: bilinear(x) > thr (M:652-656 +
+ * maskformer_fusion_head.py:169); mode 2: as mode 0 on input that rsp_sigmoid_f32 has already activated (one exp
+ * per low-resolution pixel instead of four per output pixel).
+ * Hb == 0: one resize (hm, wm) -> (H, W); Wb, crop_h, crop_w are unused.  Otherwise the mask resize of
+ * RSPrompterAnchorMaskHead._predict_by_feat_single for resized / padded images (M:1763-1777), modes 1 and 2 only:
+ * bilinear to (Hb, Wb) = batch_input_shape -> crop [:crop_h, :crop_w] (the resized, unpadded image) -> bilinear to
+ * (H, W) = ori_shape -> threshold.  The intermediate map is never formed.
+ * packed = 0: out uint8 [n, H, W], (Hr, Wr) = (H, W).  packed = 1: out holds the masks bit-packed into record slots
+ * of Hr x Wr (H <= Hr, W <= Wr, Wr % 16 == 0, out 2-byte aligned): uint8 [n, Hr, Wr/8], pixel x = bit x % 8 of byte
+ * x / 8, the (H, W) mask at the slot's top-left, every other pixel 0.  With (Hr, Wr) = (H, W) the bits are
+ * rsp_pack_mask_bits of the byte output exactly (predict_records of resized images).
+ * One resize writes bytes for W % 16 == 0; it writes bits on the x4 path only (anchor variant, M:1758-1780 when
+ * ori_shape == batch shape): (H, W) = (4*hm, 4*wm) = (Hr, Wr), wm % 4 == 0, maps 16-byte aligned, mode 1 or 2.
+ * Any other combination returns RSP_ERR_INVALID, nothing launched. */
+int rsp_mask_paste(const float* maps, uint8_t* out, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w,
+                   int H, int W, int Hr, int Wr, int packed, float thr, int mode, void* stream);
 
 /* out = 1 / (1 + exp(-in)) over n fp32 values (n % 4 == 0): mask_preds.sigmoid() (M:1758). */
 int rsp_sigmoid_f32(const float* in, float* out, long long n, void* stream);
@@ -307,24 +312,19 @@ int rsp_groupnorm_nhwc(const void* x, float* stats_ws, const float* gamma, const
 /* mmcv MultiScaleDeformableAttention core (deformable_detr_layers.py:237-249): value bf16 [B,NQ,128] (8 heads x 16,
  * already value_proj'ed), ow fp32 [B*NQ, ld_ow] = [sampling_offsets (8*L*P*2) | attention logits (8*L*P)] from one
  * GEMM, levels hs/ws (HOST int arrays, low -> high resolution, sum h*w = NQ).  Softmax over L*P, reference point =
- * the query's own cell centre, bilinear zero-padded sampling as grid_sample(align_corners=False).  out bf16. */
+ * the query's own cell centre, bilinear zero-padded sampling as grid_sample(align_corners=False).  out bf16.
+ * channels = 8 heads x 16 (128) or 8 heads x 32 (256: the stock Mask2FormerHead's pixel decoder,
+ * configs/rsprompter/_base_/samseg-mask2former.py:104-112); value and out are [B, NQ, channels]. */
 int rsp_ms_deform_attn_sample(const void* value, const float* ow, int ld_ow, const int32_t* hs, const int32_t* ws,
-                              int L, int P, int B, int NQ, void* out, void* stream);
-/* ... with channels = 8 heads x 16 (128, as above) or 8 heads x 32 (256: the stock Mask2FormerHead's pixel decoder,
- * configs/rsprompter/_base_/samseg-mask2former.py:104-112). */
-int rsp_ms_deform_attn_sample_c(const void* value, const float* ow, int ld_ow, const int32_t* hs, const int32_t* ws,
-                                int L, int P, int B, int NQ, void* out, int channels, void* stream);
+                              int L, int P, int B, int NQ, void* out, int channels, void* stream);
 
-/* nn.MultiheadAttention core, 8 heads x 16 (mma.sync flash form): Q bf16 [B,nq,ldq], K / V bf16 [B,nk,ld*],
+/* nn.MultiheadAttention core, 8 heads x head_dim (mma.sync flash form): Q bf16 [B,nq,ldq], K / V bf16 [B,nk,ld*],
  * mask_bits uint64 [B*nq, ceil(nk/64)] (bit k%64 of word k/64 set = key k masked, shared by the heads) or NULL;
- * out bf16 [B,nq,128].  Masked cross-attention / self-attention of Mask2FormerTransformerDecoderLayer
- * (mask2former_layers.py:113-135). */
+ * out bf16 [B,nq,8*head_dim].  head_dim 16 (128 channels): masked cross-attention / self-attention of
+ * Mask2FormerTransformerDecoderLayer (mask2former_layers.py:113-135); head_dim 32 (256 channels): the stock
+ * Mask2FormerTransformerDecoder of samseg-mask2former.py:120-140, where 1/sqrt(32) multiplies the fp32 scores. */
 int rsp_mha_small(const void* Q, int ldq, const void* K, int ldk, const void* V, int ldv, const uint64_t* mask_bits,
-                  int B, int nq, int nk, void* out, void* stream);
-/* ... with head_dim 16 (as above) or 32 (8 heads x 32 = 256 channels, out bf16 [B,nq,256]: the stock
- * Mask2FormerTransformerDecoder of samseg-mask2former.py:120-140; 1/sqrt(32) multiplies the fp32 scores). */
-int rsp_mha_small_hd(const void* Q, int ldq, const void* K, int ldk, const void* V, int ldv, const uint64_t* mask_bits,
-                     int B, int nq, int nk, void* out, int head_dim, void* stream);
+                  int B, int nq, int nk, void* out, int head_dim, void* stream);
 
 /* attn_mask = sigmoid(x) < 0.5 (= x < 0) per row of level-sized mask logits fp32 [rows, ld >= nk]; a row whose keys
  * are all masked is cleared (M:386-392, M:439-442).  The logits are mask_embed x (bilinearly resized
@@ -347,24 +347,19 @@ int rsp_mask_embed_src(const float* mpp, const float* const* wts, const float* e
 int rsp_sam_mask_embed(const float* masks, const float* const* wts, int B, int hm, int wm, int h, int w, float eps,
                        float* dense, void* stream);
 
-/* Mask resize of RSPrompterAnchorMaskHead._predict_by_feat_single for resized / padded images (M:1763-1777): maps
- * fp32 [n, hm, wm] (mode 2: already sigmoid-activated, >= thr; mode 1: raw, > thr) -> bilinear to (Hb, Wb) =
- * batch_input_shape -> crop [:crop_h, :crop_w] (the resized, unpadded image) -> bilinear to (H, W) = ori_shape ->
- * threshold.  The intermediate map is never formed.  out uint8 [n, H, W]. */
-int rsp_mask_paste_rescale(const float* maps, uint8_t* out, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w,
-                           int H, int W, float thr, int mode, void* stream);
-
-/* rsp_query_postprocess for resized / padded images (M:652-656 + 679-691): logits -> (Hb, Wb) -> crop -> (H, W), then
- * mask = > 0, score, tight box as below.  part_ws fp32 [n_inst, ceil(H/16), 6]. */
-int rsp_query_postprocess_rescale(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst, int hm,
-                                  int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, uint8_t* masks,
-                                  float* part_ws, float* scores, float* boxes, void* stream);
-
 /* Instance post-processing of the query variant (M:652-656; maskformer_fusion_head.py:149-182; mask/utils.py:56-77):
  * for instance i (map sel[i] of logits fp32 [*, hm, wm]): bilinear to H x W, mask = > 0, score = cls_scores[i] *
- * mean sigmoid over the positive pixels, tight box.  part_ws fp32 [n_inst, ceil(H/16), 6]. */
+ * mean sigmoid over the positive pixels, tight box.  part_ws fp32 [n_inst, ceil(Hr/16), 6].
+ * Hb == 0: one resize (hm, wm) -> (H, W); Wb, crop_h, crop_w are unused.  Otherwise resized / padded images
+ * (M:652-656 + 679-691): logits -> (Hb, Wb) -> crop [:crop_h, :crop_w] -> (H, W), then mask, score and box as above.
+ * packed = 0: masks uint8 [n_inst, H, W], (Hr, Wr) = (H, W).  packed = 1: the masks bit-packed into record slots
+ * uint8 [n_inst, Hr, Wr/8] as rsp_mask_paste writes them; scores and boxes are bit-identical to the byte layout's.
+ * One resize writes bytes for W % 4 == 0; it writes bits on the x4 path only ((H, W) = (4*hm, 4*wm) = (Hr, Wr): the
+ * mask decoder always emits image/4 logits; wm % 4 == 0, logits 16-byte aligned).  Two resizes write bits for
+ * Wr <= 16384.  Any other combination returns RSP_ERR_INVALID, nothing launched. */
 int rsp_query_postprocess(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst, int hm, int wm,
-                          int H, int W, uint8_t* masks, float* part_ws, float* scores, float* boxes, void* stream);
+                          int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr, int Wr, int packed,
+                          uint8_t* masks, float* part_ws, float* scores, float* boxes, void* stream);
 
 /* ---- global attention on grids the flash kernel does not specialise (S = 48 / 80: 768^2 / 1280^2 inputs, VS:570-602):
  * three passes per image, all heads batched (rows stacked [H*T]), the two contractions on the wgmma GEMM:
@@ -395,29 +390,6 @@ int rsp_gemm_bf16_grouped(const void* A, int lda, const void* W, int ldw, void* 
  * row of W pixels is ceil(W/8) bytes, pixel x = bit (x % 8) of byte x / 8 (numpy.packbits(bitorder='little')).  This
  * is the device-side stand-in for encode_mask_results + collect_results (coco_metric.py:346-400, :365). ---- */
 
-/* rsp_query_postprocess with H = 4*hm, W = 4*wm (the mask decoder always emits image/4 logits) and the mask written
- * bit-packed: bits uint8 [n_inst, H, W/8].  Scores / boxes as rsp_query_postprocess.  part_ws fp32 [n_inst, H/16, 6]. */
-int rsp_query_postprocess_bits(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst, int hm,
-                               int wm, uint8_t* bits, float* part_ws, float* scores, float* boxes, void* stream);
-
-/* x4 bilinear + threshold of rsp_mask_paste (modes 1, 2) with bit-packed output: bits uint8 [n, 4*hm, 4*wm/8]
- * (anchor variant, M:1758-1780 when ori_shape == batch shape). */
-int rsp_mask_paste_bits(const float* maps, uint8_t* bits, int n, int hm, int wm, float thr, int mode, void* stream);
-
-/* rsp_mask_paste_rescale (the two resizes and the threshold, M:1763-1777) with bit-packed output into record slots of
- * Hr x Wr (H <= Hr, W <= Wr, Wr % 16 == 0): bits uint8 [n, Hr, Wr/8]; the (H, W) = ori_shape mask at the slot's
- * top-left, every other pixel 0.  With (Hr, Wr) = (H, W) the bits are rsp_pack_mask_bits of rsp_mask_paste_rescale's
- * output exactly (predict_records of resized images). */
-int rsp_mask_paste_rescale_bits(const float* maps, uint8_t* bits, int n, int hm, int wm, int Hb, int Wb, int crop_h,
-                                int crop_w, int H, int W, int Hr, int Wr, float thr, int mode, void* stream);
-
-/* rsp_query_postprocess_rescale (M:652-656 + 679-691) with the masks bit-packed as above; scores and boxes are
- * bit-identical to it.  part_ws fp32 [n_inst, ceil(Hr/16), 6]; Wr <= 16384. */
-int rsp_query_postprocess_rescale_bits(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst,
-                                       int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr,
-                                       int Wr, uint8_t* bits, float* part_ws, float* scores, float* boxes,
-                                       void* stream);
-
 /* Panoptic post-processing of the query variants: MaskFormerFusionHead.panoptic_postprocess
  * (mmdet/models/seg_heads/panoptic_fusion_heads/maskformer_fusion_head.py:41-106) after the resize of
  * RSMaskFormerFusionHead.predict (M:663-715; M:652-656 up-sampling), for n_img images of nq queries each, with no host
@@ -432,53 +404,44 @@ int rsp_query_postprocess_rescale_bits(const float* logits, const int32_t* sel, 
  * double (Python's float).  Workspaces: idx_ws uint16 [n_img, H*W], bits_ws uint32 [n_img, ceil(H*W/32)].  Outputs:
  * areas int32 [2, n_img*nq] (mask_area, then original_area; 0 for queries not kept), seg int32 [n_img*nq] (the segment
  * id of q, -1 when skipped or not kept), pan int32 [n_img, H, W].  nq < 65535, num_classes < 1000.
- * This entry point: one bilinear resize (hm, wm) -> (H, W) (the batch shape). */
+ * Hb == 0: one bilinear resize (hm, wm) -> (H, W) (the batch shape); Wb, crop_h, crop_w are unused.  Otherwise the
+ * two resizes of a resized / padded image (M:652-656 + 679-691): logits -> (Hb, Wb) -> crop [:crop_h, :crop_w] ->
+ * (H, W) (ori_shape with rescale, the crop itself without). */
 int rsp_panoptic_postprocess(const float* logits, const uint8_t* keep, const float* scores, const int32_t* labels,
-                             int n_img, int nq, int hm, int wm, int H, int W, int num_things, int num_classes,
-                             const double* iou_thr, int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws,
-                             int32_t* areas, int32_t* seg, int32_t* pan, void* stream);
-
-/* rsp_panoptic_postprocess through the two resizes of a resized / padded image (M:652-656 + 679-691): logits ->
- * (Hb, Wb) -> crop [:crop_h, :crop_w] -> (H, W) (ori_shape with rescale, the crop itself without). */
-int rsp_panoptic_postprocess_rescale(const float* logits, const uint8_t* keep, const float* scores,
-                                     const int32_t* labels, int n_img, int nq, int hm, int wm, int Hb, int Wb,
-                                     int crop_h, int crop_w, int H, int W, int num_things, int num_classes,
-                                     const double* iou_thr, int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws,
-                                     int32_t* areas, int32_t* seg, int32_t* pan, void* stream);
+                             int n_img, int nq, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                             int num_things, int num_classes, const double* iou_thr, int filter_low_score,
+                             uint16_t* idx_ws, uint32_t* bits_ws, int32_t* areas, int32_t* seg, int32_t* pan,
+                             void* stream);
 
 /* SAM automatic mask generation, per candidate mask, without the original-size fp32 mask ever existing.  Replaces, for
  * one crop layer, HF SamImageProcessor.post_process_masks(binarize=False) (image_processing_sam.py:423-425) followed by
  * filter_masks (:350-363): iou_scores > pred_iou_thresh, _compute_stability_score (:449-457), masks > mask_threshold and
- * _batched_mask_to_box (:460-506).  maps fp32 [n, hm, wm] low-res logits, geometry as rsp_mask_paste_rescale_bits
- * (bilinear to (Hb, Wb), crop, bilinear to (H, W)); every pixel is that kernel's sample, so the > thr decisions are its
- * bits exactly.  Outputs per mask: counts int32 [n, 3] = pixels > thr_hi, > thr_lo, > thr (thr_hi / thr_lo = mask_threshold
- * +/- stability_score_offset, rounded to fp32 as torch compares with a python scalar); boxes int32 [n, 4] inclusive
- * pixel xyxy of > thr, [0, 0, 0, 0] when empty; stability fp32 [n] = fp32(count_hi) / fp32(count_lo) (NaN for 0 / 0).
+ * _batched_mask_to_box (:460-506).  maps fp32 [n, hm, wm] low-res logits, geometry as rsp_mask_paste's two resizes
+ * (bilinear to (Hb, Wb), crop, bilinear to (H, W); Hb > 0); every pixel is that kernel's sample, so the > thr
+ * decisions are its bits exactly.  Outputs per mask: counts int32 [n, 3] = pixels > thr_hi, > thr_lo, > thr
+ * (thr_hi / thr_lo = mask_threshold +/- stability_score_offset, rounded to fp32 as torch compares with a python
+ * scalar); boxes int32 [n, 4] inclusive pixel xyxy of > thr, [0, 0, 0, 0] when empty; stability fp32 [n] =
+ * fp32(count_hi) / fp32(count_lo) (NaN for 0 / 0).
  * With iou fp32 [n] non-null, keep uint8 [n] = (pred_iou_thresh <= 0 or iou > pred_iou_thresh) and
  * (stability_score_thresh <= 0 or stability > stability_score_thresh).  part_ws int32 [n, ceil(H / 16), 7].
+ * scene_h == 0: no crop-edge rule; crop_x0 .. scene_w are unused.  Otherwise the masks are those of one crop of a
+ * larger scene, with HF filter_masks' crop-edge rule in the keep flag (image_processing_sam.py
+ * _is_box_near_crop_edge(box, crop_box, [0, 0, scene_w, scene_h], atol=20)): the H x W masks are the crop box
+ * (crop_x0, crop_y0, crop_x1, crop_y1) of a scene_h x scene_w scene, and a mask is also dropped when a side of its box
+ * (its empty-mask [0, 0, 0, 0] included), shifted by (crop_x0, crop_y0) and rounded to fp32, lies within 20 of the
+ * crop box's side and not within 20 of the scene's.  Applied in the same launch as the other tests; iou is required.
  * Integer reductions only: two calls give identical outputs.  n > 0, H * W < 2^31, n * ceil(H / 16) < 2^31. */
 int rsp_sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
                        float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                       float stability_score_thresh, int32_t* part_ws, int32_t* counts, int32_t* boxes,
-                       float* stability, uint8_t* keep, void* stream);
-
-/* rsp_sam_mask_stats for the masks of one crop of a larger scene, with HF filter_masks' crop-edge rule in the keep flag
- * (image_processing_sam.py _is_box_near_crop_edge(box, crop_box, [0, 0, scene_w, scene_h], atol=20)): the H x W masks
- * are the crop box (crop_x0, crop_y0, crop_x1, crop_y1) of a scene_h x scene_w scene, and a mask is also dropped when a
- * side of its box (its empty-mask [0, 0, 0, 0] included), shifted by (crop_x0, crop_y0) and rounded to fp32, lies within
- * 20 of the crop box's side and not within 20 of the scene's.  Applied in the same launch as the other tests; iou is
- * required.  Every other output and argument as rsp_sam_mask_stats. */
-int rsp_sam_mask_stats_crop(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H,
-                            int W, float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                            float stability_score_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1,
-                            int scene_h, int scene_w, int32_t* part_ws, int32_t* counts, int32_t* boxes,
-                            float* stability, uint8_t* keep, void* stream);
+                       float stability_score_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1, int scene_h,
+                       int scene_w, int32_t* part_ws, int32_t* counts, int32_t* boxes, float* stability,
+                       uint8_t* keep, void* stream);
 
 /* SAM automatic mask generation's small-region removal (min_mask_region_area) on bit-packed masks.  Replaces, per
  * kept mask, segment_anything/utils/amg.py remove_small_regions(mask, area_thresh, mode) as
  * SamAutomaticMaskGenerator.postprocess_small_regions calls it (cv2.connectedComponentsWithStats(., 8) + np.isin), and
  * batched_mask_to_box of its result.  in / out uint8 [n, H, ld] bit rows (pixel x = bit x % 8 of byte x / 8, ld even,
- * 8 * ld >= W, ld <= 4 * ceil(W / 32); rsp_mask_paste_rescale_bits' ld = ceil(W / 16) * 2); bits at x >= W are
+ * 8 * ld >= W, ld <= 4 * ceil(W / 32); rsp_mask_paste's packed ld = ceil(W / 16) * 2); bits at x >= W are
  * ignored on input and written as 0; out must not overlap in.  The working mask is ~mask (mode 0, holes) or mask
  * (mode 1, islands); its 8-connected components of area < min_area are "small":
  *   holes    out = mask | (every small component)
@@ -498,8 +461,8 @@ int rsp_mask_small_regions_bits(const uint8_t* in, uint8_t* out, int n, int H, i
 int rsp_mask_paste_boxes(const float* probs, const float* boxes, uint8_t* out, int n, int hm, int wm, int H, int W,
                          float thr, int packed, void* stream);
 
-/* Generic pack / unpack between uint8 {0,1} masks [rows, W] and the payload [rows, ceil(W/8)] (masks produced by the
- * *_rescale entry points; unpack is for consumers that want torch.bool masks back). */
+/* Generic pack / unpack between uint8 {0,1} masks [rows, W] and the payload [rows, ceil(W/8)] (masks produced in
+ * the byte layout; unpack is for consumers that want torch.bool masks back). */
 int rsp_pack_mask_bits(const uint8_t* masks, uint8_t* bits, long long rows, int W, void* stream);
 int rsp_unpack_mask_bits(const uint8_t* bits, uint8_t* masks, long long rows, int W, void* stream);
 

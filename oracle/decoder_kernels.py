@@ -115,7 +115,7 @@ def _res_rows(residual, m: int, res_mod: int = 0, res_block_map=None, res_block_
 
 def ln_row(a, w, bias, residual, gamma, beta, eps: float, res_mod: int = 0, res_block_map=None,
            res_block_rows: int = 0) -> torch.Tensor:
-    """rsp_gemm_bf16_ex epi_mode 1: LayerNorm_N(a W^T + bias + residual[rrow]) * gamma + beta, float64."""
+    """rsp_gemm_bf16 epi_mode 1: LayerNorm_N(a W^T + bias + residual[rrow]) * gamma + beta, float64."""
     x = a.to(D) @ w.to(D).t()
     if bias is not None:
         x = x + bias.to(D)

@@ -1,10 +1,10 @@
 """Float64 restatements of the anchor head's and the necks' standalone kernels (include/rsp_b200.h).  TEST
 INFRASTRUCTURE ONLY.
 
-  * ``rpn_decode``: rsp_rpn_decode(_shapes), sigmoid scores and delta2bbox boxes of the top-k anchors, with the
-    ``w > min_size and h > min_size`` filter (restate_anchor.delta2bbox, grid_anchors);
-  * ``bbox_cls_decode``: rsp_bbox_cls_decode(_shapes), a (C + 1)-way softmax with the background last, per-class
-    delta2bbox, ``score > thr`` and the padding RoIs masked;
+  * ``rpn_decode``: rsp_rpn_decode with and without img_shapes, sigmoid scores and delta2bbox boxes of the top-k
+    anchors, with the ``w > min_size and h > min_size`` filter (restate_anchor.delta2bbox, grid_anchors);
+  * ``bbox_cls_decode``: rsp_bbox_cls_decode with and without img_shapes, a (C + 1)-way softmax with the background
+    last, per-class delta2bbox, ``score > thr`` and the padding RoIs masked;
   * ``roi_align``: rsp_roi_align_nhwc, torchvision's roi_align (aligned=True, sampling_ratio=0) in float64 on the level
     restate_anchor.map_roi_levels picks in fp32 (mmdet computes it in fp32); with a PE table the reference is
     roi_align(feat + pe), since RoIAlign is linear;

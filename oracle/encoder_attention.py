@@ -1,6 +1,6 @@
-"""Float64 restatements of the ViT encoder's attention kernels (include/rsp_b200.h: rsp_vit_attention[_scatter],
-rsp_vit_attention_simt and the three-pass path of rsp_split_heads, rsp_transpose_cols, rsp_attn_softmax_bias and two
-grouped GEMMs).  TEST INFRASTRUCTURE ONLY.
+"""Float64 restatements of the ViT encoder's attention kernels (include/rsp_b200.h: rsp_vit_attention with and
+without out_row_map, rsp_vit_attention_simt and the three-pass path of rsp_split_heads, rsp_transpose_cols,
+rsp_attn_softmax_bias and two grouped GEMMs).  TEST INFRASTRUCTURE ONLY.
 
 ``attention`` is SamVisionAttention's core (HF:803-831, rel-pos HF:729-801) in float64 on the kernels' layout: qkv
 [n_seq*T, 3*H*hd] with columns [q | k | v], heads contiguous inside each; out [n_seq*T, H*hd].  The scale hd^-0.5

@@ -49,10 +49,10 @@ _vp, _i, _f = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
 _SIGNATURES = {
     "rsp_abi_version": ([], _i),
     "rsp_last_error": ([], ctypes.c_char_p),
-    "rsp_gemm_bf16": ([_vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp], _i),
+    "rsp_gemm_bf16": ([_vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i,
+                       _i, _vp, _vp, _f, _vp, _i, _vp, _vp, _i, _i, _vp], _i),
     "rsp_gemm_bf16_simt": ([_vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp], _i),
-    "rsp_vit_attention": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp], _i),
-    "rsp_vit_attention_scatter": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp], _i),
+    "rsp_vit_attention": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp], _i),
     "rsp_vit_attention_simt": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp], _i),
     "rsp_layernorm": ([_vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _f, _i, _vp, _i, _vp], _i),
     "rsp_patchify16": ([_vp, _vp, _i, _i, _i, _vp], _i),
@@ -61,51 +61,41 @@ _SIGNATURES = {
     "rsp_nhwc_to_nchw": ([_vp, _i, _vp, _i, _i, _i, _vp], _i),
     "rsp_cast_f32_bf16": ([_vp, _vp, ctypes.c_longlong, _vp], _i),
     "rsp_add_table_bf16": ([_vp, _vp, _vp, ctypes.c_longlong, ctypes.c_longlong, _vp], _i),
-    "rsp_gemm_bf16_ex": ([_vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i,
-                          _i, _vp, _vp, _f, _vp, _i, _vp, _vp, _i, _i, _vp], _i),
     "rsp_add_cast_bf16": ([_vp, _vp, _vp, ctypes.c_longlong, ctypes.c_longlong, _vp], _i),
     "rsp_token_self_attention": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp], _i),
     "rsp_t2i_attention": ([_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp], _i),
     "rsp_i2t_attention": ([_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp], _i),
     "rsp_t2i_fused": ([_vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp], _i),
     "rsp_i2t_fused": ([_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp], _i),
-    "rsp_rpn_decode": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _f, _f, _f, _i, _i, _vp, _vp, _vp], _i),
-    "rsp_bbox_cls_decode": ([_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _f, _f, _f, _vp, _vp, _vp, _vp], _i),
-    "rsp_rpn_decode_shapes": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp], _i),
-    "rsp_nms_batched_topk": ([_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _i, _vp], _i),
-    "rsp_bbox_cls_decode_shapes": ([_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp], _i),
-    "rsp_nms_batched": ([_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp], _i),
+    "rsp_rpn_decode": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _f, _f, _vp, _f, _i, _i, _vp, _vp, _vp], _i),
+    "rsp_bbox_cls_decode": ([_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _f, _f, _vp, _f, _vp, _vp, _vp, _vp], _i),
+    "rsp_nms_batched": ([_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _i, _vp], _i),
     "rsp_nmm_batched": ([_vp, _vp, _vp, _i, _i, _f, _i, _vp, _vp, _vp, _vp], _i),
     "rsp_compact_keep": ([_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp], _i),
     "rsp_soft_nms_workspace_bytes": ([_i, _i, _i, _vp], _i),
     "rsp_soft_nms_batched": ([_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _f, _i, _i, _i, _vp, ctypes.c_size_t, _vp, _vp,
                               _vp, _vp, _vp, _vp], _i),
     "rsp_roi_align_nhwc": ([_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _f, _vp, _vp], _i),
-    "rsp_mask_paste": ([_vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp], _i),
+    "rsp_mask_paste": ([_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp], _i),
     "rsp_pool2_nhwc": ([_vp, _vp, _i, _i, _i, _i, _i, _vp], _i),
     "rsp_zero_border_nhwc": ([_vp, _i, _i, _i, _i, _vp], _i),
     "rsp_sigmoid_f32": ([_vp, _vp, ctypes.c_longlong, _vp], _i),
     "rsp_mask_paste_boxes": ([_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp], _i),
     "rsp_groupnorm_nhwc": ([_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp], _i),
-    "rsp_ms_deform_attn_sample": ([_vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp], _i),
-    "rsp_mha_small": ([_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _vp, _vp], _i),
-    "rsp_ms_deform_attn_sample_c": ([_vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp], _i),
-    "rsp_mha_small_hd": ([_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp], _i),
+    "rsp_ms_deform_attn_sample": ([_vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp], _i),
+    "rsp_mha_small": ([_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp], _i),
     "rsp_conv3x3_nhwc_bf16": ([_vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _vp], _i),
     "rsp_conv3x3_geometry_ok": ([_i, _i, _i, _i], _i),
-    "rsp_mask_paste_rescale": ([_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, ctypes.c_float, _i, _vp], _i),
-    "rsp_query_postprocess_rescale": ([_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp], _i),
     "rsp_attn_mask_bits": ([_vp, _i, _i, _i, _vp, _vp], _i),
     "rsp_resize_bilinear_nhwc": ([_vp, _i, _i, _i, _i, _i, _i, _vp, _vp], _i),
     "rsp_mask_embed_src": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp], _i),
-    "rsp_query_postprocess": ([_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp], _i),
+    "rsp_query_postprocess": ([_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp],
+                              _i),
     "rsp_sin_fold": ([_vp, _vp, ctypes.c_longlong, _vp], _i),
     "rsp_attn_softmax_bias": ([_vp, _i, _vp, _i, _i, _vp, _i, _i, _i, _i, _f, _vp], _i),
     "rsp_transpose_cols": ([_vp, _i, _i, _i, _i, _i, _vp, _vp], _i),
     "rsp_split_heads": ([_vp, _i, _i, _i, _i, _i, _i, _vp, _vp], _i),
     "rsp_gemm_bf16_grouped": ([_vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp], _i),
-    "rsp_query_postprocess_bits": ([_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp], _i),
-    "rsp_mask_paste_bits": ([_vp, _vp, _i, _i, _i, _f, _i, _vp], _i),
     "rsp_pack_mask_bits": ([_vp, _vp, ctypes.c_longlong, _i, _vp], _i),
     "rsp_unpack_mask_bits": ([_vp, _vp, ctypes.c_longlong, _i, _vp], _i),
     "rsp_preprocess_u8": ([_vp, _i, _i, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp, _i, _i, _vp, _vp,
@@ -115,9 +105,6 @@ _SIGNATURES = {
     "rsp_resize_aa_pad_u8_ws_bytes": ([_vp, _i, _vp], _i),
     "rsp_resize_aa_pad_u8": ([_vp, _vp, _vp, _vp, ctypes.c_longlong, _i, _vp, ctypes.c_longlong, _vp, _i, _i, _vp, _vp,
                               _i, _vp, _vp], _i),
-    "rsp_mask_paste_rescale_bits": ([_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp], _i),
-    "rsp_query_postprocess_rescale_bits": ([_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp,
-                                            _vp, _vp], _i),
     "rsp_mask_rle_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp], _i),
     "rsp_mask_rle_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
     "rsp_mask_rle_placed_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp], _i),
@@ -126,15 +113,11 @@ _SIGNATURES = {
     "rsp_mask_rle_union_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp], _i),
     "rsp_gemm_upscale_masks": ([_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _i, _vp], _i),
     "rsp_sam_mask_embed": ([_vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp], _i),
-    "rsp_sam_mask_stats": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _vp, _vp, _vp, _vp, _vp,
-                            _vp], _i),
-    "rsp_sam_mask_stats_crop": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _i, _i, _i, _i, _i,
-                                 _i, _vp, _vp, _vp, _vp, _vp, _vp], _i),
+    "rsp_sam_mask_stats": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _i, _i, _i, _i, _i, _i,
+                            _vp, _vp, _vp, _vp, _vp, _vp], _i),
     "rsp_mask_small_regions_bits": ([_vp, _vp, _i, _i, _i, _i, ctypes.c_longlong, _i, _vp, _vp, _vp, _vp], _i),
-    "rsp_panoptic_postprocess": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp,
-                                  _vp], _i),
-    "rsp_panoptic_postprocess_rescale": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i,
-                                          _vp, _vp, _vp, _vp, _vp, _vp], _i),
+    "rsp_panoptic_postprocess": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp,
+                                  _vp, _vp, _vp, _vp], _i),
 }
 
 
@@ -210,7 +193,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, *,
          row_map: torch.Tensor | None = None, out_rows: int | None = None,
          simt: bool = False, ln: tuple | None = None, ln64_gelu: tuple | None = None,
          res_block_map: torch.Tensor | None = None, res_block_rows: int = 0) -> torch.Tensor:
-    """``out[row_map[m]] = act(a @ w.T + bias) + residual`` (see rsp_gemm_bf16 / _ex in the header).
+    """``out[row_map[m]] = act(a @ w.T + bias) + residual`` (see rsp_gemm_bf16 in the header).
 
     a: bf16 [M, K] (row stride may exceed K); w: bf16 [N, K]; bias fp32 [N].
     ln=(gamma, beta, eps): LayerNorm over the whole output row after bias + residual (N <= 256).
@@ -249,16 +232,13 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, *,
         assert not simt
         if g is not None:
             assert g.dtype == torch.float32 and b.dtype == torch.float32 and g.is_contiguous() and b.is_contiguous()
-        st = _lib.rsp_gemm_bf16_ex(_ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(out), out.stride(0),
-                                   M, N, K, _ptr(bias), _ptr(residual), ldr, res_fp32, res_mod,
-                                   _ptr(row_map), ACT[act], int(out.dtype == torch.float32), epi,
-                                   _ptr(g), _ptr(b), float(eps), _ptr(res_block_map), res_block_rows,
-                                   None, None, 0, 0, _stream())
+    args = (_ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(out), out.stride(0), M, N, K, _ptr(bias), _ptr(residual),
+            ldr, res_fp32, res_mod, _ptr(row_map), ACT[act], int(out.dtype == torch.float32))
+    if simt:
+        st = _lib.rsp_gemm_bf16_simt(*args, _stream())
     else:
-        fn = _lib.rsp_gemm_bf16_simt if simt else _lib.rsp_gemm_bf16
-        st = fn(_ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(out), out.stride(0), M, N, K, _ptr(bias),
-                _ptr(residual), ldr, res_fp32, res_mod, _ptr(row_map), ACT[act],
-                int(out.dtype == torch.float32), _stream())
+        st = _lib.rsp_gemm_bf16(*args, epi, _ptr(g), _ptr(b), float(eps), _ptr(res_block_map), res_block_rows,
+                                None, None, 0, 0, _stream())
     _check(st, "rsp_gemm_bf16")
     launch_count += 1
     if not simt:
@@ -311,10 +291,10 @@ def gemm_upscale_mask(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, hype
     if out is None:
         out = torch.empty((P, 4 * grid_h, 4 * grid_w), device=a.device, dtype=torch.float32)
     assert out.is_contiguous() and out.dtype == torch.float32
-    st = _lib.rsp_gemm_bf16_ex(_ptr(a), a.stride(0), _ptr(w), w.stride(0), None, 0, M, 128, K, _ptr(bias),
-                               None, 0, 1, 0, None, 0, 0, 3, None, None, 0.0, None, 0, _ptr(hyper),
-                               _ptr(out), grid_h, grid_w, _stream())
-    _check(st, "rsp_gemm_bf16_ex(upscale_mask)")
+    st = _lib.rsp_gemm_bf16(_ptr(a), a.stride(0), _ptr(w), w.stride(0), None, 0, M, 128, K, _ptr(bias),
+                            None, 0, 1, 0, None, 0, 0, 3, None, None, 0.0, None, 0, _ptr(hyper),
+                            _ptr(out), grid_h, grid_w, _stream())
+    _check(st, "rsp_gemm_bf16(upscale_mask)")
     launch_count += 1
     _log("gemm", 2.0 * M * 128 * K)
     return out
@@ -503,19 +483,17 @@ def vit_attention(qkv: torch.Tensor, rel_h: torch.Tensor, rel_w: torch.Tensor, n
         assert not simt and out_row_map.dtype == torch.int32 and out_row_map.is_contiguous()
         assert out_row_map.numel() == n_seq * T and out_rows is not None
         _require_cuda(out_row_map)
-        if out is None:
-            out = torch.empty((out_rows, D), device=qkv.device, dtype=torch.bfloat16)
-        assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape == (out_rows, D)
-        _check(_lib.rsp_vit_attention_scatter(_ptr(qkv), _ptr(rel_h), _ptr(rel_w), _ptr(out), n_seq, T, S, H, hd,
-                                              _ptr(out_row_map), _stream()), "rsp_vit_attention_scatter")
-        launch_count += 1
-        return out
+    else:
+        out_rows = n_seq * T
     if out is None:
-        out = torch.empty((n_seq * T, D), device=qkv.device, dtype=torch.bfloat16)
-    assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape == (n_seq * T, D)
-    fn = _lib.rsp_vit_attention_simt if simt else _lib.rsp_vit_attention
-    _check(fn(_ptr(qkv), _ptr(rel_h), _ptr(rel_w), _ptr(out), n_seq, T, S, H, hd, _stream()),
-           "rsp_vit_attention")
+        out = torch.empty((out_rows, D), device=qkv.device, dtype=torch.bfloat16)
+    assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape == (out_rows, D)
+    args = (_ptr(qkv), _ptr(rel_h), _ptr(rel_w), _ptr(out), n_seq, T, S, H, hd)
+    if simt:
+        st = _lib.rsp_vit_attention_simt(*args, _stream())
+    else:
+        st = _lib.rsp_vit_attention(*args, _ptr(out_row_map), _stream())
+    _check(st, "rsp_vit_attention")
     launch_count += 1
     return out
 
@@ -711,14 +689,10 @@ def rpn_decode(head_out: torch.Tensor, topk_idx: torch.Tensor, B: int, H: int, W
     if img_shapes is not None:
         _require_cuda(img_shapes)
         assert img_shapes.dtype == torch.float32 and img_shapes.is_contiguous() and img_shapes.shape == (B, 2)
-        _check(_lib.rsp_rpn_decode_shapes(_ptr(head_out), head_out.stride(0), _ptr(topk_idx), K, B, H, W, A, stride,
-                                          _ptr(base_anchors), _host_f4(stds), _ptr(img_shapes), float(min_size), out_off,
-                                          scores.shape[1], _ptr(boxes), _ptr(scores), _stream()), "rsp_rpn_decode_shapes")
-        launch_count += 1
-        return
     _check(_lib.rsp_rpn_decode(_ptr(head_out), head_out.stride(0), _ptr(topk_idx), K, B, H, W, A, stride,
-                               _ptr(base_anchors), _host_f4(stds), float(img_hw[0]), float(img_hw[1]), float(min_size),
-                               out_off, scores.shape[1], _ptr(boxes), _ptr(scores), _stream()), "rsp_rpn_decode")
+                               _ptr(base_anchors), _host_f4(stds), float(img_hw[0]), float(img_hw[1]), _ptr(img_shapes),
+                               float(min_size), out_off, scores.shape[1], _ptr(boxes), _ptr(scores), _stream()),
+           "rsp_rpn_decode")
     launch_count += 1
 
 
@@ -740,15 +714,10 @@ def bbox_cls_decode(cls: torch.Tensor, reg: torch.Tensor, rois: torch.Tensor, ro
     if img_shapes is not None:
         _require_cuda(img_shapes)
         assert img_shapes.dtype == torch.float32 and img_shapes.is_contiguous() and img_shapes.shape[1] == 2
-        _check(_lib.rsp_bbox_cls_decode_shapes(_ptr(cls), cls.stride(0), _ptr(reg), reg.stride(0), _ptr(rois),
-                                               _ptr(roi_valid), n, C, _host_f4(stds), _ptr(img_shapes), float(score_thr),
-                                               _ptr(scores), _ptr(boxes), _ptr(labels), _stream()),
-               "rsp_bbox_cls_decode_shapes")
-    else:
-        _check(_lib.rsp_bbox_cls_decode(_ptr(cls), cls.stride(0), _ptr(reg), reg.stride(0), _ptr(rois),
-                                        _ptr(roi_valid), n, C, _host_f4(stds), float(img_hw[0]), float(img_hw[1]),
-                                        float(score_thr), _ptr(scores), _ptr(boxes), _ptr(labels), _stream()),
-               "rsp_bbox_cls_decode")
+    _check(_lib.rsp_bbox_cls_decode(_ptr(cls), cls.stride(0), _ptr(reg), reg.stride(0), _ptr(rois), _ptr(roi_valid), n,
+                                    C, _host_f4(stds), float(img_hw[0]), float(img_hw[1]), _ptr(img_shapes),
+                                    float(score_thr), _ptr(scores), _ptr(boxes), _ptr(labels), _stream()),
+           "rsp_bbox_cls_decode")
     launch_count += 1
     return scores, boxes, labels
 
@@ -767,8 +736,8 @@ def nms_batched(boxes: torch.Tensor, ids: torch.Tensor, nvalid: torch.Tensor, io
     mask_ws = torch.empty(B * n * words, device=boxes.device, dtype=torch.int64)
     mx = torch.empty(B, device=boxes.device, dtype=torch.float32)
     keep = torch.empty(B, n, device=boxes.device, dtype=torch.uint8)
-    _check(_lib.rsp_nms_batched_topk(_ptr(boxes), _ptr(ids), _ptr(nvalid), B, n, float(iou_thr), _ptr(mask_ws),
-                                     _ptr(mx), _ptr(keep), int(max_keep), _stream()), "rsp_nms_batched_topk")
+    _check(_lib.rsp_nms_batched(_ptr(boxes), _ptr(ids), _ptr(nvalid), B, n, float(iou_thr), _ptr(mask_ws), _ptr(mx),
+                                _ptr(keep), int(max_keep), _stream()), "rsp_nms_batched")
     launch_count += 3
     return keep
 
@@ -905,13 +874,18 @@ def mask_paste(logits: torch.Tensor, thr: float, *, raw: bool, size: tuple | Non
     if rescale is not None:
         assert n > 0
         (Hb, Wb), (ch, cw), (H, W) = rescale
+    else:
+        Hb = Wb = ch = cw = 0
+        H, W = size if bits is None else (4 * hm, 4 * wm)
+    Hr, Wr = H, W
     if bits is None:
-        out = torch.empty(n, *(size if rescale is None else (H, W)), device=logits.device, dtype=torch.uint8)
+        out = torch.empty(n, H, W, device=logits.device, dtype=torch.uint8)
     elif rescale is None:
         assert size is None or tuple(size) == (4 * hm, 4 * wm)
         assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.numel() == n * 4 * hm * (wm // 2)
     else:
         assert bits.dtype == torch.uint8 and bits.is_contiguous() and bits.dim() == 3 and bits.shape[0] == n
+        Hr, Wr = bits.shape[1], bits.shape[2] * 8
     if n == 0:
         return out.view(torch.bool) if bits is None else bits
     mode = 1 if raw else 2
@@ -919,19 +893,8 @@ def mask_paste(logits: torch.Tensor, thr: float, *, raw: bool, size: tuple | Non
         mode = 0   # rsp_sigmoid_f32 takes numel % 4 == 0; rsp_mask_paste's mode 0 activates the taps instead
     elif not raw:
         logits = sigmoid_f32(logits)   # activate once per low-res pixel, then paste
-    if rescale is None and bits is None:
-        _check(_lib.rsp_mask_paste(_ptr(logits), _ptr(out), n, hm, wm, size[0], size[1], float(thr), mode, _stream()),
-               "rsp_mask_paste")
-    elif rescale is None:
-        _check(_lib.rsp_mask_paste_bits(_ptr(logits), _ptr(bits), n, hm, wm, float(thr), mode, _stream()),
-               "rsp_mask_paste_bits")
-    elif bits is None:
-        _check(_lib.rsp_mask_paste_rescale(_ptr(logits), _ptr(out), n, hm, wm, Hb, Wb, ch, cw, H, W, float(thr), mode,
-                                           _stream()), "rsp_mask_paste_rescale")
-    else:
-        _check(_lib.rsp_mask_paste_rescale_bits(_ptr(logits), _ptr(bits), n, hm, wm, Hb, Wb, ch, cw, H, W, bits.shape[1],
-                                                bits.shape[2] * 8, float(thr), mode, _stream()),
-               "rsp_mask_paste_rescale_bits")
+    _check(_lib.rsp_mask_paste(_ptr(logits), _ptr(out if bits is None else bits), n, hm, wm, Hb, Wb, ch, cw, H, W, Hr,
+                               Wr, int(bits is not None), float(thr), mode, _stream()), "rsp_mask_paste")
     launch_count += 1
     return out.view(torch.bool) if bits is None else bits
 
@@ -943,7 +906,7 @@ def sam_mask_stats(logits: torch.Tensor, rescale: tuple, mask_threshold: float =
     (pad_hw, reshaped_hw, original_hw) as mask_paste's.  -> counts int32 [n, 3] (> thr + offset, > thr - offset,
     > thr), boxes int32 [n, 4] (HF's inclusive xyxy of > thr), stability fp32 [n], keep bool [n] (None without iou).
     ``crop`` = ((x0, y0, x1, y1), (scene_h, scene_w)): the masks are that crop box of a larger scene, and the keep flag
-    also applies HF's crop-edge rule (rsp_sam_mask_stats_crop; needs iou)."""
+    also applies HF's crop-edge rule (needs iou)."""
     global launch_count
     _require_cuda(logits, iou)
     assert crop is None or iou is not None, "the crop-edge rule is part of the keep flag: pass iou"
@@ -963,17 +926,11 @@ def sam_mask_stats(logits: torch.Tensor, rescale: tuple, mask_threshold: float =
     part = torch.empty(n, (H + 15) // 16, 7, device=dev, dtype=torch.int32)
     thr = float(mask_threshold)
     thr_hi, thr_lo = thr + float(stability_score_offset), thr - float(stability_score_offset)
-    if crop is None:
-        _check(_lib.rsp_sam_mask_stats(_ptr(logits), n, hm, wm, Hb, Wb, ch, cw, H, W, thr, thr_hi, thr_lo, _ptr(iou),
-                                       float(pred_iou_thresh), float(stability_score_thresh), _ptr(part), _ptr(counts),
-                                       _ptr(boxes), _ptr(stability), _ptr(keep), _stream()), "rsp_sam_mask_stats")
-    else:
-        (x0, y0, x1, y1), (sh, sw) = crop
-        _check(_lib.rsp_sam_mask_stats_crop(_ptr(logits), n, hm, wm, Hb, Wb, ch, cw, H, W, thr, thr_hi, thr_lo,
-                                            _ptr(iou), float(pred_iou_thresh), float(stability_score_thresh), int(x0),
-                                            int(y0), int(x1), int(y1), int(sh), int(sw), _ptr(part), _ptr(counts),
-                                            _ptr(boxes), _ptr(stability), _ptr(keep), _stream()),
-               "rsp_sam_mask_stats_crop")
+    (x0, y0, x1, y1), (sh, sw) = crop if crop is not None else ((0, 0, 0, 0), (0, 0))
+    _check(_lib.rsp_sam_mask_stats(_ptr(logits), n, hm, wm, Hb, Wb, ch, cw, H, W, thr, thr_hi, thr_lo, _ptr(iou),
+                                   float(pred_iou_thresh), float(stability_score_thresh), int(x0), int(y0), int(x1),
+                                   int(y1), int(sh), int(sw), _ptr(part), _ptr(counts), _ptr(boxes), _ptr(stability),
+                                   _ptr(keep), _stream()), "rsp_sam_mask_stats")
     launch_count += 2
     return counts, boxes, stability, None if keep is None else keep.view(torch.bool)
 
@@ -1145,8 +1102,9 @@ def ms_deform_attn_sample(value: torch.Tensor, ow: torch.Tensor, shapes: list, p
     hs = (ctypes.c_int32 * L)(*[s[0] for s in shapes])
     ws = (ctypes.c_int32 * L)(*[s[1] for s in shapes])
     out = torch.empty(B * NQ, E, device=value.device, dtype=torch.bfloat16)
-    _check(_lib.rsp_ms_deform_attn_sample_c(_ptr(value), _ptr(ow), ow.stride(0), ctypes.cast(hs, _vp), ctypes.cast(ws, _vp),
-                                            L, points, B, NQ, _ptr(out), E, _stream()), "rsp_ms_deform_attn_sample_c")
+    _check(_lib.rsp_ms_deform_attn_sample(_ptr(value), _ptr(ow), ow.stride(0), ctypes.cast(hs, _vp),
+                                          ctypes.cast(ws, _vp), L, points, B, NQ, _ptr(out), E, _stream()),
+           "rsp_ms_deform_attn_sample")
     launch_count += 1
     return out
 
@@ -1163,8 +1121,8 @@ def mha_small(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, B: int, nq: int
         assert mask.dtype == torch.int64 and mask.is_contiguous() and mask.shape == (B * nq, (nk + 63) // 64)
     assert head_dim in (16, 32)
     out = torch.empty(B * nq, 8 * head_dim, device=q.device, dtype=torch.bfloat16)
-    _check(_lib.rsp_mha_small_hd(_ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(mask), B, nq, nk,
-                                 _ptr(out), head_dim, _stream()), "rsp_mha_small_hd")
+    _check(_lib.rsp_mha_small(_ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(mask), B, nq, nk,
+                              _ptr(out), head_dim, _stream()), "rsp_mha_small")
     launch_count += 1
     return out
 
@@ -1228,6 +1186,7 @@ def query_postprocess(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch
     _, hm, wm = logits.shape
     assert logits.dtype == torch.float32 and logits.is_contiguous() and sel.dtype == torch.int32 and cls_scores.dtype == torch.float32
     assert size is None or rescale is None
+    Hb = Wb = ch = cw = 0
     if rescale is not None:
         (Hb, Wb), (ch, cw), (H, W) = rescale
     elif bits is not None:
@@ -1235,7 +1194,7 @@ def query_postprocess(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch
         H, W = 4 * hm, 4 * wm
     else:
         H, W = size
-    Hr = H
+    Hr, Wr = H, W
     if bits is None:
         masks = torch.empty(n, H, W, device=logits.device, dtype=torch.uint8)
     else:
@@ -1245,24 +1204,16 @@ def query_postprocess(logits: torch.Tensor, sel: torch.Tensor, cls_scores: torch
             assert bits.numel() == n * H * W // 8
         else:
             assert bits.dim() == 3 and bits.shape[0] == n
-            Hr = bits.shape[1]
+            Hr, Wr = bits.shape[1], bits.shape[2] * 8
     if scores is None:
         scores = torch.empty(n, device=logits.device, dtype=torch.float32)
     if boxes is None:
         boxes = torch.empty(n, 4, device=logits.device, dtype=torch.float32)
     assert scores.is_contiguous() and boxes.is_contiguous() and scores.numel() == n and boxes.numel() == 4 * n
     part = torch.empty(n * ((Hr + 15) // 16) * 6, device=logits.device, dtype=torch.float32)
-    args = (_ptr(logits), _ptr(sel), _ptr(cls_scores), n, hm, wm)
-    tail = (_ptr(masks if bits is None else bits), _ptr(part), _ptr(scores), _ptr(boxes), _stream())
-    if rescale is None and bits is None:
-        _check(_lib.rsp_query_postprocess(*args, H, W, *tail), "rsp_query_postprocess")
-    elif rescale is None:
-        _check(_lib.rsp_query_postprocess_bits(*args, *tail), "rsp_query_postprocess_bits")
-    elif bits is None:
-        _check(_lib.rsp_query_postprocess_rescale(*args, Hb, Wb, ch, cw, H, W, *tail), "rsp_query_postprocess_rescale")
-    else:
-        _check(_lib.rsp_query_postprocess_rescale_bits(*args, Hb, Wb, ch, cw, H, W, Hr, bits.shape[2] * 8, *tail),
-               "rsp_query_postprocess_rescale_bits")
+    _check(_lib.rsp_query_postprocess(_ptr(logits), _ptr(sel), _ptr(cls_scores), n, hm, wm, Hb, Wb, ch, cw, H, W, Hr,
+                                      Wr, int(bits is not None), _ptr(masks if bits is None else bits), _ptr(part),
+                                      _ptr(scores), _ptr(boxes), _stream()), "rsp_query_postprocess")
     launch_count += 2
     return (masks.view(torch.bool) if bits is None else bits), scores, boxes
 
@@ -1297,7 +1248,7 @@ def panoptic_postprocess(logits: torch.Tensor, keep: torch.Tensor, scores: torch
     _require_cuda(logits, keep, scores, labels)
     assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.shape[0] == B * nq
     _, hm, wm = logits.shape
-    H, W = size if rescale is None else rescale[2]
+    (Hb, Wb), (ch, cw), (H, W) = ((0, 0), (0, 0), size) if rescale is None else rescale
     dev = logits.device
     keep = keep.to(torch.uint8).contiguous()
     scores = scores.to(torch.float32).contiguous()
@@ -1308,15 +1259,10 @@ def panoptic_postprocess(logits: torch.Tensor, keep: torch.Tensor, scores: torch
     seg = torch.empty(B, nq, device=dev, dtype=torch.int32)
     pan = torch.empty(B, 1, H, W, device=dev, dtype=torch.int32)
     thr = ctypes.c_double(float(iou_thr))
-    head = (_ptr(logits), _ptr(keep), _ptr(scores), _ptr(labels), B, nq, hm, wm)
-    tail = (int(num_things), int(num_classes), ctypes.addressof(thr), int(bool(filter_low_score)), _ptr(idx), _ptr(bits),
-            _ptr(areas), _ptr(seg), _ptr(pan), _stream())
-    if rescale is None:
-        _check(_lib.rsp_panoptic_postprocess(*head, H, W, *tail), "rsp_panoptic_postprocess")
-    else:
-        (Hb, Wb), (ch, cw), _ = rescale
-        _check(_lib.rsp_panoptic_postprocess_rescale(*head, Hb, Wb, ch, cw, H, W, *tail),
-               "rsp_panoptic_postprocess_rescale")
+    _check(_lib.rsp_panoptic_postprocess(_ptr(logits), _ptr(keep), _ptr(scores), _ptr(labels), B, nq, hm, wm, Hb, Wb, ch,
+                                         cw, H, W, int(num_things), int(num_classes), ctypes.addressof(thr),
+                                         int(bool(filter_low_score)), _ptr(idx), _ptr(bits), _ptr(areas), _ptr(seg),
+                                         _ptr(pan), _stream()), "rsp_panoptic_postprocess")
     launch_count += 3
     return pan, dict(mask_area=areas[0], original_area=areas[1], segment_id=seg)
 

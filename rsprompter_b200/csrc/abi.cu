@@ -29,9 +29,15 @@ static GemmArgs make_gemm_args(const void* A, int lda, const void* W, int ldw, v
 
 int rsp_gemm_bf16(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M, int N,
                   int K, const float* bias, const void* residual, int ldr, int res_fp32, int res_mod,
-                  const int32_t* row_map, int act, int out_fp32, void* stream) {
-  return gemm_bf16(make_gemm_args(A, lda, W, ldw, out, ldo, M, N, K, bias, residual, ldr, res_fp32,
-                                  res_mod, row_map, act, out_fp32), S(stream));
+                  const int32_t* row_map, int act, int out_fp32, int epi_mode, const float* ln_gamma,
+                  const float* ln_beta, float ln_eps, const int32_t* res_block_map, int res_block_rows,
+                  const float* hyper, float* mask_out, int grid_h, int grid_w, void* stream) {
+  GemmArgs a = make_gemm_args(A, lda, W, ldw, out, ldo, M, N, K, bias, residual, ldr, res_fp32,
+                              res_mod, row_map, act, out_fp32);
+  a.epi_mode = epi_mode; a.ln_gamma = ln_gamma; a.ln_beta = ln_beta; a.ln_eps = ln_eps;
+  a.res_block_map = res_block_map; a.res_block_rows = res_block_rows;
+  a.hyper = hyper; a.mask_out = mask_out; a.grid_h = grid_h; a.grid_w = grid_w;
+  return gemm_bf16(a, S(stream));
 }
 
 int rsp_gemm_bf16_grouped(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M, int N, int K,
@@ -67,13 +73,8 @@ static AttentionArgs make_att_args(const void* qkv, const void* rel_h, const voi
   return a;
 }
 
-int rsp_vit_attention(const void* qkv, const void* rel_h, const void* rel_w, void* out, int n_seq,
-                      int T, int Sg, int H, int hd, void* stream) {
-  return vit_attention(make_att_args(qkv, rel_h, rel_w, out, n_seq, T, Sg, H, hd), S(stream));
-}
-
-int rsp_vit_attention_scatter(const void* qkv, const void* rel_h, const void* rel_w, void* out, int n_seq, int T,
-                              int Sg, int H, int hd, const int32_t* out_row_map, void* stream) {
+int rsp_vit_attention(const void* qkv, const void* rel_h, const void* rel_w, void* out, int n_seq, int T, int Sg,
+                      int H, int hd, const int32_t* out_row_map, void* stream) {
   return vit_attention(make_att_args(qkv, rel_h, rel_w, out, n_seq, T, Sg, H, hd, out_row_map), S(stream));
 }
 
@@ -140,20 +141,6 @@ int rsp_add_table_bf16(const void* x, const float* table, void* out, long long n
 
 extern "C" {
 
-int rsp_gemm_bf16_ex(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M, int N,
-                     int K, const float* bias, const void* residual, int ldr, int res_fp32, int res_mod,
-                     const int32_t* row_map, int act, int out_fp32, int epi_mode, const float* ln_gamma,
-                     const float* ln_beta, float ln_eps, const int32_t* res_block_map,
-                     int res_block_rows, const float* hyper, float* mask_out, int grid_h, int grid_w,
-                     void* stream) {
-  GemmArgs a = make_gemm_args(A, lda, W, ldw, out, ldo, M, N, K, bias, residual, ldr, res_fp32,
-                              res_mod, row_map, act, out_fp32);
-  a.epi_mode = epi_mode; a.ln_gamma = ln_gamma; a.ln_beta = ln_beta; a.ln_eps = ln_eps;
-  a.res_block_map = res_block_map; a.res_block_rows = res_block_rows;
-  a.hyper = hyper; a.mask_out = mask_out; a.grid_h = grid_h; a.grid_w = grid_w;
-  return gemm_bf16(a, S(stream));
-}
-
 int rsp_gemm_upscale_masks(const void* A, int lda, const void* W, int ldw, int M, int K, const float* bias,
                            const float* hyper, int n_out, float* mask_out, int grid_h, int grid_w, void* stream) {
   GemmArgs a = make_gemm_args(A, lda, W, ldw, nullptr, 0, M, 128, K, bias, nullptr, 0, 1, 0, nullptr, 0, 0);
@@ -198,44 +185,23 @@ int rsp_i2t_fused(const void* keys, int ldk, const void* wq, const float* qb, co
 
 extern "C" {
 
-int rsp_rpn_decode(const float* head_out, int ld, const int64_t* topk_idx, int K, int B, int H, int W,
-                   int A, int stride, const float* base_anchors, const float* stds4, float img_h, float img_w,
+int rsp_rpn_decode(const float* head_out, int ld, const int64_t* topk_idx, int K, int B, int H, int W, int A, int stride,
+                   const float* base_anchors, const float* stds4, float img_h, float img_w, const float* img_shapes,
                    float min_size, int out_off, int out_ld, float* boxes, float* scores, void* stream) {
   return rpn_decode(head_out, ld, reinterpret_cast<const long long*>(topk_idx), K, B, H, W, A, stride,
-                    base_anchors, stds4, img_h, img_w, nullptr, min_size, out_off, out_ld, boxes, scores, S(stream));
-}
-
-int rsp_rpn_decode_shapes(const float* head_out, int ld, const int64_t* topk_idx, int K, int B, int H, int W, int A,
-                          int stride, const float* base_anchors, const float* stds4, const float* img_shapes,
-                          float min_size, int out_off, int out_ld, float* boxes, float* scores, void* stream) {
-  RSP_CHECK_ARG(img_shapes, "rpn_decode_shapes: img_shapes is null");
-  return rpn_decode(head_out, ld, reinterpret_cast<const long long*>(topk_idx), K, B, H, W, A, stride,
-                    base_anchors, stds4, 0.f, 0.f, img_shapes, min_size, out_off, out_ld, boxes, scores, S(stream));
+                    base_anchors, stds4, img_h, img_w, img_shapes, min_size, out_off, out_ld, boxes, scores, S(stream));
 }
 
 int rsp_bbox_cls_decode(const float* cls, int ld_cls, const float* reg, int ld_reg, const float* rois,
                         const uint8_t* roi_valid, int n, int C, const float* stds4, float img_h, float img_w,
-                        float score_thr, float* scores, float* boxes, int64_t* labels, void* stream) {
-  return bbox_cls_decode(cls, ld_cls, reg, ld_reg, rois, roi_valid, n, C, stds4, img_h, img_w, nullptr, score_thr,
-                         scores, boxes, reinterpret_cast<long long*>(labels), S(stream));
-}
-
-int rsp_bbox_cls_decode_shapes(const float* cls, int ld_cls, const float* reg, int ld_reg, const float* rois,
-                               const uint8_t* roi_valid, int n, int C, const float* stds4, const float* img_shapes,
-                               float score_thr, float* scores, float* boxes, int64_t* labels, void* stream) {
-  RSP_CHECK_ARG(img_shapes, "bbox_cls_decode_shapes: img_shapes is null");
-  return bbox_cls_decode(cls, ld_cls, reg, ld_reg, rois, roi_valid, n, C, stds4, 0.f, 0.f, img_shapes, score_thr,
+                        const float* img_shapes, float score_thr, float* scores, float* boxes, int64_t* labels,
+                        void* stream) {
+  return bbox_cls_decode(cls, ld_cls, reg, ld_reg, rois, roi_valid, n, C, stds4, img_h, img_w, img_shapes, score_thr,
                          scores, boxes, reinterpret_cast<long long*>(labels), S(stream));
 }
 
 int rsp_nms_batched(const float* boxes, const int64_t* ids, const int32_t* nvalid, int B, int n, float thr,
-                    void* mask_ws, float* max_coord_ws, uint8_t* keep, void* stream) {
-  return nms_batched(boxes, reinterpret_cast<const long long*>(ids), nvalid, B, n, thr,
-                     static_cast<unsigned long long*>(mask_ws), max_coord_ws, keep, 0, S(stream));
-}
-
-int rsp_nms_batched_topk(const float* boxes, const int64_t* ids, const int32_t* nvalid, int B, int n, float thr,
-                         void* mask_ws, float* max_coord_ws, uint8_t* keep, int max_keep, void* stream) {
+                    void* mask_ws, float* max_coord_ws, uint8_t* keep, int max_keep, void* stream) {
   return nms_batched(boxes, reinterpret_cast<const long long*>(ids), nvalid, B, n, thr,
                      static_cast<unsigned long long*>(mask_ws), max_coord_ws, keep, max_keep, S(stream));
 }
@@ -274,9 +240,9 @@ int rsp_roi_align_nhwc(const void* const* feats, const float* const* pes, const 
   return roi_align_nhwc(feats, pes, Hs, Ws, scales, num_levels, rois, n, C, P, finest_scale, out, S(stream));
 }
 
-int rsp_mask_paste(const float* logits, uint8_t* out, int n, int hm, int wm, int H, int W, float thr,
-                   int mode, void* stream) {
-  return mask_paste(logits, out, n, hm, wm, H, W, thr, mode, S(stream));
+int rsp_mask_paste(const float* maps, uint8_t* out, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w,
+                   int H, int W, int Hr, int Wr, int packed, float thr, int mode, void* stream) {
+  return mask_paste(maps, out, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, Hr, Wr, packed, thr, mode, S(stream));
 }
 
 int rsp_sigmoid_f32(const float* in, float* out, long long n, void* stream) {
@@ -307,23 +273,12 @@ int rsp_groupnorm_nhwc(const void* x, float* stats_ws, const float* gamma, const
 }
 
 int rsp_ms_deform_attn_sample(const void* value, const float* ow, int ld_ow, const int32_t* hs, const int32_t* ws,
-                              int L, int P, int B, int NQ, void* out, void* stream) {
-  return ms_deform_attn_sample(value, ow, ld_ow, hs, ws, L, P, B, NQ, out, 128, S(stream));
-}
-
-int rsp_ms_deform_attn_sample_c(const void* value, const float* ow, int ld_ow, const int32_t* hs, const int32_t* ws,
-                                int L, int P, int B, int NQ, void* out, int channels, void* stream) {
+                              int L, int P, int B, int NQ, void* out, int channels, void* stream) {
   return ms_deform_attn_sample(value, ow, ld_ow, hs, ws, L, P, B, NQ, out, channels, S(stream));
 }
 
 int rsp_mha_small(const void* Q, int ldq, const void* K, int ldk, const void* V, int ldv, const uint64_t* mask_bits,
-                  int B, int nq, int nk, void* out, void* stream) {
-  return mha_small(Q, ldq, K, ldk, V, ldv, reinterpret_cast<const unsigned long long*>(mask_bits), B, nq, nk, out, 16,
-                   S(stream));
-}
-
-int rsp_mha_small_hd(const void* Q, int ldq, const void* K, int ldk, const void* V, int ldv, const uint64_t* mask_bits,
-                     int B, int nq, int nk, void* out, int head_dim, void* stream) {
+                  int B, int nq, int nk, void* out, int head_dim, void* stream) {
   return mha_small(Q, ldq, K, ldk, V, ldv, reinterpret_cast<const unsigned long long*>(mask_bits), B, nq, nk, out,
                    head_dim, S(stream));
 }
@@ -346,26 +301,11 @@ int rsp_sam_mask_embed(const float* masks, const float* const* wts, int B, int h
   return sam_mask_embed(masks, wts, B, hm, wm, h, w, eps, dense, S(stream));
 }
 
-int rsp_mask_paste_rescale(const float* maps, uint8_t* out, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w,
-                           int H, int W, float thr, int mode, void* stream) {
-  return mask_paste_rescale(maps, out, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, thr, mode, S(stream));
-}
-
-int rsp_query_postprocess_rescale(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst, int hm,
-                                  int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, uint8_t* masks,
-                                  float* part_ws, float* scores, float* boxes, void* stream) {
-  return query_postprocess_rescale(logits, sel, cls_scores, n_inst, hm, wm, Hb, Wb, crop_h, crop_w, H, W, masks, part_ws,
-                                   scores, boxes, S(stream));
-}
-
 int rsp_query_postprocess(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst, int hm, int wm,
-                          int H, int W, uint8_t* masks, float* part_ws, float* scores, float* boxes, void* stream) {
-  return query_postprocess(logits, sel, cls_scores, n_inst, hm, wm, H, W, masks, part_ws, scores, boxes, S(stream));
-}
-
-int rsp_query_postprocess_bits(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst, int hm,
-                               int wm, uint8_t* bits, float* part_ws, float* scores, float* boxes, void* stream) {
-  return query_postprocess_bits(logits, sel, cls_scores, n_inst, hm, wm, bits, part_ws, scores, boxes, S(stream));
+                          int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr, int Wr, int packed,
+                          uint8_t* masks, float* part_ws, float* scores, float* boxes, void* stream) {
+  return query_postprocess(logits, sel, cls_scores, n_inst, hm, wm, Hb, Wb, crop_h, crop_w, H, W, Hr, Wr, packed, masks,
+                           part_ws, scores, boxes, S(stream));
 }
 
 int rsp_mask_paste_boxes(const float* probs, const float* boxes, uint8_t* out, int n, int hm, int wm, int H, int W,
@@ -373,57 +313,23 @@ int rsp_mask_paste_boxes(const float* probs, const float* boxes, uint8_t* out, i
   return mask_paste_boxes(probs, boxes, out, n, hm, wm, H, W, thr, packed, S(stream));
 }
 
-int rsp_mask_paste_bits(const float* maps, uint8_t* bits, int n, int hm, int wm, float thr, int mode, void* stream) {
-  return mask_paste_bits(maps, bits, n, hm, wm, thr, mode, S(stream));
-}
-
-int rsp_mask_paste_rescale_bits(const float* maps, uint8_t* bits, int n, int hm, int wm, int Hb, int Wb, int crop_h,
-                                int crop_w, int H, int W, int Hr, int Wr, float thr, int mode, void* stream) {
-  return mask_paste_rescale_bits(maps, bits, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, Hr, Wr, thr, mode, S(stream));
-}
-
-int rsp_query_postprocess_rescale_bits(const float* logits, const int32_t* sel, const float* cls_scores, int n_inst,
-                                       int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr,
-                                       int Wr, uint8_t* bits, float* part_ws, float* scores, float* boxes,
-                                       void* stream) {
-  return query_postprocess_rescale_bits(logits, sel, cls_scores, n_inst, hm, wm, Hb, Wb, crop_h, crop_w, H, W, Hr, Wr,
-                                        bits, part_ws, scores, boxes, S(stream));
-}
-
 int rsp_panoptic_postprocess(const float* logits, const uint8_t* keep, const float* scores, const int32_t* labels,
-                             int n_img, int nq, int hm, int wm, int H, int W, int num_things, int num_classes,
-                             const double* iou_thr, int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws,
-                             int32_t* areas, int32_t* seg, int32_t* pan, void* stream) {
-  return panoptic_postprocess(logits, keep, scores, labels, n_img, nq, hm, wm, H, W, num_things, num_classes, iou_thr,
-                              filter_low_score, idx_ws, bits_ws, areas, seg, pan, S(stream));
-}
-
-int rsp_panoptic_postprocess_rescale(const float* logits, const uint8_t* keep, const float* scores,
-                                     const int32_t* labels, int n_img, int nq, int hm, int wm, int Hb, int Wb,
-                                     int crop_h, int crop_w, int H, int W, int num_things, int num_classes,
-                                     const double* iou_thr, int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws,
-                                     int32_t* areas, int32_t* seg, int32_t* pan, void* stream) {
-  return panoptic_postprocess_rescale(logits, keep, scores, labels, n_img, nq, hm, wm, Hb, Wb, crop_h, crop_w, H, W,
-                                      num_things, num_classes, iou_thr, filter_low_score, idx_ws, bits_ws, areas, seg,
-                                      pan, S(stream));
+                             int n_img, int nq, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                             int num_things, int num_classes, const double* iou_thr, int filter_low_score,
+                             uint16_t* idx_ws, uint32_t* bits_ws, int32_t* areas, int32_t* seg, int32_t* pan,
+                             void* stream) {
+  return panoptic_postprocess(logits, keep, scores, labels, n_img, nq, hm, wm, Hb, Wb, crop_h, crop_w, H, W, num_things,
+                              num_classes, iou_thr, filter_low_score, idx_ws, bits_ws, areas, seg, pan, S(stream));
 }
 
 int rsp_sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
                        float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                       float stability_score_thresh, int32_t* part_ws, int32_t* counts, int32_t* boxes,
-                       float* stability, uint8_t* keep, void* stream) {
+                       float stability_score_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1, int scene_h,
+                       int scene_w, int32_t* part_ws, int32_t* counts, int32_t* boxes, float* stability, uint8_t* keep,
+                       void* stream) {
   return sam_mask_stats(maps, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, thr, thr_hi, thr_lo, iou, pred_iou_thresh,
-                        stability_score_thresh, part_ws, counts, boxes, stability, keep, S(stream));
-}
-
-int rsp_sam_mask_stats_crop(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H,
-                            int W, float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                            float stability_score_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1,
-                            int scene_h, int scene_w, int32_t* part_ws, int32_t* counts, int32_t* boxes,
-                            float* stability, uint8_t* keep, void* stream) {
-  return sam_mask_stats_crop(maps, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, thr, thr_hi, thr_lo, iou, pred_iou_thresh,
-                             stability_score_thresh, crop_x0, crop_y0, crop_x1, crop_y1, scene_h, scene_w, part_ws,
-                             counts, boxes, stability, keep, S(stream));
+                        stability_score_thresh, crop_x0, crop_y0, crop_x1, crop_y1, scene_h, scene_w, part_ws, counts,
+                        boxes, stability, keep, S(stream));
 }
 
 }  // extern "C"

@@ -1024,25 +1024,48 @@ static int paste_px(const Sampler& s, unsigned char* out, int n, int H, int W, i
   return RSP_OK;
 }
 
-int mask_paste_rescale(const float* maps, unsigned char* out, int n, int hm, int wm, int Hb, int Wb, int crop_h,
-                       int crop_w, int H, int W, float thr, int mode, cudaStream_t stream) {
-  RSP_CHECK_ARG(maps && out && n > 0 && hm > 0 && wm > 0 && Hb > 0 && Wb > 0 && crop_h > 0 && crop_w > 0 &&
-                crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 && (mode == 1 || mode == 2),
-                "mask_paste_rescale: bad args (mode 1: > thr on raw maps, 2: >= thr on activated maps)");
-  const TwoResizes s{maps, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
-  return mode == 1 ? paste_px<1, false>(s, out, n, H, W, H, W, thr, stream)
-                   : paste_px<2, false>(s, out, n, H, W, H, W, thr, stream);
+// MODE 1 for mode 1, MODE 2 otherwise
+template <bool BITS, class Sampler>
+static int paste_px12(const Sampler& s, unsigned char* out, int n, int H, int W, int Hr, int Wr, float thr, int mode,
+                      cudaStream_t stream) {
+  return mode == 1 ? paste_px<1, BITS>(s, out, n, H, W, Hr, Wr, thr, stream)
+                   : paste_px<2, BITS>(s, out, n, H, W, Hr, Wr, thr, stream);
 }
 
-int mask_paste_rescale_bits(const float* maps, unsigned char* bits, int n, int hm, int wm, int Hb, int Wb, int crop_h,
-                            int crop_w, int H, int W, int Hr, int Wr, float thr, int mode, cudaStream_t stream) {
-  RSP_CHECK_ARG(maps && bits && n > 0 && hm > 0 && wm > 0 && Hb > 0 && Wb > 0 && crop_h > 0 && crop_w > 0 &&
-                crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 && H <= Hr && W <= Wr && Wr % 16 == 0 &&
-                (reinterpret_cast<uintptr_t>(bits) & 1) == 0 && (mode == 1 || mode == 2),
-                "mask_paste_rescale_bits: bad args (H <= Hr, W <= Wr, Wr % 16 == 0, 2-byte aligned bits; mode 1 or 2)");
+int mask_paste(const float* maps, unsigned char* out, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w,
+               int H, int W, int Hr, int Wr, int packed, float thr, int mode, cudaStream_t stream) {
+  RSP_CHECK_ARG(maps && out && n > 0 &&
+                (packed ? H <= Hr && W <= Wr && Wr % 16 == 0 && (reinterpret_cast<uintptr_t>(out) & 1) == 0
+                        : Hr == H && Wr == W),
+                "mask_paste: bad output (bytes: (Hr, Wr) = (H, W); bits: H <= Hr, W <= Wr, Wr % 16 == 0, 2-byte aligned)");
+  if (Hb == 0) {   // one resize (hm, wm) -> (H, W)
+    const bool x4 = H == 4 * hm && W == 4 * wm && wm % 4 == 0 && (reinterpret_cast<uintptr_t>(maps) & 15) == 0;
+    RSP_CHECK_ARG(packed ? x4 && Hr == H && Wr == W && (mode == 1 || mode == 2) : W % 16 == 0,
+                  "mask_paste: one resize needs W % 16 == 0; bit-packed, the x4 path only ((H, W) = (4hm, 4wm) = "
+                  "(Hr, Wr), wm % 4 == 0, 16-byte aligned maps; mode 1: > thr on raw maps, 2: >= thr on activated maps)");
+    if (x4 && mode != 0) {
+      const long long tiles = static_cast<long long>(n) * hm * (wm / 4);
+      const unsigned blocks = static_cast<unsigned>((tiles + 127) / 128);
+      if (packed) {
+        if (mode == 1) mask_paste_x4_kernel<1, true><<<blocks, 128, 0, stream>>>(maps, out, n, hm, wm, thr);
+        else mask_paste_x4_kernel<2, true><<<blocks, 128, 0, stream>>>(maps, out, n, hm, wm, thr);
+      } else {
+        if (mode == 1) mask_paste_x4_kernel<1, false><<<blocks, 128, 0, stream>>>(maps, out, n, hm, wm, thr);
+        else mask_paste_x4_kernel<2, false><<<blocks, 128, 0, stream>>>(maps, out, n, hm, wm, thr);
+      }
+      RSP_CHECK_LAUNCH();
+      return RSP_OK;
+    }
+    if (mode == 0) return paste_px<0, false>(OneResize<true, false>{maps, hm, wm, H, W}, out, n, H, W, H, W, thr, stream);
+    return paste_px12<false>(OneResize<false, false>{maps, hm, wm, H, W}, out, n, H, W, H, W, thr, mode, stream);
+  }
+  RSP_CHECK_ARG(hm > 0 && wm > 0 && Hb > 0 && Wb > 0 && crop_h > 0 && crop_w > 0 && crop_h <= Hb && crop_w <= Wb &&
+                H > 0 && W > 0 && (mode == 1 || mode == 2),
+                "mask_paste: bad args for two resizes (crop within (Hb, Wb); mode 1: > thr on raw maps, 2: >= thr on "
+                "activated maps)");
   const TwoResizes s{maps, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
-  return mode == 1 ? paste_px<1, true>(s, bits, n, H, W, Hr, Wr, thr, stream)
-                   : paste_px<2, true>(s, bits, n, H, W, Hr, Wr, thr, stream);
+  return packed ? paste_px12<true>(s, out, n, H, W, Hr, Wr, thr, mode, stream)
+                : paste_px12<false>(s, out, n, H, W, H, W, thr, mode, stream);
 }
 
 int mask_paste_boxes(const float* probs, const float* boxes, unsigned char* out, int n, int hm, int wm, int H, int W,
@@ -1057,7 +1080,7 @@ int mask_paste_boxes(const float* probs, const float* boxes, unsigned char* out,
 // ---------------------------------------------------------------------------------------
 // SAM automatic mask generation, per candidate mask (HF SamImageProcessor.post_process_masks(binarize=False) followed
 // by filter_masks' _compute_stability_score, > mask_threshold and _batched_mask_to_box): every pixel of the original-size
-// mask comes from the TwoResizes sampler of mask_paste_rescale_bits, so its > thr decision is that kernel's bit, and
+// mask comes from the TwoResizes sampler of mask_paste's two resizes, so its > thr decision is that kernel's bit, and
 // only integers leave a block.  Block m * bands + band covers rows [band * SMS_ROWS, +SMS_ROWS) of mask m (the bands of
 // a mask are consecutive blocks, so its low-res map is read while it is in L2); thread = 16 consecutive pixels of a
 // row, as in mask_paste_px_kernel.  part: int32 [n, bands, 7] = (count > thr_hi,
@@ -1200,11 +1223,16 @@ __global__ void crop_mask_stats_finish_kernel(const int* __restrict__ part, int 
                               crop);
 }
 
-static int sam_mask_stats_impl(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H,
-                               int W, float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                               float stability_thresh, int* part_ws, int* counts, int* boxes, float* stability,
-                               unsigned char* keep, const CropEdge* edge, cudaStream_t stream) {
+int sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
+                   float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
+                   float stability_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1, int scene_h,
+                   int scene_w, int* part_ws, int* counts, int* boxes, float* stability, unsigned char* keep,
+                   cudaStream_t stream) {
   const int bands = (H + SMS_ROWS - 1) / SMS_ROWS;
+  const bool crop = scene_h != 0;
+  RSP_CHECK_ARG(!crop || (iou && crop_x0 >= 0 && crop_y0 >= 0 && crop_x1 > crop_x0 && crop_y1 > crop_y0 &&
+                          crop_x1 <= scene_w && crop_y1 <= scene_h && crop_x1 - crop_x0 == W && crop_y1 - crop_y0 == H),
+                "sam_mask_stats: bad crop-edge args (iou needed; the crop box is the H x W mask's place in the scene)");
   RSP_CHECK_ARG(maps && part_ws && counts && boxes && stability && (!iou || keep) && n > 0 && hm > 0 && wm > 0 &&
                 Hb > 0 && Wb > 0 && crop_h > 0 && crop_w > 0 && crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 &&
                 static_cast<long long>(H) * W <= INT_MAX && static_cast<long long>(n) * bands <= INT_MAX,
@@ -1213,36 +1241,15 @@ static int sam_mask_stats_impl(const float* maps, int n, int hm, int wm, int Hb,
   sam_mask_stats_kernel<<<static_cast<unsigned>(n) * bands, SMS_THREADS, 0, stream>>>(s, H, W, thr, thr_hi, thr_lo,
                                                                                      bands, part_ws);
   RSP_CHECK_LAUNCH();
-  if (edge)
-    crop_mask_stats_finish_kernel<<<(n + 7) / 8, 256, 0, stream>>>(part_ws, n, bands, iou, pred_iou_thresh,
-                                                                    stability_thresh, counts, boxes, stability, keep,
-                                                                    *edge);
+  if (crop)
+    crop_mask_stats_finish_kernel<<<(n + 7) / 8, 256, 0, stream>>>(
+        part_ws, n, bands, iou, pred_iou_thresh, stability_thresh, counts, boxes, stability, keep,
+        CropEdge{crop_x0, crop_y0, crop_x1, crop_y1, scene_h, scene_w});
   else
     sam_mask_stats_finish_kernel<<<(n + 7) / 8, 256, 0, stream>>>(part_ws, n, bands, iou, pred_iou_thresh,
                                                                    stability_thresh, counts, boxes, stability, keep);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
-}
-
-int sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
-                   float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                   float stability_thresh, int* part_ws, int* counts, int* boxes, float* stability,
-                   unsigned char* keep, cudaStream_t stream) {
-  return sam_mask_stats_impl(maps, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, thr, thr_hi, thr_lo, iou, pred_iou_thresh,
-                             stability_thresh, part_ws, counts, boxes, stability, keep, nullptr, stream);
-}
-
-int sam_mask_stats_crop(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
-                        float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                        float stability_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1, int scene_h,
-                        int scene_w, int* part_ws, int* counts, int* boxes, float* stability, unsigned char* keep,
-                        cudaStream_t stream) {
-  RSP_CHECK_ARG(iou && crop_x0 >= 0 && crop_y0 >= 0 && crop_x1 > crop_x0 && crop_y1 > crop_y0 &&
-                crop_x1 <= scene_w && crop_y1 <= scene_h && crop_x1 - crop_x0 == W && crop_y1 - crop_y0 == H,
-                "sam_mask_stats_crop: bad args (iou needed; the crop box is the H x W mask's place in the scene)");
-  const CropEdge edge{crop_x0, crop_y0, crop_x1, crop_y1, scene_h, scene_w};
-  return sam_mask_stats_impl(maps, n, hm, wm, Hb, Wb, crop_h, crop_w, H, W, thr, thr_hi, thr_lo, iou, pred_iou_thresh,
-                             stability_thresh, part_ws, counts, boxes, stability, keep, &edge, stream);
 }
 
 __global__ void sigmoid_f32_kernel(const float4* __restrict__ in, float4* __restrict__ out, long long n4) {
@@ -1259,36 +1266,6 @@ int sigmoid_f32(const float* in, float* out, long long n, cudaStream_t stream) {
       reinterpret_cast<const float4*>(in), reinterpret_cast<float4*>(out), n / 4);
   RSP_CHECK_LAUNCH();
   return RSP_OK;
-}
-
-int mask_paste_bits(const float* maps, unsigned char* bits, int n, int hm, int wm, float thr, int mode,
-                    cudaStream_t stream) {
-  RSP_CHECK_ARG(maps && bits && n > 0 && wm % 4 == 0 && (mode == 1 || mode == 2) &&
-                (reinterpret_cast<uintptr_t>(maps) & 15) == 0 && (reinterpret_cast<uintptr_t>(bits) & 1) == 0,
-                "mask_paste_bits: x4 path only (wm % 4 == 0, mode 1: > thr on raw maps, 2: >= thr on activated maps)");
-  const long long tiles = static_cast<long long>(n) * hm * (wm / 4);
-  const unsigned blocks = static_cast<unsigned>((tiles + 127) / 128);
-  if (mode == 1) mask_paste_x4_kernel<1, true><<<blocks, 128, 0, stream>>>(maps, bits, n, hm, wm, thr);
-  else mask_paste_x4_kernel<2, true><<<blocks, 128, 0, stream>>>(maps, bits, n, hm, wm, thr);
-  RSP_CHECK_LAUNCH();
-  return RSP_OK;
-}
-
-int mask_paste(const float* logits, unsigned char* out, int n, int hm, int wm, int H, int W, float thr,
-               int mode, cudaStream_t stream) {
-  RSP_CHECK_ARG(logits && out && n > 0 && W % 16 == 0, "mask_paste: W must be a multiple of 16");
-  if (mode != 0 && H == 4 * hm && W == 4 * wm && wm % 4 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0) {
-    const long long tiles = static_cast<long long>(n) * hm * (wm / 4);
-    const unsigned blocks = static_cast<unsigned>((tiles + 127) / 128);
-    if (mode == 1) mask_paste_x4_kernel<1, false><<<blocks, 128, 0, stream>>>(logits, out, n, hm, wm, thr);
-    else mask_paste_x4_kernel<2, false><<<blocks, 128, 0, stream>>>(logits, out, n, hm, wm, thr);
-    RSP_CHECK_LAUNCH();
-    return RSP_OK;
-  }
-  if (mode == 0) return paste_px<0, false>(OneResize<true, false>{logits, hm, wm, H, W}, out, n, H, W, H, W, thr, stream);
-  const OneResize<false, false> s{logits, hm, wm, H, W};
-  return mode == 1 ? paste_px<1, false>(s, out, n, H, W, H, W, thr, stream)
-                   : paste_px<2, false>(s, out, n, H, W, H, W, thr, stream);
 }
 
 // ---------------------------------------------------------------------------------------

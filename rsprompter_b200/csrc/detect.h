@@ -27,25 +27,15 @@ int soft_nms_batched(const float* boxes, const float* scores, const long long* i
 int roi_align_nhwc(const void* const* feats, const float* const* pes, const int* Hs, const int* Ws,
                    const float* scales, int num_levels, const float* rois, int n, int C, int P,
                    float finest_scale, void* out, cudaStream_t stream);
-int mask_paste_rescale(const float* maps, unsigned char* out, int n, int hm, int wm, int Hb, int Wb, int crop_h,
-                       int crop_w, int H, int W, float thr, int mode, cudaStream_t stream);
-int mask_paste_rescale_bits(const float* maps, unsigned char* bits, int n, int hm, int wm, int Hb, int Wb, int crop_h,
-                            int crop_w, int H, int W, int Hr, int Wr, float thr, int mode, cudaStream_t stream);
-int mask_paste(const float* logits, unsigned char* out, int n, int hm, int wm, int H, int W, float thr,
-               int mode, cudaStream_t stream);
-int mask_paste_bits(const float* maps, unsigned char* bits, int n, int hm, int wm, float thr, int mode,
-                    cudaStream_t stream);
+int mask_paste(const float* maps, unsigned char* out, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w,
+               int H, int W, int Hr, int Wr, int packed, float thr, int mode, cudaStream_t stream);   // Hb = 0: one resize
 int mask_paste_boxes(const float* probs, const float* boxes, unsigned char* out, int n, int hm, int wm, int H, int W,
                      float thr, int packed, cudaStream_t stream);
 int sam_mask_stats(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
                    float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                   float stability_thresh, int* part_ws, int* counts, int* boxes, float* stability,
-                   unsigned char* keep, cudaStream_t stream);
-int sam_mask_stats_crop(const float* maps, int n, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
-                        float thr, float thr_hi, float thr_lo, const float* iou, float pred_iou_thresh,
-                        float stability_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1, int scene_h,
-                        int scene_w, int* part_ws, int* counts, int* boxes, float* stability, unsigned char* keep,
-                        cudaStream_t stream);
+                   float stability_thresh, int crop_x0, int crop_y0, int crop_x1, int crop_y1, int scene_h,
+                   int scene_w, int* part_ws, int* counts, int* boxes, float* stability, unsigned char* keep,
+                   cudaStream_t stream);   // scene_h = 0: no crop-edge rule
 int sigmoid_f32(const float* in, float* out, long long n, cudaStream_t stream);
 int pool2_nhwc(const void* in, void* out, int B, int H, int W, int C, int mode, cudaStream_t stream);
 int zero_border_nhwc(void* x, int N, int H, int W, int C, cudaStream_t stream);

@@ -17,7 +17,7 @@ struct GemmArgs {
   int act = 0;        // 0 none, 1 GELU (erf; gelu_fast on the wgmma kernel), 2 ReLU   (applied before the residual add)
   int out_fp32 = 0;
   int res_fp32 = 1;
-  // epilogue variants used by the mask decoder (see rsp_gemm_bf16_ex in rsp_b200.h)
+  // epilogue variants used by the mask decoder (see rsp_gemm_bf16 in rsp_b200.h)
   int epi_mode = 0;                   // 0 standard, 1 row LayerNorm, 2 LN over 64-column groups + GELU,
                                       // 3 GELU + hypernetwork dot + 2x2 mask scatter
   const float* ln_gamma = nullptr;

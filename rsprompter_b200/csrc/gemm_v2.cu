@@ -99,7 +99,7 @@ struct Dev {
   int res_fp32;
   int num_n_blocks;
   int num_tiles;
-  // EPI 1 - 3 (the mask decoder's fused epilogues, see rsp_gemm_bf16_ex in rsp_b200.h for the maths)
+  // EPI 1 - 3 (the mask decoder's fused epilogues, see rsp_gemm_bf16 in rsp_b200.h for the maths)
   const float* ln_gamma;
   const float* ln_beta;
   float ln_eps;

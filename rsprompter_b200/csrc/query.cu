@@ -1004,50 +1004,33 @@ static int query_px(const Sampler& s, const int* sel, const float* cls_scores, i
   return query_finalize(part_ws, nblk, cls_scores, n_inst, H, W, scores, boxes, stream);
 }
 
-int query_postprocess(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm, int H,
-                      int W, unsigned char* masks, float* part_ws, float* scores, float* boxes, cudaStream_t stream) {
-  RSP_CHECK_ARG(logits && sel && cls_scores && masks && part_ws && scores && boxes && n_inst > 0 && W % 4 == 0,
-                "query_postprocess: bad args");
-  if (H == 4 * hm && W == 4 * wm && wm % 4 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0) {
-    const int nblk = (H + QP_ROWS - 1) / QP_ROWS;
-    query_mask_x4_kernel<false><<<dim3(nblk, n_inst), 256, 0, stream>>>(logits, sel, hm, wm, masks, part_ws);
-    return query_finalize(part_ws, nblk, cls_scores, n_inst, H, W, scores, boxes, stream);
+int query_postprocess(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm, int Hb,
+                      int Wb, int crop_h, int crop_w, int H, int W, int Hr, int Wr, int packed, unsigned char* masks,
+                      float* part_ws, float* scores, float* boxes, cudaStream_t stream) {
+  RSP_CHECK_ARG(logits && sel && cls_scores && masks && part_ws && scores && boxes && n_inst > 0 &&
+                (packed || (Hr == H && Wr == W)), "query_postprocess: bad args (bytes: (Hr, Wr) = (H, W))");
+  if (Hb == 0) {   // one resize (hm, wm) -> (H, W)
+    const bool x4 = H == 4 * hm && W == 4 * wm && wm % 4 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0;
+    RSP_CHECK_ARG(packed ? x4 && Hr == H && Wr == W && (reinterpret_cast<uintptr_t>(masks) & 1) == 0 : W % 4 == 0,
+                  "query_postprocess: one resize needs W % 4 == 0; bit-packed, the x4 path only ((H, W) = (4hm, 4wm) = "
+                  "(Hr, Wr), wm % 4 == 0, 16-byte aligned logits)");
+    if (x4) {
+      const int nblk = (H + QP_ROWS - 1) / QP_ROWS;
+      if (packed) query_mask_x4_kernel<true><<<dim3(nblk, n_inst), 256, 0, stream>>>(logits, sel, hm, wm, masks, part_ws);
+      else query_mask_x4_kernel<false><<<dim3(nblk, n_inst), 256, 0, stream>>>(logits, sel, hm, wm, masks, part_ws);
+      return query_finalize(part_ws, nblk, cls_scores, n_inst, H, W, scores, boxes, stream);
+    }
+    return query_px<4, false>(OneResize<false, true>{logits, hm, wm, H, W}, sel, cls_scores, n_inst, H, W, H, W, masks,
+                              part_ws, scores, boxes, stream);
   }
-  return query_px<4, false>(OneResize<false, true>{logits, hm, wm, H, W}, sel, cls_scores, n_inst, H, W, H, W, masks, part_ws,
-                            scores, boxes, stream);
-}
-
-int query_postprocess_bits(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm,
-                           unsigned char* bits, float* part_ws, float* scores, float* boxes, cudaStream_t stream) {
-  RSP_CHECK_ARG(logits && sel && cls_scores && bits && part_ws && scores && boxes && n_inst > 0 && wm % 4 == 0 &&
-                (reinterpret_cast<uintptr_t>(logits) & 15) == 0 && (reinterpret_cast<uintptr_t>(bits) & 1) == 0,
-                "query_postprocess_bits: needs wm % 4 == 0 and 16-byte aligned logits (x4 path only)");
-  const int H = 4 * hm, W = 4 * wm;
-  const int nblk = (H + QP_ROWS - 1) / QP_ROWS;
-  query_mask_x4_kernel<true><<<dim3(nblk, n_inst), 256, 0, stream>>>(logits, sel, hm, wm, bits, part_ws);
-  return query_finalize(part_ws, nblk, cls_scores, n_inst, H, W, scores, boxes, stream);
-}
-
-int query_postprocess_rescale(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm,
-                              int Hb, int Wb, int crop_h, int crop_w, int H, int W, unsigned char* masks, float* part_ws,
-                              float* scores, float* boxes, cudaStream_t stream) {
-  RSP_CHECK_ARG(logits && sel && cls_scores && masks && part_ws && scores && boxes && n_inst > 0 && crop_h > 0 &&
-                crop_w > 0 && crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0, "query_postprocess_rescale: bad args");
+  RSP_CHECK_ARG(crop_h > 0 && crop_w > 0 && crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 &&
+                (!packed || (H <= Hr && W <= Wr && Wr % 16 == 0 && Wr <= 16384 &&
+                             (reinterpret_cast<uintptr_t>(masks) & 1) == 0)),
+                "query_postprocess: bad args for two resizes (crop within (Hb, Wb); bits: H <= Hr, W <= Wr, "
+                "Wr % 16 == 0, Wr <= 16384, 2-byte aligned)");
   const TwoResizes s{logits, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
-  return query_px<1, false>(s, sel, cls_scores, n_inst, H, W, H, W, masks, part_ws, scores, boxes, stream);
-}
-
-int query_postprocess_rescale_bits(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm,
-                                   int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr, int Wr,
-                                   unsigned char* bits, float* part_ws, float* scores, float* boxes,
-                                   cudaStream_t stream) {
-  RSP_CHECK_ARG(logits && sel && cls_scores && bits && part_ws && scores && boxes && n_inst > 0 && crop_h > 0 &&
-                crop_w > 0 && crop_h <= Hb && crop_w <= Wb && H > 0 && W > 0 && H <= Hr && W <= Wr &&
-                Wr % 16 == 0 && Wr <= 16384 && (reinterpret_cast<uintptr_t>(bits) & 1) == 0,
-                "query_postprocess_rescale_bits: bad args (H <= Hr, W <= Wr, Wr % 16 == 0, Wr <= 16384, 2-byte "
-                "aligned bits)");
-  const TwoResizes s{logits, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
-  return query_px<1, true>(s, sel, cls_scores, n_inst, H, W, Hr, Wr, bits, part_ws, scores, boxes, stream);
+  return packed ? query_px<1, true>(s, sel, cls_scores, n_inst, H, W, Hr, Wr, masks, part_ws, scores, boxes, stream)
+                : query_px<1, false>(s, sel, cls_scores, n_inst, H, W, H, W, masks, part_ws, scores, boxes, stream);
 }
 
 // ------------------------------------------------------------------------------------ panoptic post-process
@@ -1205,33 +1188,23 @@ static int panoptic_run(const Sampler& s, const uint8_t* keep, const float* scor
   return RSP_OK;
 }
 
-#define RSP_PANOPTIC_ARGS_OK                                                                                          \
-  (logits && keep && scores && labels && idx_ws && bits_ws && areas && seg && pan && n_img > 0 && n_img <= 65535 &&     \
-   nq > 0 && nq < PAN_NONE && hm > 0 && wm > 0 && H > 0 && W > 0 &&                                                     \
-   static_cast<long long>(H) * W <= 0x7fffffffLL - PAN_TILE && num_things >= 0 && num_things <= num_classes &&      \
-   num_classes < PAN_INSTANCE_OFFSET &&                                                                              \
-   static_cast<long long>(nq) * PAN_INSTANCE_OFFSET + num_classes <= 0x7fffffffLL && iou_thr)
-
 int panoptic_postprocess(const float* logits, const uint8_t* keep, const float* scores, const int* labels, int n_img,
-                         int nq, int hm, int wm, int H, int W, int num_things, int num_classes, const double* iou_thr,
-                         int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws, int* areas, int* seg, int* pan,
-                         cudaStream_t stream) {
-  RSP_CHECK_ARG(RSP_PANOPTIC_ARGS_OK, "panoptic_postprocess: bad args (nq < 65535, num_classes < 1000)");
-  return panoptic_run(OneResize<false, true>{logits, hm, wm, H, W}, keep, scores, labels, n_img, nq, H, W, num_things,
-                      num_classes, *iou_thr, filter_low_score, idx_ws, bits_ws, areas, seg, pan, stream);
-}
-
-int panoptic_postprocess_rescale(const float* logits, const uint8_t* keep, const float* scores, const int* labels,
-                                 int n_img, int nq, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
-                                 int num_things, int num_classes, const double* iou_thr, int filter_low_score,
-                                 uint16_t* idx_ws, uint32_t* bits_ws, int* areas, int* seg, int* pan,
-                                 cudaStream_t stream) {
-  RSP_CHECK_ARG(RSP_PANOPTIC_ARGS_OK && crop_h > 0 && crop_w > 0 && crop_h <= Hb && crop_w <= Wb,
-                "panoptic_postprocess_rescale: bad args (nq < 65535, num_classes < 1000, crop within the batch shape)");
+                         int nq, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int num_things,
+                         int num_classes, const double* iou_thr, int filter_low_score, uint16_t* idx_ws,
+                         uint32_t* bits_ws, int* areas, int* seg, int* pan, cudaStream_t stream) {
+  RSP_CHECK_ARG(logits && keep && scores && labels && idx_ws && bits_ws && areas && seg && pan && n_img > 0 &&
+                n_img <= 65535 && nq > 0 && nq < PAN_NONE && hm > 0 && wm > 0 && H > 0 && W > 0 &&
+                static_cast<long long>(H) * W <= 0x7fffffffLL - PAN_TILE && num_things >= 0 &&
+                num_things <= num_classes && num_classes < PAN_INSTANCE_OFFSET &&
+                static_cast<long long>(nq) * PAN_INSTANCE_OFFSET + num_classes <= 0x7fffffffLL && iou_thr &&
+                (Hb == 0 || (crop_h > 0 && crop_w > 0 && crop_h <= Hb && crop_w <= Wb)),
+                "panoptic_postprocess: bad args (nq < 65535, num_classes < 1000, crop within the batch shape)");
+  if (Hb == 0)   // one resize (hm, wm) -> (H, W)
+    return panoptic_run(OneResize<false, true>{logits, hm, wm, H, W}, keep, scores, labels, n_img, nq, H, W, num_things,
+                        num_classes, *iou_thr, filter_low_score, idx_ws, bits_ws, areas, seg, pan, stream);
   const TwoResizes s{logits, {hm, wm, Hb, Wb, crop_h, crop_w, H, W}};
   return panoptic_run(s, keep, scores, labels, n_img, nq, H, W, num_things, num_classes, *iou_thr, filter_low_score,
                       idx_ws, bits_ws, areas, seg, pan, stream);
 }
-#undef RSP_PANOPTIC_ARGS_OK
 
 }  // namespace rsp

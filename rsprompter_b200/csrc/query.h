@@ -15,26 +15,12 @@ int mask_embed_src(const float* mpp, const float* const* wts, const float* emb, 
                    int hm, int wm, int h, int w, float eps, void* src, void* src_pe, cudaStream_t stream);
 int sam_mask_embed(const float* masks, const float* const* wts, int B, int hm, int wm, int h, int w, float eps,
                    float* dense, cudaStream_t stream);
-int query_postprocess(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm, int H,
-                      int W, unsigned char* masks, float* part_ws, float* scores, float* boxes, cudaStream_t stream);
-
-int query_postprocess_bits(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm,
-                           unsigned char* bits, float* part_ws, float* scores, float* boxes, cudaStream_t stream);
-int query_postprocess_rescale(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm,
-                              int Hb, int Wb, int crop_h, int crop_w, int H, int W, unsigned char* masks, float* part_ws,
-                              float* scores, float* boxes, cudaStream_t stream);
-int query_postprocess_rescale_bits(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm,
-                                   int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int Hr, int Wr,
-                                   unsigned char* bits, float* part_ws, float* scores, float* boxes,
-                                   cudaStream_t stream);
+int query_postprocess(const float* logits, const int* sel, const float* cls_scores, int n_inst, int hm, int wm, int Hb,
+                      int Wb, int crop_h, int crop_w, int H, int W, int Hr, int Wr, int packed, unsigned char* masks,
+                      float* part_ws, float* scores, float* boxes, cudaStream_t stream);   // Hb = 0: one resize
 int panoptic_postprocess(const float* logits, const uint8_t* keep, const float* scores, const int* labels, int n_img,
-                         int nq, int hm, int wm, int H, int W, int num_things, int num_classes, const double* iou_thr,
-                         int filter_low_score, uint16_t* idx_ws, uint32_t* bits_ws, int* areas, int* seg, int* pan,
-                         cudaStream_t stream);
-int panoptic_postprocess_rescale(const float* logits, const uint8_t* keep, const float* scores, const int* labels,
-                                 int n_img, int nq, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W,
-                                 int num_things, int num_classes, const double* iou_thr, int filter_low_score,
-                                 uint16_t* idx_ws, uint32_t* bits_ws, int* areas, int* seg, int* pan,
-                                 cudaStream_t stream);
+                         int nq, int hm, int wm, int Hb, int Wb, int crop_h, int crop_w, int H, int W, int num_things,
+                         int num_classes, const double* iou_thr, int filter_low_score, uint16_t* idx_ws,
+                         uint32_t* bits_ws, int* areas, int* seg, int* pan, cudaStream_t stream);   // Hb = 0: one resize
 
 }  // namespace rsp

@@ -8,11 +8,11 @@ de-duplicates with a box NMS (post_process_for_mask_generation :432-446).  Here:
   * every image of the call is encoded in one batch, and the grids of all images run through the mask decoder in
     calls of ``points_per_batch`` prompts (prompts of several images share a call through the decoder's block maps);
   * ``rsp_sam_mask_stats`` reduces each call's low-res logits to three pixel counts, a box and the keep flag,
-    sampling every original-size pixel with the two-resizes-and-crop sampler of ``rsp_mask_paste_rescale_bits``:
+    sampling every original-size pixel with the two-resizes-and-crop sampler of ``rsp_mask_paste``:
     the original-size fp32 mask never exists;
   * one ``rsp_nms_batched`` + ``rsp_compact_keep`` per call de-duplicates every image's survivors, ties broken by
     candidate order (point-major, mask-minor, HF's ``flatten(0, 1)``);
-  * only the kept masks are pasted, as bits, by ``rsp_mask_paste_rescale_bits``; ``output_rle_mask=True`` encodes
+  * only the kept masks are pasted, as bits, by ``rsp_mask_paste``; ``output_rle_mask=True`` encodes
     them as COCO RLE on the GPU.
 
 The low-res logits of every candidate of every image of the call stay on the device until the NMS has run: 256 KB
@@ -29,7 +29,7 @@ components of the bit-packed masks by a block-based union-find), and a second ``
 changed after those it left alone: one more host synchronisation per call.
 
 ``generate_scene_masks`` runs the same stages over the overlapping windows of a whole scene (large_image's slicing),
-with HF's crop-edge rule applied in ``rsp_sam_mask_stats_crop``, RLE of the whole scene from each window's bits, and
+with HF's crop-edge rule applied in ``rsp_sam_mask_stats``, RLE of the whole scene from each window's bits, and
 one cross-window box NMS; ``coarse_patch_sizes`` adds layers of larger windows up to the whole scene, resized by
 ``rsp_resize_aa_pad_u8`` (SamImageProcessor's antialiased resize) and merged under the finer layers as SAM merges
 its crop layers.
@@ -150,7 +150,7 @@ def _candidates(sam, emb_nhwc, sizes, reshaped, p, crops=None) -> dict:
     """The grids of every image through the decoder in calls of points_per_batch prompts, each call's logits through
     rsp_sam_mask_stats.  -> per-candidate device tensors, candidate c of image b at [b, c] (point c // 3, mask c % 3).
     ``crops``: per image, ((x0, y0, x1, y1), (H, W)) when it is that crop box of an H x W scene; the keep flags then
-    include the crop-edge rule (rsp_sam_mask_stats_crop)."""
+    include the crop-edge rule (rsp_sam_mask_stats with scene_h > 0)."""
     B, g, C = emb_nhwc.shape[0], emb_nhwc.shape[1], emb_nhwc.shape[3]
     S = sam.varch.image_size
     dev = emb_nhwc.device

@@ -5,7 +5,7 @@ Registry types (M:744-759, 881-914): ``RSSamMaskDecoder``, ``RSSamPositionalEmbe
 ``pytorch_model.bin`` loads unchanged.
 
 Decoder data flow (HF:461-543 over HF:306-405), N prompts, Tt = 5 + P tokens, HW image tokens:
-  * every Linear / ConvTranspose is ``rsp_gemm_bf16(_ex)``; the LayerNorm that follows an
+  * every Linear / ConvTranspose is ``rsp_gemm_bf16``; the LayerNorm that follows an
     out_proj / lin2 is fused into that GEMM's epilogue (epi_mode 1), so the pre-norm sums never
     reach HBM;
   * ``k_proj(keys + pe) = k_proj(keys) + k_proj(pe)``: the positional half is projected once

@@ -219,7 +219,7 @@ def post_process_masks(masks, original_sizes, reshaped_input_sizes, mask_thresho
                        binarize: bool = True, pad_size=(1024, 1024)) -> list:
     """HF SamProcessor.post_process_masks on the device: per image, low-res logits [pb, n_out, h, w] -> bilinear to
     pad_size -> crop to the reshaped (resized, unpadded) input size -> bilinear to the original size -> > threshold, in
-    one fused kernel (rsp_mask_paste_rescale, the SAMDet path).  -> list of bool [pb, n_out, H, W]."""
+    one fused kernel (rsp_mask_paste through two resizes, the SAMDet path).  -> list of bool [pb, n_out, H, W]."""
     if not binarize:
         raise ValueError("post_process_masks computes binary masks only (binarize=False is not supported)")
     if len(original_sizes) != len(masks) or len(reshaped_input_sizes) != len(masks):
@@ -276,7 +276,7 @@ class RSSamModel(BaseModule):
 class SAMDet(BaseModule):
     """M:1060-1215: boxes from ``detector`` (or the ground truth with test_cfg.oracle_on, the reference's default)
     prompt the SAM ``segmentor``; masks go low-res logits -> img_shape -> crop to the resized image -> ori_shape -> > 0
-    in one fused kernel per image (rsp_mask_paste_rescale, no intermediate maps)."""
+    in one fused kernel per image (rsp_mask_paste through two resizes, no intermediate maps)."""
 
     def __init__(self, detector, segmentor, data_preprocessor=None, test_cfg=None, init_cfg=None):
         BaseModule.__init__(self, init_cfg=None)

@@ -332,8 +332,8 @@ def test_predict_attaches_per_image_shapes(model_and_sd):
 
 @pytest.mark.parametrize("n,K", [(3000, 50), (700, 1000), (64, 1)])
 def test_nms_early_stop_keeps_the_same_first_k(n, K):
-    """rsp_nms_batched_topk: stopping the greedy scan after max_keep kept candidates leaves the first K kept ones (all a
-    caller of batched_nms(...)[:max_per_img] reads) unchanged."""
+    """rsp_nms_batched with max_keep > 0: stopping the greedy scan after max_keep kept candidates leaves the first K kept
+    ones (all a caller of batched_nms(...)[:max_per_img] reads) unchanged."""
     from rsprompter_b200 import _lib
     g = torch.Generator().manual_seed(n + K)
     B = 3

@@ -150,7 +150,7 @@ def test_upscale2_bugs_are_far(h, w, one_hot):
 
 
 # ---------------------------------------------------------------------------------------------------- alignment
-def test_epilogue_shape_and_alignment_rejected_before_launch():
+def test_gemm_epilogue_shape_and_alignment_rejected_before_launch():
     """Every alignment the fused epilogues' vector accesses need, and the column count of epi_mode 2, is checked on
     the host: a call that breaks one returns RSP_ERR_INVALID before any device work (so these addresses are never
     dereferenced), with a message that names what was broken."""
@@ -162,9 +162,9 @@ def test_epilogue_shape_and_alignment_rejected_before_launch():
            out_fp32=0):
         M = 4 * grid[0] * grid[1] if epi == 3 else 256
         K = 64 if epi == 3 else 256
-        st = _lib._lib.rsp_gemm_bf16_ex(A, K, W, K, out, ldo, M, N, K, bias, res, 256 if res else 0, res_fp32, 0,
-                                        None, 0, out_fp32, epi, g, e, 1e-6, None, 0, hyper, mask, grid[0], grid[1],
-                                        None)
+        st = _lib._lib.rsp_gemm_bf16(A, K, W, K, out, ldo, M, N, K, bias, res, 256 if res else 0, res_fp32, 0,
+                                     None, 0, out_fp32, epi, g, e, 1e-6, None, 0, hyper, mask, grid[0], grid[1],
+                                     None)
         return st, (_lib._lib.rsp_last_error() or b"").decode()
 
     cases = [

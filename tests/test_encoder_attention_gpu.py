@@ -86,7 +86,7 @@ def test_flash_production_windows(name, H, hd):
 @pytest.mark.parametrize("grid", [32, 48, 64, 80])
 @pytest.mark.parametrize("H,hd", [(3, 80), (2, 64)])
 def test_scatter_store(grid, H, hd):
-    """rsp_vit_attention_scatter: windows of a B = 2 grid (padded to 42 / 56 / 70 / 84) stored through window_maps
+    """rsp_vit_attention with out_row_map: windows of a B = 2 grid (padded to 42 / 56 / 70 / 84) stored through window_maps
     into a NaN-prefilled [B g g, D] output.  Every token row is written and within the bound; with a second map that
     drops some real rows (-1), exactly those rows keep the NaN."""
     from rsprompter_b200 import _lib

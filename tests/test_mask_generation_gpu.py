@@ -1,5 +1,5 @@
 """Segment-everything on the GPU (ViT-B synthetic weights, seeded as in test_sam_prompts_gpu.py): rsp_sam_mask_stats
-against a float64 restatement of the two resizes and against the pasted bits of rsp_mask_paste_rescale_bits; then
+against a float64 restatement of the two resizes and against the bits rsp_mask_paste pastes through them; then
 generate_masks end to end against oracle.restate_mask_generation applied to the decoder outputs the GPU produced for the
 same grid, its batch and points_per_batch invariance, empty results, RLE strings, host synchronisations and the CLI."""
 import json

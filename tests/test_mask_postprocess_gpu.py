@@ -35,9 +35,9 @@ def _slot_bits(bytes_, Hr, Wr):
 
 @pytest.mark.parametrize("ori", [(150, 200), (151, 203), (97, 61)])
 @pytest.mark.parametrize("mode", [1, 2])
-def test_paste_rescale_bits_equal_packed_bytes(ori, mode):
-    """rsp_mask_paste_rescale_bits into (H, round_up16(W)) slots and into larger slots equals the bytes of
-    rsp_mask_paste_rescale, packed; at odd W the bits past column W are 0."""
+def test_paste_two_resize_bits_equal_packed_bytes(ori, mode):
+    """rsp_mask_paste through two resizes into bits in (H, round_up16(W)) slots and in larger slots equals its bytes,
+    packed; at odd W the bits past column W are 0."""
     H, W = ori
     maps = _logits(5, 64, 64, H * W + mode)
     thr = 0.0 if mode == 1 else 0.5
@@ -45,18 +45,18 @@ def test_paste_rescale_bits_equal_packed_bytes(ori, mode):
         maps = maps.sigmoid().contiguous()
     geo = (64, 64, *BATCH, *CROP, H, W)
     bytes_ = _u8(5, H, W)
-    _c("mask_paste_rescale", maps, bytes_, 5, *geo, thr, mode)
+    _c("mask_paste", maps, bytes_, 5, *geo, H, W, 0, thr, mode)
     assert 0 < bytes_.sum() < bytes_.numel()
     for Hr, Wr in [(H, (W + 15) // 16 * 16), (H + 9, (W + 15) // 16 * 16 + 32)]:
         bits = _u8(5, Hr, Wr // 8)
-        _c("mask_paste_rescale_bits", maps, bits, 5, *geo, Hr, Wr, thr, mode)
+        _c("mask_paste", maps, bits, 5, *geo, Hr, Wr, 1, thr, mode)
         assert torch.equal(bits, _slot_bits(bytes_, Hr, Wr))
 
 
 @pytest.mark.parametrize("ori", [(150, 200), (151, 203)])
-def test_query_rescale_bits_equal_packed_bytes(ori):
-    """rsp_query_postprocess_rescale_bits: the bits are the packed bytes of rsp_query_postprocess_rescale, and the
-    scores and boxes are identical, also for slots with more rows than the mask."""
+def test_query_two_resize_bits_equal_packed_bytes(ori):
+    """rsp_query_postprocess through two resizes: the bits are its packed bytes, and the scores and boxes are
+    identical, also for slots with more rows than the mask."""
     H, W = ori
     logits = _logits(9, 64, 64, W)
     sel = torch.tensor([3, 0, 8, 3, 5, 5], dtype=torch.int32, device="cuda")
@@ -66,13 +66,13 @@ def test_query_rescale_bits_equal_packed_bytes(ori):
     bytes_ = _u8(n, H, W)
     part = torch.empty(n * ((H + 15) // 16) * 6, device="cuda")
     s0, b0 = torch.empty(n, device="cuda"), torch.empty(n, 4, device="cuda")
-    _c("query_postprocess_rescale", logits, sel, cls, n, *geo, bytes_, part, s0, b0)
+    _c("query_postprocess", logits, sel, cls, n, *geo, H, W, 0, bytes_, part, s0, b0)
     assert 0 < bytes_.sum() < bytes_.numel()
     for Hr, Wr in [(H, (W + 15) // 16 * 16), (H + 40, (W + 15) // 16 * 16 + 16)]:
         bits = _u8(n, Hr, Wr // 8)
         part = torch.empty(n * ((Hr + 15) // 16) * 6, device="cuda")
         s1, b1 = torch.empty(n, device="cuda"), torch.empty(n, 4, device="cuda")
-        _c("query_postprocess_rescale_bits", logits, sel, cls, n, *geo, Hr, Wr, bits, part, s1, b1)
+        _c("query_postprocess", logits, sel, cls, n, *geo, Hr, Wr, 1, bits, part, s1, b1)
         assert torch.equal(bits, _slot_bits(bytes_, Hr, Wr))
         assert torch.equal(s0, s1) and torch.equal(b0, b1)
 
@@ -91,7 +91,7 @@ def test_paste_boxes_packed_equals_packed_bytes():
 
 
 @pytest.mark.parametrize("shape,size", [((3, 5, 7), (24, 32)), ((1, 9, 13), (16, 48)), ((2, 15, 11), (64, 16))])
-def test_paste_mode0_equals_sigmoid_then_mode2(shape, size):
+def test_paste_one_resize_mode0_equals_sigmoid_then_mode2(shape, size):
     """n * hm * wm not divisible by 4: rsp_mask_paste's mode 0 activates the taps in the kernel, with the arithmetic of
     rsp_sigmoid_f32 followed by mode 2."""
     from rsprompter_b200 import _lib
@@ -99,10 +99,10 @@ def test_paste_mode0_equals_sigmoid_then_mode2(shape, size):
     logits = _logits(n, hm, wm, hm * wm)
     assert logits.numel() % 4
     got, ref = _u8(n, *size), _u8(n, *size)
-    _c("mask_paste", logits, got, n, hm, wm, *size, 0.5, 0)
+    _c("mask_paste", logits, got, n, hm, wm, 0, 0, 0, 0, *size, *size, 0, 0.5, 0)
     pad = torch.zeros((logits.numel() + 3) // 4 * 4, device="cuda")
     pad[:logits.numel()] = logits.reshape(-1)
     act = _lib.sigmoid_f32(pad)
-    _c("mask_paste", act, ref, n, hm, wm, *size, 0.5, 2)
+    _c("mask_paste", act, ref, n, hm, wm, 0, 0, 0, 0, *size, *size, 0, 0.5, 2)
     assert 0 < ref.sum() < ref.numel()
     assert torch.equal(got, ref)

@@ -15,14 +15,14 @@ from rsprompter_b200.sam_config import SamDecoderArch, SamVisionArch, VISION_ARC
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_header_and_binding_export_the_same_symbols():
+def test_header_binding_and_library_export_the_same_abi_3_symbols():
     hdr = open(os.path.join(ROOT, "include", "rsp_b200.h")).read()
     declared = set(re.findall(r"\b(rsp_[a-z0-9_]+)\s*\(", hdr))
     assert declared == set(_lib.declared_symbols())
     lib = ctypes.CDLL(str(_lib.LIB_PATH))
     for name in declared:
         assert hasattr(lib, name), f"{name} missing from librsp_b200.so"
-    assert lib.rsp_abi_version() == 2
+    assert lib.rsp_abi_version() == 3
 
 
 def test_arch_name_parsing():

@@ -134,10 +134,14 @@ def test_device_transforms_reject_float_inputs():
         dp(dict(inputs=[torch.zeros(3, 40, 50, dtype=torch.float32)]))
 
 
-def test_header_declares_the_resize_entry_points():
+def test_header_declares_the_folded_resize_entry_points():
     from rsprompter_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "rsp_b200.h")).read()
-    for name in ("rsp_resize_pad_u8", "rsp_mask_paste_rescale_bits", "rsp_query_postprocess_rescale_bits"):
+    for name in ("rsp_resize_pad_u8", "rsp_mask_paste", "rsp_query_postprocess"):
         assert re.search(r"\bint\s+" + name + r"\s*\(", hdr), name
         assert name in _lib.declared_symbols()
-    assert re.search(r"#define\s+RSP_ABI_VERSION\s+2\b", hdr)
+    for name in ("rsp_mask_paste", "rsp_query_postprocess"):   # the rescale geometry and the record-slot bits
+        proto = re.search(r"\bint\s+" + name + r"\s*\(([^)]*)\)", hdr).group(1)
+        assert re.search(r"int Hb,\s*int Wb,\s*int crop_h,\s*int crop_w,\s*int H,\s*int W,\s*int Hr,\s*int Wr,\s*int packed",
+                         proto), name
+    assert re.search(r"#define\s+RSP_ABI_VERSION\s+3\b", hdr)

@@ -1,5 +1,5 @@
 """Segment-everything over a whole scene on the GPU (ViT-B synthetic weights, seeded as in test_mask_generation_gpu.py):
-rsp_sam_mask_stats_crop against rsp_sam_mask_stats and the oracle's crop-edge rule; generate_scene_masks on one window
+rsp_sam_mask_stats with the crop-edge rule against it without and the oracle's crop-edge rule; generate_scene_masks on one window
 against generate_masks; on six windows against oracle.restate_scene_mask_generation, with structured decoder outputs
 and end to end; batch-size invariance, host synchronisations, the refusals and the CLI."""
 import json
