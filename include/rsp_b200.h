@@ -509,6 +509,38 @@ int rsp_mask_rle_union_lengths(const uint8_t* src, int packed, const int64_t* de
 int rsp_mask_rle_union_write(const uint8_t* src, int packed, const int64_t* desc, int n, const int64_t* parts,
                              const int64_t* offsets, char* pool, int32_t* lengths, void* stream);
 
+/* ---- Mask borders as polygons: cv2.findContours(mask, RETR_CCOMP, approx) of every canvas, the call
+ * mmdet.structures.mask.bitmap_to_polygon makes per mask on the host (mmdet/structures/mask/structures.py:1166-1194:
+ * outs = cv2.findContours(bitmap.astype(np.uint8), cv2.RETR_CCOMP, cv2.CHAIN_APPROX_NONE)), which DetLocalVisualizer
+ * calls on every drawn mask.  approx = 1 (cv2.CHAIN_APPROX_NONE) or 2 (cv2.CHAIN_APPROX_SIMPLE).  Canvases are
+ * addressed as in rsp_mask_rle_union_* with bit-packed parts (pixel x = bit x % 8 of byte x / 8): desc int64 [n, 4] =
+ * (canvas H, W, first part, K), parts int64 [num_parts, 7] = (byte offset from src, row bytes, rows, visible h, w,
+ * origin y0, x0), in DEVICE memory and desc_host / parts_host, the same values in host memory.  One part covers a
+ * record slot or a tile mask placed in a scene; K > 1 the OR of greedy_nmm's members.  The union is formed only in
+ * the workspace, over the rectangle bounding the parts plus a one-pixel zero border; points are canvas coordinates.
+ * RSP_ERR_INVALID, nothing launched, on rsp_mask_rle_union_lengths's descriptor checks (with their messages), on a
+ * bounding rectangle of more than 2^31 - 1 pixels with its border, or on a workspace smaller than
+ * rsp_mask_contours_ws_bytes's (17 bytes per rectangle pixel, plus 40 per canvas).
+ *   rsp_mask_contours_lengths  contour_offsets int64 [n + 1]: first contour of canvas i, [n] = all contours;
+ *                              point_offsets int64 [n + 1]: first point of canvas i, [n] = all points (negative if a
+ *                              canvas has 2^31 points or more)
+ *   rsp_mask_contours_write    with the descriptors, approx and workspace the lengths call was given (it reads what
+ *                              that call left there) and its two arrays (canvas_points = its point_offsets):
+ *                              points int32 [all points, 2] of (x, y); point_offsets int64 [num_contours + 1], the
+ *                              first point of every contour; parents int32 [num_contours], the index of a hole's outer
+ *                              border within its canvas's list, -1 for an outer border.
+ * Per canvas, the contours come in cv2's order with cv2's start points; cv2's hierarchy follows from the parents.
+ * Atomics touch intermediate labels only: two calls give identical bytes. */
+int rsp_mask_contours_ws_bytes(const int64_t* desc_host, int n, const int64_t* parts_host, int num_parts,
+                               long long* bytes);
+int rsp_mask_contours_lengths(const uint8_t* src, const int64_t* desc, const int64_t* desc_host, int n,
+                              const int64_t* parts, const int64_t* parts_host, int num_parts, int approx, void* ws,
+                              long long ws_bytes, int64_t* contour_offsets, int64_t* point_offsets, void* stream);
+int rsp_mask_contours_write(const int64_t* desc_host, int n, const int64_t* parts_host, int num_parts, int approx,
+                            const void* ws, long long ws_bytes, const int64_t* contour_offsets,
+                            const int64_t* canvas_points, long long num_contours, int32_t* points,
+                            int64_t* point_offsets, int32_t* parents, void* stream);
+
 /* ---- DetDataPreprocessor on the device (SURVEY 8(f2); data_preprocessor.py:110-148, ImgDataPreprocessor.forward,
  * BatchFixedSizePad :300).  mean3 / std3: HOST arrays of 3 floats in OUTPUT channel order. ---- */
 

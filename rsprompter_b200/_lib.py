@@ -111,6 +111,10 @@ _SIGNATURES = {
     "rsp_mask_rle_placed_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp], _i),
     "rsp_mask_rle_union_lengths": ([_vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp], _i),
     "rsp_mask_rle_union_write": ([_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp], _i),
+    "rsp_mask_contours_ws_bytes": ([_vp, _i, _vp, _i, _vp], _i),
+    "rsp_mask_contours_lengths": ([_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, ctypes.c_longlong, _vp, _vp, _vp], _i),
+    "rsp_mask_contours_write": ([_vp, _i, _vp, _i, _i, _vp, ctypes.c_longlong, _vp, _vp, ctypes.c_longlong, _vp, _vp,
+                                 _vp, _vp], _i),
     "rsp_gemm_upscale_masks": ([_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _i, _vp], _i),
     "rsp_sam_mask_embed": ([_vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp], _i),
     "rsp_sam_mask_stats": ([_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _f, _f, _i, _i, _i, _i, _i, _i,
@@ -1543,3 +1547,128 @@ def _rle_strings(base: int, packed: bool, rows: list, dev, placed: bool, parts: 
         out.append(buf[p:p + ln])
         p += ln
     return out
+
+
+# ------------------------------------------------------------------------------ mask contours
+CHAIN_APPROX_NONE, CHAIN_APPROX_SIMPLE = 1, 2      # cv2's values
+# workspace bound of one contours call: canvases are split into calls that stay under it (a canvas larger than the
+# bound goes alone); 17 bytes per pixel of each canvas's padded parts rectangle
+CONTOURS_WS_BOUND = 1 << 30
+
+
+def mask_contours(sources: list, canvases: list, approx: int, ws_bound: int | None = None) -> list:
+    """cv2.findContours(canvas, cv2.RETR_CCOMP, approx) of canvases that are each the OR of one or more placed
+    bit-packed masks, neither the canvas nor the OR formed outside the workspace.  ``sources`` are contiguous uint8
+    CUDA tensors of bit-packed rows (pixel x = bit x % 8 of byte x // 8); ``canvases`` = [(H, W, parts)] exactly as
+    mask_rle_union takes them.  approx: CHAIN_APPROX_NONE or CHAIN_APPROX_SIMPLE.  -> per canvas (contours, hierarchy):
+    int32 [k, 2] (x, y) arrays in canvas coordinates and int32 [1, n, 4] (None without contours), cv2's output point for
+    point.  The canvases go in calls whose workspace stays under ``ws_bound`` bytes (CONTOURS_WS_BOUND); each call
+    synchronises with the host twice, for the totals and for the copy."""
+    import numpy as np
+    if approx not in (CHAIN_APPROX_NONE, CHAIN_APPROX_SIMPLE):
+        raise ValueError(f"approx must be CHAIN_APPROX_NONE (1) or CHAIN_APPROX_SIMPLE (2), got {approx}")
+    canvases = [(int(H), int(W), list(pl)) for H, W, pl in canvases]
+    if not canvases:
+        return []
+    if any(not pl for _, _, pl in canvases):
+        raise ValueError("every canvas needs at least one part")
+    _require_cuda(*sources)
+    base = min(t.data_ptr() for t in sources)
+    for t in sources:
+        assert t.is_contiguous() and t.dtype == torch.uint8, "sources are bit-packed uint8 rows"
+    rows, parts, need = [], [], []
+    for H, W, pl in canvases:
+        rows.append((H, W, len(parts), len(pl)))
+        y0 = x0 = 1 << 62
+        y1 = x1 = 0
+        for p in pl:
+            si, off, ld, nrows, h, w, py, px = (int(v) for v in p)
+            t = sources[si]
+            assert 0 <= off and off + (h - 1) * ld + (w + 7) // 8 <= t.numel(), "mask outside src"
+            parts.append((off + t.data_ptr() - base, ld, nrows, h, w, py, px))
+            y0, x0, y1, x1 = min(y0, py), min(x0, px), max(y1, py + h), max(x1, px + w)
+        need.append(40 + 17 * (y1 - y0 + 2) * (x1 - x0 + 2))
+    dev = sources[0].device
+    parts_host = torch.tensor(parts, dtype=torch.int64).pin_memory()
+    parts_d = parts_host.to(dev, non_blocking=True)
+    bound = CONTOURS_WS_BOUND if ws_bound is None else int(ws_bound)
+    out, i = [], 0
+    while i < len(rows):
+        j, acc = i + 1, need[i]
+        while j < len(rows) and acc + need[j] <= bound:
+            acc += need[j]
+            j += 1
+        out += _contours_call(base, rows[i:j], parts_d, parts_host, approx, dev, np)
+        i = j
+    return out
+
+
+def _contours_call(base: int, rows: list, parts_d, parts_host, approx: int, dev, np) -> list:
+    n = len(rows)
+    offs_host, points, point_offsets, parents = _contours_device(base, rows, parts_d, parts_host, approx, dev)
+    C, P = int(offs_host[0, n]), int(offs_host[1, n])
+    h_pts = torch.empty(points.shape, dtype=torch.int32, pin_memory=True)
+    h_po = torch.empty(C + 1, dtype=torch.int64, pin_memory=True)
+    h_par = torch.empty(parents.shape, dtype=torch.int32, pin_memory=True)
+    h_pts.copy_(points, non_blocking=True)
+    h_po.copy_(point_offsets, non_blocking=True)
+    h_par.copy_(parents, non_blocking=True)
+    torch.cuda.current_stream().synchronize()            # host sync 2: points, offsets, parents
+    pts, par = h_pts.numpy()[:P], h_par.numpy()
+    po = h_po.tolist()
+    contours = [pts[a:b] for a, b in zip(po[:-1], po[1:])]   # views; np.split costs 4x as much per contour
+    out = []
+    for i in range(n):
+        c0, c1 = int(offs_host[0, i]), int(offs_host[0, i + 1])
+        out.append((contours[c0:c1], _ccomp_hierarchy(par[c0:c1], np)))
+    return out
+
+
+def _contours_device(base: int, rows: list, parts_d, parts_host, approx: int, dev) -> tuple:
+    """The device half of one contours call: the lengths pass, host sync 1 for the totals, the write pass.  -> (host
+    int64 [2, n + 1] contour and point offsets per canvas, device points, point offsets, parents), written once the
+    stream reaches them."""
+    global launch_count
+    n, num_parts = len(rows), parts_host.shape[0]
+    desc_host = torch.tensor(rows, dtype=torch.int64).pin_memory()
+    desc = desc_host.to(dev, non_blocking=True)
+    nb = ctypes.c_longlong(0)
+    _check(_lib.rsp_mask_contours_ws_bytes(desc_host.data_ptr(), n, parts_host.data_ptr(), num_parts, ctypes.byref(nb)),
+           "rsp_mask_contours_ws_bytes")
+    ws = torch.empty(nb.value, dtype=torch.uint8, device=dev)
+    offs = torch.empty(2, n + 1, dtype=torch.int64, device=dev)
+    _check(_lib.rsp_mask_contours_lengths(base, _ptr(desc), desc_host.data_ptr(), n, _ptr(parts_d),
+                                          parts_host.data_ptr(), num_parts, approx, _ptr(ws), nb.value, _ptr(offs[0]),
+                                          _ptr(offs[1]), _stream()), "rsp_mask_contours_lengths")
+    offs_host = offs.cpu().numpy()                       # host sync 1: the totals
+    C, P = int(offs_host[0, n]), int(offs_host[1, n])
+    if P < 0:
+        raise RspError("rsp_mask_contours_lengths: a canvas has 2^31 or more contour points")
+    points = torch.empty(max(P, 1), 2, dtype=torch.int32, device=dev)
+    point_offsets = torch.empty(C + 1, dtype=torch.int64, device=dev)
+    parents = torch.empty(max(C, 1), dtype=torch.int32, device=dev)
+    _check(_lib.rsp_mask_contours_write(desc_host.data_ptr(), n, parts_host.data_ptr(), num_parts, approx, _ptr(ws),
+                                        nb.value, _ptr(offs[0]), _ptr(offs[1]), C, _ptr(points), _ptr(point_offsets),
+                                        _ptr(parents), _stream()), "rsp_mask_contours_write")
+    launch_count += 8
+    return offs_host, points, point_offsets, parents
+
+
+def _ccomp_hierarchy(par, np):
+    """cv2's RETR_CCOMP hierarchy [1, m, 4] = (next, prev, first child, parent) from the parents in list order, where
+    every outer border is followed by its holes; None for no contours."""
+    m = len(par)
+    if m == 0:
+        return None
+    h = np.full((m, 4), -1, np.int32)
+    h[:, 3] = par
+    o = np.flatnonzero(par < 0)
+    h[o[:-1], 0] = o[1:]
+    h[o[1:], 1] = o[:-1]
+    hole = par >= 0
+    s = np.flatnonzero(hole[1:] & (par[1:] == par[:-1])) + 1      # holes after a sibling
+    h[s, 1] = s - 1
+    h[s - 1, 0] = s
+    f = np.flatnonzero(hole[1:] & (par[1:] == np.arange(m - 1)))  # outer borders followed by their first hole
+    h[f, 2] = f + 1
+    return h[None]

@@ -425,6 +425,40 @@ int rsp_mask_rle_union_write(const uint8_t* src, int packed, const int64_t* desc
 
 }  // extern "C"
 
+#include "contours.h"
+
+extern "C" {
+
+int rsp_mask_contours_ws_bytes(const int64_t* desc_host, int n, const int64_t* parts_host, int num_parts,
+                               long long* bytes) {
+  return mask_contours_ws_bytes(reinterpret_cast<const long long*>(desc_host), n,
+                                reinterpret_cast<const long long*>(parts_host), num_parts, bytes);
+}
+
+int rsp_mask_contours_lengths(const uint8_t* src, const int64_t* desc, const int64_t* desc_host, int n,
+                              const int64_t* parts, const int64_t* parts_host, int num_parts, int approx, void* ws,
+                              long long ws_bytes, int64_t* contour_offsets, int64_t* point_offsets, void* stream) {
+  return mask_contours_lengths(src, reinterpret_cast<const long long*>(desc),
+                               reinterpret_cast<const long long*>(desc_host), n,
+                               reinterpret_cast<const long long*>(parts),
+                               reinterpret_cast<const long long*>(parts_host), num_parts, approx, ws, ws_bytes,
+                               reinterpret_cast<long long*>(contour_offsets), reinterpret_cast<long long*>(point_offsets),
+                               S(stream));
+}
+
+int rsp_mask_contours_write(const int64_t* desc_host, int n, const int64_t* parts_host, int num_parts, int approx,
+                            const void* ws, long long ws_bytes, const int64_t* contour_offsets,
+                            const int64_t* canvas_points, long long num_contours, int32_t* points,
+                            int64_t* point_offsets, int32_t* parents, void* stream) {
+  return mask_contours_write(reinterpret_cast<const long long*>(desc_host), n,
+                             reinterpret_cast<const long long*>(parts_host), num_parts, approx, ws, ws_bytes,
+                             reinterpret_cast<const long long*>(contour_offsets),
+                             reinterpret_cast<const long long*>(canvas_points), num_contours, points,
+                             reinterpret_cast<long long*>(point_offsets), parents, S(stream));
+}
+
+}  // extern "C"
+
 #include "regions.h"
 
 extern "C" {

@@ -34,6 +34,7 @@ import torch
 
 from . import _lib
 from .detectors import RSPrompterAnchor, RSPrompterQuery, SAMSegMaskRCNN
+from .geojson import feature_collection
 from .registry import DetDataSample, InstanceData
 from .results import ResultRecord, _align16
 
@@ -229,7 +230,8 @@ def _record_nbytes(B: int, M: int, hw: tuple) -> int:
 @torch.no_grad()
 def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr: float = 0.25,
                         score_thr: float = 0.0, batch_size: int = 8, patch_size: int | None = None,
-                        merge_nms_type: str = "nms", merge_match_metric: str = "ios") -> DetDataSample:
+                        merge_nms_type: str = "nms", merge_match_metric: str = "ios",
+                        output_polygons: bool = False) -> DetDataSample:
     """Detect a whole scene: slice, run the tiles in batches, merge across tiles, encode the kept masks.
 
     ``image`` is the scene as mmcv.imread decodes it, uint8 [H, W, 3] BGR: a numpy array or a tensor on the host
@@ -249,7 +251,9 @@ def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr
 
     Returns a DetDataSample with ori_shape = img_shape = (H, W), scale_factor (1, 1) and pred_instances: bboxes,
     scores, labels on the device in descending score order, masks a list of {'size': [H, W], 'counts': bytes} (the
-    test_cfg.rle_masks convention, passed through by CocoMetric.process)."""
+    test_cfg.rle_masks convention, passed through by CocoMetric.process).  ``output_polygons`` adds
+    pred_instances.polygons: per mask, mask_polygons' (contours, hierarchy) of the same scene mask, in scene pixel
+    coordinates (two more host synchronisations)."""
     _check_merge_args(merge_nms_type, merge_match_metric)
     records, batches = run_tiles(model, image, overlap_ratio, batch_size, patch_size=patch_size,
                                  merge_nms_type=merge_nms_type)
@@ -258,13 +262,16 @@ def predict_large_image(model, image, overlap_ratio: float = 0.25, merge_iou_thr
     merged = merge_tile_records(records, batches, (H, W), merge_iou_thr=merge_iou_thr, score_thr=score_thr,
                                 window=window, nms_type=merge_nms_type, match_metric=merge_match_metric)
     if merge_nms_type == "greedy_nmm":
-        masks = encode_merged_masks(records, batches, merged["members"], merged["member_offsets"], (H, W),
-                                    window=window)
+        canvases = _merged_canvases(records, batches, merged["members"], merged["member_offsets"], (H, W), window)
+        masks = _merged_rle(records, canvases)
     else:
-        masks = encode_kept_masks(records, batches, merged["source"], (H, W), window=window)
+        canvases = _kept_canvases(records, batches, merged["source"], (H, W), window)
+        masks = _kept_rle(records, canvases)
     ds = DetDataSample(metainfo=dict(ori_shape=(H, W), img_shape=(H, W), scale_factor=(1.0, 1.0)))
     ds.pred_instances = InstanceData(bboxes=merged["bboxes"], scores=merged["scores"], labels=merged["labels"],
                                      masks=masks)
+    if output_polygons:
+        ds.pred_instances.polygons = mask_polygons(records, canvases)
     return ds
 
 
@@ -365,21 +372,58 @@ def _run_resized_tiles(model, scene, batches, B, M, S, P, rec_hw, norm):
     return records
 
 
+def _kept_canvases(records: list, origins: list, source: torch.Tensor, scene_hw: tuple, window: tuple | None) -> list:
+    """Union-mode canvases of the kept masks (``source`` rows (record, image, slot)), one part each: the record's mask
+    placed at its tile origin in the H x W scene, cut to its tile window."""
+    H, W = int(scene_hw[0]), int(scene_hw[1])
+    return [(H, W, [_part(records, origins, r, b, s, H, W, window)]) for r, b, s in source.tolist()]
+
+
+def _merged_canvases(records: list, origins: list, members: torch.Tensor, member_offsets: torch.Tensor,
+                     scene_hw: tuple, window: tuple | None) -> list:
+    """Union-mode canvases of greedy_nmm's merged rows: row i's parts are its members'
+    members[member_offsets[i]:member_offsets[i + 1]] masks, placed as in _kept_canvases."""
+    H, W = int(scene_hw[0]), int(scene_hw[1])
+    mem = members.tolist()
+    offs = member_offsets.tolist()
+    return [(H, W, [_part(records, origins, r, b, s, H, W, window) for r, b, s in mem[offs[i]:offs[i + 1]]])
+            for i in range(len(offs) - 1)]
+
+
+def _part(records: list, origins: list, r: int, b: int, s: int, H: int, W: int, window: tuple | None) -> tuple:
+    """(record, byte offset, row bytes, rows, h, w, y0, x0) of slot s of image b of record r in the scene."""
+    rec = records[r]
+    P, M = rec.hw[0], rec.slots
+    ph, pw = window or rec.hw
+    ld = rec.hw[1] // 8
+    x0, y0 = origins[r][b]
+    return (r, (b * M + s) * P * ld, ld, P, min(ph, H - y0), min(pw, W - x0), y0, x0)
+
+
+def _kept_rle(records: list, canvases: list) -> list:
+    groups = [(records[r].buf, [(off, ld, rows, h, w, H, W, y0, x0)])
+              for H, W, [(r, off, ld, rows, h, w, y0, x0)] in canvases]
+    return [dict(size=[H, W], counts=c) for (H, W, _), c in zip(canvases, _lib.mask_rle_placed(groups, packed=True))]
+
+
+def _merged_rle(records: list, canvases: list) -> list:
+    return [dict(size=[H, W], counts=c) for (H, W, _), c in
+            zip(canvases, _lib.mask_rle_union([rec.buf for rec in records], canvases, packed=True))]
+
+
+def mask_polygons(records: list, canvases: list) -> list:
+    """Per canvas (_kept_canvases / _merged_canvases) the (contours, hierarchy) of cv2.findContours(scene mask,
+    RETR_CCOMP, CHAIN_APPROX_SIMPLE), traced on the GPU from the records' bits: int32 [k, 2] (x, y) scene pixel
+    indices and int32 [1, n, 4] (None for an empty mask); two host synchronisations per workspace-bounded call."""
+    return _lib.mask_contours([rec.buf for rec in records], canvases, _lib.CHAIN_APPROX_SIMPLE)
+
+
 def encode_kept_masks(records: list, origins: list, source: torch.Tensor, scene_hw: tuple,
                       window: tuple | None = None) -> list:
     """COCO RLE dicts of the kept masks (``source`` rows (record, image, slot) from merge_tile_records) as masks of
     the whole H x W scene, encoded from the records' bits; two host synchronisations.  ``window`` as in
     merge_tile_records."""
-    H, W = int(scene_hw[0]), int(scene_hw[1])
-    groups = []
-    for r, b, s in source.tolist():
-        rec = records[r]
-        P, M = rec.hw[0], rec.slots
-        ph, pw = window or rec.hw
-        ld = rec.hw[1] // 8
-        x0, y0 = origins[r][b]
-        groups.append((rec.buf, [((b * M + s) * P * ld, ld, P, min(ph, H - y0), min(pw, W - x0), H, W, y0, x0)]))
-    return [dict(size=[H, W], counts=c) for c in _lib.mask_rle_placed(groups, packed=True)]
+    return _kept_rle(records, _kept_canvases(records, origins, source, scene_hw, window))
 
 
 def encode_merged_masks(records: list, origins: list, members: torch.Tensor, member_offsets: torch.Tensor,
@@ -388,22 +432,7 @@ def encode_merged_masks(records: list, origins: list, members: torch.Tensor, mem
     member_offsets[i + 1]] (rows (record, image, slot) from merge_tile_records), each placed in the H x W scene at its
     tile origin and cut to its tile window, encoded by rsp_mask_rle_union_* from the records' bits (a group of one is
     the placed encode's string); two host synchronisations.  ``window`` as in merge_tile_records."""
-    H, W = int(scene_hw[0]), int(scene_hw[1])
-    mem = members.tolist()
-    offs = member_offsets.tolist()
-    canvases = []
-    for i in range(len(offs) - 1):
-        parts = []
-        for r, b, s in mem[offs[i]:offs[i + 1]]:
-            rec = records[r]
-            P, M = rec.hw[0], rec.slots
-            ph, pw = window or rec.hw
-            ld = rec.hw[1] // 8
-            x0, y0 = origins[r][b]
-            parts.append((r, (b * M + s) * P * ld, ld, P, min(ph, H - y0), min(pw, W - x0), y0, x0))
-        canvases.append((H, W, parts))
-    return [dict(size=[H, W], counts=c)
-            for c in _lib.mask_rle_union([rec.buf for rec in records], canvases, packed=True)]
+    return _merged_rle(records, _merged_canvases(records, origins, members, member_offsets, scene_hw, window))
 
 
 def coco_results(ds: DetDataSample, image_id=0, label_to_cat=None) -> list:
@@ -437,10 +466,14 @@ def build_parser() -> argparse.ArgumentParser:
                     help="window size; each window is resized to the model size (default: model-size windows, "
                          "not resized)")
     ap.add_argument("--out", default=None, help="JSON file for the result dicts (default: stdout)")
+    ap.add_argument("--out-format", default="coco", choices=("coco", "geojson"),
+                    help="coco: COCO result dicts with RLE masks; geojson: a FeatureCollection, one Feature per result "
+                         "with the mask's outlines as a MultiPolygon in pixel coordinates")
     return ap
 
 
-def main(argv=None) -> list:
+def main(argv=None):
+    """The CLI: the result dicts (--out-format coco) or the GeoJSON FeatureCollection, also returned."""
     args = build_parser().parse_args(argv)
 
     import cv2
@@ -457,8 +490,12 @@ def main(argv=None) -> list:
         raise FileNotFoundError(args.image)
     ds = predict_large_image(model, img, overlap_ratio=args.patch_overlap_ratio, merge_iou_thr=args.merge_iou_thr,
                              score_thr=args.score_thr, batch_size=args.batch_size, patch_size=args.patch_size,
-                             merge_nms_type=args.merge_nms_type, merge_match_metric=args.merge_match_metric)
+                             merge_nms_type=args.merge_nms_type, merge_match_metric=args.merge_match_metric,
+                             output_polygons=args.out_format == "geojson")
     res = coco_results(ds)
+    if args.out_format == "geojson":
+        res = feature_collection([{k: v for k, v in r.items() if k != "segmentation"} for r in res],
+                                 ds.pred_instances.polygons)
     text = json.dumps(res)
     if args.out:
         with open(args.out, "w") as f:

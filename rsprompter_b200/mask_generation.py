@@ -49,6 +49,7 @@ import numbers
 import torch
 
 from . import _lib
+from .geojson import feature_collection
 
 # SamImageProcessor defaults (image_processing_sam.py:61-75): ImageNet mean / std on [0, 1] pixels
 IMAGE_MEAN = (0.485, 0.456, 0.406)
@@ -307,9 +308,11 @@ def _remove_small_regions(out: list, min_area: float, iou_thr: float) -> list:
     return res
 
 
-def _add_rle(out: list, places: list | None = None) -> None:
-    """COCO RLE strings of every image's masks, in one batch on the GPU.  ``places``: per image, (SH, SW, y0, x0) to
-    encode its masks as masks of an SH x SW canvas that is zero but for the image at (y0, x0)."""
+def _add_rle(out: list, places: list | None = None, rle: bool = True, polygons: bool = False) -> None:
+    """COCO RLE strings (``rle``) and polygons (``polygons``) of every image's masks, each in one batch on the GPU from
+    the same placed descriptors.  ``places``: per image, (SH, SW, y0, x0) to encode its masks as masks of an SH x SW
+    canvas that is zero but for the image at (y0, x0).  Polygons are (contours, hierarchy) of cv2.findContours(canvas,
+    RETR_CCOMP, CHAIN_APPROX_SIMPLE): int32 [k, 2] (x, y) canvas pixel indices and int32 [1, n, 4] (None when empty)."""
     rle_groups, sizes = [], []
     for b, r in enumerate(out):
         bits = r["masks"]
@@ -319,9 +322,16 @@ def _add_rle(out: list, places: list | None = None) -> None:
         if k:
             ld = bits.shape[2]
             rle_groups.append((bits, [(j * H * ld, ld, H, H, W, SH, SW, y0, x0) for j in range(k)]))
-    strings = iter(_lib.mask_rle_placed(rle_groups, packed=True))
-    for r, size in zip(out, sizes):
-        r["rle"] = [dict(size=list(size), counts=next(strings)) for _ in range(r["masks"].shape[0])]
+    if rle:
+        strings = iter(_lib.mask_rle_placed(rle_groups, packed=True))
+        for r, size in zip(out, sizes):
+            r["rle"] = [dict(size=list(size), counts=next(strings)) for _ in range(r["masks"].shape[0])]
+    if polygons:
+        canvases = [(SH, SW, [(g, off, ld, rows, h, w, y0, x0)])
+                    for g, (_, pl) in enumerate(rle_groups) for off, ld, rows, h, w, SH, SW, y0, x0 in pl]
+        polys = iter(_lib.mask_contours([bits for bits, _ in rle_groups], canvases, _lib.CHAIN_APPROX_SIMPLE))
+        for r in out:
+            r["polygons"] = [next(polys) for _ in range(r["masks"].shape[0])]
 
 
 @torch.no_grad()
@@ -330,7 +340,7 @@ def generate_masks(model, images=None, *, pixel_values=None, original_sizes=None
                    stability_score_thresh: float = 0.95, stability_score_offset: float = 1.0,
                    mask_threshold: float = 0.0, crops_nms_thresh: float = 0.7, crops_n_layers: int = 0,
                    max_hole_area=None, max_sprinkle_area=None, min_mask_region_area: float = 0,
-                   output_rle_mask: bool = False) -> list:
+                   output_rle_mask: bool = False, output_polygons: bool = False) -> list:
     """Every mask of each image, as HF's mask-generation pipeline finds them with crops_n_layers=0.
 
     ``model``: an RSSamModel or SamModelB200.  Images go in one of two forms:
@@ -366,6 +376,8 @@ def generate_masks(model, images=None, *, pixel_values=None, original_sizes=None
       candidates        int64 [k] (host) candidate index: point * 3 + output mask
       size              (H, W)
       rle               with output_rle_mask: COCO compressed RLE dicts {'size': [H, W], 'counts': bytes}
+      polygons          with output_polygons: per mask (contours, hierarchy), cv2.findContours(mask, RETR_CCOMP,
+                        CHAIN_APPROX_SIMPLE) traced on the GPU from the same bits (two host synchronisations)
     All tensors but ``candidates`` are on the model's device.
 
     Memory: the low-res logits of every candidate of every image stay resident until the NMS, 3 x points_per_side^2 x
@@ -384,8 +396,8 @@ def generate_masks(model, images=None, *, pixel_values=None, original_sizes=None
     out = _outputs(cand, idx, counts, idx_host, float(mask_threshold), sam.varch.image_size)
     if min_area > 0:
         out = _remove_small_regions(out, min_area, float(crops_nms_thresh))
-    if output_rle_mask:
-        _add_rle(out)
+    if output_rle_mask or output_polygons:
+        _add_rle(out, rle=output_rle_mask, polygons=output_polygons)
     return out
 
 
@@ -454,7 +466,7 @@ def _chunks(counts: list, per_mask: list, budget: int) -> list:
 
 
 def _coarse_outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch.Tensor, p: dict, target_size: int,
-                    min_area: float, nms_thr: float, places: list) -> list:
+                    min_area: float, nms_thr: float, places: list, polygons: bool = False) -> list:
     """_outputs, then _remove_small_regions with min_area > 0, then _add_rle(places), for a batch of coarse-layer
     windows, with the kept masks pasted, cleaned and encoded in groups of at most COARSE_MASK_BYTES: the same rows and
     strings, without the masks.  Host synchronisations: the RLE's per group, one more for the second NMS."""
@@ -466,6 +478,7 @@ def _coarse_outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch
     valid = torch.zeros(B, K, device=dev, dtype=torch.bool)
     boxes = cand["boxes"].gather(1, idx[:, :K, None].expand(-1, -1, 4)).contiguous()
     rle = [[] for _ in range(B)]
+    polys = [[] for _ in range(B)]
     for group in _chunks(counts, per_mask, COARSE_MASK_BYTES):
         parts = []
         for b, j0, j1 in group:
@@ -473,9 +486,10 @@ def _coarse_outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch
             if min_area > 0:
                 unchanged[b, j0:j1], boxes[b, j0:j1] = _clean(bits, cand["sizes"][b][1], min_area)
             parts.append(dict(masks=bits, size=cand["sizes"][b]))
-        _add_rle(parts, places=[places[b] for b, _, _ in group])
+        _add_rle(parts, places=[places[b] for b, _, _ in group], polygons=polygons)
         for (b, _, _), r in zip(group, parts):
             rle[b].extend(r["rle"])
+            polys[b].extend(r.get("polygons", ()))
     out = []
     for b in range(B):
         k = counts[b]
@@ -485,6 +499,8 @@ def _coarse_outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch
                         stability_scores=cand["stability"][b].index_select(0, ci), boxes=boxes[b, :k].long(),
                         points=cand["points"][b].index_select(0, ci // cand["n_out"]),
                         candidates=idx_host[b, :k].clone(), rle=rle[b], size=cand["sizes"][b]))
+        if polygons:
+            out[-1]["polygons"] = polys[b]
     if min_area <= 0 or K == 0:
         return out
     rows_d, cnt, rows_h = _nms(unchanged, valid, boxes, nms_thr)
@@ -493,6 +509,8 @@ def _coarse_outputs(cand: dict, idx: torch.Tensor, counts: list, idx_host: torch
         r.update(scores=r["scores"].index_select(0, rows), stability_scores=r["stability_scores"].index_select(0, rows),
                  boxes=boxes[b].index_select(0, rows).long(), points=r["points"].index_select(0, rows),
                  candidates=r["candidates"][rh], rle=[r["rle"][i] for i in rh.tolist()])
+        if polygons:
+            r["polygons"] = [r["polygons"][i] for i in rh.tolist()]
     return out
 
 
@@ -518,7 +536,7 @@ def generate_scene_masks(model, scene, *, patch_size: int | None = None, overlap
                          stability_score_offset: float = 1.0, mask_threshold: float = 0.0,
                          crops_nms_thresh: float = 0.7, crops_n_layers: int = 0, max_hole_area=None,
                          max_sprinkle_area=None, min_mask_region_area: float = 0,
-                         coarse_patch_sizes: tuple = ()) -> dict:
+                         coarse_patch_sizes: tuple = (), output_polygons: bool = False) -> dict:
     """Every mask of a whole scene: generate_masks on overlapping windows, merged across windows.
 
     ``scene``: uint8 RGB [3, H, W] with any strides (a permuted HWC array is fine), on the host or the device; it is
@@ -567,6 +585,8 @@ def generate_scene_masks(model, scene, *, patch_size: int | None = None, overlap
 
     Returns one dict, rows in the merge's keep order, all in scene coordinates:
       rle               COCO compressed RLE dicts {'size': [H, W], 'counts': bytes}
+      polygons          with output_polygons: per mask (contours, hierarchy) of the same scene mask as generate_masks
+                        gives them, traced with the RLE from the same bits (two more host synchronisations each time)
       scores            fp32 [k] predicted IoU
       stability_scores  fp32 [k]
       boxes             int64 [k, 4] inclusive pixel xyxy
@@ -638,23 +658,24 @@ def generate_scene_masks(model, scene, *, patch_size: int | None = None, overlap
             idx, counts, idx_host = _nms(cand["iou"], cand["keep"], cand["boxes"], nms_thr)
             places = [(H, W, y0, x0) for x0, y0, _, _ in boxes_b]
             if l:
-                out = _coarse_outputs(cand, idx, counts, idx_host, p, S, min_area, nms_thr, places)
+                out = _coarse_outputs(cand, idx, counts, idx_host, p, S, min_area, nms_thr, places,
+                                      polygons=output_polygons)
                 del cand, idx
             else:
                 out = _outputs(cand, idx, counts, idx_host, p["mask_threshold"], S)
                 del cand, idx                                   # the batch's low-res logits
                 if min_area > 0:
                     out = _remove_small_regions(out, min_area, nms_thr)
-                _add_rle(out, places=places)
+                _add_rle(out, places=places, polygons=output_polygons)
                 for r in out:
                     del r["masks"]                              # only the rows and strings stay
             tiles.extend(out)
-        merged.append((l, _merge_tiles(tiles, crops, (H, W), nms_thr, dev)))
+        merged.append((l, _merge_tiles(tiles, crops, (H, W), nms_thr, dev, output_polygons)))
     if len(merged) == 1:
         res = merged[0][1]
         res["layers"] = torch.zeros(len(res["rle"]), device=dev, dtype=torch.int64)
         return res
-    return _merge_layers(merged, nms_thr, dev)
+    return _merge_layers(merged, nms_thr, dev, output_polygons)
 
 
 def _check_merge(N: int, what: str, dev) -> None:
@@ -669,7 +690,7 @@ def _check_merge(N: int, what: str, dev) -> None:
                            f"on {dev}; {free / 2**30:.2f} GiB are free")
 
 
-def _merge_layers(merged: list, nms_thr: float, dev) -> dict:
+def _merge_layers(merged: list, nms_thr: float, dev, polygons: bool = False) -> dict:
     """SAM's crop-layer rule over every layer's merged rows (``merged`` = [(layer, _merge_tiles result)], base first):
     one box NMS over their concatenation ranked by position (equal scores and a stable sort), so a row is dropped only
     by an earlier kept row, of its own layer or a finer one.  One host synchronisation."""
@@ -680,6 +701,8 @@ def _merge_layers(merged: list, nms_thr: float, dev) -> dict:
     cat = {key: torch.cat([m[key] for _, m in merged])
            for key in ("scores", "stability_scores", "boxes", "points", "tiles", "crop_boxes", "candidates")}
     res = dict(size=merged[0][1]["size"])
+    if polygons:
+        res["polygons"] = []
     if N == 0:
         return dict(res, rle=[], layers=layer_h.to(dev), **cat)
     idx, cnt, idx_host = _nms(torch.zeros(1, N, device=dev), torch.ones(1, N, device=dev, dtype=torch.bool),
@@ -689,10 +712,13 @@ def _merge_layers(merged: list, nms_thr: float, dev) -> dict:
     res.update({key: v.index_select(0, rows) for key, v in cat.items() if key != "candidates"})
     res.update(rle=[rle[i] for i in rows_h.tolist()], candidates=cat["candidates"][rows_h],
                layers=layer_h[rows_h].pin_memory().to(dev, non_blocking=True))
+    if polygons:
+        polys = [s for _, m in merged for s in m["polygons"]]
+        res["polygons"] = [polys[i] for i in rows_h.tolist()]
     return res
 
 
-def _merge_tiles(tiles: list, crops: list, hw: tuple, nms_thr: float, dev) -> dict:
+def _merge_tiles(tiles: list, crops: list, hw: tuple, nms_thr: float, dev, polygons: bool = False) -> dict:
     """The cross-window NMS of generate_scene_masks over every window's rows (in slice order, each in keep order)."""
     counts = [r["scores"].shape[0] for r in tiles]
     N = sum(counts)
@@ -704,6 +730,8 @@ def _merge_tiles(tiles: list, crops: list, hw: tuple, nms_thr: float, dev) -> di
                tiles=torch.zeros(0, device=dev, dtype=torch.int64),
                crop_boxes=torch.zeros(0, 4, device=dev, dtype=torch.int64),
                candidates=torch.zeros(0, dtype=torch.int64), size=(int(hw[0]), int(hw[1])))
+    if polygons:
+        res["polygons"] = []
     if N == 0:
         return res
     crop_d = crop_h.pin_memory().to(dev, non_blocking=True)
@@ -720,6 +748,9 @@ def _merge_tiles(tiles: list, crops: list, hw: tuple, nms_thr: float, dev) -> di
                boxes=boxes.index_select(0, rows), points=points.index_select(0, rows),
                tiles=tile_h[rows_h].pin_memory().to(dev, non_blocking=True), crop_boxes=crop_d.index_select(0, rows),
                candidates=torch.cat([r["candidates"] for r in tiles])[rows_h])
+    if polygons:
+        polys = [s for r in tiles for s in r["polygons"]]
+        res["polygons"] = [polys[i] for i in rows_h.tolist()]
     return res
 
 
@@ -750,7 +781,8 @@ def mask_dicts(result: dict) -> list:
     return out
 
 
-def main(argv=None) -> list:
+def main(argv=None):
+    """The CLI: the mask dicts (--out-format coco) or the GeoJSON FeatureCollection, also returned."""
     ap = argparse.ArgumentParser(description="Segment everything in one image with SAM (HF mask-generation, one crop "
                                              "layer) and write the masks as COCO RLE; with --patch-size, in a whole "
                                              "scene cut into overlapping windows")
@@ -778,6 +810,9 @@ def main(argv=None) -> list:
                          ">= the scene's long side is the whole scene) that find objects larger than the overlap; "
                          "each dict then has the \"layer\" it came from (0 = the --patch-size windows)")
     ap.add_argument("--out", default=None, help="JSON file for the mask dicts (default: stdout)")
+    ap.add_argument("--out-format", default="coco", choices=("coco", "geojson"),
+                    help="coco: the mask dicts with COCO RLE segmentations; geojson: a FeatureCollection, one Feature "
+                         "per mask with its outlines as a MultiPolygon in pixel coordinates")
     args = ap.parse_args(argv)
     if args.coarse_patch_sizes is not None and args.patch_size is None:
         ap.error("--coarse-patch-sizes needs --patch-size (scene mode)")
@@ -790,6 +825,7 @@ def main(argv=None) -> list:
     img = cv2.imread(args.image, cv2.IMREAD_COLOR)
     if img is None:
         raise FileNotFoundError(args.image)
+    geo = args.out_format == "geojson"
     kw = dict(points_per_side=args.points_per_side, points_per_batch=args.points_per_batch,
               pred_iou_thresh=args.pred_iou_thresh, stability_score_thresh=args.stability_score_thresh,
               stability_score_offset=args.stability_score_offset, mask_threshold=args.mask_threshold,
@@ -798,14 +834,16 @@ def main(argv=None) -> list:
         rgb = torch.from_numpy(cv2.cvtColor(img, cv2.COLOR_BGR2RGB)).permute(2, 0, 1)      # [3, H, W] view of HWC
         res = generate_scene_masks(model, rgb, patch_size=args.patch_size, overlap_ratio=args.patch_overlap_ratio,
                                    batch_size=args.batch_size, coarse_patch_sizes=tuple(args.coarse_patch_sizes or ()),
-                                   **kw)
+                                   output_polygons=geo, **kw)
     else:
         rgb = torch.from_numpy(img).permute(2, 0, 1).flip(0)                 # BGR HWC -> RGB [3, H, W] view
-        res = generate_masks(model, rgb.contiguous(), output_rle_mask=True, **kw)[0]
+        res = generate_masks(model, rgb.contiguous(), output_rle_mask=True, output_polygons=geo, **kw)[0]
     rows = mask_dicts(res)
     if args.coarse_patch_sizes is not None:
         for row, layer in zip(rows, res["layers"].tolist()):
             row["layer"] = layer
+    if geo:
+        rows = feature_collection([{k: v for k, v in r.items() if k != "segmentation"} for r in rows], res["polygons"])
     text = json.dumps(rows)
     if args.out:
         with open(args.out, "w") as f:

@@ -185,6 +185,51 @@ def record_to_coco_results(rec: "ResultRecord", image_ids: list, label_to_cat=No
     return out
 
 
+# ---- mask polygons ------------------------------------------------------------------------------------------------
+# What mmdet's DetLocalVisualizer does to every drawn mask: mmdet.structures.mask.bitmap_to_polygon
+# (mmdet/structures/mask/structures.py:1166-1194), cv2.findContours(RETR_CCOMP, CHAIN_APPROX_NONE) per mask on the host.
+# csrc/contours.cu computes the same contours on the device from the bit-packed masks; only the points are copied.
+def _polygons_from_bits(groups: list, approx: int) -> list:
+    """groups = [(bits uint8 [n, H, ceil(W/8)], W)] -> per mask (contours, hierarchy) in group order."""
+    from . import _lib
+    groups = [(b.contiguous(), int(W)) for b, W in groups if b.shape[0] > 0]
+    if not groups:
+        return []
+    canvases = []
+    for si, (b, W) in enumerate(groups):
+        n, H, ld = b.shape
+        canvases += [(H, W, [(si, j * H * ld, ld, H, H, W, 0, 0)]) for j in range(n)]
+    return _lib.mask_contours([b for b, _ in groups], canvases, approx)
+
+
+def _with_hole(contours, hierarchy):
+    if hierarchy is None:
+        return [], False
+    return contours, bool((hierarchy.reshape(-1, 4)[:, 3] >= 0).any())
+
+
+def bitmap_to_polygon(masks: torch.Tensor) -> list:
+    """Device counterpart of mmdet's bitmap_to_polygon for a batch: CUDA bool / uint8 masks [n, H, W] (nonzero = set)
+    -> one (contours, with_hole) per mask, contours int32 [k, 2] (x, y) arrays, exactly what the mmdet function returns
+    for that mask.  The masks are bit-packed and traced on the GPU in one call."""
+    from . import _lib
+    m = masks.contiguous()
+    if m.dtype == torch.uint8:
+        m = m != 0
+    return [_with_hole(c, h) for c, h in _polygons_from_bits([(_lib.pack_mask_bits(m), m.shape[-1])],
+                                                             _lib.CHAIN_APPROX_NONE)]
+
+
+def record_polygons(rec: "ResultRecord") -> list:
+    """Per image of a device record, one (contours, with_hole) per valid slot: bitmap_to_polygon of its masks, traced
+    from the record's bits."""
+    from . import _lib
+    W = rec.hw[1]
+    counts = rec.counts.tolist()
+    polys = iter(_polygons_from_bits([(rec.mask_bits[b, :n], W) for b, n in enumerate(counts)], _lib.CHAIN_APPROX_NONE))
+    return [[_with_hole(*next(polys)) for _ in range(n)] for n in counts]
+
+
 # ---- round-1 helpers kept for callers that only exchange the detection rows -------------------------------------
 def pack_records(bboxes: torch.Tensor, scores: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
     """[B,M,4], [B,M], [B,M] -> fp32 [B, M, 6]."""
