@@ -111,7 +111,9 @@ int rsp_vit_attention_simt(const void* qkv, const void* rel_h, const void* rel_w
  * copy_out (bf16 [rows_in, ld_copy] or NULL, fp32 input only): every source row read is also written back as bf16 -
  * the hidden states RSFeatureAggregator consumes (M:1046-1050) leave the encoder without a separate cast pass.
  * Replaces nn.LayerNorm (HF:894-896), SamLayerNorm channels_first (HF:147-170), mmpretrain
- * LayerNorm2d (norm.py:64-89) and LN2d (M:33-50) on channels-last data. */
+ * LayerNorm2d (norm.py:64-89) and LN2d (M:33-50) on channels-last data.
+ * C % 4 == 0, C <= 1280, ld_in and ld_out multiples of 4; in and out 16-byte aligned when fp32, 8-byte when bf16;
+ * gamma and beta 16-byte aligned; copy_out 8-byte aligned.  Anything else returns RSP_ERR_INVALID. */
 int rsp_layernorm(const void* in, int in_fp32, int ld_in, void* out, int out_fp32, int ld_out,
                   const float* gamma, const float* beta, const int32_t* src_map, int rows_out, int C,
                   float eps, int act, void* copy_out, int ld_copy, void* stream);
@@ -126,10 +128,13 @@ int rsp_layernorm_add(const void* x, const void* res, int res_fp32, const int32_
                       int pos_mod, void* out_pe, long long rows, int C, float eps, void* stream);
 
 /* fp32 NCHW image [B,3,H,W] -> bf16 [B*(H/16)*(W/16), 768] patch rows, k = c*256 + ky*16 + kx,
- * so that patch embedding (HF:116,128; mmcv PatchEmbed VS:455) is one rsp_gemm_bf16. */
+ * so that patch embedding (HF:116,128; mmcv PatchEmbed VS:455) is one rsp_gemm_bf16.
+ * B, H, W > 0, H and W multiples of 16, img and out 16-byte aligned; else RSP_ERR_INVALID. */
 int rsp_patchify16(const float* img, void* out, int B, int H, int W, void* stream);
 
-/* bf16 NHWC [B,H,W,C] -> [B*Ho*Wo, KH*KW*C] rows, k = (ky*KW + kx)*C + c, zero padding. */
+/* bf16 NHWC [B,H,W,C] -> [B*Ho*Wo, KH*KW*C] rows, k = (ky*KW + kx)*C + c, zero padding;
+ * Ho = (H + 2 pad - KH) / stride + 1, Wo likewise.  B, H, W > 0, C a positive multiple of 8, KH, KW, stride >= 1,
+ * pad >= 0, KH <= H + 2 pad and KW <= W + 2 pad (Ho, Wo >= 1), in and out 16-byte aligned; else RSP_ERR_INVALID. */
 int rsp_im2col_nhwc(const void* in, void* out, int B, int H, int W, int C, int KH, int KW,
                     int stride, int pad, void* stream);
 
@@ -592,11 +597,13 @@ int rsp_resize_aa_pad_u8(const int64_t* desc, const int64_t* desc_host, const in
 int rsp_patchify16_u8(const uint8_t* img, int hwc, void* out, int B, int H, int W, const float* mean3, const float* std3,
                       int swap_rb, void* stream);
 
-/* fp32 -> bf16 (n % 4 == 0): feeds fp32 hidden states to the bf16 tensor-core GEMMs. */
+/* fp32 -> bf16, round to nearest even (n % 4 == 0, in 16-byte and out 8-byte aligned): feeds fp32 hidden states to
+ * the bf16 tensor-core GEMMs. */
 int rsp_cast_f32_bf16(const float* in, void* out, long long n, void* stream);
 
 /* out = bf16(x + table[i % period]) on bf16 x: the RoI head's extra positional encoding added to one pyramid level
- * (x = [xi + pe_i ...], M:1566-1574), table fp32 [H*W*C], n and period multiples of 8. */
+ * (x = [xi + pe_i ...], M:1566-1574), table fp32 [H*W*C], n and period multiples of 8, x, table and out 16-byte
+ * aligned. */
 int rsp_add_table_bf16(const void* x, const float* table, void* out, long long n, long long period, void* stream);
 
 #ifdef __cplusplus

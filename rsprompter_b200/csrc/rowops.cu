@@ -13,6 +13,8 @@
 
 namespace rsp {
 
+static bool aligned(const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; }
+
 template <typename T>
 __device__ __forceinline__ float load_as_float(const T* p);
 template <>
@@ -140,6 +142,11 @@ int layernorm_rows(const LayerNormArgs& a, cudaStream_t stream) {
   RSP_CHECK_ARG(a.rows_out > 0 && a.C > 0 && a.C % 4 == 0 && a.C <= 1280, "layernorm: C=%d", a.C);
   RSP_CHECK_ARG(a.ld_in % 4 == 0 && a.ld_out % 4 == 0, "layernorm: ld must be multiple of 4");
   RSP_CHECK_ARG(!a.copy_out || (a.in_fp32 && a.ld_copy % 4 == 0 && a.ld_copy >= a.C), "layernorm: copy_out needs fp32 input");
+  // 4 elements per access: float4 / uint2 loads and stores of in, out and copy_out, float4 loads of gamma and beta
+  RSP_CHECK_ARG(aligned(a.in, a.in_fp32 ? 16 : 8), "layernorm: in must be %d-byte aligned", a.in_fp32 ? 16 : 8);
+  RSP_CHECK_ARG(aligned(a.out, a.out_fp32 ? 16 : 8), "layernorm: out must be %d-byte aligned", a.out_fp32 ? 16 : 8);
+  RSP_CHECK_ARG(aligned(a.gamma, 16) && aligned(a.beta, 16), "layernorm: gamma / beta must be 16-byte aligned");
+  RSP_CHECK_ARG(aligned(a.copy_out, 8), "layernorm: copy_out must be 8-byte aligned");
   if (a.in_fp32 && !a.out_fp32) return launch_ln<float, __nv_bfloat16>(a, stream);
   if (a.in_fp32 && a.out_fp32) return launch_ln<float, float>(a, stream);
   if (!a.in_fp32 && !a.out_fp32) return launch_ln<__nv_bfloat16, __nv_bfloat16>(a, stream);
@@ -178,7 +185,10 @@ __global__ void patchify16_kernel(const float* __restrict__ img, __nv_bfloat16* 
 
 int patchify16(const float* img, void* out, int B, int Himg, int Wimg, cudaStream_t stream) {
   RSP_CHECK_ARG(img && out, "patchify: null pointer");
-  RSP_CHECK_ARG(B > 0 && Himg % 16 == 0 && Wimg % 16 == 0, "patchify: bad shape");
+  RSP_CHECK_ARG(B > 0 && Himg > 0 && Wimg > 0 && Himg % 16 == 0 && Wimg % 16 == 0,
+                "patchify: shape B=%d H=%d W=%d (positive, H and W multiples of 16)", B, Himg, Wimg);
+  // float4 image loads, uint4 patch-row stores
+  RSP_CHECK_ARG(aligned(img, 16) && aligned(out, 16), "patchify: img / out must be 16-byte aligned");
   const long long total = static_cast<long long>(B) * (Himg / 16) * (Wimg / 16) * 48;
   const int threads = 256;
   patchify16_kernel<<<static_cast<unsigned>((total + threads - 1) / threads), threads, 0, stream>>>(
@@ -215,7 +225,15 @@ __global__ void im2col_nhwc_kernel(const __nv_bfloat16* __restrict__ in,
 int im2col_nhwc(const void* in, void* out, int B, int H, int W, int C, int KH, int KW, int stride,
                 int pad, cudaStream_t stream) {
   RSP_CHECK_ARG(in && out, "im2col: null pointer");
-  RSP_CHECK_ARG(C % 8 == 0 && B > 0 && H > 0 && W > 0, "im2col: C must be a multiple of 8");
+  RSP_CHECK_ARG(C > 0 && C % 8 == 0 && B > 0 && H > 0 && W > 0,
+                "im2col: shape B=%d H=%d W=%d C=%d (positive, C a multiple of 8)", B, H, W, C);
+  RSP_CHECK_ARG(KH >= 1 && KW >= 1 && stride >= 1 && pad >= 0, "im2col: kernel %dx%d stride %d pad %d", KH, KW, stride,
+                pad);
+  // at least one output pixel per axis, checked before the division that would otherwise round a negative span to 0
+  RSP_CHECK_ARG(H + 2 * pad >= KH && W + 2 * pad >= KW, "im2col: kernel %dx%d larger than the padded %dx%d input", KH,
+                KW, H + 2 * pad, W + 2 * pad);
+  // 8 channels (16 bytes) per access
+  RSP_CHECK_ARG(aligned(in, 16) && aligned(out, 16), "im2col: in / out must be 16-byte aligned");
   const int Ho = (H + 2 * pad - KH) / stride + 1, Wo = (W + 2 * pad - KW) / stride + 1;
   const long long total = static_cast<long long>(B) * Ho * Wo * KH * KW * (C / 8);
   const int threads = 256;
@@ -266,6 +284,7 @@ __global__ void cast_f32_bf16_kernel(const float4* __restrict__ in, uint2* __res
 
 int cast_f32_bf16(const float* in, void* out, long long n, cudaStream_t stream) {
   RSP_CHECK_ARG(in && out && n > 0 && n % 4 == 0, "cast: n must be a positive multiple of 4");
+  RSP_CHECK_ARG(aligned(in, 16) && aligned(out, 8), "cast: in must be 16-byte and out 8-byte aligned");   // float4 / uint2
   const long long n4 = n / 4;
   cast_f32_bf16_kernel<<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, stream>>>(
       reinterpret_cast<const float4*>(in), static_cast<uint2*>(out), n4);
@@ -394,6 +413,8 @@ __global__ void add_table_bf16_kernel(const uint4* __restrict__ x, const float* 
 
 int add_table_bf16(const void* x, const float* table, void* out, long long n, long long period, cudaStream_t stream) {
   RSP_CHECK_ARG(x && table && out && n > 0 && n % 8 == 0 && period > 0 && period % 8 == 0, "add_table: bad args");
+  // uint4 loads and stores of 8 bf16, float4 table loads
+  RSP_CHECK_ARG(aligned(x, 16) && aligned(table, 16) && aligned(out, 16), "add_table: x / table / out must be 16-byte aligned");
   const long long n8 = n / 8;
   add_table_bf16_kernel<<<static_cast<unsigned>((n8 + 255) / 256), 256, 0, stream>>>(
       static_cast<const uint4*>(x), table, static_cast<uint4*>(out), n8, period);
